@@ -43,6 +43,9 @@ def parse():
     ap.add_argument("--dp-diag", default="", choices=["", "nocomm"], help="multi-GPU diagnosis only: 'nocomm' skips the gradient allreduce")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the short BASELINE configs[2]/[3] side measurements")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write what the last timed step computed (its outputs and a fixed sample of the updated parameters) "
+                         "as DIR/<name>.npy, to compare two builds output for output")
     return ap.parse_args()
 
 
@@ -52,7 +55,8 @@ def measured_peaks():
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], bf16_tflops=d["bf16_tflops"], bf16_tflops_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0,
+                source="NVIDIA H100 SXM data sheet (dense bf16, 700 W card; not measured)")
 
 
 class ClockSampler(object):
@@ -138,7 +142,7 @@ def cpu_oracle_pairs_per_s(sample_b, steps, warmup, loss_type):
 
 
 def workload(loss_type):
-    """The same string in both arms (the driver compares the arms' configs)."""
+    """The same string in both arms, so that their results can be compared."""
     return "train step (BASELINE configs[1]): synthetic rho=45, 128x128 2-ch patches, batch 128 per GPU, loss_type=%s" % loss_type
 
 
@@ -160,6 +164,23 @@ def run_reference(args):
         "gpu_launches": 0,
     }
     print(json.dumps(line))
+
+
+DUMP_PARAM_SAMPLE = 1 << 20      # updated parameters written by --dump-outputs: a fixed, seeded sample (4 MB of 137 MB)
+
+
+def dump_outputs(d, out, params):
+    """The arrays a caller of train_step receives (pred_h4p, H_mat, pred_I2, photometric and h4p losses, lr) plus a fixed
+    sample of the parameters the step updated, as d/<name>.npy in float32 (float64 where the source is)."""
+    import numpy as np
+    import torch
+    os.makedirs(d, exist_ok=True)
+    arrays = {k: v for k, v in out.items() if not k.startswith("_")}
+    idx = np.sort(np.random.default_rng(0).choice(params.numel(), size=min(DUMP_PARAM_SAMPLE, params.numel()), replace=False))
+    arrays["params_sample"] = params[torch.from_numpy(idx).to(params.device)]
+    for k, v in arrays.items():
+        a = v.detach().cpu().numpy() if isinstance(v, torch.Tensor) else np.asarray(v)
+        np.save(os.path.join(d, k + ".npy"), a.astype(np.float64 if a.dtype == np.float64 else np.float32))
 
 
 def run_ours(args):
@@ -209,11 +230,13 @@ def run_ours(args):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for i in range(K):
-        eng.train_step(batches[i % nb])
+        out = eng.train_step(batches[i % nb])
     e1.record()
     barrier()
     ms_total = e0.elapsed_time(e1)
     launches = _lib.lib.udh_launch_count() - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out, eng.params)
     # ---- the same K steps again with the library's per-phase CUDA-event brackets (udh_prof_*): per-kernel durations for the
     # roofline.  Kept out of the headline region because ~80 event records per step serialise kernel boundaries. ----
     _lib.lib.udh_prof_enable(1); _lib.lib.udh_prof_reset()
@@ -299,9 +322,9 @@ def run_ours(args):
             if li == 0 or not tc:
                 add("conv3x3 fp32 CUDA-core kernels" if not tc else "conv1_1 CUDA-core kernels", tms, cnt, flops)
             elif kind == "wgrad":
-                add("tc_wgrad%s_kernel (tcgen05 weight gradient, conv1_2..conv4_2)" % ("_x3" if numeric == "bf16x3" else ""), tms, cnt, flops)
+                add("tc_wgrad%s_kernel (wgmma weight gradient, conv1_2..conv4_2)" % ("_x3" if numeric == "bf16x3" else ""), tms, cnt, flops)
             else:
-                add("tc_conv%s_kernel (tcgen05 implicit-GEMM conv fwd+dgrad, conv1_2..conv4_2)" % ("_x3" if numeric == "bf16x3" else ""), tms, cnt, flops)
+                add("tc_conv%s_kernel (wgmma implicit-GEMM conv fwd+dgrad, conv1_2..conv4_2)" % ("_x3" if numeric == "bf16x3" else ""), tms, cnt, flops)
         elif name == "adam":
             add("adam_kernel", tms, cnt, 0.0, 28.0 * 34192264 * cnt)
         elif name.startswith("fc"):
@@ -326,12 +349,6 @@ def run_ours(args):
             roof = {"kernel": name, "bound": "hbm", "achieved": ach, "peak": peaks["hbm_gbs"], "unit": "GB/s",
                     "frac": ach / peaks["hbm_gbs"] if ach else None, "traffic": None, "peak_source": peaks["source"],
                     "launches_per_step": cnt / K, "ms_per_step": tms / K, "share_of_step": share}
-        tr = os.path.join(ROOT, "profiles", "roofline_traffic.json")
-        if roof and os.path.exists(tr):
-            try:
-                roof["traffic"] = json.load(open(tr)).get(name.split(" ")[0])
-            except Exception:
-                pass
     extras = None
     if world == 1 and not args.no_extras:
         extras = other_configs(torch, _lib, engine, synthetic, numeric, peaks, dev)
@@ -341,7 +358,7 @@ def run_ours(args):
         v, ms_cpu, cores = cpu_oracle_pairs_per_s(sb, 2, 1, args.loss_type)
         cpu = {"value": v, "unit": "pairs/s", "cores": cores, "kind": "port",
                "sample": "%d-pair sample of the 128-pair batch, 1 warm-up + 2 timed train steps of oracle/ (PyTorch-CPU fp32 restatement)" % sb}
-    dtype = {"bf16x3": "bf16x3 (two bf16 limbs per fp32 value, lo.hi + hi.hi + hi.lo on tcgen05, fp32 TMEM accumulation: fp32-grade, parity-certified)",
+    dtype = {"bf16x3": "bf16x3 (two bf16 limbs per fp32 value, lo.hi + hi.hi + hi.lo on wgmma, fp32 register accumulation: fp32-grade, parity-certified)",
              "bf16": "bf16 (single pass, fp32 accumulation: throughput mode, NOT parity-certified)", "fp32": "fp32 (CUDA cores)"}[numeric]
     parity = None
     if world == 1 and not args.no_extras:
@@ -353,7 +370,7 @@ def run_ours(args):
         "config": {"workload": workload(args.loss_type),
                    "per_gpu_batch": B, "global_batch": B * world, "parallelism": "dp%d" % world, "numeric_mode": numeric,
                    "dropout": "on (keep 0.5)", "optimizer": "TF-Adam lr 5e-4 staircase",
-                   "l2_policy": "inputs larger than L2: %d rotating batches, 135 MB of inputs + ~1.7 GB of activations touched per step (L2 = 126 MB)" % nb},
+                   "l2_policy": "inputs larger than L2: %d rotating batches, 135 MB of inputs + ~1.7 GB of activations touched per step (L2 = 50 MB)" % nb},
         "clocks": clocks, "e2e": e2e, "gpu_launches": int(launches), "roofline": roof, "cpu_baseline": cpu,
         "tflops_algorithmic": TRAIN_FLOP_PER_PAIR * B * world / (ms_step * 1e-3) / 1e12,
         "phases_ms_per_step": {k: round(v[0] / K, 4) for k, v in sorted(phases.items(), key=lambda kv: -kv[1][0])},
@@ -423,7 +440,7 @@ def other_configs(torch, _lib, engine, synthetic, numeric, peaks, dev):
         out["configs[2] error"] = repr(e)[:200]
     try:
         B4, Hh, W = 64, 240, 320
-        nb = 4                                                 # 4 x 39.3 MB of inputs rotate through the 126 MB L2
+        nb = 4                                                 # 4 x 39.3 MB of inputs rotate through the 50 MB L2
         g = torch.Generator(device=dev).manual_seed(5)
         src = [torch.randn(B4, Hh, W, 1, device=dev, generator=g) for _ in range(nb)]
         tgt = [torch.randn(B4, Hh, W, 1, device=dev, generator=g) for _ in range(nb)]
@@ -449,7 +466,7 @@ def other_configs(torch, _lib, engine, synthetic, numeric, peaks, dev):
             "pairs_per_s": B4 / (ms * 1e-3), "us_per_launch": ms * 1e3,
             "roofline": {"bound": "hbm", "achieved": byts / (ms * 1e-3) / 1e9, "peak": peaks["hbm_gbs"], "unit": "GB/s",
                          "frac": byts / (ms * 1e-3) / 1e9 / peaks["hbm_gbs"], "algorithmic_bytes_per_launch": byts,
-                         "l2_policy": "4 rotating input sets of 39.3 MB (157 MB > 126 MB L2)"}}
+                         "l2_policy": "4 rotating input sets of 39.3 MB (157 MB > 50 MB L2)"}}
     except Exception as e:
         out["configs[3] error"] = repr(e)[:200]
     return out

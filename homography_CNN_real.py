@@ -7,7 +7,7 @@
   * test: the ground truth is four hand-picked correspondences per pair; the error is the RMSE of the predicted positions of
     those points on the full-size images, bounded by the identity error (:578-612; real_metrics.correspondence_errors).
 Images are 142 x 190 at the network (AREA-resized from 240 x 320 "full" images), patches 128 x 128, RHO = 24 (:17-23).
-The arithmetic runs in libudh's sm_100a kernels exactly as for the synthetic path (same engine, one process per GPU).
+The arithmetic runs in libudh's sm_90a kernels exactly as for the synthetic path (same engine, one process per GPU).
 The classical baselines (RANSAC / direct, --do_report) and the visualisations are out of scope (DESIGN.md §8).
 
 New flags: --synthetic N (on-device stand-in pairs at the real-data geometry: the aerial set is private), --seed,

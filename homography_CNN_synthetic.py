@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Drop-in entry point for the reference's `code/homography_CNN_synthetic.py` (flags :49-85, train() :151-389,
 TestHomography :391-580): same flags, modes, printed metrics and checkpoint cadence; the arithmetic runs in libudh's
-sm_100a CUDA kernels, one process per GPU (torchrun) with one NCCL gradient allreduce per step.
+sm_90a CUDA kernels, one process per GPU (torchrun) with one NCCL gradient allreduce per step.
 
 New flags: --synthetic N (generate N pairs on the device instead of reading <data_path>/I, I_prime — MS-COCO is not
 available offline), --seed, --numeric {bf16x3,bf16,fp32} (default bf16x3: the parity-certified tensor-core mode),
@@ -69,7 +69,7 @@ def build_parser():
     # new
     p.add_argument('--synthetic', type=int, default=0, help='generate this many pairs on the device instead of reading data_path')
     p.add_argument('--seed', type=int, default=0)
-    # bf16x3 = tcgen05 tensor cores with two-limb (fp32-grade) operands: the parity-certified default.  bf16 = single-pass
+    # bf16x3 = wgmma tensor cores with two-limb (fp32-grade) operands: the parity-certified default.  bf16 = single-pass
     # throughput mode (tenths of a pixel from fp32 on a trained net), fp32 = CUDA cores.
     p.add_argument('--numeric', type=str, default='bf16x3', choices=['fp32', 'bf16', 'bf16x3'])
     p.add_argument('--num_total_steps', type=int, default=150000)

@@ -1,5 +1,5 @@
 /*
- * libudh.so — C ABI of the B200-native unsupervised-deep-homography hot path.
+ * libudh.so — C ABI of the H100-native unsupervised-deep-homography hot path.
  *
  * The reference (tynguyen/unsupervisedDeepHomographyRAL2018) is a pure-Python TF1 graph and has no FFI of its
  * own; each entry point below replaces the group of TF ops cited next to it (file:line under /root/reference/code).
@@ -32,11 +32,11 @@ extern "C" {
 #define UDH_EWS (-4)    /* workspace too small                              */
 
 /* numeric mode of the regressor (udh_cnn_*).  FP32: CUDA-core fp32 everywhere — the parity mode.
- * BF16: tcgen05 bf16 tensor-core tiles with fp32 TMEM accumulation, fp32 master weights — the throughput mode. */
+ * BF16: wgmma bf16 tensor-core tiles with fp32 register accumulation, fp32 master weights — the throughput mode. */
 #define UDH_NUMERIC_FP32 0
 #define UDH_NUMERIC_BF16 1
-/* BF16X3: the same tcgen05 tiles with ERROR-COMPENSATED operands: every fp32 activation / gradient / weight travels as two
- * 16-bit limbs (x = hi + lo) and every product is evaluated as lo.hi + hi.hi + hi.lo with fp32 TMEM accumulation, so the
+/* BF16X3: the same wgmma tiles with ERROR-COMPENSATED operands: every fp32 activation / gradient / weight travels as two
+ * 16-bit limbs (x = hi + lo) and every product is evaluated as lo.hi + hi.hi + hi.lo with fp32 register accumulation, so the
  * regressor reproduces fp32 arithmetic to ~1e-5 relative (the tensor-core parity mode; three MMA passes per product). */
 #define UDH_NUMERIC_BF16X3 2
 
@@ -303,8 +303,7 @@ const char* udh_prof_tag_name(int tag);
 int udh_prof_read(int tag, float* total_ms, int* count);
 
 /* ---- debug / test entry points of the tensor-core path ---------------------------------------------------------
- * (the hardware probes of the TMA / tcgen05 conventions live in their own library: include/udh_probe.h, libudh_probe.so)
- * udh_debug_tc_conv: ONE tcgen05 3x3 convolution on fp32 NHWC tensors (pads + casts to bf16 internally), so tests can
+ * udh_debug_tc_conv: ONE wgmma 3x3 convolution on fp32 NHWC tensors (pads + casts to bf16 internally), so tests can
  * compare the tensor-core kernel with a reference convolution layer by layer; dgrad != 0 runs the mirrored kernel. */
 size_t udh_debug_tc_conv_scratch_bytes(int B, int H, int W, int cin, int cout);
 int udh_debug_tc_conv(const float* x, const float* w, const float* bias, float* out, void* scratch, int B, int H, int W,

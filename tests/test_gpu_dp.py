@@ -1,5 +1,5 @@
 """Row G on real GPUs: the repo's HomographyEngine data-parallel over NCCL (needs >= 2 GPUs; run with
-`gpurun --gpus 2 -- python -m pytest tests/test_gpu_dp.py -m gpu`).  Asserts, for the certified tensor-core mode and the
+`python -m pytest tests/test_gpu_dp.py -m gpu` on a machine with two GPUs; it skips on one).  Asserts, for the certified tensor-core mode and the
 bf16 throughput mode:
   * the gradient left by the overlapped two-phase allreduce (fc slice on the communication stream under the conv
     backward, conv slice afterwards), divided by N, equals the mean over ranks of the single-GPU gradients to 1e-5

@@ -1,4 +1,4 @@
-"""GPU tests of the tensor-core (UDH_NUMERIC_BF16) path: tcgen05/TMA plumbing, each tcgen05 kernel against a torch
+"""GPU tests of the tensor-core (UDH_NUMERIC_BF16) path: each wgmma kernel against a torch
 reference on bf16-rounded operands (so the only difference is fp32 summation order: tolerance 1e-4 relative to the
 largest output), and the whole bf16 engine against the fp32 engine / the oracle.
 
@@ -10,7 +10,7 @@ arithmetic: a bf16 perturbation of a pre-activation that sits within rounding of
 arg-max), which switches that unit's whole gradient path on or off.  Measured on this test: relative L2 difference
 0.7 % at fc2, 7 % at fc1, growing to 23 % at conv1_1, cosine similarity 0.97-0.9999 — so the end-to-end check is a
 direction check (cosine >= 0.9 per tensor, norm ratio within 15 %), and exactness of the backward kernels is established
-layer by layer above (each tcgen05 kernel vs torch on identical bf16 operands)."""
+layer by layer above (each wgmma kernel vs torch on identical bf16 operands)."""
 import ctypes
 import os
 
@@ -41,27 +41,6 @@ def udh():
 
 
 P = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-
-def test_tcgen05_descriptor_conventions(udh):
-    """TMA(SW128) -> smem -> tcgen05.mma -> TMEM: K-major and MN-major operands, descriptor starts shifted by whole
-    128-byte rows (what the conv / wgrad kernels rely on), M = 64 accumulator layout."""
-    g = torch.Generator(device="cuda").manual_seed(1)
-    A = torch.randn(144, 64, device="cuda", generator=g).bfloat16().contiguous()
-    B = torch.randn(64, 64, device="cuda", generator=g).bfloat16().contiguous()
-    out = torch.zeros(128, 512, device="cuda")
-    probes = udh.lib.load_probes()                       # libudh_probe.so: the product library carries no probe kernels
-    assert probes.udh_debug_umma_probe(P(A), 144, P(B), 64, P(out), 0, 0, None) == 0
-    torch.cuda.synchronize()
-    for s in range(8):
-        assert (out[:, 64 * s:64 * s + 64] - A[s:s + 128].float() @ B.float().t()).abs().max() < 1e-3
-    G = torch.randn(128, 128, device="cuda", generator=g).bfloat16()
-    Gb = torch.cat([G[:, :64], G[:, 64:]], dim=0).contiguous()
-    X = torch.randn(144, 64, device="cuda", generator=g).bfloat16().contiguous()
-    assert probes.udh_debug_umma_probe(P(Gb), 256, P(X), 144, P(out), 1, 0, None) == 0
-    torch.cuda.synchronize()
-    for s in range(8):
-        assert (out[:, 64 * s:64 * s + 64] - G.float().t() @ X[s:s + 128].float()).abs().max() < 1e-3
 
 
 CONV_CASES = [(2, 128, 64, 64), (3, 64, 64, 64), (2, 32, 64, 128), (2, 32, 128, 128), (5, 16, 128, 128), (1, 16, 128, 128)]

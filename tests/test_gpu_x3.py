@@ -1,5 +1,5 @@
 """GPU tests of the error-compensated tensor-core mode (UDH_NUMERIC_BF16X3): every fp32 value travels as two 16-bit limbs
-and every product is three tcgen05 passes (lo.hi + hi.hi + hi.lo) into an fp32 TMEM accumulator.
+and every product is three wgmma passes (lo.hi + hi.hi + hi.lo) into an fp32 register accumulator.
 
 Unlike the single-pass bf16 tests, the operands here are FULL fp32 tensors (not pre-rounded to bf16) and the reference is
 plain fp32 / fp64 arithmetic, so these tests bound the approximation itself.  Tolerances (relative to the largest

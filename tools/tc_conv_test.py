@@ -1,4 +1,4 @@
-"""Layer-by-layer check of the tcgen05 conv kernel against torch conv2d on bf16-rounded inputs (GPU)."""
+"""Layer-by-layer check of the wgmma conv kernel against torch conv2d on bf16-rounded inputs (GPU)."""
 import ctypes, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 print("importing torch", flush=True)

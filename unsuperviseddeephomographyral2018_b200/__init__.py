@@ -1,4 +1,4 @@
-"""B200-native unsupervised deep homography hot path (see DESIGN.md).
+"""H100-native unsupervised deep homography hot path (see DESIGN.md).
 
 Public surface (mirrors the reference's names for this path):
     homography_model.HomographyModel, homography_model.homography_model_params

@@ -153,13 +153,3 @@ def prof_read_all():
         if n.value:
             out[lib.udh_prof_tag_name(t).decode()] = (ms.value, n.value)
     return out
-
-
-def load_probes():
-    """libudh_probe.so (include/udh_probe.h): hardware probes, built on demand, never loaded by the product path."""
-    plib = ctypes.CDLL(build_ext.build_probes())
-    plib.udh_debug_umma_probe.restype = c_int
-    plib.udh_debug_umma_probe.argtypes = [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]
-    plib.udh_debug_umma2_probe.restype = c_int
-    plib.udh_debug_umma2_probe.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]
-    return plib

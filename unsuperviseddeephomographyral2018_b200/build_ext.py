@@ -1,4 +1,4 @@
-"""Build libudh.so in-tree with nvcc for sm_100a (no torch in the link line: the library is a plain C ABI).
+"""Build libudh.so in-tree with nvcc for sm_90a (no torch in the link line: the library is a plain C ABI).
 
 Concurrency: several ranks (torchrun) may import the package at once on a fresh clone.  The build runs under an exclusive
 fcntl lock on `build/.lock`, compiles into a per-variant object directory, links to a temporary name and publishes the
@@ -6,7 +6,7 @@ library with an atomic rename — a concurrent importer either waits for the loc
 loads the previous complete file; it never sees a half-written one.
 
 Variants: UDH_LIB_VARIANT=<name> builds libudh_<name>.so with the extra nvcc flags VARIANTS[name] into its own object
-directory (used for A/B experiments on the GPU box; the product is the default variant and the only one listed).
+directory (for A/B experiments; the product is the default variant and the only one listed).
 """
 import fcntl
 import glob
@@ -35,7 +35,7 @@ def lib_path(v=None):
 LIB = lib_path("")
 
 NVCC_FLAGS = [
-    "-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+    "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
 ]
 
@@ -81,30 +81,11 @@ def build(force=False, verbose=False, v=None):
             if not ok:
                 raise RuntimeError("nvcc failed building %s" % os.path.basename(lib))
             tmp = "%s.tmp.%d" % (lib, os.getpid())
-            subprocess.check_call([nvcc, "-shared", "-o", tmp] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"])
+            subprocess.check_call([nvcc, "-shared", "-o", tmp] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"])
             os.replace(tmp, lib)                        # atomic publish
         finally:
             fcntl.flock(lock, fcntl.LOCK_UN)
     return lib
-
-
-PROBE_LIB = os.path.join(HERE, "libudh_probe.so")
-
-
-def build_probes(force=False):
-    """Hardware probes (csrc/probes/: TMA / tcgen05 descriptor conventions, CTA-pair MMAs, MMA issue rates) live in their OWN
-    library, libudh_probe.so, declared in include/udh_probe.h — the product library carries no debug kernels.  Links against
-    libudh.so for the shared error / launch-count helpers."""
-    lib = build()
-    srcs = sorted(glob.glob(os.path.join(CSRC, "probes", "*.cu")))
-    if not force and os.path.exists(PROBE_LIB) and all(os.path.getmtime(s) < os.path.getmtime(PROBE_LIB) for s in srcs) \
-            and os.path.getmtime(lib) < os.path.getmtime(PROBE_LIB):
-        return PROBE_LIB
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    tmp = "%s.tmp.%d" % (PROBE_LIB, os.getpid())
-    subprocess.check_call([nvcc] + NVCC_FLAGS + ["-shared", "-o", tmp] + srcs + ["-L" + HERE, "-l:libudh.so", "-Xlinker", "-rpath=$ORIGIN"])
-    os.replace(tmp, PROBE_LIB)
-    return PROBE_LIB
 
 
 if __name__ == "__main__":

@@ -1,5 +1,5 @@
 // Launchers of the regressor's building blocks (Row C).  fp32 CUDA-core kernels live in cnn_simt.cu; the
-// tcgen05 tensor-core path lives in conv_tc.cu.  All tensors NHWC fp32 unless noted.
+// wgmma tensor-core path lives in conv_tc.cu.  All tensors NHWC fp32 unless noted.
 #pragma once
 #include <cuda_bf16.h>
 

@@ -1,6 +1,6 @@
 // fp32 CUDA-core building blocks of the 4-point regressor (Row C; code/homography_model.py:88-133).
 // This is the PARITY numeric mode (UDH_NUMERIC_FP32): fp32 FFMA implicit-GEMM convolutions, max-pool, SGEMM for
-// the two fully connected layers, dropout, and their backward passes.  The throughput mode (bf16 tcgen05) is in
+// the two fully connected layers, dropout, and their backward passes.  The throughput mode (bf16 wgmma) is in
 // conv_tc.cu and is validated against these kernels.
 #include "cnn_kernels.cuh"
 
@@ -270,7 +270,7 @@ __global__ void maxpool_bwd_kernel(const float* __restrict__ in, const float* __
 __global__ void __launch_bounds__(256) sgemm_kernel(const float* __restrict__ A, int64_t a_rs, int64_t a_cs,
                                                     const float* __restrict__ Bm, int64_t b_rs, int64_t b_cs,
                                                     float* __restrict__ C, int64_t ldc, int M, int N, int K, int k_chunk,
-                                                    int atomic) {
+                                                    int atomic, float* __restrict__ slab) {
   pdl_wait(); pdl_trigger();   // launched through launch_chain (common.cuh)
   __shared__ __align__(16) float As[16][68];
   __shared__ __align__(16) float Bs[16][68];
@@ -311,6 +311,8 @@ __global__ void __launch_bounds__(256) sgemm_kernel(const float* __restrict__ A,
         for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
     }
   }
+  // split-K: each split stores its partial product in its own slab ([split][M][N]); the launcher adds them in split order
+  float* part = slab ? slab + (size_t)blockIdx.z * M * N : nullptr;
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int m = m0 + ty * 4 + i;
@@ -319,6 +321,7 @@ __global__ void __launch_bounds__(256) sgemm_kernel(const float* __restrict__ A,
     for (int j = 0; j < 4; ++j) {
       const int n = n0 + tx * 4 + j;
       if (n >= N) continue;
+      if (part) { part[(size_t)m * N + n] = acc[i][j]; continue; }
       float* dst = C + (int64_t)m * ldc + n;
       if (atomic) atomicAdd(dst, acc[i][j]); else *dst = acc[i][j];
     }
@@ -356,13 +359,14 @@ __global__ void drop_relu_bwd_kernel(float* __restrict__ g, const uint8_t* __res
   }
 }
 
-__global__ void colsum_kernel(const float* __restrict__ g, float* __restrict__ db, int rows, int cols) {
+// partial column sums of the row slices blockIdx.y, one slab each ([slice][cols]); the launcher adds them in slice order
+__global__ void colsum_kernel(const float* __restrict__ g, float* __restrict__ part, int rows, int cols) {
   pdl_wait(); pdl_trigger();   // launched through launch_chain (common.cuh)
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= cols) return;
   float s = 0.f;
   for (int r = blockIdx.y; r < rows; r += gridDim.y) s += g[(size_t)r * cols + c];
-  atomicAdd(db + c, s);
+  part[(size_t)blockIdx.y * cols + c] = s;
 }
 
 }  // namespace
@@ -387,14 +391,14 @@ int wgrad3x3_simt(const float* x0, const float* x1, const float* g, float* dW, f
   const int tiles = B * (H / TH) * (W / TW);
   if (x1) {
     UDH_REQUIRE(Cin == 2, "wgrad3x3: two-plane input needs Cin == 2");
-    const int ctas = min(tiles, 148 * 4 / (Cout / 64));
+    const int ctas = min(tiles, kSmCount * 4 / (Cout / 64));
     const int per = (tiles + ctas - 1) / ctas;
     dim3 grid((tiles + per - 1) / per, 1, Cout / 64);
     wgrad3x3_kernel<2, true><<<grid, 256, 0, st>>>(x0, x1, g, dW, db, B, H, W, Cin, Cout, per);
   } else {
     UDH_REQUIRE(Cin % 16 == 0, "wgrad3x3: Cin must be a multiple of 16 (got %d)", Cin);
     const int groups = (Cin / 16) * (Cout / 64);
-    const int ctas = max(1, min(tiles, (148 * 4 + groups - 1) / groups));
+    const int ctas = max(1, min(tiles, (kSmCount * 4 + groups - 1) / groups));
     const int per = (tiles + ctas - 1) / ctas;
     dim3 grid((tiles + per - 1) / per, Cin / 16, Cout / 64);
     wgrad3x3_kernel<16, false><<<grid, 256, 0, st>>>(x0, nullptr, g, dW, db, B, H, W, Cin, Cout, per);
@@ -411,14 +415,14 @@ int rotate_weights(const float* w, float* wrot, int Cin, int Cout, cudaStream_t 
 int maxpool2x2_fwd(const float* in, float* out, int B, int H, int W, int C, cudaStream_t st) {
   UDH_REQUIRE(H % 2 == 0 && W % 2 == 0 && C % 4 == 0, "maxpool: unsupported shape");
   const size_t total = (size_t)B * (H / 2) * (W / 2) * (C / 4);
-  maxpool_fwd_kernel<<<grid1d((total + 255) / 256, 148 * 32), 256, 0, st>>>(in, out, B, H, W, C);
+  maxpool_fwd_kernel<<<grid1d((total + 255) / 256, kSmCount * 32), 256, 0, st>>>(in, out, B, H, W, C);
   return check_launch("maxpool2x2_fwd");
 }
 
 int maxpool2x2_bwd(const float* in, const float* dout, float* din, int B, int H, int W, int C, cudaStream_t st) {
   UDH_REQUIRE(H % 2 == 0 && W % 2 == 0 && C % 4 == 0, "maxpool: unsupported shape");
   const size_t total = (size_t)B * (H / 2) * (W / 2) * (C / 4);
-  maxpool_bwd_kernel<<<grid1d((total + 255) / 256, 148 * 32), 256, 0, st>>>(in, dout, din, B, H, W, C);
+  maxpool_bwd_kernel<<<grid1d((total + 255) / 256, kSmCount * 32), 256, 0, st>>>(in, dout, din, B, H, W, C);
   return check_launch("maxpool2x2_bwd");
 }
 
@@ -428,15 +432,26 @@ int sgemm_simt(const float* A, int64_t a_rs, int64_t a_cs, const float* Bm, int6
   int k_chunk = ((K + split_k - 1) / split_k + 15) / 16 * 16;
   split_k = (K + k_chunk - 1) / k_chunk;
   dim3 grid((N + 63) / 64, (M + 63) / 64, split_k);
+  float* slab = nullptr;
+  if (split_k > 1) {
+    UDH_REQUIRE(ldc == N, "sgemm: split-K needs a dense output (ldc %lld, N %d)", (long long)ldc, N);
+    slab = slab_scratch((size_t)split_k * M * N, st);
+    if (!slab) return UDH_ECUDA;
+  }
   launch_chain(sgemm_kernel, grid, dim3(256), 0, st, A, a_rs, a_cs, Bm, b_rs, b_cs, C, ldc, M, N, K, k_chunk,
-               (split_k > 1 || accumulate) ? 1 : 0);
-  return check_launch("sgemm_simt");
+               accumulate ? 1 : 0, slab);
+  if (int rc = check_launch("sgemm_simt")) return rc;
+  if (!slab) return UDH_OK;
+  SlabSegments t;
+  t.count = 1;
+  t.s[0] = SlabSegment{slab, C, (size_t)M * N, split_k, M * N};
+  return slab_reduce(t, st);
 }
 
 int bias_act_dropout(const float* x, const float* bias, float* act, float* drop, uint8_t* mask, int rows, int cols,
                      int relu, int gen_mask, uint64_t seed, uint64_t salt, cudaStream_t st) {
   const size_t total = (size_t)rows * cols;
-  launch_chain(bias_act_dropout_kernel, dim3(grid1d((total + 255) / 256, 148 * 16)), dim3(256), 0, st,
+  launch_chain(bias_act_dropout_kernel, dim3(grid1d((total + 255) / 256, kSmCount * 16)), dim3(256), 0, st,
                x, bias, act, drop, mask, rows, cols, relu, gen_mask, seed, salt);
   return check_launch("bias_act_dropout");
 }
@@ -446,14 +461,20 @@ int dropout_fwd(const float* x, float* drop, uint8_t* mask, size_t n, uint64_t s
 }
 
 int drop_relu_bwd(float* g, const uint8_t* mask, const float* act, size_t n, cudaStream_t st) {
-  launch_chain(drop_relu_bwd_kernel, dim3(grid1d((n + 255) / 256, 148 * 16)), dim3(256), 0, st, g, mask, act, n);
+  launch_chain(drop_relu_bwd_kernel, dim3(grid1d((n + 255) / 256, kSmCount * 16)), dim3(256), 0, st, g, mask, act, n);
   return check_launch("drop_relu_bwd");
 }
 
 int colsum_accum(const float* g, float* db, int rows, int cols, cudaStream_t st) {
   dim3 grid((cols + 127) / 128, min(rows, 16));
-  launch_chain(colsum_kernel, grid, dim3(128), 0, st, g, db, rows, cols);
-  return check_launch("colsum_accum");
+  float* part = slab_scratch((size_t)grid.y * cols, st);
+  if (!part) return UDH_ECUDA;
+  launch_chain(colsum_kernel, grid, dim3(128), 0, st, g, part, rows, cols);
+  if (int rc = check_launch("colsum_accum")) return rc;
+  SlabSegments t;
+  t.count = 1;
+  t.s[0] = SlabSegment{part, db, (size_t)cols, (int)grid.y, cols};
+  return slab_reduce(t, st);
 }
 
 }  // namespace udh

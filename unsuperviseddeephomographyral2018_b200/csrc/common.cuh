@@ -24,9 +24,11 @@ extern unsigned long long g_launches;
 extern int g_sm_reserve;      // SMs the persistent tensor-core kernels leave free (udh_set_sm_reserve)
 extern int g_sm_reserve_top;  // SMs the conv4_x backward kernels leave free (udh_set_sm_reserve_top): these few launches run
                               // while the fc-gradient allreduce occupies SMs; they have <= 2 items per CTA either way
+// SMs of the H100 SXM: sizes the grids of the grid-stride (non-persistent) kernels
+constexpr int kSmCount = 132;
 // CTAs a persistent one-CTA-per-SM kernel should launch on the current device
 inline int persistent_ctas() {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = kSmCount;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int n = sms - g_sm_reserve;
@@ -48,6 +50,15 @@ struct ProfScope {
   ProfScope(int t, cudaStream_t s) : tag(t), st(s) { prof_begin(tag, st); }
   ~ProfScope() { prof_end(tag, st); }
 };
+
+// ---- split reductions with a result that does not depend on CTA timing ----
+// Floating-point addition does not associate, so CTAs adding partial results of the same outputs with atomics give a
+// result that changes from run to run (and Adam amplifies the difference over the steps).  Such CTAs instead store their
+// partials in their own slab of a scratch buffer, and slab_reduce adds the slabs to the outputs in slab order.
+struct SlabSegment { const float* slab; float* dst; size_t stride; int nslab; int n; };   // dst[e] += sum_k slab[k*stride + e]
+struct SlabSegments { int count; SlabSegment s[16]; };
+float* slab_scratch(size_t floats, cudaStream_t st);   // grow-only buffer of the current device; nullptr (+ error) on failure
+int slab_reduce(const SlabSegments& segs, cudaStream_t st);
 
 inline int check_launch(const char* what) {
   ++g_launches;
@@ -80,7 +91,7 @@ static inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStre
 
 // ---- programmatic dependent launch (PDL) for the back-to-back kernels of the bf16 step ---------------------------------
 // A kernel launched through launch_chain() may be scheduled while its predecessor in the stream is still draining: its CTAs
-// take over SMs as the predecessor's CTAs exit and run their prologue (barrier init, TMEM allocation, tensor-map prefetch)
+// take over SMs as the predecessor's CTAs exit and run their prologue (barrier init, tensor-map prefetch)
 // early.  Every such kernel calls pdl_wait() before its first global-memory access (it returns once the predecessor grid
 // has completed and its writes are visible) and pdl_trigger() right after, so completion is transitive along the chain.
 // UDH_PDL=0 in the environment falls back to plain launches (griddepcontrol.wait is then a no-op).

@@ -1,4 +1,4 @@
-// UDH_NUMERIC_BF16: the regressor's conv stack on tcgen05 tensor cores (see conv_tc_kernels.cuh for the kernel design).
+// UDH_NUMERIC_BF16: the regressor's conv stack on wgmma tensor cores (see conv_tc_kernels.cuh for the kernel design).
 // Activations and activation gradients are zero-bordered NHWC bf16 ("padded streams"); parameters, parameter gradients,
 // the fully connected head and all reductions stay fp32.
 #include "conv_tc.cuh"
@@ -282,7 +282,7 @@ int tc_conv(const __nv_bfloat16* x, const __nv_bfloat16* wpk, const float* bias,
   if (cin == 64 && cout == 64) return launch_conv<64, 1, 2, true>(x, wpk, bias, mask_src, mask_bits, mask_out, out_bf, out_f32, relu, B, H, W, st);
   if (cin == 64 && cout == 128) return launch_conv<128, 1, 1, true>(x, wpk, bias, mask_src, mask_bits, mask_out, out_bf, out_f32, relu, B, H, W, st);
   if (cin == 128 && cout == 64) return launch_conv<64, 2, 2, false>(x, wpk, bias, mask_src, mask_bits, mask_out, out_bf, out_f32, relu, B, H, W, st);
-  if (cin == 128 && cout == 128) return launch_conv<128, 2, 2, false>(x, wpk, bias, mask_src, mask_bits, mask_out, out_bf, out_f32, relu, B, H, W, st);
+  if (cin == 128 && cout == 128) return launch_conv<128, 2, 1, false>(x, wpk, bias, mask_src, mask_bits, mask_out, out_bf, out_f32, relu, B, H, W, st);
   set_error("tc_conv: unsupported channel combination %d -> %d", cin, cout);
   return UDH_ENOSUP;
 }
@@ -294,23 +294,53 @@ int pack_weights(const float* w, __nv_bfloat16* dst, int cin, int cout, int dgra
 }
 int pad_cast(const float* src, __nv_bfloat16* dst, int B, int H, int W, int C, cudaStream_t st) {
   const size_t total = (size_t)B * H * W * (C / 4);
-  launch_chain(pad_cast_kernel, dim3(grid1d((total + 255) / 256, 148 * 32)), dim3(256), 0, st, src, dst, B, H, W, C);
+  launch_chain(pad_cast_kernel, dim3(grid1d((total + 255) / 256, kSmCount * 32)), dim3(256), 0, st, src, dst, B, H, W, C);
   return check_launch("pad_cast");
 }
 int unpad_cast(const __nv_bfloat16* src, float* dst, int B, int H, int W, int C, cudaStream_t st) {
   const size_t total = (size_t)B * H * W * (C / 4);
-  unpad_cast_kernel<<<grid1d((total + 255) / 256, 148 * 32), 256, 0, st>>>(src, dst, B, H, W, C);
+  unpad_cast_kernel<<<grid1d((total + 255) / 256, kSmCount * 32), 256, 0, st>>>(src, dst, B, H, W, C);
   return check_launch("unpad_cast");
 }
 int pool_fwd_bf16(const __nv_bfloat16* in, __nv_bfloat16* out, uint32_t* codes, int B, int H, int W, int C, cudaStream_t st) {
   const size_t total = (size_t)B * (H / 2) * (W / 2) * (C / 8);
-  launch_chain(pool_fwd_bf16_kernel, dim3(grid1d((total + 255) / 256, 148 * 32)), dim3(256), 0, st, in, out, codes, B, H, W, C);
+  launch_chain(pool_fwd_bf16_kernel, dim3(grid1d((total + 255) / 256, kSmCount * 32)), dim3(256), 0, st, in, out, codes, B, H, W, C);
   return check_launch("pool_fwd_bf16");
 }
 int pool_bwd_bf16(const uint32_t* codes, const __nv_bfloat16* gout, __nv_bfloat16* gin, int B, int H, int W, int C, cudaStream_t st) {
   const size_t total = (size_t)B * (H / 2) * (W / 2) * (C / 8);
-  launch_chain(pool_bwd_bf16_kernel, dim3(grid1d((total + 255) / 256, 148 * 32)), dim3(256), 0, st, codes, gout, gin, B, H, W, C);
+  launch_chain(pool_bwd_bf16_kernel, dim3(grid1d((total + 255) / 256, kSmCount * 32)), dim3(256), 0, st, codes, gout, gin, B, H, W, C);
   return check_launch("pool_bwd_bf16");
+}
+
+// slab reductions of the weight-gradient kernels (wgrad_tc_kernels.cuh): generic kernels, one 128 x N_OUT slab per CTA
+template <int N_OUT, int CBX>
+inline int wgrad_reduce(const float* slab, const tc::WgradGeom& g, float* dW, float* db, cudaStream_t st) {
+  constexpr size_t S = (size_t)128 * N_OUT;
+  SlabSegments t;
+  t.count = 0;
+  for (int s = 0; s < g.num_slices; ++s) {
+    const int gi = g.slice_group[s], first = g.slice_cta[s], n = g.slice_cta[s + 1] - first;
+    const float* sl = slab + (size_t)first * S;
+    int rows = 128, bias_row = -1;
+    float* dst;
+    if (CBX == 1) { dst = dW + (size_t)2 * gi * 64 * N_OUT; if (gi == 4) { rows = 64; bias_row = 64; } }
+    else if (gi < 9) dst = dW + (size_t)gi * 128 * N_OUT;
+    else { rows = 0; bias_row = 0; dst = nullptr; }
+    if (rows) t.s[t.count++] = SlabSegment{sl, dst, S, n, rows * N_OUT};
+    if (bias_row >= 0 && db) t.s[t.count++] = SlabSegment{sl + (size_t)bias_row * N_OUT, db, S, n, N_OUT};
+  }
+  return slab_reduce(t, st);
+}
+// N = 192 kernels: even CTAs (group 0) hold taps 0-5, odd CTAs (group 1) taps 6-8 and then db, in dW's layout
+inline int wgrad64_reduce(const float* slab, int per_group, float* dW, float* db, cudaStream_t st) {
+  constexpr size_t S = tc::kWgrad64SlabFloats;
+  SlabSegments t;
+  t.count = 0;
+  t.s[t.count++] = SlabSegment{slab, dW, 2 * S, per_group, 6 * 4096};
+  t.s[t.count++] = SlabSegment{slab + S, dW + 6 * 4096, 2 * S, per_group, 3 * 4096};
+  if (db) t.s[t.count++] = SlabSegment{slab + S + 3 * 4096, db, 2 * S, per_group, 64};
+  return slab_reduce(t, st);
 }
 
 template <int N_OUT, int CBX, int T>
@@ -324,8 +354,7 @@ int launch_wgrad(const __nv_bfloat16* x, const __nv_bfloat16* gsrc, float* dW, f
   g.xrows = T * 128 + 2 * g.hh;
   g.num_groups = CBX == 1 ? 5 : 10;
   const int sms = persistent_ctas();
-  const int max_groups = 512 / N_OUT;                              // accumulators of one slice fit TMEM
-  g.num_slices = (g.num_groups + max_groups - 1) / max_groups;
+  g.num_slices = g.num_groups;                                      // one group per CTA (its accumulators fill the registers)
   g.slice_group[0] = 0; g.slice_cta[0] = 0;
   for (int s = 0; s < g.num_slices; ++s) {
     g.slice_group[s + 1] = g.slice_group[s] + g.num_groups / g.num_slices + (s < g.num_groups % g.num_slices ? 1 : 0);
@@ -346,8 +375,11 @@ int launch_wgrad(const __nv_bfloat16* x, const __nv_bfloat16* gsrc, float* dW, f
   UDH_REQUIRE(smem <= 232448, "tc wgrad: %zu bytes of shared memory exceed the 227 KiB limit", smem);
   auto kern = tc::tc_wgrad_kernel<N_OUT, CBX, T>;
   UDH_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  launch_chain(kern, dim3(g.slice_cta[g.num_slices]), dim3(256), smem, st, tmX128, tmXhh, tmG, g, dW, db);
-  return check_launch("tc_wgrad_kernel");
+  float* slab = slab_scratch((size_t)g.slice_cta[g.num_slices] * 128 * N_OUT, st);
+  if (!slab) return UDH_ECUDA;
+  launch_chain(kern, dim3(g.slice_cta[g.num_slices]), dim3(384), smem, st, tmX128, tmXhh, tmG, g, slab);
+  TRY(check_launch("tc_wgrad_kernel"));
+  return wgrad_reduce<N_OUT, CBX>(slab, g, dW, db, st);
 }
 
 // 64 -> 64 layers: the N = 192 kernel (see wgrad_tc_kernels.cuh)
@@ -372,8 +404,12 @@ int launch_wgrad64(const __nv_bfloat16* x, const __nv_bfloat16* gsrc, float* dW,
   auto kern = tc::tc_wgrad64_kernel<T>;
   UDH_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int sms = persistent_ctas();
-  launch_chain(kern, dim3(g.num_items < sms ? g.num_items : sms), dim3(256), smem, st, tmX128, tmXhh, tmG136, g, dW, db);
-  return check_launch("tc_wgrad64_kernel");
+  const int per_group = g.num_items < sms / 2 ? g.num_items : sms / 2;   // even CTAs: group 0, odd CTAs: group 1
+  float* slab = slab_scratch((size_t)2 * per_group * tc::kWgrad64SlabFloats, st);
+  if (!slab) return UDH_ECUDA;
+  launch_chain(kern, dim3(2 * per_group), dim3(384), smem, st, tmX128, tmXhh, tmG136, g, slab);
+  TRY(check_launch("tc_wgrad64_kernel"));
+  return wgrad64_reduce(slab, per_group, dW, db, st);
 }
 
 // dW (HWIO fp32) += X^T-shifted . G ; db += sum G   for one layer, on padded bf16 streams
@@ -396,7 +432,7 @@ __global__ void cast_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* _
   }
 }
 int cast_bf16(const float* src, __nv_bfloat16* dst, size_t n, cudaStream_t st) {
-  launch_chain(cast_bf16_kernel, dim3(grid1d((n / 4 + 255) / 256, 148 * 16)), dim3(256), 0, st, src, dst, n / 4);
+  launch_chain(cast_bf16_kernel, dim3(grid1d((n / 4 + 255) / 256, kSmCount * 16)), dim3(256), 0, st, src, dst, n / 4);
   return check_launch("cast_bf16");
 }
 
@@ -410,11 +446,11 @@ int conv1_tc_fwd(const float* I1, const float* I2, const float* w, const float* 
   uint64_t dims[2] = {64, Q}, str[2] = {2, 128};
   uint32_t box[2] = {64, 32};
   TRY(tc::make_tmap_bf16(&tmOut, out_pad, 2, dims, str, box));
-  const size_t smem = 1024 + 2 * 16384 + 8192 + 16384 + 256;
+  const size_t smem = tc::kConv1FwdSmem;
   UDH_CUDA(cudaFuncSetAttribute(tc::conv1_tc_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int want = tc::kConv1CtasPerSm * persistent_ctas();
   const int grid = g.tiles < want ? g.tiles : want;
-  launch_chain(tc::conv1_tc_fwd_kernel, dim3(grid), dim3(160), smem, st, tmOut, g, I1, I2, w, bias, mask_out);
+  launch_chain(tc::conv1_tc_fwd_kernel, dim3(grid), dim3(128), smem, st, tmOut, g, I1, I2, w, bias, mask_out);
   return check_launch("conv1_tc_fwd_kernel");
 }
 
@@ -427,12 +463,19 @@ int conv1_tc_wgrad(const float* I1, const float* I2, const __nv_bfloat16* G_pad,
   uint64_t dims[2] = {64, Q}, str[2] = {2, 128};
   uint32_t box[2] = {64, 128};
   TRY(tc::make_tmap_bf16(&tmG, G_pad, 2, dims, str, box));
-  const size_t smem = 1024 + 4 * 16384 + 256;
+  const size_t smem = tc::kConv1WgradSmem;
   UDH_CUDA(cudaFuncSetAttribute(tc::conv1_tc_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int want = tc::kConv1CtasPerSm * persistent_ctas();
   const int grid = g.tiles < want ? g.tiles : want;
-  launch_chain(tc::conv1_tc_wgrad_kernel, dim3(grid), dim3(160), smem, st, tmG, g, I1, I2, dW, db);
-  return check_launch("conv1_tc_wgrad_kernel");
+  float* slab = slab_scratch((size_t)grid * tc::kConv1SlabFloats, st);
+  if (!slab) return UDH_ECUDA;
+  launch_chain(tc::conv1_tc_wgrad_kernel, dim3(grid), dim3(128), smem, st, tmG, g, I1, I2, slab);
+  TRY(check_launch("conv1_tc_wgrad_kernel"));
+  SlabSegments t;
+  t.count = 0;
+  t.s[t.count++] = SlabSegment{slab, dW, (size_t)tc::kConv1SlabFloats, grid, 18 * 64};
+  if (db) t.s[t.count++] = SlabSegment{slab + 18 * 64, db, (size_t)tc::kConv1SlabFloats, grid, 64};
+  return slab_reduce(t, st);
 }
 
 }  // namespace
@@ -470,7 +513,7 @@ int tc_cnn_fwd_convs(const float* params, const size_t* poff, const float* I1, c
     TRY(check_launch("pack_all_weights"));
   }
   {
-    // conv1_1 (K = 18): im2col tile in shared memory + tcgen05, writing the padded bf16 stream and its 1-bit ReLU mask
+    // conv1_1 (K = 18): im2col tile in shared memory + wgmma, writing the padded bf16 stream and its 1-bit ReLU mask
     ProfScope ps(PROF_CONV_FWD0, st);
     TRY(conv1_tc_fwd(I1, I2, params + poff[0], params + poff[1], Pb(0), reinterpret_cast<uint32_t*>(tcw + L.Mb[0]), B, P, P, st));
   }

@@ -1,4 +1,4 @@
-// tcgen05 / TMEM / TMA tensor-core path of the regressor's convolutions (UDH_NUMERIC_BF16).
+// wgmma / TMA tensor-core path of the regressor's convolutions (UDH_NUMERIC_BF16).
 #pragma once
 #include "common.cuh"
 

@@ -1,6 +1,6 @@
-// UDH_NUMERIC_BF16X3: the regressor on tcgen05 tensor cores with fp32-grade results.  Every fp32 value (activations,
+// UDH_NUMERIC_BF16X3: the regressor on wgmma tensor cores with fp32-grade results.  Every fp32 value (activations,
 // activation gradients, weights) travels as two 16-bit limbs, x = hi + lo, and every product is evaluated as
-// lo.hi + hi.hi + hi.lo with fp32 TMEM accumulation (conv_x3_kernels.cuh, wgrad_x3_kernels.cuh, conv1_x3_kernels.cuh, and
+// lo.hi + hi.hi + hi.lo with fp32 register accumulation (conv_x3_kernels.cuh, wgrad_x3_kernels.cuh, conv1_x3_kernels.cuh, and
 // the segment mechanism of gemm_tc_kernels.cuh for fc1).  Bias, ReLU, masks, pooling decisions, dropout, fc2, losses,
 // DLT, warp and Adam are fp32 exactly as in the other modes.  Reference arithmetic matched: fp32 everywhere,
 // code/homography_model.py:67,88-133.
@@ -228,11 +228,11 @@ __global__ void pool_bwd_x3_kernel(const uint32_t* __restrict__ codes, const uin
 }
 
 // ---------------------------------------------------------------------------------------------------- launchers
-template <int N_OUT, int CB, int T, int FA, int FW, int FO, bool WIDE, int STAGES>
+template <int N_OUT, int CB, int T, int FA, int FW, int FO, bool WIDE>
 int launch_conv_x3_impl(const CUtensorMap& tmA128, const CUtensorMap& tmAhh, const CUtensorMap& tmW, const CUtensorMap& tmOut, const tc::ConvGeom& g,
                         int stages, size_t smem, const float* bias, const uint32_t* mask_bits, uint32_t* mask_out, float* out_f32, int relu,
                         float out_scale, cudaStream_t st) {
-  auto kern = tc::tc_conv_x3_kernel<N_OUT, CB, T, FA, FW, FO, WIDE, STAGES>;
+  auto kern = tc::tc_conv_x3_kernel<N_OUT, CB, T, FA, FW, FO, WIDE>;
   UDH_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int sms = persistent_ctas();
   const int grid = g.num_items < sms ? g.num_items : sms;
@@ -263,25 +263,10 @@ int launch_conv_x3(const uint16_t* x, const uint16_t* wpk, const float* bias, co
   uint32_t boxO[2] = {64, 32};
   TRY(tc::make_tmap_bf16(&tmOut, out_limbs, 2, dimsO, strO, boxO));
   using S = tc::ConvX3Smem<N_OUT, CB, T, WIDE>;
-  int stages = S::stages(g.abuf_rows);
+  const int stages = S::stages(g.abuf_rows);          // weight-ring depth: as many stages as shared memory holds (<= 6)
   UDH_REQUIRE(stages >= 2, "tc conv x3: activation rows (%d x %d blocks) leave no room for the weight ring", g.abuf_rows, 2 * CB);
-  // static ring (unrolled issue loop) when a depth of 6 or 3 fits: both divide the 18*CB (WIDE) / 27*CB stages of an item
-  // (measured: the 128-channel / CB = 2 instances are better off with the deeper runtime ring, so only WIDE uses it)
-  static const int static_env = [] { const char* e = getenv("UDH_X3_STATIC_RING"); return (e && e[0] == '0') ? 0 : 1; }();
-  const int use_static = WIDE ? static_env : 0;
-  constexpr int kSPI = (WIDE ? 18 : 27) * CB;
-  if constexpr (kSPI % 6 == 0) if (use_static && stages >= 6) {
-    stages = 6;
-    return launch_conv_x3_impl<N_OUT, CB, T, FA, FW, FO, WIDE, 6>(tmA128, tmAhh, tmW, tmOut, g, stages, S::fixed_bytes(g.abuf_rows) + (size_t)stages * S::kWStageBytes,
-                                                                  bias, mask_bits, mask_out, out_f32, relu, out_scale, st);
-  }
-  if (use_static && stages >= 3) {
-    stages = 3;
-    return launch_conv_x3_impl<N_OUT, CB, T, FA, FW, FO, WIDE, 3>(tmA128, tmAhh, tmW, tmOut, g, stages, S::fixed_bytes(g.abuf_rows) + (size_t)stages * S::kWStageBytes,
-                                                                  bias, mask_bits, mask_out, out_f32, relu, out_scale, st);
-  }
-  return launch_conv_x3_impl<N_OUT, CB, T, FA, FW, FO, WIDE, 0>(tmA128, tmAhh, tmW, tmOut, g, stages, S::fixed_bytes(g.abuf_rows) + (size_t)stages * S::kWStageBytes,
-                                                                bias, mask_bits, mask_out, out_f32, relu, out_scale, st);
+  return launch_conv_x3_impl<N_OUT, CB, T, FA, FW, FO, WIDE>(tmA128, tmAhh, tmW, tmOut, g, stages, S::fixed_bytes(g.abuf_rows) + (size_t)stages * S::kWStageBytes,
+                                                             bias, mask_bits, mask_out, out_f32, relu, out_scale, st);
 }
 
 // conv1_2 on row tiles (64 -> 64 channels, 128-wide images): ROWS = 1 forward fused with pool1 (writes the pooled two-limb
@@ -307,11 +292,11 @@ int launch_conv_x3_rows(const uint16_t* x, const uint16_t* wpk, const float* bia
   TRY(tc::make_tmap_bf16(&tmW, wpk, 2, dimsW, strW, boxW));
   // ROWS = 1 stores the pooled stream with plain vector stores (the map is only a placeholder there)
   TRY(tc::make_tmap_bf16(&tmOut, ROWS == 2 ? out_limbs : const_cast<uint16_t*>(x), 2, dimsA, strA, boxO));
-  using S = tc::ConvX3Smem<64, 1, 2, true>;
+  using S = tc::ConvX3Smem<64, 1, 2, false>;
   constexpr int kStages = 3;
   const size_t smem = S::fixed_bytes(g.abuf_rows) + (size_t)kStages * S::kWStageBytes;
   UDH_REQUIRE(smem <= 232448, "tc conv x3 rows: %zu bytes of shared memory exceed the 227 KiB limit", smem);
-  auto kern = tc::tc_conv_x3_kernel<64, 1, 2, FA, FW, FO, true, kStages, ROWS>;
+  auto kern = tc::tc_conv_x3_kernel<64, 1, 2, FA, FW, FO, false, ROWS>;
   UDH_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int sms = persistent_ctas();
   const int grid = g.num_items < sms ? g.num_items : sms;
@@ -325,15 +310,47 @@ int launch_conv_x3_rows(const uint16_t* x, const uint16_t* wpk, const float* bia
 template <int FA, int FW, int FO>
 int tc_conv_x3(const uint16_t* x, const uint16_t* wpk, const float* bias, const uint32_t* mask_bits, uint32_t* mask_out,
                uint16_t* out_limbs, float* out_f32, int relu, int B, int H, int W, int cin, int cout, cudaStream_t st) {
-  static const int wide = [] { const char* e = getenv("UDH_X3_WIDE"); return (e && e[0] == '0') ? 0 : 1; }();
-  if (cin == 64 && cout == 64 && wide) return launch_conv_x3<64, 1, 2, FA, FW, FO, true>(x, wpk, bias, mask_bits, mask_out, out_limbs, out_f32, relu, B, H, W, 1.0f, st);
-  if (cin == 64 && cout == 64 && W >= 128) return launch_conv_x3<64, 1, 3, FA, FW, FO>(x, wpk, bias, mask_bits, mask_out, out_limbs, out_f32, relu, B, H, W, 1.0f, st);
-  if (cin == 64 && cout == 64) return launch_conv_x3<64, 1, 4, FA, FW, FO>(x, wpk, bias, mask_bits, mask_out, out_limbs, out_f32, relu, B, H, W, 1.0f, st);
-  if (cin == 64 && cout == 128) return launch_conv_x3<128, 1, 2, FA, FW, FO>(x, wpk, bias, mask_bits, mask_out, out_limbs, out_f32, relu, B, H, W, 1.0f, st);
+  // WIDE (one N = 128 MMA against [W_hi | W_lo], a MAIN and an AUX accumulator) is opt-in (UDH_X3_WIDE=1): the default
+  // instance sums in the same order as the row-tile kernel of conv1_2, so the two paths agree bit for bit
+  static const int wide = [] { const char* e = getenv("UDH_X3_WIDE"); return (e && e[0] == '1') ? 1 : 0; }();
+  // items of T tiles: T * (accumulator columns per tile) / 2 fp32 registers per MMA thread, kept at 64
+  if (cin == 64 && cout == 64 && wide) return launch_conv_x3<64, 1, 1, FA, FW, FO, true>(x, wpk, bias, mask_bits, mask_out, out_limbs, out_f32, relu, B, H, W, 1.0f, st);
+  if (cin == 64 && cout == 64) return launch_conv_x3<64, 1, 2, FA, FW, FO>(x, wpk, bias, mask_bits, mask_out, out_limbs, out_f32, relu, B, H, W, 1.0f, st);
+  if (cin == 64 && cout == 128) return launch_conv_x3<128, 1, 1, FA, FW, FO>(x, wpk, bias, mask_bits, mask_out, out_limbs, out_f32, relu, B, H, W, 1.0f, st);
   if (cin == 128 && cout == 64) return launch_conv_x3<64, 2, 2, FA, FW, FO>(x, wpk, bias, mask_bits, mask_out, out_limbs, out_f32, relu, B, H, W, 1.0f, st);
-  if (cin == 128 && cout == 128) return launch_conv_x3<128, 2, 2, FA, FW, FO>(x, wpk, bias, mask_bits, mask_out, out_limbs, out_f32, relu, B, H, W, 1.0f, st);
+  if (cin == 128 && cout == 128) return launch_conv_x3<128, 2, 1, FA, FW, FO>(x, wpk, bias, mask_bits, mask_out, out_limbs, out_f32, relu, B, H, W, 1.0f, st);
   set_error("tc_conv_x3: unsupported channel combination %d -> %d", cin, cout);
   return UDH_ENOSUP;
+}
+
+// slab reductions of the weight-gradient kernels (wgrad_tc_kernels.cuh): generic kernels, one 128 x N_OUT slab per CTA
+template <int N_OUT, int CBX>
+inline int wgrad_reduce(const float* slab, const tc::WgradGeom& g, float* dW, float* db, cudaStream_t st) {
+  constexpr size_t S = (size_t)128 * N_OUT;
+  SlabSegments t;
+  t.count = 0;
+  for (int s = 0; s < g.num_slices; ++s) {
+    const int gi = g.slice_group[s], first = g.slice_cta[s], n = g.slice_cta[s + 1] - first;
+    const float* sl = slab + (size_t)first * S;
+    int rows = 128, bias_row = -1;
+    float* dst;
+    if (CBX == 1) { dst = dW + (size_t)2 * gi * 64 * N_OUT; if (gi == 4) { rows = 64; bias_row = 64; } }
+    else if (gi < 9) dst = dW + (size_t)gi * 128 * N_OUT;
+    else { rows = 0; bias_row = 0; dst = nullptr; }
+    if (rows) t.s[t.count++] = SlabSegment{sl, dst, S, n, rows * N_OUT};
+    if (bias_row >= 0 && db) t.s[t.count++] = SlabSegment{sl + (size_t)bias_row * N_OUT, db, S, n, N_OUT};
+  }
+  return slab_reduce(t, st);
+}
+// N = 192 kernels: even CTAs (group 0) hold taps 0-5, odd CTAs (group 1) taps 6-8 and then db, in dW's layout
+inline int wgrad64_reduce(const float* slab, int per_group, float* dW, float* db, cudaStream_t st) {
+  constexpr size_t S = tc::kWgrad64SlabFloats;
+  SlabSegments t;
+  t.count = 0;
+  t.s[t.count++] = SlabSegment{slab, dW, 2 * S, per_group, 6 * 4096};
+  t.s[t.count++] = SlabSegment{slab + S, dW + 6 * 4096, 2 * S, per_group, 3 * 4096};
+  if (db) t.s[t.count++] = SlabSegment{slab + S + 3 * 4096, db, 2 * S, per_group, 64};
+  return slab_reduce(t, st);
 }
 
 template <int N_OUT, int CBX, int T>
@@ -347,8 +364,7 @@ int launch_wgrad_x3(const uint16_t* x, const uint16_t* gsrc, float* dW, float* d
   g.xrows = T * 128 + 2 * g.hh;
   g.num_groups = CBX == 1 ? 5 : 10;
   const int sms = persistent_ctas();
-  const int max_groups = 512 / N_OUT;                              // accumulators of one slice fit TMEM
-  g.num_slices = (g.num_groups + max_groups - 1) / max_groups;
+  g.num_slices = g.num_groups;                                      // one group per CTA (its accumulators fill the registers)
   g.slice_group[0] = 0; g.slice_cta[0] = 0;
   for (int s = 0; s < g.num_slices; ++s) {
     g.slice_group[s + 1] = g.slice_group[s] + g.num_groups / g.num_slices + (s < g.num_groups % g.num_slices ? 1 : 0);
@@ -368,8 +384,11 @@ int launch_wgrad_x3(const uint16_t* x, const uint16_t* gsrc, float* dW, float* d
   UDH_REQUIRE(smem <= 232448, "tc wgrad x3: %zu bytes of shared memory exceed the 227 KiB limit", smem);
   auto kern = tc::tc_wgrad_x3_kernel<N_OUT, CBX, T, kFwd, kGrad>;
   UDH_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  launch_chain(kern, dim3(g.slice_cta[g.num_slices]), dim3(256), smem, st, tmX128, tmXhh, tmG, g, dW, db);
-  return check_launch("tc_wgrad_x3_kernel");
+  float* slab = slab_scratch((size_t)g.slice_cta[g.num_slices] * 128 * N_OUT, st);
+  if (!slab) return UDH_ECUDA;
+  launch_chain(kern, dim3(g.slice_cta[g.num_slices]), dim3(384), smem, st, tmX128, tmXhh, tmG, g, slab);
+  TRY(check_launch("tc_wgrad_x3_kernel"));
+  return wgrad_reduce<N_OUT, CBX>(slab, g, dW, db, st);
 }
 
 int launch_wgrad64_x3(const uint16_t* x, const uint16_t* gsrc, float* dW, float* db, int B, int H, int W, cudaStream_t st) {
@@ -392,8 +411,12 @@ int launch_wgrad64_x3(const uint16_t* x, const uint16_t* gsrc, float* dW, float*
   auto kern = tc::tc_wgrad64_x3_kernel<T, kFwd, kGrad>;
   UDH_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int sms = persistent_ctas();
-  launch_chain(kern, dim3(g.num_items < sms ? g.num_items : sms), dim3(256), smem, st, tmX128, tmXhh, tmG136, g, dW, db);
-  return check_launch("tc_wgrad64_x3_kernel");
+  const int per_group = g.num_items < sms / 2 ? g.num_items : sms / 2;   // even CTAs: group 0, odd CTAs: group 1
+  float* slab = slab_scratch((size_t)2 * per_group * tc::kWgrad64SlabFloats, st);
+  if (!slab) return UDH_ECUDA;
+  launch_chain(kern, dim3(2 * per_group), dim3(384), smem, st, tmX128, tmXhh, tmG136, g, slab);
+  TRY(check_launch("tc_wgrad64_x3_kernel"));
+  return wgrad64_reduce(slab, per_group, dW, db, st);
 }
 
 int tc_wgrad_x3(const uint16_t* x, const uint16_t* gsrc, float* dW, float* db, int B, int H, int W, int cin, int cout, cudaStream_t st) {
@@ -406,30 +429,30 @@ int tc_wgrad_x3(const uint16_t* x, const uint16_t* gsrc, float* dW, float* db, i
 
 int pad_cast_x3(const float* src, uint16_t* dst, int B, int H, int W, int C, bool grad, cudaStream_t st) {
   const size_t total = (size_t)B * H * W * (C / 4);
-  if (grad) launch_chain(pad_cast_x3_kernel<kGrad>, dim3(grid1d((total + 255) / 256, 148 * 32)), dim3(256), 0, st, src, dst, B, H, W, C);
-  else launch_chain(pad_cast_x3_kernel<kFwd>, dim3(grid1d((total + 255) / 256, 148 * 32)), dim3(256), 0, st, src, dst, B, H, W, C);
+  if (grad) launch_chain(pad_cast_x3_kernel<kGrad>, dim3(grid1d((total + 255) / 256, kSmCount * 32)), dim3(256), 0, st, src, dst, B, H, W, C);
+  else launch_chain(pad_cast_x3_kernel<kFwd>, dim3(grid1d((total + 255) / 256, kSmCount * 32)), dim3(256), 0, st, src, dst, B, H, W, C);
   return check_launch("pad_cast_x3");
 }
 int unpad_cast_x3(const uint16_t* src, float* dst, int B, int H, int W, int C, bool grad, cudaStream_t st) {
   const size_t total = (size_t)B * H * W * (C / 4);
-  if (grad) unpad_cast_x3_kernel<kGrad><<<grid1d((total + 255) / 256, 148 * 32), 256, 0, st>>>(src, dst, B, H, W, C);
-  else unpad_cast_x3_kernel<kFwd><<<grid1d((total + 255) / 256, 148 * 32), 256, 0, st>>>(src, dst, B, H, W, C);
+  if (grad) unpad_cast_x3_kernel<kGrad><<<grid1d((total + 255) / 256, kSmCount * 32), 256, 0, st>>>(src, dst, B, H, W, C);
+  else unpad_cast_x3_kernel<kFwd><<<grid1d((total + 255) / 256, kSmCount * 32), 256, 0, st>>>(src, dst, B, H, W, C);
   return check_launch("unpad_cast_x3");
 }
 int cast_x3(const float* src, uint16_t* dst, size_t rows, int cols, bool grad, cudaStream_t st) {
   const size_t total = rows * (cols / 4);
-  if (grad) launch_chain(cast_x3_kernel<kGrad>, dim3(grid1d((total + 255) / 256, 148 * 16)), dim3(256), 0, st, src, dst, rows, cols);
-  else launch_chain(cast_x3_kernel<kFwd>, dim3(grid1d((total + 255) / 256, 148 * 16)), dim3(256), 0, st, src, dst, rows, cols);
+  if (grad) launch_chain(cast_x3_kernel<kGrad>, dim3(grid1d((total + 255) / 256, kSmCount * 16)), dim3(256), 0, st, src, dst, rows, cols);
+  else launch_chain(cast_x3_kernel<kFwd>, dim3(grid1d((total + 255) / 256, kSmCount * 16)), dim3(256), 0, st, src, dst, rows, cols);
   return check_launch("cast_x3");
 }
 int pool_fwd_x3(const uint16_t* in, uint16_t* out, uint32_t* codes, int B, int H, int W, int C, cudaStream_t st) {
   const size_t total = (size_t)B * (H / 2) * (W / 2) * (C / 8);
-  launch_chain(pool_fwd_x3_kernel<kFwd>, dim3(grid1d((total + 255) / 256, 148 * 32)), dim3(256), 0, st, in, out, codes, B, H, W, C);
+  launch_chain(pool_fwd_x3_kernel<kFwd>, dim3(grid1d((total + 255) / 256, kSmCount * 32)), dim3(256), 0, st, in, out, codes, B, H, W, C);
   return check_launch("pool_fwd_x3");
 }
 int pool_bwd_x3(const uint32_t* codes, const uint16_t* gout, uint16_t* gin, int B, int H, int W, int C, cudaStream_t st) {
   const size_t total = (size_t)B * (H / 2) * (W / 2) * (C / 8);
-  launch_chain(pool_bwd_x3_kernel, dim3(grid1d((total + 255) / 256, 148 * 32)), dim3(256), 0, st, codes, gout, gin, B, H, W, C);
+  launch_chain(pool_bwd_x3_kernel, dim3(grid1d((total + 255) / 256, kSmCount * 32)), dim3(256), 0, st, codes, gout, gin, B, H, W, C);
   return check_launch("pool_bwd_x3");
 }
 
@@ -442,12 +465,12 @@ int conv1_x3_fwd(const float* I1, const float* I2, const float* w, const float* 
   uint64_t dims[2] = {128, Q}, str[2] = {2, 256};
   uint32_t box[2] = {64, 32};
   TRY(tc::make_tmap_bf16(&tmOut, out_limbs, 2, dims, str, box));
-  const size_t smem = 1024 + 2 * 16384 + 16384 + 16384 + 256;
+  const size_t smem = tc::kConv1X3FwdSmem;
   auto kern = tc::conv1_x3_fwd_kernel<kFwd>;
   UDH_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int want = tc::kConv1X3CtasPerSm * persistent_ctas();
   const int grid = g.tiles < want ? g.tiles : want;
-  launch_chain(kern, dim3(grid), dim3(160), smem, st, tmOut, g, I1, I2, w, bias, mask_out);
+  launch_chain(kern, dim3(grid), dim3(128), smem, st, tmOut, g, I1, I2, w, bias, mask_out);
   return check_launch("conv1_x3_fwd_kernel");
 }
 
@@ -459,13 +482,20 @@ int conv1_x3_wgrad(const float* I1, const float* I2, const uint16_t* G_limbs, fl
   uint64_t dims[2] = {128, Q}, str[2] = {2, 256};
   uint32_t box[2] = {64, 128};
   TRY(tc::make_tmap_bf16(&tmG, G_limbs, 2, dims, str, box));
-  const size_t smem = 1024 + 2 * 16384 + 4 * 16384 + 256;
+  const size_t smem = tc::kConv1X3WgradSmem;
   auto kern = tc::conv1_x3_wgrad_kernel<kFwd, kGrad>;
   UDH_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int want = tc::kConv1X3WgradCtasPerSm * persistent_ctas();
   const int grid = g.tiles < want ? g.tiles : want;
-  launch_chain(kern, dim3(grid), dim3(160), smem, st, tmG, g, I1, I2, dW, db);
-  return check_launch("conv1_x3_wgrad_kernel");
+  float* slab = slab_scratch((size_t)grid * tc::kConv1SlabFloats, st);
+  if (!slab) return UDH_ECUDA;
+  launch_chain(kern, dim3(grid), dim3(128), smem, st, tmG, g, I1, I2, slab);
+  TRY(check_launch("conv1_x3_wgrad_kernel"));
+  SlabSegments t;
+  t.count = 0;
+  t.s[t.count++] = SlabSegment{slab, dW, (size_t)tc::kConv1SlabFloats, grid, 18 * 64};
+  if (db) t.s[t.count++] = SlabSegment{slab + 18 * 64, db, (size_t)tc::kConv1SlabFloats, grid, 64};
+  return slab_reduce(t, st);
 }
 
 inline uint16_t* U16(char* base, size_t off) { return reinterpret_cast<uint16_t*>(base + off); }
@@ -603,7 +633,7 @@ int x3_fc1_fwd(const float* x, const float* w, float* acc, void* ws, size_t tc_o
   TRY(cast_x3(x, xb, (size_t)B, (int)feat, false, st));
   if (!w_mirror_current) {
     const size_t n4 = feat * 1024 / 4;
-    launch_chain(cast_planes_x3_kernel<kFwd>, dim3(grid1d((n4 + 255) / 256, 148 * 16)), dim3(256), 0, st, w, wb, wb + feat * 1024, n4);
+    launch_chain(cast_planes_x3_kernel<kFwd>, dim3(grid1d((n4 + 255) / 256, kSmCount * 16)), dim3(256), 0, st, w, wb, wb + feat * 1024, n4);
     TRY(check_launch("cast_planes_x3"));
   }
   const int kb = 3 * (int)(feat / 64);

@@ -98,10 +98,10 @@ extern "C" int udh_dp_shard_update(const void* mc_grads, const float* params, vo
                   (uintptr_t)mc_mirror % 8 == 0, "udh_dp_shard_update: buffers must be 16-byte aligned");
   UDH_REQUIRE(!mc_mirror || (shard_begin >= mirror_begin && shard_begin + shard_count <= mirror_begin + mirror_count),
               "udh_dp_shard_update: the shard must lie inside the mirrored tensor");
-  UDH_REQUIRE(grid >= 0 && grid <= 148 * 2, "udh_dp_shard_update: grid must be in 0..296");
+  UDH_REQUIRE(grid >= 0 && grid <= udh::kSmCount * 2, "udh_dp_shard_update: grid must be in 0..%d", udh::kSmCount * 2);
   if (shard_count == 0) return UDH_OK;
   const size_t n4 = shard_count / 4, per = (size_t)udh::kDpThreads * udh::kDpUnroll;
-  const size_t full = (n4 + per - 1) / per, cap = grid > 0 ? (size_t)grid : (size_t)148;
+  const size_t full = (n4 + per - 1) / per, cap = grid > 0 ? (size_t)grid : (size_t)udh::kSmCount;
   const unsigned blocks = (unsigned)(full < cap ? full : cap);
   cudaStream_t st = udh::as_stream(stream);
   udh::ProfScope ps(udh::PROF_ADAM, st);

@@ -1,11 +1,11 @@
-// tcgen05 GEMM for the fully connected head (fc1: 32768 -> 1024), bf16 operands, fp32 TMEM accumulation.
-//   D[M][N] (+)= A . B over K, tiles of 128 x 256, k-blocks of 64, 4-stage TMA ring, two TMEM accumulator sets.
+// wgmma GEMM for the fully connected head (fc1: 32768 -> 1024), bf16 operands, fp32 register accumulation.
+//   D[M][N] (+)= A . B over K, tiles of 128 x 256 (two MMA warpgroups of 64 rows), k-blocks of 64, 3-stage TMA ring.
 // Each operand is either K-major (contraction index contiguous in memory: tile = [rows][64 k], box (64, rows)) or
 // MN-major (row/column index contiguous: tile = 64-wide column blocks of [64 k][64 mn]), which covers
-//   forward   y  = x . W        A = x [B][F] K-major,      B = W [F][N] MN-major,   split-K, atomic accumulation
+//   forward   y  = x . W        A = x [B][F] K-major,      B = W [F][N] MN-major,   split-K (partials summed in split order)
 //   dgrad     dx = dy . W^T     A = dy [B][N] K-major,     B = W [F][N] as [n=f][k] K-major
 //   wgrad     dW = x^T . dy     A = x [B][F] MN-major,     B = dy [B][N] MN-major   (K = batch)
-// with no transposed copies.  warp 0: TMA | warp 1: MMA | warp 2: TMEM alloc | warps 4-7: epilogue.
+// with no transposed copies.  warpgroup 0: TMA producer (warp 0) | warpgroups 1-2: MMA + epilogue.
 #pragma once
 #include "tc_common.cuh"
 
@@ -25,39 +25,34 @@ struct GemmGeom {
   int64_t ldc;
 };
 
-constexpr int kGemmStages = 4;
+constexpr int kGemmStages = 3;
 constexpr int kGemmStageBytes = 16384 + 32768;   // A 128 x 64, B 256 x 64 (bf16)
 
-constexpr int kGemmEpiBytes = 2 * 4 * 32 * 128;  // TMA-store staging of the non-atomic epilogue: 2 x (32 rows x 32 floats) per warp
+constexpr int kGemmEpiBytes = 8 * 32 * 128;      // TMA-store staging of the non-atomic epilogue: 32 rows x 32 floats per warp
 
-// ATOMIC: split-K partial tiles are added with 16-byte vector reductions.  Otherwise the tile is stored through a swizzled
+// SPLIT: every split stores its partial tile in its own slab of a scratch buffer ([split][M][N]); the launcher adds the
+// slabs in split order (slab_reduce), so the sum does not depend on CTA timing.  Otherwise the tile is stored through a swizzled
 // shared-memory staging block and TMA (full 128-byte lines; rows / columns beyond M / N are clipped by the tensor map).
-template <bool A_MN, bool B_MN, bool ATOMIC, int FMT_A = kFmtBF16, int FMT_B = kFmtBF16>
-__global__ void __launch_bounds__(256, 1)
+template <bool A_MN, bool B_MN, bool SPLIT, int FMT_A = kFmtBF16, int FMT_B = kFmtBF16>
+__global__ void __launch_bounds__(384, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmC,
-               const GemmGeom g, float* __restrict__ C) {
+               const GemmGeom g, float* __restrict__ slab) {
+  static_assert(FMT_A == kFmtBF16 && FMT_B == kFmtBF16, "wgmma multiplies operands of one format");
   extern __shared__ uint8_t raw[];
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* sEpi = base + (size_t)kGemmStages * kGemmStageBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sEpi + (ATOMIC ? 0 : kGemmEpiBytes));
+  float* sStg = reinterpret_cast<float*>(sEpi + (SPLIT ? 0 : kGemmEpiBytes));   // [2 warpgroups][kStgBytes]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sStg) + 2 * kStgBytes);
   uint64_t* full = bars;                       // [stages]
   uint64_t* empty = bars + kGemmStages;        // [stages]
-  uint64_t* t_full = bars + 2 * kGemmStages;   // [2]
-  uint64_t* t_empty = t_full + 2;              // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(t_empty + 2);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < kGemmStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&t_full[i], 1); mbar_init(&t_empty[i], 128); }
+    for (int i = 0; i < kGemmStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 256); }
     fence_barrier_init();
   }
   if (warp == 0 && lane == 0) { prefetch_tmap(&tmA); prefetch_tmap(&tmB); }
-  if (warp == 2) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int num_tiles = g.m_tiles * g.n_tiles * g.k_splits;
   pdl_wait();                  // predecessor grid complete: global memory may be touched from here on
   pdl_trigger();
@@ -69,8 +64,9 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     mt = tile / g.n_tiles;
   };
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    regs_dec<40>();
+    if (warp == 0 && lane == 0) {
       uint32_t cnt = 0;
       for (int i = 0; i < my_tiles; ++i) {
         int mt, nt, ks;
@@ -98,65 +94,66 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-  } else if (warp == 1) {
-    // whole warp converged; one elected lane issues
-    constexpr uint32_t idesc = make_idesc_f16kind(128, 256, A_MN ? 1 : 0, B_MN ? 1 : 0, FMT_A, FMT_B);
+  } else {
+    regs_inc<232>();
+    const int cw = (warp - 4) >> 2;              // MMA warpgroup: rows [64 cw, 64 cw + 64) of the tile
+    const int wi = warp & 3;
+    const int ew = 2 * cw + (wi & 1);            // row quarter this warp stores
+    const int eg = wi >> 1;                      // 32-column chunk parity this warp stores
+    const int erow = 32 * (wi & 1) + lane;
+    float* stg = sStg + cw * (kStgBytes / 4);
+    uint8_t* stg_tma = sEpi + (warp - 4) * 4096;  // this warp's TMA-store staging block
+    const int sw = lane & 7;
+    bool store_pending = false;
     uint32_t cnt = 0;
+    float acc[128];
     for (int i = 0; i < my_tiles; ++i) {
-      const int b = i & 1;
-      mbar_wait(&t_empty[b], ((i >> 1) & 1) ^ 1);
-      tc_fence_after();
+      int mt, nt, ks;
+      decode((int)blockIdx.x + i * (int)gridDim.x, mt, nt, ks);
+      acc_fence(acc);
+      int prev = -1;
       for (int kb = 0; kb < g.kb_per_split; ++kb, ++cnt) {
         const int s = cnt % kGemmStages;
         mbar_wait(&full[s], (cnt / kGemmStages) & 1);
-        tc_fence_after();
-        const uint32_t a_addr = smem_u32(base + (size_t)s * kGemmStageBytes), b_addr = a_addr + 16384;
-        const uint32_t a_lo = desc_lo(a_addr, A_MN ? 8192 : 16), b_lo = desc_lo(b_addr, B_MN ? 8192 : 16);
-        if (elect_one()) {
+        // this warpgroup's 64 rows: the second 64-wide column block (MN-major) or 64 rows further (K-major), 8 KB either way
+        const uint32_t a_addr = smem_u32(base + (size_t)s * kGemmStageBytes) + (uint32_t)cw * 8192, b_addr = smem_u32(base + (size_t)s * kGemmStageBytes) + 16384;
+        const uint32_t a_lo = desc_lo(a_addr, 16), b_lo = desc_lo(b_addr, B_MN ? 8192 : 16);
+        wg_fence();
 #pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_bf16(tmem_base + (uint32_t)(b * 256), desc_from_lo(a_lo + k * (A_MN ? 128 : 2)), desc_from_lo(b_lo + k * (B_MN ? 128 : 2)),
-                      idesc, (kb > 0 || k > 0) ? 1u : 0u);
-          umma_commit(&empty[s]);
-        }
-        __syncwarp();
+        for (int k = 0; k < 4; ++k)
+          wgmma_bf16<256, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, desc_from_lo(a_lo + k * (A_MN ? 128 : 2)), desc_from_lo(b_lo + k * (B_MN ? 128 : 2)),
+                                                      (kb > 0 || k > 0) ? 1u : 0u);
+        wg_commit();
+        wg_wait<1>();
+        if (prev >= 0) mbar_arrive(&empty[prev]);
+        prev = s;
       }
-      if (elect_one()) umma_commit(&t_full[b]);
-      __syncwarp();
-    }
-  } else if (warp >= 4) {
-    const int ew = warp - 4;
-    uint8_t* stg0 = sEpi + ew * 8192;            // two staging blocks per warp: chunk c fills one while the TMA store
-    const int sw = lane & 7;                      // of chunk c-1 still reads the other
-    int stores_in_flight = 0;
-    for (int i = 0; i < my_tiles; ++i) {
-      const int b = i & 1;
-      int mt, nt, ks;
-      decode((int)blockIdx.x + i * (int)gridDim.x, mt, nt, ks);
-      mbar_wait(&t_full[b], (i >> 1) & 1);
-      tc_fence_after();
+      wg_wait<0>();
+      if (prev >= 0) mbar_arrive(&empty[prev]);
+      acc_fence(acc);
       const int m = mt * 128 + ew * 32 + lane;
-      float* crow = C + (int64_t)m * g.ldc + nt * 256;
+      float* prow = slab + ((size_t)ks * g.M + m) * g.N + nt * 256;     // SPLIT: this split's partial row
 #pragma unroll 1
-      for (int c = 0; c < 8; ++c) {
+      for (int cc = 0; cc < 4; ++cc) {
+        const int c = 2 * cc + eg;
         float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)(b * 256 + c * 32), v);
+        named_sync(5 + cw, 128); stage_acc64(acc, cc, stg); named_sync(5 + cw, 128);
+        stg_read32(stg, erow, eg * 32, v);
         const int n0 = nt * 256 + c * 32;
-        if (ATOMIC) {
+        if (SPLIT) {
           if (m < g.M) {
             if (n0 + 32 <= g.N) {
 #pragma unroll
-              for (int j = 0; j < 8; ++j) red_add_v4(crow + c * 32 + 4 * j, v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+              for (int j = 0; j < 8; ++j) reinterpret_cast<float4*>(prow + c * 32)[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
             } else {
 #pragma unroll
               for (int j = 0; j < 32; ++j)
-                if (n0 + j < g.N) atomicAdd(crow + c * 32 + j, v[j]);
+                if (n0 + j < g.N) prow[c * 32 + j] = v[j];
             }
           }
         } else {
-          uint8_t* stg = stg0 + (c & 1) * 4096;
-          const uint32_t my_row = smem_u32(stg) + lane * 128;
-          if (stores_in_flight >= 2) { if (lane == 0) bulk_wait_read1(); __syncwarp(); stores_in_flight = 1; }
+          const uint32_t my_row = smem_u32(stg_tma) + lane * 128;
+          if (store_pending) { if (lane == 0) bulk_wait_read0(); __syncwarp(); }
 #pragma unroll
           for (int j4 = 0; j4 < 8; ++j4)
             asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(my_row + (uint32_t)((j4 ^ sw) << 4)), "f"(v[4 * j4]), "f"(v[4 * j4 + 1]),
@@ -164,27 +161,22 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           fence_proxy_async();
           __syncwarp();
           if (lane == 0) {                          // (always commit, possibly an empty group, so the group count stays uniform)
-            if (n0 < g.N && mt * 128 + ew * 32 < g.M) tma_store_2d(&tmC, stg, n0, mt * 128 + ew * 32);
+            if (n0 < g.N && mt * 128 + ew * 32 < g.M) tma_store_2d(&tmC, stg_tma, n0, mt * 128 + ew * 32);
             bulk_commit();
           }
-          ++stores_in_flight;
+          store_pending = true;
         }
       }
-      tc_fence_before();
-      mbar_arrive(&t_empty[b]);
     }
-    if (!ATOMIC) { if (lane == 0) bulk_wait0(); __syncwarp(); }
+    if (!SPLIT) { if (lane == 0) bulk_wait0(); __syncwarp(); }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, 512);
 }
 
 // Host launcher.  C[M][N] (+)= A . B on tensor cores.  a_inner/a_outer: dims of A's tensor (innermost first); same for B.
 // seg (nullable): offsets of the contraction segments (see GemmGeom), K is the length of ONE segment.
 struct GemmSegments { int n; int a_koff[3], a_moff[3], b_koff[3], b_noff[3]; };
 
-template <bool A_MN, bool B_MN, bool ATOMIC, int FMT_A = kFmtBF16, int FMT_B = kFmtBF16>
+template <bool A_MN, bool B_MN, bool SPLIT, int FMT_A = kFmtBF16, int FMT_B = kFmtBF16>
 inline int launch_gemm(const void* A, uint64_t a_inner, uint64_t a_outer, const void* Bm, uint64_t b_inner, uint64_t b_outer,
                        float* C, int64_t ldc, int M, int N, int K, int k_splits, const GemmSegments* seg, cudaStream_t st) {
   GemmGeom g;
@@ -215,13 +207,24 @@ inline int launch_gemm(const void* A, uint64_t a_inner, uint64_t a_outer, const 
   uint32_t boxC[2] = {32, 32};
   rc = make_tmap(&tmC, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, C, 2, dC, sC, boxC);
   if (rc != UDH_OK) return rc;
-  const size_t smem = 1024 + (size_t)kGemmStages * kGemmStageBytes + (ATOMIC ? 0 : kGemmEpiBytes) + 256;
-  auto kern = tc_gemm_kernel<A_MN, B_MN, ATOMIC, FMT_A, FMT_B>;
+  const size_t smem = 1024 + (size_t)kGemmStages * kGemmStageBytes + (SPLIT ? 0 : kGemmEpiBytes) + 2 * kStgBytes + 256;
+  auto kern = tc_gemm_kernel<A_MN, B_MN, SPLIT, FMT_A, FMT_B>;
   UDH_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int sms = persistent_ctas();
   const int tiles = g.m_tiles * g.n_tiles * g.k_splits;
-  launch_chain(kern, dim3(tiles < sms ? tiles : sms), dim3(256), smem, st, tmA, tmB, tmC, g, C);
-  return check_launch("tc_gemm_kernel");
+  float* slab = nullptr;
+  if (SPLIT) {
+    UDH_REQUIRE(ldc == N, "tc gemm: split-K needs a dense output (ldc %lld, N %d)", (long long)ldc, N);
+    slab = slab_scratch((size_t)k_splits * M * N, st);
+    if (!slab) return UDH_ECUDA;
+  }
+  launch_chain(kern, dim3(tiles < sms ? tiles : sms), dim3(384), smem, st, tmA, tmB, tmC, g, slab);
+  if (int rc2 = check_launch("tc_gemm_kernel")) return rc2;
+  if (!SPLIT) return UDH_OK;
+  SlabSegments t;
+  t.count = 1;
+  t.s[0] = SlabSegment{slab, C, (size_t)M * N, k_splits, M * N};
+  return slab_reduce(t, st);
 }
 
 }  // namespace tc

@@ -182,7 +182,7 @@ extern "C" int udh_bwd_marker_wait(void* stream) {
 }
 
 extern "C" int udh_set_adam_grid(int blocks) {
-  UDH_REQUIRE(blocks >= 0 && blocks <= 148 * 16, "udh_set_adam_grid: blocks must be in 0..2368");
+  UDH_REQUIRE(blocks >= 0 && blocks <= udh::kSmCount * 16, "udh_set_adam_grid: blocks must be in 0..%d", udh::kSmCount * 16);
   udh::g_adam_grid = blocks;
   return UDH_OK;
 }
@@ -256,7 +256,7 @@ extern "C" int udh_adam_step_mirror_ex(float* p, float* g, float* m, float* v, s
   UDH_REQUIRE(((uintptr_t)p | (uintptr_t)g | (uintptr_t)m | (uintptr_t)v) % 16 == 0, "udh_adam_step: buffers must be 16-byte aligned");
   if (n == 0) return UDH_OK;
   const size_t n4 = n / 4;
-  const size_t full = (n4 + 255) / 256, cap = udh::g_adam_grid > 0 ? (size_t)udh::g_adam_grid : (size_t)148 * 16;
+  const size_t full = (n4 + 255) / 256, cap = udh::g_adam_grid > 0 ? (size_t)udh::g_adam_grid : (size_t)udh::kSmCount * 16;
   const unsigned blocks = (unsigned)(full < cap ? full : cap);
   udh::ProfScope ps(udh::PROF_ADAM, udh::as_stream(stream));
   udh::launch_chain(udh::adam_kernel, dim3(blocks), dim3(256), 0, udh::as_stream(stream), (float4*)p, (float4*)g, (float4*)m, (float4*)v, n4, alpha_t,
@@ -265,3 +265,50 @@ extern "C" int udh_adam_step_mirror_ex(float* p, float* g, float* m, float* v, s
                                                               (mirror && mirror_limbs == 2) ? (uint2*)((char*)mirror + mirror_count * 2) : (uint2*)nullptr);
   return udh::check_launch("udh_adam_step");
 }
+
+// ---------------------------------------------------------------------------------------------------- slab reductions
+namespace udh {
+namespace {
+__global__ void slab_reduce_kernel(SlabSegments t) {
+  pdl_wait(); pdl_trigger();   // launched through launch_chain (common.cuh)
+  const SlabSegment sg = t.s[blockIdx.y];
+  for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < sg.n; e += gridDim.x * blockDim.x) {
+    float sum = 0.f;
+    for (int k = 0; k < sg.nslab; ++k) sum += sg.slab[(size_t)k * sg.stride + e];
+    sg.dst[e] += sum;
+  }
+}
+}  // namespace
+
+float* slab_scratch(size_t floats, cudaStream_t st) {
+  constexpr int kMaxDevices = 64;
+  static float* buf[kMaxDevices];
+  static size_t cap[kMaxDevices];
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) { set_error("slab_scratch: no usable device"); return nullptr; }
+  if (floats > cap[dev]) {
+    if (buf[dev]) {                     // the previous buffer may still be read by work queued on this stream
+      cudaStreamSynchronize(st);
+      cudaFree(buf[dev]);
+      buf[dev] = nullptr; cap[dev] = 0;
+    }
+    if (cudaMalloc(&buf[dev], floats * sizeof(float)) != cudaSuccess) {
+      buf[dev] = nullptr;
+      set_error("slab_scratch: cannot allocate %zu bytes", floats * sizeof(float));
+      return nullptr;
+    }
+    cap[dev] = floats;
+  }
+  return buf[dev];
+}
+
+int slab_reduce(const SlabSegments& segs, cudaStream_t st) {
+  UDH_REQUIRE(segs.count >= 1 && segs.count <= 16, "slab_reduce: %d segments", segs.count);
+  int n = 0;
+  for (int i = 0; i < segs.count; ++i) n = segs.s[i].n > n ? segs.s[i].n : n;
+  const int gx = (n + 255) / 256 < 256 ? (n + 255) / 256 : 256;
+  launch_chain(slab_reduce_kernel, dim3(gx > 0 ? gx : 1, segs.count), dim3(256), 0, st, segs);
+  return check_launch("slab_reduce");
+}
+}  // namespace udh
+

@@ -53,7 +53,7 @@ extern "C" int udh_prep_inputs_u8(const uint8_t* I, const uint8_t* I_prime, cons
   cudaStream_t st = udh::as_stream(stream);
   udh::ProfScope ps(udh::PROF_ELTWISE, st);
   const size_t n4 = (size_t)B * img_h * img_w * 3 / 4;
-  udh::normalise_u8_kernel<<<(unsigned)((n4 + 255) / 256 < 148 * 16 ? (n4 + 255) / 256 : 148 * 16), 256, 0, st>>>(I, I_aug, n4);
+  udh::normalise_u8_kernel<<<(unsigned)((n4 + 255) / 256 < udh::kSmCount * 16 ? (n4 + 255) / 256 : udh::kSmCount * 16), 256, 0, st>>>(I, I_aug, n4);
   int rc = udh::check_launch("normalise_u8");
   if (rc) return rc;
   udh::patches_u8_kernel<<<dim3((P * P + 255) / 256 < 16 ? (P * P + 255) / 256 : 16, B), 256, 0, st>>>(I, I_prime, pts1, I1, I2, patch_origin,

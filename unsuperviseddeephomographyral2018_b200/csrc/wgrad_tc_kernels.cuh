@@ -1,17 +1,18 @@
-// tcgen05 weight-gradient kernel on the padded bf16 streams (see conv_tc_kernels.cuh for the layout).
+// wgmma weight-gradient kernel on the padded bf16 streams (see conv_tc_kernels.cuh for the layout).
 //
 //   dW[tap][ci][co] = sum_q X[q + off_tap][ci] * G[q][co],   off_tap = (ky-1)*Wp + (kx-1)
 // summed over EVERY flattened position q: G is zero on the borders, so border terms vanish and no masking is needed.
 // Positions are the contraction (K) dimension, channels are contiguous in memory, so both operands are MN-major:
 //   A = rows of X shifted by off_tap (M = input channels), B = rows of G (N = output channels), K = 16 positions / MMA.
-// M is always 128:
-//   Cin = 64  : TWO TAPS per MMA — the second 64-row M block is the same smem buffer shifted by (off_b - off_a) rows,
-//               expressed through the descriptor's leading-dimension byte offset; the odd tap 8 is paired with a block
-//               of ones, whose 64 identical result rows are the bias gradient sum_q G[q][co];
-//   Cin = 128 : one tap per MMA, the two 64-channel blocks of X are the two M blocks; a tenth group is an M = 64 MMA
-//               of the ones block against G, whose (identical) result rows are the bias gradient.
-// Accumulators stay in TMEM for the CTA's whole run (split-K over CTAs); one epilogue at the end adds them to the fp32
-// gradient buffer with atomics.  warp 0: TMA producer | warp 1: MMA issuer | warp 2: TMEM alloc | warps 4-7: epilogue.
+// A GROUP is 128 accumulator rows; MMA warpgroup cw owns rows [64 cw, 64 cw + 64):
+//   Cin = 64  : TWO TAPS per group — warpgroup 1 reads the same staged X rows shifted by (off_b - off_a); the odd tap 8 is
+//               paired with a block of ones, whose 64 identical result rows are the bias gradient sum_q G[q][co];
+//   Cin = 128 : one tap per group, the two 64-channel blocks of X are the two warpgroups' A operands; a tenth group
+//               multiplies the ones block with G (bias gradient, its first row is used).
+// Every CTA owns ONE group (the accumulators of a group fill the MMA warpgroups' registers): the groups are slices of the
+// 1-D grid, each with a share of the CTAs, and every CTA reduces its group over its positions (split-K) into its own slab of
+// a scratch buffer; the launcher adds the slabs to the fp32 gradient buffer in CTA order.
+// warpgroup 0: TMA producer (warp 0) | warpgroups 1-2: MMA + epilogue.
 #pragma once
 #include "tc_common.cuh"
 
@@ -23,20 +24,25 @@ struct WgradGeom {
   int num_items;     // ceil(ceil(Q/128) / T)
   int xrows;         // T*128 + 2*hh rows staged per 64-channel block of X
   int num_groups;    // CBX == 1: 5 (4 tap pairs + tap 8 | ones);  CBX == 2: 10 (9 taps + ones)
-  // The accumulators of all groups do not fit the 512 TMEM columns when N_OUT = 128, so the groups are cut into slices;
   // slice s owns groups [slice_group[s], slice_group[s+1]) and CTAs [slice_cta[s], slice_cta[s+1]) of the 1-D grid
-  // (CTA counts proportional to the slice's group count, so every CTA issues about the same number of MMAs).
+  // (CTA counts proportional to the slice's group count, so every CTA issues about the same number of MMAs); the kernels
+  // take one group per slice.
   int num_slices;
-  int slice_group[5];
-  int slice_cta[5];
+  int slice_group[11];
+  int slice_cta[11];
 };
 
+// Every CTA stores its group's accumulators in its own slab of a scratch buffer; the launcher then adds the slabs to the
+// fp32 gradient buffer in a fixed order (slab_reduce), so the gradient does not depend on CTA timing.
+//   generic kernels: slab = the group's 128 rows x N_OUT columns, in the order of the gradient rows they feed;
+//   N = 192 kernels: slab = the group's taps in the HWIO layout of dW (group 0: taps 0-5; group 1: taps 6-8, then db).
+constexpr int kWgrad64SlabFloats = 6 * 64 * 64;
+
 template <int N_OUT, int CBX, int T>
-__global__ void __launch_bounds__(256, 1)
+__global__ void __launch_bounds__(384, 1)
 tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmX128, const __grid_constant__ CUtensorMap tmXhh,
-                const __grid_constant__ CUtensorMap tmG, const WgradGeom g, float* __restrict__ dW, float* __restrict__ db) {
+                const __grid_constant__ CUtensorMap tmG, const WgradGeom g, float* __restrict__ slab) {
   constexpr int CBO = N_OUT / 64;
-  constexpr int CIN = CBX * 64;
   extern __shared__ uint8_t raw[];
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw) + 1023) & ~(uintptr_t)1023);
   const int xblk_bytes = g.xrows * 128;                         // one 64-channel block of X of one stage
@@ -47,16 +53,12 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmX128, const __grid_constan
   uint64_t* bars = reinterpret_cast<uint64_t*>(sOnes + 16384);
   uint64_t* full = bars;        // [2]
   uint64_t* empty = bars + 2;   // [2]
-  uint64_t* acc_full = bars + 4;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 5);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int sl = 0;
   while (sl + 1 < g.num_slices && (int)blockIdx.x >= g.slice_cta[sl + 1]) ++sl;
   const int bx = (int)blockIdx.x - g.slice_cta[sl], gxs = g.slice_cta[sl + 1] - g.slice_cta[sl];
-  const int g_begin = g.slice_group[sl];
-  const int g_count = g.slice_group[sl + 1] - g_begin;
-  constexpr int kTmemCols = 512;
+  const int gi = g.slice_group[sl];                             // this CTA's group
 
   {
     // ones block: every 16-byte chunk is identical, so the 128-byte swizzle leaves it unchanged
@@ -65,22 +67,18 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmX128, const __grid_constan
     fence_proxy_async();                                        // generic-proxy writes -> visible to the tensor (async) proxy
   }
   if (threadIdx.x == 0) {
-    for (int i = 0; i < 2; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    mbar_init(acc_full, 1);
+    for (int i = 0; i < 2; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 256); }
     fence_barrier_init();
   }
   if (warp == 0 && lane == 0) { prefetch_tmap(&tmX128); prefetch_tmap(&tmXhh); prefetch_tmap(&tmG); }
-  if (warp == 2) tmem_alloc(tmem_slot, kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();                  // predecessor grid complete: global memory may be touched from here on
   pdl_trigger();
   const int my_items = (g.num_items - bx + gxs - 1) / gxs;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    regs_dec<40>();
+    if (warp == 0 && lane == 0) {
       for (int it = 0; it < my_items; ++it) {
         const int s = it & 1;
         const int q0 = (bx + it * gxs) * T * 128;
@@ -98,105 +96,58 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmX128, const __grid_constan
             tma_load_2d(st + (size_t)CBX * xblk_bytes + (size_t)cb * gblk_bytes + (size_t)t * 16384, &tmG, cb * 64, q0 + t * 128, &full[s]);
       }
     }
-  } else if (warp == 1) {
-    // whole warp converged; one elected lane issues (see conv_tc_kernels.cuh)
-    constexpr uint32_t idesc = make_idesc_bf16(128, N_OUT, 1, 1);
-    constexpr uint32_t idesc_ones = make_idesc_bf16(64, N_OUT, 1, 1);
+  } else {                                                      // (CTAs without items store zero slabs)
+    regs_inc<232>();
+    const int cw = (warp - 4) >> 2;
     const uint32_t ones_addr = smem_u32(sOnes);
+    // A operand of this warpgroup: a row shift of X (channel block xcb), or the ones block
+    int off = 0, xcb = 0;
+    bool ones = false;
+    if (CBX == 1) {
+      const int tap = 2 * gi + cw;
+      if (tap == 9) ones = true;
+      else off = (tap / 3 - 1) * g.Wp + (tap % 3 - 1);
+    } else if (gi < 9) {
+      off = (gi / 3 - 1) * g.Wp + (gi % 3 - 1);
+      xcb = cw;
+    } else {
+      ones = true;
+    }
+    float acc[N_OUT / 2];
+    acc_zero(acc);
     for (int it = 0; it < my_items; ++it) {
       const int s = it & 1;
       mbar_wait(&full[s], (it >> 1) & 1);
-      tc_fence_after();
       const uint32_t x_addr = smem_u32(sStage + (size_t)s * stage_bytes);
       const uint32_t g_addr = x_addr + (uint32_t)(CBX * xblk_bytes);
+      acc_fence(acc);
+      wg_fence();
 #pragma unroll 1
       for (int t = 0; t < T; ++t) {
-#pragma unroll 1
-        for (int gl = 0; gl < g_count; ++gl) {
-          const int gi = g_begin + gl;
-          uint32_t a_start, lbo;
-          if (CBX == 1) {
-            const int tap0 = 2 * gi;
-            const int off0 = (tap0 / 3 - 1) * g.Wp + (tap0 % 3 - 1);
-            a_start = x_addr + (uint32_t)(g.hh + t * 128 + off0) * 128;
-            if (gi < 4) {
-              const int tap1 = tap0 + 1;
-              const int off1 = (tap1 / 3 - 1) * g.Wp + (tap1 % 3 - 1);
-              lbo = (uint32_t)(off1 - off0) * 128;
-            } else {
-              lbo = ones_addr - a_start;                      // second M block = the ones rows (bias gradient)
-            }
-          } else if (gi < 9) {
-            const int off = (gi / 3 - 1) * g.Wp + (gi % 3 - 1);
-            a_start = x_addr + (uint32_t)(g.hh + t * 128 + off) * 128;
-            lbo = (uint32_t)xblk_bytes;                       // second M block = channels 64..127
-          } else {
-            a_start = ones_addr; lbo = 0;                     // M = 64 rows of ones (bias gradient)
-          }
-          const uint32_t id = (CBX == 2 && gi == 9) ? idesc_ones : idesc;
-          const uint32_t a_lo = desc_lo(a_start, lbo);
-          const uint32_t b_lo = desc_lo(g_addr + (uint32_t)t * 16384, (uint32_t)gblk_bytes);
-          const uint32_t d_tmem = tmem_base + (uint32_t)(gl * N_OUT);
-          if (elect_one()) {
+        const uint32_t a_start = ones ? ones_addr : x_addr + (uint32_t)xcb * xblk_bytes + (uint32_t)(g.hh + t * 128 + off) * 128;
+        const uint32_t a_lo = desc_lo(a_start, 0);
+        const uint32_t b_lo = desc_lo(g_addr + (uint32_t)t * 16384, (uint32_t)gblk_bytes);
 #pragma unroll
-            for (int kk = 0; kk < 8; ++kk)                     // 16 positions = 2048 bytes = 128 sixteen-byte units per k-step
-              umma_bf16(d_tmem, desc_from_lo(a_lo + kk * 128), desc_from_lo(b_lo + kk * 128), id, (it > 0 || t > 0 || kk > 0) ? 1u : 0u);
-          }
-          __syncwarp();
-        }
+        for (int kk = 0; kk < 8; ++kk)                     // 16 positions = 2048 bytes = 128 sixteen-byte units per k-step
+          wgmma_bf16<N_OUT, 1, 1>(acc, desc_from_lo(a_lo + kk * 128), desc_from_lo(b_lo + kk * 128), 1u);
       }
-      if (elect_one()) umma_commit(&empty[s]);
-      __syncwarp();
+      wg_commit();
+      wg_wait<0>();
+      acc_fence(acc);
+      mbar_arrive(&empty[s]);
     }
-    if (elect_one()) umma_commit(acc_full);
-    __syncwarp();
-  } else if (warp >= 4 && my_items > 0) {
-    const int ew = warp - 4;
-    const int m = ew * 32 + lane;                               // accumulator row == TMEM lane
-    mbar_wait(acc_full, 0);
-    tc_fence_after();
-#pragma unroll 1
-    for (int gl = 0; gl < g_count; ++gl) {
-      const int gi = g_begin + gl;
-      int tap, ci;
-      bool is_ones = false;
-      if (CBX == 1) {
-        ci = m & 63;
-        tap = 2 * gi + (m >> 6);
-        if (tap == 9) is_ones = true;
-      } else {
-        ci = m; tap = gi;
-        if (gi == 9) is_ones = true;
-      }
-      float* dst = is_ones ? db : dW + ((size_t)tap * CIN + ci) * N_OUT;
-      const bool active = is_ones ? (m == (CBX == 1 ? 64 : 0) && db != nullptr) : true;
-#pragma unroll 1
-      for (int c = 0; c < N_OUT / 32; ++c) {
-        float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)(gl * N_OUT + c * 32), v);
-        if (active) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j)                                  // 16-byte vector reductions: 4x fewer L2 atomics
-            red_add_v4(dst + c * 32 + 4 * j, v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-        }
-      }
-    }
+    float* mine = slab + (size_t)blockIdx.x * 128 * N_OUT + (size_t)cw * 64 * N_OUT;
+    store_acc(acc, [&](int r, int c) -> float* { return mine + (size_t)r * N_OUT + c; });
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, kTmemCols);
 }
 
 
 // ---------------------------------------------------------------------------------------------------------------------
 // 64 -> 64 channel layers (conv1_2, conv2_1, conv2_2): N = 192 variant.
-// An (M128, N64, K16) MMA is capped at ~50 clk by the rate at which the 4 KB A operand can be fetched from shared memory
-// (64 % of the tensor peak, measured with tools/tc_probe2.py; pairing CTAs does not change it), so here the N side is
-// widened instead: B is THREE row shifts of the gradient rows, c = -1, 0, +1 (three 64-wide MN blocks, leading-dimension
-// byte offset = one 128-byte row), A is two row shifts of X (ky and ky' rows of the 3x3 window, as above).  Since
+// The N side is widened: B is THREE row shifts of the gradient rows, c = -1, 0, +1 (three 64-wide MN blocks, leading-dimension
+// byte offset = one 128-byte row), A is a row shift of X (one per MMA warpgroup: the ky and ky' rows of the 3x3 window).  Since
 //   sum_q X[q + a][ci] * G[q + c][co]  =  dW at tap offset (a - c),
-// one (M128, N192, K16) MMA yields the six taps (ky, ky') x (kx = -c), and the whole 3x3 window + bias gradient takes
-// TWO MMAs per 16 positions (96 clk each) instead of five (50 clk each):
+// one (M128, N192) group yields the six taps (ky, ky') x (kx = -c), and the whole 3x3 window + bias gradient takes two groups:
 //   group 0: A = X[q - Wp] | X[q]          -> taps ky = -1, 0 ; kx = +1, 0, -1 (N blocks 0, 1, 2)
 //   group 1: A = X[q + Wp] | ones          -> taps ky = +1    ; rows 64.. = bias gradient (taken from N block 1)
 // G needs one halo row on each side (8 are staged to keep the 1024-byte swizzle-atom alignment of the TMA boxes).
@@ -207,9 +158,9 @@ struct Wgrad64Geom {
 };
 
 template <int T>
-__global__ void __launch_bounds__(256, 1)
+__global__ void __launch_bounds__(384, 1)
 tc_wgrad64_kernel(const __grid_constant__ CUtensorMap tmX128, const __grid_constant__ CUtensorMap tmXhh,
-                  const __grid_constant__ CUtensorMap tmG136, const Wgrad64Geom g, float* __restrict__ dW, float* __restrict__ db) {
+                  const __grid_constant__ CUtensorMap tmG136, const Wgrad64Geom g, float* __restrict__ slab) {
   static_assert(T == 2, "G is staged as two 136-row boxes");
   extern __shared__ uint8_t raw[];
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw) + 1023) & ~(uintptr_t)1023);
@@ -222,10 +173,9 @@ tc_wgrad64_kernel(const __grid_constant__ CUtensorMap tmX128, const __grid_const
   uint64_t* bars = reinterpret_cast<uint64_t*>(sOnes + 16384);
   uint64_t* full = bars;        // [2]
   uint64_t* empty = bars + 2;   // [2]
-  uint64_t* acc_full = bars + 4;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 5);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr int kTmemCols = 512;                                // 2 groups x 192 columns
+  // even CTAs own group 0, odd CTAs group 1 (a group's 128 x 192 accumulators fill the MMA warpgroups' registers)
+  const int gl = (int)blockIdx.x & 1, bx = (int)blockIdx.x >> 1, gxs = (int)gridDim.x >> 1;
 
   {
     uint32_t* o = reinterpret_cast<uint32_t*>(sOnes);
@@ -233,25 +183,21 @@ tc_wgrad64_kernel(const __grid_constant__ CUtensorMap tmX128, const __grid_const
     fence_proxy_async();
   }
   if (threadIdx.x == 0) {
-    for (int i = 0; i < 2; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    mbar_init(acc_full, 1);
+    for (int i = 0; i < 2; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 256); }
     fence_barrier_init();
   }
   if (warp == 0 && lane == 0) { prefetch_tmap(&tmX128); prefetch_tmap(&tmXhh); prefetch_tmap(&tmG136); }
-  if (warp == 2) tmem_alloc(tmem_slot, kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();                  // predecessor grid complete: global memory may be touched from here on
   pdl_trigger();
-  const int my_items = (g.num_items - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+  const int my_items = (g.num_items - bx + gxs - 1) / gxs;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    regs_dec<40>();
+    if (warp == 0 && lane == 0) {
       for (int it = 0; it < my_items; ++it) {
         const int s = it & 1;
-        const int q0 = ((int)blockIdx.x + it * (int)gridDim.x) * T * 128;
+        const int q0 = (bx + it * gxs) * T * 128;
         mbar_wait(&empty[s], ((it >> 1) & 1) ^ 1);
         mbar_arrive_expect_tx(&full[s], (uint32_t)stage_bytes);
         uint8_t* dst = sStage + (size_t)s * stage_bytes;
@@ -263,66 +209,44 @@ tc_wgrad64_kernel(const __grid_constant__ CUtensorMap tmX128, const __grid_const
         tma_load_2d(gd + 136 * 128, &tmG136, 0, q0 + 128, &full[s]);
       }
     }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = make_idesc_bf16(128, 192, 1, 1);
+  } else {                                                      // (CTAs without items store zero slabs)
+    regs_inc<232>();
+    const int cw = (warp - 4) >> 2;
     const uint32_t ones_addr = smem_u32(sOnes);
+    // rows of the group: group 0 = [X[q - Wp] | X[q]], group 1 = [X[q + Wp] | ones]
+    const int shift = gl == 0 ? (cw == 0 ? -g.Wp : 0) : g.Wp;
+    const bool ones = gl == 1 && cw == 1;
+    float acc[96];
+    acc_zero(acc);
     for (int it = 0; it < my_items; ++it) {
       const int s = it & 1;
       mbar_wait(&full[s], (it >> 1) & 1);
-      tc_fence_after();
       const uint32_t x_addr = smem_u32(sStage + (size_t)s * stage_bytes);
       const uint32_t g_addr = x_addr + (uint32_t)xblk_bytes;
+      acc_fence(acc);
+      wg_fence();
 #pragma unroll 1
       for (int t = 0; t < T; ++t) {
         const uint32_t b_lo = desc_lo(g_addr + (uint32_t)(8 + t * 128 - 1) * 128, 128);     // G[q-1] | G[q] | G[q+1]
+        const uint32_t a_lo = desc_lo(ones ? ones_addr : x_addr + (uint32_t)(g.hh + t * 128 + shift) * 128, 0);
 #pragma unroll
-        for (int gl = 0; gl < 2; ++gl) {
-          const uint32_t a_start = x_addr + (uint32_t)(g.hh + t * 128 + (gl == 0 ? -g.Wp : g.Wp)) * 128;
-          const uint32_t lbo = gl == 0 ? (uint32_t)g.Wp * 128 : ones_addr - a_start;
-          const uint32_t a_lo = desc_lo(a_start, lbo);
-          const uint32_t d_tmem = tmem_base + (uint32_t)(gl * 192);
-          if (elect_one()) {
-#pragma unroll
-            for (int kk = 0; kk < 8; ++kk)
-              umma_bf16(d_tmem, desc_from_lo(a_lo + kk * 128), desc_from_lo(b_lo + kk * 128), idesc, (it > 0 || t > 0 || kk > 0) ? 1u : 0u);
-          }
-          __syncwarp();
-        }
+        for (int kk = 0; kk < 8; ++kk)
+          wgmma_bf16<192, 1, 1>(acc, desc_from_lo(a_lo + kk * 128), desc_from_lo(b_lo + kk * 128), 1u);
       }
-      if (elect_one()) umma_commit(&empty[s]);
-      __syncwarp();
+      wg_commit();
+      wg_wait<0>();
+      acc_fence(acc);
+      mbar_arrive(&empty[s]);
     }
-    if (elect_one()) umma_commit(acc_full);
-    __syncwarp();
-  } else if (warp >= 4 && my_items > 0) {
-    const int ew = warp - 4;
-    const int m = ew * 32 + lane;
-    const int ci = m & 63;
-    mbar_wait(acc_full, 0);
-    tc_fence_after();
-#pragma unroll 1
-    for (int gl = 0; gl < 2; ++gl) {
-      const int ky = gl == 0 ? (m >> 6) - 1 : 1;                  // rows 64.. of group 1 are the ones rows
-      const bool is_ones = gl == 1 && m >= 64;
-#pragma unroll 1
-      for (int c = 0; c < 6; ++c) {
-        const int j = c >> 1;                                     // N block: G shift c = j - 1  ->  kx = 1 - j
-        const int tap = (ky + 1) * 3 + (2 - j);
-        float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)(gl * 192 + c * 32), v);
-        float* dst = is_ones ? db : dW + ((size_t)tap * 64 + ci) * 64;
-        const bool active = is_ones ? (m == 64 && j == 1 && db != nullptr) : true;
-        if (active) {
-#pragma unroll
-          for (int jj = 0; jj < 8; ++jj)
-            red_add_v4(dst + (c & 1) * 32 + 4 * jj, v[4 * jj], v[4 * jj + 1], v[4 * jj + 2], v[4 * jj + 3]);
-        }
-      }
-    }
+    float* mine = slab + (size_t)blockIdx.x * kWgrad64SlabFloats;
+    store_acc(acc, [&](int r, int c) -> float* {
+      const int m = 64 * cw + r, ci = m & 63, jb = c >> 6, co = c & 63;   // N block jb: G shift jb - 1 -> kx = 1 - jb
+      if (gl == 1 && m >= 64) return (m == 64 && jb == 1) ? mine + 3 * 4096 + co : nullptr;   // ones rows: db
+      const int ky = gl == 0 ? (m >> 6) - 1 : 1;
+      const int tap = (ky + 1) * 3 + (2 - jb);
+      return mine + ((size_t)(tap - 6 * gl) * 64 + ci) * 64 + co;
+    });
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, kTmemCols);
 }
 
 }  // namespace tc

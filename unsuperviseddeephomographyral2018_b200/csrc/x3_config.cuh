@@ -1,9 +1,8 @@
 // Limb formats of the two-limb mode (UDH_NUMERIC_BF16X3): forward operands (activations, forward weights, fc1's weight
 // mirror) and backward operands (gradients, mirrored conv weights).
-// Measured on B200 (round 2, gpurun_out/x3_fp16fwd.log): kind::f16 MMAs with fp16 on one side and bf16 on the other raise
-// an illegal-instruction error, so both operands of every MMA must share a format.  fp16 limbs would carry 22 bits
-// instead of 16, but the weight gradient multiplies activations with gradients, and gradients (1e-8 .. 1e-2) do not fit
-// fp16's range without per-tensor loss scaling; bf16 limbs need no scaling anywhere, so every stream uses them.
+// wgmma multiplies operands of one format, so both operands of every MMA share a limb format.  fp16 limbs would carry 22
+// bits instead of 16, but the weight gradient multiplies activations with gradients, and gradients (1e-8 .. 1e-2) do not
+// fit fp16's range without per-tensor loss scaling; bf16 limbs need no scaling anywhere, so every stream uses them.
 #pragma once
 #include "tc_common.cuh"
 

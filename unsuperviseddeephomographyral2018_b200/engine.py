@@ -105,8 +105,8 @@ class HomographyEngine(object):
         self._mv_sharded = False
         self._mc = self._dp_setup_multicast() if self._symm else None
         # second stream: Row G of the fully connected slice under the conv backward.  UDH_OVERLAP_UPDATE=1 also moves that
-        # slice's Adam there at N = 1; measured on B200 it gains nothing (whichever conv kernel starts next waits for the
-        # update's CTAs to leave its SMs: profiles/r2_dp_overlap_experiments.md), so it is off by default.
+        # slice's Adam there at N = 1; whichever conv kernel starts next waits for the update's CTAs to leave its SMs, so it
+        # is off by default.
         self._overlap_update = os.environ.get("UDH_OVERLAP_UPDATE", "0") == "1"
         self._comm_stream = torch.cuda.Stream(device=self.device) if (world_size > 1 or self._overlap_update) else None
         # SM policy of this engine's steps (library-global knobs, applied at the start of every step).  A conv CTA with 200+ KB
@@ -121,7 +121,7 @@ class HomographyEngine(object):
         self._sm_policy = dict(reserve=int(os.environ.get("UDH_SM_RESERVE", "0")) if world_size > 1 else 0,
                                top=int(os.environ.get("UDH_SM_RESERVE_TOP", "32")) if (world_size > 1 and self._mc is None) else 0,
                                marker=int(os.environ.get("UDH_DP_MARKER_LAYER", "3")) if side_kernel else -1, marker_sms=sms)
-        self._side_adam_grid = int(os.environ.get("UDH_SIDE_ADAM_GRID", str(sms * 8 if sms else 296)))
+        self._side_adam_grid = int(os.environ.get("UDH_SIDE_ADAM_GRID", str(sms * 8 if sms else 264)))   # 2 CTAs per H100 SM
         # static per-step outputs of the one-call step (udh_step_forward_backward): reused every step
         B, Pz, dev = self.B, self.Pz, self.device
         self._sb = dict(h4p=torch.zeros(B, 8, device=dev), H=torch.zeros(B, 3, 3, device=dev), pred=torch.zeros(B, Pz, Pz, 1, device=dev),
@@ -285,8 +285,7 @@ class HomographyEngine(object):
     # ------------------------------------------------------------------ Row G over NVSwitch multicast memory
     def _dp_want_multicast(self):
         """UDH_DP_MODE = nccl (default) | multicast.  `multicast` selects the fused switch-reduce / sharded-Adam / weight-multicast
-        kernel (csrc/dp_update.cu) for fc1's weights; it is parity-tested but measured no faster than the NCCL path on B200
-        (DESIGN.md section 6), hence opt-in."""
+        kernel (csrc/dp_update.cu) for fc1's weights; it is parity-tested and opt-in (DESIGN.md section 6)."""
         mode = os.environ.get("UDH_DP_MODE", "nccl")
         if mode not in ("nccl", "multicast"):
             raise ValueError("UDH_DP_MODE must be nccl or multicast")
