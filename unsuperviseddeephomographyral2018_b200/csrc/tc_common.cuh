@@ -85,15 +85,12 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
   return t;
 }
 // Bounded wait: a protocol bug traps after ~2 s (launch error) instead of hanging the GPU.
+// No printf here: any call in a kernel makes ptxas serialise every wgmma of it (C7510).
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const uint64_t t0 = globaltimer_ns();
   while (!mbar_try_wait(bar, parity)) {
-    if (globaltimer_ns() - t0 > 2000000000ull) {
-      printf("libudh: mbarrier wait timed out (block %d thread %d bar 0x%x parity %u)\n", (int)blockIdx.x, (int)threadIdx.x,
-             smem_u32(bar), parity);
-      asm volatile("trap;");
-    }
+    if (globaltimer_ns() - t0 > 2000000000ull) asm volatile("trap;");
   }
 }
 

@@ -244,7 +244,8 @@ tc_wgrad64_x3_kernel(const __grid_constant__ CUtensorMap tmX128, const __grid_co
         const uint32_t const_addr = xl ? zeros_addr : ones_addr;
         acc_fence(acc);
         wg_fence();
-#pragma unroll 1
+        // unrolled: a loop back-edge between the MMAs would make ptxas wait for them (C7519)
+#pragma unroll
         for (int t = 0; t < T; ++t) {
           const uint32_t b_lo = desc_lo(g_addr + (uint32_t)(8 + t * 128 - 1) * 128, 128);     // G[q-1] | G[q] | G[q+1]
           const uint32_t a_start = x_addr + (uint32_t)(g.hh + t * 128 + shift) * 128;
