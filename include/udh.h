@@ -245,6 +245,32 @@ int udh_prep_inputs_u8_ex(const uint8_t* I, const uint8_t* I_prime, const float*
 int udh_synth_scene_u8(uint8_t* I, float* pts1, float* gt, int B, int img_h, int img_w, int P, int rho, uint64_t seed, void* stream);
 int udh_warp_image_u8(const uint8_t* U, const float* H, uint8_t* out, int B, int img_h, int img_w, void* stream);
 
+/* ---- direct-method baseline: cv2.findTransformECC, MOTION_HOMOGRAPHY (utils/direct_homography.py:8-57) ----------------
+ * as homography_conventional_synthetic.py:186-223 runs it on the test set, batched.  Images are uint8 planes
+ * [B,img_h,img_w]; W [B,9] row-major fp32 maps template pixels into the input image (WARP_INVERSE_MAP).
+ * udh_ecc_prep_u8: the two gray planes the reference hands to ECC from the decoded I, I' [B,img_h,img_w,3] and the
+ *   augmentation table of udh_prep_inputs_u8_ex (nullable): augment + normalise (fp32), denorm_img (fp64), astype(uint8),
+ *   cvtColor(RGB2GRAY) (utils/utils.py:406-413, homography_conventional_synthetic.py:190-191).
+ * udh_ecc_homography: gray_I is the template, gray_I' the input image; W_init [B,9] (nullable = identity); runs up to
+ *   max_iters iterations, stopping early when |rho - rho_last| < eps.  Writes W, rho [B] (the last correlation coefficient),
+ *   iters [B] (iterations entered) and status [B]: UDH_ECC_* — where cv2 raises, the sample stops with W as it was before
+ *   that iteration's update.  workspace: udh_ecc_workspace_bytes.
+ * udh_ecc_h4p: pred_h4p [B,8] = perspectiveTransform(pts1, inv(W)) - pts1 (zeros when status != 0 or W is singular),
+ *   then values >= rho_clamp become 2 rho_clamp and values <= -rho_clamp become -2 rho_clamp.  With gt (nullable):
+ *   h_loss [B] = RMSE(pred, gt) and fail [B] = 1 (not found; scores as pred = 0) or 2 (identity < h_loss: h_loss becomes
+ *   the identity RMSE), else 0 — the harness's rules, not udh_h4p_loss's. */
+#define UDH_ECC_OK 0
+#define UDH_ECC_NAN 1     /* rho is NaN ("NaN encountered.")                                     */
+#define UDH_ECC_NOCONV 2  /* lambda_d <= 0 ("The algorithm stopped before its convergence ...") */
+size_t udh_ecc_workspace_bytes(int B, int img_h, int img_w);
+int udh_ecc_prep_u8(const uint8_t* I, const uint8_t* I_prime, const float* aug, uint8_t* gray_I, uint8_t* gray_I_prime, int B,
+                    int img_h, int img_w, void* stream);
+int udh_ecc_homography(const uint8_t* tmpl, const uint8_t* input, const float* W_init, int max_iters, double eps, float* W,
+                       double* rho, int32_t* iters, int32_t* status, void* ws, size_t ws_bytes, int B, int img_h, int img_w,
+                       void* stream);
+int udh_ecc_h4p(const float* W, const int32_t* status, const float* pts1, const float* gt, float rho_clamp, float* pred_h4p,
+                float* h_loss, int32_t* fail, int B, void* stream);
+
 /* ---- instrumentation read by bench.py -------------------------------------------------------------------------
  * udh_launch_count: kernels this library has launched in this process (monotonic).
  * udh_prof_*: when enabled, every tagged phase is bracketed by CUDA events recorded on the launching stream;

@@ -16,6 +16,7 @@ LOSS_L1, LOSS_REC, LOSS_L1_SMOOTH, LOSS_NCC, LOSS_CUSTOM = 0, 1, 2, 3, 4
 NSUMS, NLOSSES, NMETRICS = 8, 8, 4
 L_REC, L_SSIM, L_L1, L_L1_SMOOTH, L_NCC = 0, 1, 2, 3, 4
 M_H_LOSS, M_BOUNDED_H_LOSS, M_NUM_FAIL, M_ACE = 0, 1, 2, 3
+ECC_OK, ECC_NAN, ECC_NOCONV = 0, 1, 2
 
 class StepArgs(ctypes.Structure):
     """udh_step_args (include/udh.h)."""
@@ -100,6 +101,11 @@ SIGNATURES = {
                                       c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "udh_synth_scene_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_uint64, c_void_p]),
     "udh_warp_image_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "udh_ecc_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "udh_ecc_prep_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "udh_ecc_homography": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_double, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                   c_size_t, c_int, c_int, c_int, c_void_p]),
+    "udh_ecc_h4p": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "udh_launch_count": (c_ulonglong, []),
     "udh_set_sm_reserve": (c_int, [c_int]),
     "udh_set_sm_reserve_top": (c_int, [c_int]),

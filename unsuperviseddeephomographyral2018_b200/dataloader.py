@@ -203,8 +203,10 @@ class Dataloader(object):
             aug[j, 6:11] = a if self.mode == 'train' else draw()                                   # joint (train) / disjoint (test)
         pts1 = torch.tensor(self.pts1[idx], dtype=torch.float32, device=dev)
         gt = torch.tensor(self.gt[idx], dtype=torch.float32, device=dev) if self.gt is not None else None
-        out = synthetic.prep_u8(I_u8, Ip_u8, pts1, torch.tensor(aug, device=dev), P, want_rgb=True)
+        aug_dev = torch.tensor(aug, device=dev)
+        out = synthetic.prep_u8(I_u8, Ip_u8, pts1, aug_dev, P, want_rgb=True)
         out["gt"] = gt
+        out.update(I_u8=I_u8, I_prime_u8=Ip_u8, aug=aug_dev)       # the decoded images and their augmentation (direct-method baseline)
         out["I_aug"] = out.pop("I_aug_rgb")                        # the reference contract: [B,Hh,W,3] normalised (augmented) I
         return out
 

@@ -170,6 +170,58 @@ def h4p_loss(pred, gt, want_grad=False, want_per_sample=False):
     return metrics, per, dpred
 
 
+# ------------------------------------------------------------------ direct method (cv2.findTransformECC, MOTION_HOMOGRAPHY)
+def ecc_prep_u8(I_u8, Ip_u8, aug=None):
+    """Decoded I, I' [B,H,W,3] uint8 (+ the [B,11] augmentation table or None) -> the two uint8 gray planes [B,H,W] the
+    reference hands to ECC: cvtColor(denorm_img(I_aug).astype(uint8), RGB2GRAY)."""
+    _req(I_u8, torch.uint8, "I"); _req(Ip_u8, torch.uint8, "I_prime")
+    if aug is not None:
+        _req(aug, torch.float32, "aug")
+    B, Hh, W, _ = I_u8.shape
+    g1 = torch.empty(B, Hh, W, device=I_u8.device, dtype=torch.uint8)
+    g2 = torch.empty_like(g1)
+    check(lib.udh_ecc_prep_u8(_ptr(I_u8), _ptr(Ip_u8), _ptr(aug), _ptr(g1), _ptr(g2), B, Hh, W, _stream()), "udh_ecc_prep_u8")
+    return g1, g2
+
+
+def find_homography_ecc(template, image, W_init=None, max_iters=8, eps=1e-10):
+    """Batched cv2.findTransformECC(template, image, W, MOTION_HOMOGRAPHY, (COUNT|EPS, max_iters, eps)) on uint8 planes
+    [B,H,W].  Returns (W [B,3,3] fp32, rho [B] fp64, iterations [B] int32, status [B] int32 in _lib.ECC_*)."""
+    _req(template, torch.uint8, "template"); _req(image, torch.uint8, "image")
+    if template.shape != image.shape or template.dim() != 3:
+        raise _lib.UdhError("template and image must both be [B,H,W] (got %s and %s)" % (tuple(template.shape), tuple(image.shape)))
+    B, Hh, W = template.shape
+    if W_init is not None:
+        W_init = W_init.reshape(B, 9).contiguous()
+        _req(W_init, torch.float32, "W_init")
+    dev = template.device
+    Wout = torch.empty(B, 3, 3, device=dev, dtype=torch.float32)
+    rho = torch.empty(B, device=dev, dtype=torch.float64)
+    iters = torch.empty(B, device=dev, dtype=torch.int32)
+    status = torch.empty(B, device=dev, dtype=torch.int32)
+    nbytes = lib.udh_ecc_workspace_bytes(B, Hh, W)
+    ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+    check(lib.udh_ecc_homography(_ptr(template), _ptr(image), _ptr(W_init), int(max_iters), float(eps), _ptr(Wout), _ptr(rho),
+                                 _ptr(iters), _ptr(status), _ptr(ws), nbytes, B, Hh, W, _stream()), "udh_ecc_homography")
+    return Wout, rho, iters, status
+
+
+def ecc_h4p(W, status, pts1, gt=None, rho=45.0):
+    """-> (pred_h4p [B,8], h_loss [B] or None, fail [B] int32 or None): the direct method's corner displacements and the
+    harness's clamp / failure rules (0 = ok, 1 = not found, 2 = worse than identity)."""
+    W = W.reshape(-1, 9).contiguous()
+    _req(W, torch.float32, "W"); _req(status, torch.int32, "status"); _req(pts1, torch.float32, "pts1")
+    if gt is not None:
+        _req(gt, torch.float32, "gt")
+    B = W.shape[0]
+    pred = torch.empty(B, 8, device=W.device, dtype=torch.float32)
+    h = torch.empty(B, device=W.device, dtype=torch.float32) if gt is not None else None
+    fail = torch.empty(B, device=W.device, dtype=torch.int32) if gt is not None else None
+    check(lib.udh_ecc_h4p(_ptr(W), _ptr(status), _ptr(pts1), _ptr(gt), float(rho), _ptr(pred), _ptr(h), _ptr(fail), B, _stream()),
+          "udh_ecc_h4p")
+    return pred, h, fail
+
+
 # ------------------------------------------------------------------ Adam
 def adam_step(p, g, m, v, alpha_t, beta1=0.9, beta2=0.999, eps=1e-8, grad_scale=1.0, zero_grad=True):
     for t, n in ((p, "p"), (g, "g"), (m, "m"), (v, "v")):
