@@ -271,6 +271,47 @@ int udh_ecc_homography(const uint8_t* tmpl, const uint8_t* input, const float* W
 int udh_ecc_h4p(const float* W, const int32_t* status, const float* pts1, const float* gt, float rho_clamp, float* pred_h4p,
                 float* h_loss, int32_t* fail, int B, void* stream);
 
+/* ---- baseline-JPEG decode, bit-identical to cv2.imread(..., IMREAD_COLOR) + BGR->RGB (libjpeg-turbo defaults) --------
+ * Accepted: baseline Huffman 8-bit (SOF0, SOF1), one interleaved scan, gray or YCbCr with luma sampling 1x1, 2x1 or 2x2 and
+ * chroma 1x1; any size; restart intervals; APPn / COM skipped.  Everything else is rejected with a UDH_JPEG_R_* reason.
+ * udh_jpeg_parse (host): one file -> info; returns UDH_OK with info->reason set, or UDH_EINVAL on a null pointer.
+ * udh_jpeg_plan_bytes / udh_jpeg_plan (host): N files, concatenated in `data` with file k at [offsets[k], offsets[k+1]),
+ *   all h x w and supported -> the packed descriptor (tables + restart segments).  plan_bytes returns 0 when the plan
+ *   cannot be built; udh_jpeg_plan then returns UDH_ENOSUP (a file is not supported) or UDH_EINVAL (wrong size).
+ * udh_jpeg_decode (device): plan_host is the plan as udh_jpeg_plan wrote it, plan_dev a 16-byte aligned device copy,
+ *   data the same concatenated bytes on the device; writes out [N,h,w,3] uint8 RGB and status [N] (0, or a
+ *   UDH_JPEG_E_* code: that image's output is undefined, the other images are unaffected).
+ *   workspace: udh_jpeg_workspace_bytes(N, h, w), 16-byte aligned. */
+#define UDH_JPEG_R_OK 0
+#define UDH_JPEG_R_NOT_JPEG 1      /* no SOI marker (PNG, ...)                                         */
+#define UDH_JPEG_R_TRUNCATED 2     /* malformed or truncated header                                     */
+#define UDH_JPEG_R_NOT_BASELINE 3  /* progressive, lossless, hierarchical or arithmetic-coded           */
+#define UDH_JPEG_R_PRECISION 4     /* not 8-bit samples                                                 */
+#define UDH_JPEG_R_COMPONENTS 5    /* 2 or 4 components                                                 */
+#define UDH_JPEG_R_RGB 6           /* RGB-coded (Adobe transform 0, or component ids 'R','G','B')       */
+#define UDH_JPEG_R_SAMPLING_H 7    /* horizontal sampling other than 4:4:4 / 4:2:x (e.g. 4:1:1)         */
+#define UDH_JPEG_R_SAMPLING_V 8    /* vertical-only chroma subsampling (e.g. 4:4:0)                     */
+#define UDH_JPEG_R_ORIENTATION 9   /* EXIF orientation other than 1 (cv2.imread rotates the image)      */
+#define UDH_JPEG_R_MULTI_SCAN 10   /* components spread over several scans                              */
+#define UDH_JPEG_E_TRUNCATED 1     /* entropy-coded data ran out                                        */
+#define UDH_JPEG_E_HUFFMAN 2       /* invalid Huffman code                                              */
+#define UDH_JPEG_E_COEF 3          /* coefficient index past 63                                         */
+typedef struct udh_jpeg_info {
+  int32_t width, height, components;
+  int32_t h_samp[3], v_samp[3];
+  int32_t restart_interval; /* MCUs per restart interval, 0 = none */
+  int32_t reason;           /* UDH_JPEG_R_*                         */
+} udh_jpeg_info;
+int udh_jpeg_parse(const uint8_t* data, int64_t nbytes, udh_jpeg_info* info);
+size_t udh_jpeg_plan_bytes(const uint8_t* data, const int64_t* offsets, int n, int h, int w);
+int udh_jpeg_plan(const uint8_t* data, const int64_t* offsets, int n, int h, int w, void* plan, size_t plan_bytes);
+size_t udh_jpeg_workspace_bytes(int n, int h, int w);
+int udh_jpeg_decode(const void* plan_host, const void* plan_dev, const uint8_t* data, uint8_t* out, int32_t* status, void* ws,
+                    size_t ws_bytes, void* stream);
+/* Lanes per image in the entropy-decode kernel (32: one warp per image, the default; 1: eight images share a warp).  For
+ * the timing tool's comparison; process-wide. */
+int udh_debug_jpeg_set_lanes(int lanes);
+
 /* ---- instrumentation read by bench.py -------------------------------------------------------------------------
  * udh_launch_count: kernels this library has launched in this process (monotonic).
  * udh_prof_*: when enabled, every tagged phase is bracketed by CUDA events recorded on the launching stream;

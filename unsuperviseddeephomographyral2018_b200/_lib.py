@@ -33,6 +33,18 @@ class StepArgs(ctypes.Structure):
 FWD_FC1_MIRROR_CURRENT = 1
 
 
+class JpegInfo(ctypes.Structure):
+    """udh_jpeg_info (include/udh.h)."""
+    _fields_ = [("width", c_int), ("height", c_int), ("components", c_int), ("h_samp", c_int * 3), ("v_samp", c_int * 3),
+                ("restart_interval", c_int), ("reason", c_int)]
+
+
+# udh_jpeg_parse reasons (UDH_JPEG_R_*) and udh_jpeg_decode statuses (UDH_JPEG_E_*)
+JPEG_R = dict(OK=0, NOT_JPEG=1, TRUNCATED=2, NOT_BASELINE=3, PRECISION=4, COMPONENTS=5, RGB=6, SAMPLING_H=7, SAMPLING_V=8,
+              ORIENTATION=9, MULTI_SCAN=10)
+JPEG_E = dict(TRUNCATED=1, HUFFMAN=2, COEF=3)
+
+
 STEP_ALL, STEP_FWD_HEAD, STEP_CONVS, STEP_FWD_ONLY = 0, 1, 2, 3
 STEP_LOSS = {"h_loss": 0, "l1_loss": 1, "rec_loss": 2, "l1_smooth_loss": 3, "ncc_loss": 4, "ssim_loss": 5}
 
@@ -106,6 +118,12 @@ SIGNATURES = {
     "udh_ecc_homography": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_double, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                    c_size_t, c_int, c_int, c_int, c_void_p]),
     "udh_ecc_h4p": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
+    "udh_jpeg_parse": (c_int, [c_void_p, c_int64, POINTER(JpegInfo)]),
+    "udh_jpeg_plan_bytes": (c_size_t, [c_void_p, c_void_p, c_int, c_int, c_int]),
+    "udh_jpeg_plan": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_size_t]),
+    "udh_jpeg_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "udh_jpeg_decode": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "udh_debug_jpeg_set_lanes": (c_int, [c_int]),
     "udh_launch_count": (c_ulonglong, []),
     "udh_set_sm_reserve": (c_int, [c_int]),
     "udh_set_sm_reserve_top": (c_int, [c_int]),

@@ -2,11 +2,13 @@
 
 Produces, per batch, the nine post-dataloader tensors the model consumes (`*_batch` attributes / dict keys):
 I1, I2, I1_aug, I2_aug [B,P,P,1]; I (=I_aug), I_prime (=I_prime_aug) [B,Hh,W,3]; pts1, gt [B,8]; patch_indices [B,P*P].
-JPEG decode and list parsing run on the host (as in the reference: queue-runner threads); photometric augmentation,
-normalisation, gray conversion and patch gather run on the device.  `synthetic=N` replaces the on-disk set by N
+JPEG decode runs on the device for the baseline files cv2.imwrite produces (bit-identical to cv2.imread; other files are
+decoded on the host); list parsing runs on the host; photometric augmentation, normalisation, gray conversion and patch
+gather run on the device.  `synthetic=N` replaces the on-disk set by N
 on-device generated pairs (synthetic.make_batch) — MS-COCO is not available offline.
 """
 import os
+import time
 from collections import namedtuple
 
 import numpy as np
@@ -75,6 +77,8 @@ class Dataloader(object):
         self.rho = rho
         self._rng = np.random.default_rng(seed)
         self._step = 0
+        self._reader, self._pending, self._ready = None, None, []
+        self.decode_stats = dict(groups=0, read_s=0.0, wait_s=0.0, group_s=0.0, device_images=0, host_images=0, decode_errors=0)
         if not self.synthetic_pairs:
             self.names, self.pts1, self.gt = read_img_and_gt(params.filenames_file, params.pts1_file, params.gt_file)
             self.num_samples = len(self.names)
@@ -84,19 +88,23 @@ class Dataloader(object):
             self.num_samples = self.synthetic_pairs
 
     # ---- on-disk path -------------------------------------------------------------------------------------------
-    def _read_pair(self, idx):
-        import cv2
+    def _pair_paths(self, idx):
         name = self.names[idx][1] if len(self.names[idx]) > 1 else self.names[idx][0]   # dataloader.py:143-144 (column 1 for both)
-        imgs = []
-        for sub in ("I", "I_prime"):
-            im = cv2.imread(os.path.join(self.params.data_path, sub, name), cv2.IMREAD_COLOR)
-            if im is None:
-                raise IOError("cannot read %s" % os.path.join(self.params.data_path, sub, name))
-            im = cv2.cvtColor(im, cv2.COLOR_BGR2RGB)
-            if im.shape[0] != self.params.img_h or im.shape[1] != self.params.img_w:
-                im = cv2.resize(im, (self.params.img_w, self.params.img_h), interpolation=cv2.INTER_AREA)    # dataloader.py:245
-            imgs.append(im)
-        return imgs
+        return [os.path.join(self.params.data_path, sub, name) for sub in ("I", "I_prime")]
+
+    def _read_image(self, path):
+        """The host decode: cv2.imread + BGR -> RGB, INTER_AREA-resized to the network size when it differs."""
+        import cv2
+        im = cv2.imread(path, cv2.IMREAD_COLOR)
+        if im is None:
+            raise IOError("cannot read %s" % path)
+        im = cv2.cvtColor(im, cv2.COLOR_BGR2RGB)
+        if im.shape[0] != self.params.img_h or im.shape[1] != self.params.img_w:
+            im = cv2.resize(im, (self.params.img_w, self.params.img_h), interpolation=cv2.INTER_AREA)    # dataloader.py:245
+        return im
+
+    def _read_pair(self, idx):
+        return [self._read_image(path) for path in self._pair_paths(idx)]
 
     def _next_indices(self, B):
         out = []
@@ -182,17 +190,21 @@ class Dataloader(object):
         b["gt"] = None                                                                            # the real path never sees a 4-point gt
         return b
 
-    def _disk_batch(self):
+    # Device decode of the on-disk set.  A group of DECODE_BATCHES batches is decoded in one launch: the indices and the
+    # augmentation table of each batch are drawn from the host RNG batch after batch, exactly as the host path draws them,
+    # so the batches are the same whichever decoder ran.  A background thread reads (and parses) the next group's files
+    # while the current group is being consumed.  Files the device decoder does not take (progressive, PNG, another size,
+    # a decode error, ...) go through _read_image.  Because a group is built at once, a missing or unreadable file raises
+    # its IOError when the first batch of its group is requested (up to DECODE_BATCHES - 1 batches before its own).
+    # decode_stats counts, over the loader's life, the groups, the reader thread's seconds, the seconds next_batch spent
+    # waiting for it, the seconds next_batch spent building groups (wait included), and the images decoded on the device, on the host, and sent to the host after a device decode error.
+    # DECODE_BATCHES: see DESIGN §4.
+    DECODE_BATCHES = 4
+
+    def _draw_batch(self):
         p = self.params
-        B, P, Hh, W = p.batch_size, p.patch_size, p.img_h, p.img_w
+        B = p.batch_size
         idx = self._next_indices(B)
-        I = np.empty((B, Hh, W, 3), np.uint8); Ip = np.empty_like(I)
-        for j, i in enumerate(idx):
-            I[j], Ip[j] = self._read_pair(i)
-        dev = self.device
-        I_u8 = torch.from_numpy(I).to(dev); Ip_u8 = torch.from_numpy(Ip).to(dev)
-        if 'normalize' not in p.augment_list:
-            raise NotImplementedError("augment_list without 'normalize' is not supported (the reference default is ['normalize'])")
         # augmentation parameters on the host RNG (reproducible order), applied by the fused device kernel
         aug = np.zeros((B, 11), np.float32)
         aug[:, 0] = self._rng.uniform(0, 1, size=B) > (1 - p.do_augment)                          # dataloader.py:163-169
@@ -201,6 +213,70 @@ class Dataloader(object):
             a = draw()
             aug[j, 1:6] = a
             aug[j, 6:11] = a if self.mode == 'train' else draw()                                   # joint (train) / disjoint (test)
+        return idx, aug
+
+    def _read_group(self, paths):
+        """Background thread: file bytes -> (device-decodable file positions, JpegPlan or None).  File reads and the
+        ctypes parser calls release the GIL."""
+        from . import ops
+        t0 = time.perf_counter()
+        blobs, take = [], []
+        for k, path in enumerate(paths):
+            try:
+                with open(path, "rb") as f:
+                    b = f.read()
+            except OSError:
+                continue                                       # _read_image raises the host path's error
+            info = ops.jpeg_parse(b)
+            if info.reason == 0 and info.height == self.params.img_h and info.width == self.params.img_w:
+                blobs.append(b); take.append(k)
+        plan = ops.JpegPlan(blobs, self.params.img_h, self.params.img_w) if blobs else None
+        return take, plan, time.perf_counter() - t0
+
+    def _submit_group(self):
+        draws = [self._draw_batch() for _ in range(self.DECODE_BATCHES)]
+        paths = [path for idx, _ in draws for i in idx for path in self._pair_paths(i)]
+        if self._reader is None:
+            import concurrent.futures
+            self._reader = concurrent.futures.ThreadPoolExecutor(max_workers=1, thread_name_prefix="udh-jpeg-reader")
+        return draws, paths, self._reader.submit(self._read_group, paths)
+
+    def _decode_group(self):
+        t_group = time.perf_counter()
+        if self._pending is None:
+            self._pending = self._submit_group()
+        draws, paths, fut = self._pending
+        self._pending = self._submit_group()                   # read the next group while this one is decoded and consumed
+        t0 = time.perf_counter()
+        take, plan, read_s = fut.result()
+        st = self.decode_stats
+        st["groups"] += 1; st["read_s"] += read_s; st["wait_s"] += time.perf_counter() - t0
+        p, dev = self.params, self.device
+        imgs = torch.empty(len(paths), p.img_h, p.img_w, 3, dtype=torch.uint8, device=dev)
+        host = sorted(set(range(len(paths))) - set(take))
+        if plan is not None:
+            out, status = plan.decode(dev)
+            imgs[torch.tensor(take, device=dev)] = out
+            bad = [take[k] for k in np.flatnonzero(status.cpu().numpy())]
+            host = sorted(host + bad)
+            st["device_images"] += len(take) - len(bad); st["decode_errors"] += len(bad)
+        st["host_images"] += len(host)
+        if host:
+            h = np.stack([self._read_image(paths[k]) for k in host])
+            imgs[torch.tensor(host, device=dev)] = torch.from_numpy(h).to(dev)
+        imgs = imgs.view(len(draws), p.batch_size, 2, p.img_h, p.img_w, 3)
+        self._ready = [(idx, aug, imgs[d, :, 0].contiguous(), imgs[d, :, 1].contiguous()) for d, (idx, aug) in enumerate(draws)]
+        st["group_s"] += time.perf_counter() - t_group
+
+    def _disk_batch(self):
+        p = self.params
+        B, P, Hh, W = p.batch_size, p.patch_size, p.img_h, p.img_w
+        if 'normalize' not in p.augment_list:
+            raise NotImplementedError("augment_list without 'normalize' is not supported (the reference default is ['normalize'])")
+        if not self._ready:
+            self._decode_group()
+        idx, aug, I_u8, Ip_u8 = self._ready.pop(0)
+        dev = self.device
         pts1 = torch.tensor(self.pts1[idx], dtype=torch.float32, device=dev)
         gt = torch.tensor(self.gt[idx], dtype=torch.float32, device=dev) if self.gt is not None else None
         aug_dev = torch.tensor(aug, device=dev)

@@ -2,6 +2,7 @@
 autograd bookkeeping; all arithmetic happens in libudh's CUDA kernels.  Every function requires CUDA tensors."""
 import ctypes
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -220,6 +221,60 @@ def ecc_h4p(W, status, pts1, gt=None, rho=45.0):
     check(lib.udh_ecc_h4p(_ptr(W), _ptr(status), _ptr(pts1), _ptr(gt), float(rho), _ptr(pred), _ptr(h), _ptr(fail), B, _stream()),
           "udh_ecc_h4p")
     return pred, h, fail
+
+
+# ------------------------------------------------------------------ baseline-JPEG decode
+def jpeg_parse(blob):
+    """One file's bytes -> _lib.JpegInfo (host only): size, sampling, restart interval and `reason`, 0 when the device
+    decoder takes the file, else one of _lib.JPEG_R."""
+    info = _lib.JpegInfo()
+    buf = np.frombuffer(blob, np.uint8) if len(blob) else np.zeros(1, np.uint8)
+    check(lib.udh_jpeg_parse(buf.ctypes.data, len(blob), ctypes.byref(info)), "udh_jpeg_parse")
+    return info
+
+
+class JpegPlan:
+    """Host side of one decode launch: the files concatenated in pinned memory and the packed descriptor."""
+
+    def __init__(self, blobs, h, w):
+        offs = np.zeros(len(blobs) + 1, np.int64)
+        offs[1:] = np.cumsum([len(b) for b in blobs])
+        self.n, self.h, self.w = len(blobs), h, w
+        pin = torch.cuda.is_available()                  # the plan itself is host-only; pinning needs a device
+        self.data = torch.empty(max(int(offs[-1]), 1), dtype=torch.uint8, pin_memory=pin)
+        dv = self.data.numpy()
+        for k, b in enumerate(blobs):
+            dv[offs[k]:offs[k + 1]] = np.frombuffer(b, np.uint8)
+        nb = lib.udh_jpeg_plan_bytes(dv.ctypes.data, offs.ctypes.data, self.n, h, w)
+        if nb == 0:
+            raise _lib.UdhError("udh_jpeg_plan_bytes: %s" % lib.udh_last_error().decode())
+        self.plan = torch.empty(nb, dtype=torch.uint8, pin_memory=pin)
+        check(lib.udh_jpeg_plan(dv.ctypes.data, offs.ctypes.data, self.n, h, w, self.plan.data_ptr(), nb), "udh_jpeg_plan")
+
+    def decode(self, device=None):
+        """-> (uint8 [N,h,w,3] RGB, int32 [N] status) on the current stream; nonzero status = that image failed."""
+        dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        plan_d = self.plan.to(dev, non_blocking=True)
+        data_d = self.data.to(dev, non_blocking=True)
+        out = torch.empty(self.n, self.h, self.w, 3, device=dev, dtype=torch.uint8)
+        status = torch.empty(self.n, device=dev, dtype=torch.int32)
+        nbytes = lib.udh_jpeg_workspace_bytes(self.n, self.h, self.w)
+        ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+        check(lib.udh_jpeg_decode(self.plan.data_ptr(), _ptr(plan_d), _ptr(data_d), _ptr(out), _ptr(status), _ptr(ws), nbytes,
+                                  _stream()), "udh_jpeg_decode")
+        return out, status
+
+
+def decode_jpeg(blobs, h, w):
+    """Baseline JPEG files (bytes), all h x w -> (uint8 [N,h,w,3] CUDA tensor, int32 [N] status): bit-identical to
+    cv2.imread(..., IMREAD_COLOR)[..., ::-1].  Raises UdhError naming the first file the device could not decode."""
+    _lib.require_device()
+    out, status = JpegPlan(blobs, h, w).decode()
+    st = status.cpu().numpy()
+    bad = np.flatnonzero(st)
+    if len(bad):
+        raise _lib.UdhError("decode_jpeg: image %d failed with status %d (%d of %d images failed)" % (bad[0], st[bad[0]], len(bad), len(st)))
+    return out, status
 
 
 # ------------------------------------------------------------------ Adam
