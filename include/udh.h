@@ -392,6 +392,22 @@ int udh_debug_x3_set_rows(int on);
 size_t udh_debug_x3_scratch_bytes(int B, int H, int W, int cin, int cout);
 int udh_debug_x3_conv(const float* x, const float* w, const float* bias, float* out, void* scratch, int B, int H, int W, int cin,
                       int cout, int relu, int dgrad, void* stream);
+/* udh_debug_x3_conv with the fused ReLU-mask epilogues of the train step.  Both masks are uint32 words over the PADDED
+ * positions q = (n (H+2) + y + 1) (W+2) + x + 1 of the output, kout / 32 words per position (kout = cout, or cin when
+ * dgrad != 0): bit j of word k of position q is channel 32k + j.  mask_bits (nullable, in) zeroes every output element whose
+ * bit is clear (after bias and ReLU); mask_out (nullable, out, B (H+2) (W+2) kout / 32 words) receives out > 0, with zero
+ * words at border positions. */
+int udh_debug_x3_conv_ex(const float* x, const float* w, const float* bias, const uint32_t* mask_bits, uint32_t* mask_out,
+                         float* out, void* scratch, int B, int H, int W, int cin, int cout, int relu, int dgrad, void* stream);
+/* conv1_2's row-tile kernels (64 -> 64 channels, W == 128, even H), as the train step runs them:
+ *   rows = 1: forward + bias + ReLU fused with the 2x2 max-pool; x [B,H,128,64] -> out = pooled [B,H/2,64,64] fp32 and
+ *             codes [B,H/2,64,8] uint32 (3 bits per channel at (c % 8) * 3 of word c / 8: window index 0-3 of the maximum in
+ *             row-major order, 4 where the maximum is not positive); bias and codes are required;
+ *   rows = 2: dgrad (mirrored weights, no bias) of g [B,H,128,64] with the mask words of udh_debug_x3_conv_ex fused
+ *             (mask_bits nullable); out [B,H,128,64]; codes is ignored.
+ * scratch: udh_debug_x3_scratch_bytes(B, H, W, 64, 64). */
+int udh_debug_x3_conv_rows(const float* x, const float* w, const float* bias, const uint32_t* mask_bits, float* out, uint32_t* codes,
+                           void* scratch, int B, int H, int W, int rows, void* stream);
 int udh_debug_x3_wgrad(const float* x, const float* g, float* dW, float* db, void* scratch, int B, int H, int W, int cin, int cout,
                        void* stream);
 int udh_debug_x3_conv1(const float* I1, const float* I2, const float* w, const float* bias, float* out, const float* g, float* dW,

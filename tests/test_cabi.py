@@ -56,6 +56,31 @@ def test_no_cpu_fallback_without_a_gpu():
         ops.dlt_forward(torch.zeros(1, 8), torch.zeros(1, 8))
 
 
+def test_x3_mask_and_row_tile_debug_entries_reject_bad_arguments():
+    """udh_debug_x3_conv_ex / udh_debug_x3_conv_rows are exported and check their arguments before touching the device."""
+    from unsuperviseddeephomographyral2018_b200 import _lib
+    L = _lib.lib
+    raw = ctypes.CDLL(_lib.LIB_PATH)
+    assert hasattr(raw, "udh_debug_x3_conv_ex") and hasattr(raw, "udh_debug_x3_conv_rows")
+    p = ctypes.c_void_p(256)                          # never dereferenced: every call below fails its argument checks
+    for i in (0, 1, 5, 6):                            # x, w, out, scratch
+        a = [p, p, None, None, None, p, p]
+        a[i] = None
+        assert L.udh_debug_x3_conv_ex(*a, 2, 16, 16, 64, 64, 1, 0, None) == _lib.EINVAL
+        assert b"udh_debug_x3_conv_ex: null pointer" in L.udh_last_error()
+    for i in (0, 1, 4, 6):                            # x, w, out, scratch
+        a = [p, p, p, None, p, p, p]
+        a[i] = None
+        assert L.udh_debug_x3_conv_rows(*a, 2, 16, 128, 1, None) == _lib.EINVAL
+        assert b"udh_debug_x3_conv_rows: null pointer" in L.udh_last_error()
+    assert L.udh_debug_x3_conv_rows(p, p, None, None, p, p, p, 2, 16, 128, 1, None) == _lib.EINVAL      # pooled forward: no bias
+    assert L.udh_debug_x3_conv_rows(p, p, p, None, p, None, p, 2, 16, 128, 1, None) == _lib.EINVAL      # pooled forward: no codes
+    assert L.udh_debug_x3_conv_rows(p, p, p, None, p, p, p, 2, 16, 128, 3, None) == _lib.EINVAL        # rows must be 1 or 2
+    assert L.udh_debug_x3_conv_rows(p, p, None, None, p, None, p, 2, 16, 64, 2, None) == _lib.EINVAL    # W != 128
+    assert L.udh_debug_x3_conv_rows(p, p, None, None, p, None, p, 2, 15, 128, 2, None) == _lib.EINVAL   # odd height
+    assert b"udh_debug_x3_conv_rows" in L.udh_last_error()
+
+
 def test_schedule_matches_reference_constants():
     from unsuperviseddeephomographyral2018_b200 import engine
     assert engine.decay_steps(1e-4, 0.9e-4) == 58117 and engine.decay_steps(5e-4, 0.9e-4) == 3570

@@ -98,6 +98,10 @@ SIGNATURES = {
     "udh_debug_x3_scratch_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
     "udh_debug_x3_conv": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
                                   c_void_p]),
+    "udh_debug_x3_conv_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                     c_int, c_int, c_int, c_void_p]),
+    "udh_debug_x3_conv_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                       c_void_p]),
     "udh_debug_x3_wgrad": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "udh_debug_x3_conv1": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                    c_int, c_void_p]),

@@ -683,8 +683,8 @@ __global__ void pack_one_x3_kernel(const float* __restrict__ w, uint16_t* __rest
   }
 }
 
-int x3_debug_conv(const float* x, const float* w, const float* bias, float* out, void* scratch, int B, int H, int W, int cin, int cout,
-                  int relu, int dgrad, cudaStream_t st) {
+int x3_debug_conv(const float* x, const float* w, const float* bias, const uint32_t* mask_bits, uint32_t* mask_out, float* out,
+                  void* scratch, int B, int H, int W, int cin, int cout, int relu, int dgrad, cudaStream_t st) {
   const int kin = dgrad ? cout : cin, kout = dgrad ? cin : cout;
   char* s = reinterpret_cast<char*>(scratch);
   uint16_t* xp = reinterpret_cast<uint16_t*>(s);
@@ -694,9 +694,30 @@ int x3_debug_conv(const float* x, const float* w, const float* bias, float* out,
   TRY(pad_cast_x3(x, xp, B, H, W, kin, dgrad != 0, st));
   pack_one_x3_kernel<<<(9 * cin * cout + 255) / 256, 256, 0, st>>>(w, wp, cin, cout, dgrad);
   TRY(check_launch("pack_one_x3"));
-  if (dgrad) TRY((tc_conv_x3<kGrad, kGrad, kGrad>(xp, wp, bias, nullptr, nullptr, op, nullptr, relu, B, H, W, kin, kout, st)));
-  else TRY((tc_conv_x3<kFwd, kFwd, kFwd>(xp, wp, bias, nullptr, nullptr, op, nullptr, relu, B, H, W, kin, kout, st)));
+  if (dgrad) TRY((tc_conv_x3<kGrad, kGrad, kGrad>(xp, wp, bias, mask_bits, mask_out, op, nullptr, relu, B, H, W, kin, kout, st)));
+  else TRY((tc_conv_x3<kFwd, kFwd, kFwd>(xp, wp, bias, mask_bits, mask_out, op, nullptr, relu, B, H, W, kin, kout, st)));
   return unpad_cast_x3(op, out, B, H, W, kout, dgrad != 0, st);
+}
+
+// conv1_2's row-tile kernels (64 -> 64 channels, W == 128).  rows = 1: forward + bias + ReLU fused with the 2x2 max-pool ->
+// pooled fp32 [B,H/2,W/2,64] and routing codes; rows = 2: dgrad (mirrored weights) with the ReLU mask words fused.
+int x3_debug_conv_rows(const float* x, const float* w, const float* bias, const uint32_t* mask_bits, float* out, uint32_t* codes,
+                       void* scratch, int B, int H, int W, int rows, cudaStream_t st) {
+  char* s = reinterpret_cast<char*>(scratch);
+  const size_t stream_bytes = al256((size_t)B * (H + 2) * (W + 2) * 64 * 4);
+  uint16_t* xp = reinterpret_cast<uint16_t*>(s);
+  uint16_t* op = reinterpret_cast<uint16_t*>(s + stream_bytes);
+  uint16_t* wp = reinterpret_cast<uint16_t*>(s + 2 * stream_bytes);
+  UDH_CUDA(cudaMemsetAsync(scratch, 0, x3_debug_scratch_bytes(B, H, W, 64, 64), st));
+  TRY(pad_cast_x3(x, xp, B, H, W, 64, rows == 2, st));
+  pack_one_x3_kernel<<<(9 * 64 * 64 + 255) / 256, 256, 0, st>>>(w, wp, 64, 64, rows == 2);
+  TRY(check_launch("pack_one_x3"));
+  if (rows == 1) {
+    TRY((launch_conv_x3_rows<1, kFwd, kFwd, kFwd>(xp, wp, bias, nullptr, codes, op, 1, B, H, W, st)));
+    return unpad_cast_x3(op, out, B, H / 2, W / 2, 64, false, st);
+  }
+  TRY((launch_conv_x3_rows<2, kGrad, kGrad, kGrad>(xp, wp, nullptr, mask_bits, nullptr, op, 0, B, H, W, st)));
+  return unpad_cast_x3(op, out, B, H, W, 64, true, st);
 }
 
 int x3_debug_wgrad(const float* x, const float* gsrc, float* dW, float* db, void* scratch, int B, int H, int W, int cin, int cout, cudaStream_t st) {
@@ -740,7 +761,22 @@ extern "C" size_t udh_debug_x3_scratch_bytes(int B, int H, int W, int cin, int c
 extern "C" int udh_debug_x3_conv(const float* x, const float* w, const float* bias, float* out, void* scratch, int B, int H, int W,
                                  int cin, int cout, int relu, int dgrad, void* stream) {
   UDH_REQUIRE(x && w && out && scratch, "udh_debug_x3_conv: null pointer");
-  return udh::x3_debug_conv(x, w, bias, out, scratch, B, H, W, cin, cout, relu, dgrad, udh::as_stream(stream));
+  return udh::x3_debug_conv(x, w, bias, nullptr, nullptr, out, scratch, B, H, W, cin, cout, relu, dgrad, udh::as_stream(stream));
+}
+
+extern "C" int udh_debug_x3_conv_ex(const float* x, const float* w, const float* bias, const uint32_t* mask_bits, uint32_t* mask_out,
+                                    float* out, void* scratch, int B, int H, int W, int cin, int cout, int relu, int dgrad, void* stream) {
+  UDH_REQUIRE(x && w && out && scratch, "udh_debug_x3_conv_ex: null pointer");
+  return udh::x3_debug_conv(x, w, bias, mask_bits, mask_out, out, scratch, B, H, W, cin, cout, relu, dgrad, udh::as_stream(stream));
+}
+
+extern "C" int udh_debug_x3_conv_rows(const float* x, const float* w, const float* bias, const uint32_t* mask_bits, float* out,
+                                      uint32_t* codes, void* scratch, int B, int H, int W, int rows, void* stream) {
+  UDH_REQUIRE(x && w && out && scratch, "udh_debug_x3_conv_rows: null pointer");
+  UDH_REQUIRE(rows == 1 || rows == 2, "udh_debug_x3_conv_rows: rows must be 1 (forward + pool) or 2 (dgrad), not %d", rows);
+  UDH_REQUIRE(rows == 2 || (bias && codes), "udh_debug_x3_conv_rows: the pooled forward needs bias and codes");
+  UDH_REQUIRE(B > 0 && W == 128 && H > 0 && H % 2 == 0, "udh_debug_x3_conv_rows: needs B > 0, W == 128 and an even height");
+  return udh::x3_debug_conv_rows(x, w, bias, mask_bits, out, codes, scratch, B, H, W, rows, udh::as_stream(stream));
 }
 
 extern "C" int udh_debug_x3_wgrad(const float* x, const float* g, float* dW, float* db, void* scratch, int B, int H, int W, int cin,
