@@ -228,11 +228,11 @@ __global__ void pool_bwd_x3_kernel(const uint32_t* __restrict__ codes, const uin
 }
 
 // ---------------------------------------------------------------------------------------------------- launchers
-template <int N_OUT, int CB, int T, int FA, int FW, int FO, bool WIDE>
+template <int N_OUT, int CB, int T, int FA, int FW, int FO>
 int launch_conv_x3_impl(const CUtensorMap& tmA128, const CUtensorMap& tmAhh, const CUtensorMap& tmW, const CUtensorMap& tmOut, const tc::ConvGeom& g,
                         int stages, size_t smem, const float* bias, const uint32_t* mask_bits, uint32_t* mask_out, float* out_f32, int relu,
                         float out_scale, cudaStream_t st) {
-  auto kern = tc::tc_conv_x3_kernel<N_OUT, CB, T, FA, FW, FO, WIDE>;
+  auto kern = tc::tc_conv_x3_kernel<N_OUT, CB, T, FA, FW, FO>;
   UDH_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int sms = persistent_ctas();
   const int grid = g.num_items < sms ? g.num_items : sms;
@@ -240,7 +240,7 @@ int launch_conv_x3_impl(const CUtensorMap& tmA128, const CUtensorMap& tmAhh, con
   return check_launch("tc_conv_x3_kernel");
 }
 
-template <int N_OUT, int CB, int T, int FA, int FW, int FO, bool WIDE = false>
+template <int N_OUT, int CB, int T, int FA, int FW, int FO>
 int launch_conv_x3(const uint16_t* x, const uint16_t* wpk, const float* bias, const uint32_t* mask_bits, uint32_t* mask_out,
                    uint16_t* out_limbs, float* out_f32, int relu, int B, int H, int W, float out_scale, cudaStream_t st) {
   tc::ConvGeom g;
@@ -262,10 +262,10 @@ int launch_conv_x3(const uint16_t* x, const uint16_t* wpk, const float* bias, co
   uint64_t dimsO[2] = {(uint64_t)2 * N_OUT, (uint64_t)g.Q}, strO[2] = {2, (uint64_t)2 * N_OUT * 2};
   uint32_t boxO[2] = {64, 32};
   TRY(tc::make_tmap_bf16(&tmOut, out_limbs, 2, dimsO, strO, boxO));
-  using S = tc::ConvX3Smem<N_OUT, CB, T, WIDE>;
+  using S = tc::ConvX3Smem<N_OUT, CB, T>;
   const int stages = S::stages(g.abuf_rows);          // weight-ring depth: as many stages as shared memory holds (<= 6)
   UDH_REQUIRE(stages >= 2, "tc conv x3: activation rows (%d x %d blocks) leave no room for the weight ring", g.abuf_rows, 2 * CB);
-  return launch_conv_x3_impl<N_OUT, CB, T, FA, FW, FO, WIDE>(tmA128, tmAhh, tmW, tmOut, g, stages, S::fixed_bytes(g.abuf_rows) + (size_t)stages * S::kWStageBytes,
+  return launch_conv_x3_impl<N_OUT, CB, T, FA, FW, FO>(tmA128, tmAhh, tmW, tmOut, g, stages, S::fixed_bytes(g.abuf_rows) + (size_t)stages * S::kWStageBytes,
                                                              bias, mask_bits, mask_out, out_f32, relu, out_scale, st);
 }
 
@@ -292,16 +292,16 @@ int launch_conv_x3_rows(const uint16_t* x, const uint16_t* wpk, const float* bia
   TRY(tc::make_tmap_bf16(&tmW, wpk, 2, dimsW, strW, boxW));
   // ROWS = 1 stores the pooled stream with plain vector stores (the map is only a placeholder there)
   TRY(tc::make_tmap_bf16(&tmOut, ROWS == 2 ? out_limbs : const_cast<uint16_t*>(x), 2, dimsA, strA, boxO));
-  using S = tc::ConvX3Smem<64, 1, 2, false>;
-  constexpr int kStages = 3;
-  const size_t smem = S::fixed_bytes(g.abuf_rows) + (size_t)kStages * S::kWStageBytes;
-  UDH_REQUIRE(smem <= 232448, "tc conv x3 rows: %zu bytes of shared memory exceed the 227 KiB limit", smem);
-  auto kern = tc::tc_conv_x3_kernel<64, 1, 2, FA, FW, FO, false, ROWS>;
+  using S = tc::ConvX3Smem<64, 1, 2>;
+  const int stages = S::stages(g.abuf_rows);          // weight-ring depth: as many stages as shared memory holds (<= kX3MaxStages)
+  UDH_REQUIRE(stages >= 2, "tc conv x3 rows: activation rows (%d) leave no room for the weight ring", g.abuf_rows);
+  const size_t smem = S::fixed_bytes(g.abuf_rows) + (size_t)stages * S::kWStageBytes;
+  auto kern = tc::tc_conv_x3_kernel<64, 1, 2, FA, FW, FO, ROWS>;
   UDH_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int sms = persistent_ctas();
   const int grid = g.num_items < sms ? g.num_items : sms;
   // ROWS = 1: `out_f32` carries the pooled stream pointer and `mask_out` the routing codes
-  launch_chain(kern, dim3(grid), dim3(384), smem, st, tmA128, tmAhh, tmW, tmOut, g, kStages, bias, mask_bits, codes_or_mask,
+  launch_chain(kern, dim3(grid), dim3(384), smem, st, tmA128, tmAhh, tmW, tmOut, g, stages, bias, mask_bits, codes_or_mask,
                ROWS == 1 ? reinterpret_cast<float*>(out_limbs) : (float*)nullptr, relu, 1.0f);
   return check_launch("tc_conv_x3_kernel(rows)");
 }
@@ -310,11 +310,7 @@ int launch_conv_x3_rows(const uint16_t* x, const uint16_t* wpk, const float* bia
 template <int FA, int FW, int FO>
 int tc_conv_x3(const uint16_t* x, const uint16_t* wpk, const float* bias, const uint32_t* mask_bits, uint32_t* mask_out,
                uint16_t* out_limbs, float* out_f32, int relu, int B, int H, int W, int cin, int cout, cudaStream_t st) {
-  // WIDE (one N = 128 MMA against [W_hi | W_lo], a MAIN and an AUX accumulator) is opt-in (UDH_X3_WIDE=1): the default
-  // instance sums in the same order as the row-tile kernel of conv1_2, so the two paths agree bit for bit
-  static const int wide = [] { const char* e = getenv("UDH_X3_WIDE"); return (e && e[0] == '1') ? 1 : 0; }();
-  // items of T tiles: T * (accumulator columns per tile) / 2 fp32 registers per MMA thread, kept at 64
-  if (cin == 64 && cout == 64 && wide) return launch_conv_x3<64, 1, 1, FA, FW, FO, true>(x, wpk, bias, mask_bits, mask_out, out_limbs, out_f32, relu, B, H, W, 1.0f, st);
+  // items of T tiles: T * N_OUT / 2 fp32 accumulator registers per MMA thread, kept at 64
   if (cin == 64 && cout == 64) return launch_conv_x3<64, 1, 2, FA, FW, FO>(x, wpk, bias, mask_bits, mask_out, out_limbs, out_f32, relu, B, H, W, 1.0f, st);
   if (cin == 64 && cout == 128) return launch_conv_x3<128, 1, 1, FA, FW, FO>(x, wpk, bias, mask_bits, mask_out, out_limbs, out_f32, relu, B, H, W, 1.0f, st);
   if (cin == 128 && cout == 64) return launch_conv_x3<64, 2, 2, FA, FW, FO>(x, wpk, bias, mask_bits, mask_out, out_limbs, out_f32, relu, B, H, W, 1.0f, st);

@@ -12,12 +12,17 @@
 // next item's phase LO — each limb buffer has its own full/empty mbarrier pair, and a dedicated producer warp so that the
 // weight ring (a second producer warp) never waits behind an activation buffer.  Weights always stream through a TMA ring
 // (hi + lo of all 9 taps do not fit next to the activations); each ring block is reused by the T tiles of the item.
-//   warpgroup 0: weight-ring producer (warp 0), activation producer (warp 3) | warpgroups 1-2: MMA + epilogue, each owning
-//   64 of the 128 rows of every tile (accumulators in registers, drained through stage_acc32 as in the bf16 kernel).
+//   warpgroup 0: weight-ring producer (warp 0), activation producer (warp 3) | warpgroups 1-2: MMA + epilogue.
 // Phase order: HI first (its first MMA initialises the accumulators), then LO.
-// WIDE (64 -> 64 channels): phase HI issues ONE N = 128 MMA per k-step against the ring stage [W_hi | W_lo] into a MAIN and
-// an AUX accumulator (adjacent columns of one fragment) instead of two N = 64 MMAs; phase LO adds A_lo x W_hi into MAIN;
-// the epilogue reads MAIN + AUX.
+// 128 output channels: each MMA warpgroup owns 64 of the 128 rows of every tile, D[pos][co] = X . W with the activation
+// rows as A and the ring stage as B (m64n128k16), drained through stage_acc32 as in the bf16 kernel.
+// 64 output channels (TR): the tile is transposed, D^T[co][pos] = W . X^T: the ring stage [64 co][64 ci] is the A operand
+// and 128 activation rows are the B operand, so each MMA is an m64n128k16 (2 KB + 4 KB of shared memory per 131 072 MACs)
+// instead of two m64n64k16 (4 KB + 4 KB); at N = 64 the operand reads alone would need all 128 B/clk of shared memory at
+// tensor peak.  MMA warpgroup cw owns the whole tile t = cw.  Every output element sees the same chain of k16 partial
+// products as in the untransposed tile (same stages, same k-step order, same first / accumulate flags).  The epilogue
+// transposes the fragment back through shared memory (stage_acc_tr) so that, as for 128 channels, one thread works on 32
+// channels of one position.
 #pragma once
 #include "conv_tc_kernels.cuh"
 
@@ -26,9 +31,9 @@ namespace tc {
 
 constexpr int kX3MaxStages = 6;
 
-template <int N_OUT, int CB, int T, bool WIDE = false>
+template <int N_OUT, int CB, int T>
 struct ConvX3Smem {
-  static constexpr int kWStageBytes = N_OUT * 128 * (WIDE ? 2 : 1);
+  static constexpr int kWStageBytes = N_OUT * 128;
   // fixed part: alignment slack + both limbs of the A rows + epilogue staging + accumulator transpose blocks + barriers
   static size_t fixed_bytes(int abuf_rows) { return 1024 + (size_t)2 * CB * abuf_rows * 128 + kEpiStageBytes + 2 * kStg32Bytes + 256; }
   static int stages(int abuf_rows) {
@@ -38,15 +43,39 @@ struct ConvX3Smem {
   }
 };
 
+// Transposed fragment (TR: rows = 64 channels, columns = 128 positions) -> positions [32 r, 32 r + 32), all 64 channels, as a
+// [32 positions][kStgStride] fp32 block (r may be a runtime value: every register index stays static).  The bank of element
+// (pos, co) is 4 pos + co mod 32, so a warp's stores are conflict-free, and so are lds_read32's row reads.
+// Stores go through a 32-bit shared address: the 16 offsets then fold into immediates instead of 16 generic pointers.
+__device__ __forceinline__ void stage_acc_tr(const float (&d)[64], int r, float* stg) {
+  const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
+  const uint32_t p0 = smem_u32(stg) + (uint32_t)(2 * (lane & 3) * kStgStride + 16 * w + (lane >> 2)) * 4;
+#pragma unroll
+  for (int i = 0; i < 64; ++i) {
+    if ((i >> 4) != r) continue;
+    const uint32_t off = (uint32_t)((8 * ((i >> 2) & 3) + (i & 1)) * kStgStride + 8 * ((i >> 1) & 1)) * 4;
+    asm volatile("st.shared.f32 [%0], %1;" ::"r"(p0 + off), "f"(d[i]) : "memory");
+  }
+}
+// v[j] = 32 consecutive fp32 at shared address addr (a row of a stage_acc_tr block)
+__device__ __forceinline__ void lds_read32(uint32_t addr, float (&v)[32]) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j)
+    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v[4 * j]), "=f"(v[4 * j + 1]), "=f"(v[4 * j + 2]), "=f"(v[4 * j + 3])
+                 : "r"(addr + 16 * j) : "memory");
+}
+static_assert(32 * kStgStride * 4 <= kStg32Bytes, "a transposed quarter tile fits a warpgroup's staging block");
+
 // The weight ring has `stages` slots (a runtime value: as many as shared memory holds next to the activation rows).
-// ROWS (W == 128 images, 64 -> 64 channels, T == 2, not WIDE: conv1_2).  An item is the interior of two consecutive image rows
+// ROWS (W == 128 images, 64 -> 64 channels, T == 2: conv1_2).  An item is the interior of two consecutive image rows
 // (2y, 2y+1): tile t starts at the first interior position of row 2y + t, i.e. the tiles are Wp (not 128) positions apart in
-// the same staged rows, no border position is computed, and the epilogue thread of column x holds both rows of that column.
-//   ROWS == 1: forward fused with the 2x2 max-pool — bias + ReLU, maximum (vertical in registers, horizontal with one lane
-//              exchange), then the POOLED two-limb stream and the 3-bit routing codes of the max-pool backward are written; the
+// the same staged rows, and no border position is computed.
+//   ROWS == 1: forward fused with the 2x2 max-pool — each warpgroup stages a quarter of its row, the epilogue thread of
+//              column x reads that column from both staging blocks; bias + ReLU, maximum (vertical in registers,
+//              horizontal with one lane exchange), then the POOLED two-limb stream and the 3-bit routing codes of the max-pool backward are written; the
 //              full-resolution activation (554 MB in this mode) is never written or re-read;
 //   ROWS == 2: the ordinary epilogue (bias / ReLU-backward mask / limb split / TMA store) on row tiles (the dgrad).
-template <int N_OUT, int CB, int T, int FMT_A, int FMT_W, int FMT_O, bool WIDE = false, int ROWS = 0>
+template <int N_OUT, int CB, int T, int FMT_A, int FMT_W, int FMT_O, int ROWS = 0>
 __global__ void __launch_bounds__(384, 1)
 tc_conv_x3_kernel(const __grid_constant__ CUtensorMap tmA128, const __grid_constant__ CUtensorMap tmAhh,
                   const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmOut, const ConvGeom g,
@@ -58,16 +87,15 @@ tc_conv_x3_kernel(const __grid_constant__ CUtensorMap tmA128, const __grid_const
   const int abuf_bytes = g.abuf_rows * 128;                       // one 64-channel block of one limb
   uint8_t* sA = base;                                             // [2 limbs][CB][abuf_rows][128]
   uint8_t* sW = base + (size_t)2 * CB * abuf_bytes;               // [stages][N_OUT][128]
-  static_assert(!WIDE || (N_OUT == 64 && T <= 2), "WIDE: 64 output channels, two accumulators per tile");
+  constexpr bool TR = N_OUT == 64;                                // transposed tile (see the top of this file)
+  static_assert(!TR || T == 2, "transposed tile: one 128-position tile per MMA warpgroup");
   static_assert(ROWS == 0 || (N_OUT == 64 && CB == 1 && T == 2), "row tiles: the 64-channel instance with two tiles");
   constexpr bool POOL = ROWS == 1;
   // first position of an item and distance between its tiles (in positions)
   auto item_q0 = [&](int item) { return ROWS ? ((item / (g.H >> 1)) * g.Hp + 2 * (item % (g.H >> 1)) + 1) * g.Wp + 1 : item * T * 128; };
   const int tstep = ROWS ? g.Wp : 128;
-  constexpr int kAcc = WIDE ? 2 : 1;                              // accumulators per tile (MAIN | AUX)
-  constexpr int kTileCols = N_OUT * kAcc;                         // accumulator columns per tile
-  constexpr int kTileRegs = kTileCols / 2;                        // fragment registers per tile
-  constexpr int kStageBytes = N_OUT * 128 * kAcc;                 // one ring stage: [W_hi] or [W_hi | W_lo]
+  constexpr int kTileRegs = N_OUT / 2;                            // fragment registers per tile
+  constexpr int kStageBytes = N_OUT * 128;                        // one ring stage: [N_OUT][64] of one limb
   uint8_t* sEpi = sW + (size_t)stages * kStageBytes;              // [4 quarters][32 rows][128 B]
   float* sStg = reinterpret_cast<float*>(sEpi + kEpiStageBytes);  // [2 warpgroups][kStg32Bytes]
   uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sStg) + 2 * kStg32Bytes);
@@ -114,31 +142,29 @@ tc_conv_x3_kernel(const __grid_constant__ CUtensorMap tmA128, const __grid_const
     } else if (warp == 0 && lane == 0) {
       // ===================================== weight-ring producer =====================================
       uint32_t ws = 0, wpar = 1;                                  // first pass over the ring: the slots are free
-      auto push = [&](int block, int nblocks) {                  // `nblocks` consecutive [N_OUT][64] blocks into one stage
+      auto push = [&](int block) {                                // one [N_OUT][64] block into one stage
         mbar_wait(&w_empty[ws], wpar);
-        mbar_arrive_expect_tx(&w_full[ws], (uint32_t)(nblocks * N_OUT * 128));
-        for (int i = 0; i < nblocks; ++i)
-          tma_load_2d(sW + (size_t)ws * kStageBytes + (size_t)i * N_OUT * 128, &tmW, 0, (block + i) * N_OUT, &w_full[ws]);
+        mbar_arrive_expect_tx(&w_full[ws], (uint32_t)kStageBytes);
+        tma_load_2d(sW + (size_t)ws * kStageBytes, &tmW, 0, block * N_OUT, &w_full[ws]);
         if (++ws == (uint32_t)stages) { ws = 0; wpar ^= 1u; }
       };
       for (int it = 0; it < my_items; ++it) {
-        for (int kb = 0; kb < 9 * CB; ++kb) {                                     // phase HI: A_hi x W_hi, A_hi x W_lo
-          if (WIDE) push(kb * 2, 2);
-          else { push(kb * 2, 1); push(kb * 2 + 1, 1); }
-        }
-        for (int kb = 0; kb < 9 * CB; ++kb) push(kb * 2, 1);                      // phase LO: A_lo x W_hi
+        for (int kb = 0; kb < 9 * CB; ++kb) { push(kb * 2); push(kb * 2 + 1); }  // phase HI: A_hi x W_hi, A_hi x W_lo
+        for (int kb = 0; kb < 9 * CB; ++kb) push(kb * 2);                         // phase LO: A_lo x W_hi
       }
     }
   } else {
     regs_inc<232>();
-    const int cw = (warp - 4) >> 2;               // MMA warpgroup: rows [64 cw, 64 cw + 64) of every tile
+    const int cw = (warp - 4) >> 2;               // MMA warpgroup: TR: tile cw; else rows [64 cw, 64 cw + 64) of every tile
     const int wi = warp & 3;
-    const int ew = 2 * cw + (wi & 1);             // row quarter of the tile this warp drains
-    const int eg = wi >> 1;                       // 32-column chunk parity this warp drains
+    const int ew = 2 * cw + (wi & 1);             // staging block (pair of warps) this warp drains through
+    const int eg = wi >> 1;                       // 32-channel chunk this warp drains
     const int erow = 32 * (wi & 1) + lane;
     float* stg = sStg + cw * (kStg32Bytes / 4);
     auto wg_sync = [&]() { named_sync(5 + cw, 128); };
-    const uint32_t a_addr0 = smem_u32(sA) + (uint32_t)cw * 64 * 128, w_addr0 = smem_u32(sW);
+    // first position of the 32 this warp drains in epilogue slot s (a tile of the item; TR: a half of the warpgroup's tile)
+    auto slot_q0 = [&](int q0, int s) { return TR ? q0 + cw * tstep + (2 * s + (wi & 1)) * 32 : q0 + ew * 32 + s * tstep; };
+    const uint32_t a_addr0 = smem_u32(sA) + (uint32_t)(TR ? cw * tstep : 64 * cw) * 128, w_addr0 = smem_u32(sW);
     const uint32_t w_stage_units = (uint32_t)kStageBytes >> 4;
     const uint32_t w_lo0 = desc_lo(w_addr0, 16);
     const uint32_t cb_units = (uint32_t)abuf_bytes >> 4;
@@ -154,6 +180,15 @@ tc_conv_x3_kernel(const __grid_constant__ CUtensorMap tmA128, const __grid_const
         if (e == eg) stg32_read32(stg, erow, v);
       }
     };
+    // TR: channel chunk eg of position 32 (2 s + (wi & 1)) + lane of the warpgroup's tile (two quarter rounds)
+    const uint32_t my_stg_row = smem_u32(stg) + (uint32_t)(lane * kStgStride + 32 * eg) * 4;
+    auto fetch_tr = [&](int s, float (&v)[32]) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        wg_sync(); stage_acc_tr(acc, 2 * s + e, stg); wg_sync();
+        if (e == (wi & 1)) lds_read32(my_stg_row, v);
+      }
+    };
     const int HpWp = g.Hp * g.Wp;
     uint8_t* estg = sEpi + ew * 4096;
     const uint32_t my_row = smem_u32(estg) + lane * 128;
@@ -163,13 +198,13 @@ tc_conv_x3_kernel(const __grid_constant__ CUtensorMap tmA128, const __grid_const
     bool store_pending = false;
     for (int it = 0; it < my_items; ++it) {
       const int item = (int)blockIdx.x + it * (int)gridDim.x;
-      const int q0w0 = item_q0(item) + ew * 32;
-      // ReLU-backward mask words (1 bit / element) of all T tiles, requested before the MMAs
+      const int q0 = item_q0(item);
+      // ReLU-backward mask words (1 bit / element) of all T epilogue slots, requested before the MMAs
       uint32_t mbt[T][2];
       if (!POOL) {
 #pragma unroll
         for (int t = 0; t < T; ++t) {
-          const int qt = q0w0 + t * tstep + lane;
+          const int qt = slot_q0(q0, t) + lane;
           const bool ok = mask_bits && qt < g.Q;
           if (N_OUT == 64) {
             mbt[t][0] = ok ? __ldg(mask_bits + (size_t)qt * 2 + eg) : 0u; mbt[t][1] = 0u;
@@ -195,23 +230,22 @@ tc_conv_x3_kernel(const __grid_constant__ CUtensorMap tmA128, const __grid_const
           const uint32_t a_lo = a_tap0 + (uint32_t)ky * wp8 + (uint32_t)(kx * 8) + (uint32_t)cb * cb_units;
 #pragma unroll
           for (int wl = 0; wl < 2; ++wl) {
-            if (wl == 1 && (ph == 1 || WIDE)) continue;           // phase LO multiplies with W_hi only; WIDE: one [hi | lo] stage
+            if (wl == 1 && ph == 1) continue;                     // phase LO multiplies with W_hi only
             mbar_wait(&w_full[ws], wpar);
             const uint32_t w_lo = w_lo0 + ws * w_stage_units;
             wg_fence();
+            if constexpr (TR) {
 #pragma unroll
-            for (int t = 0; t < T; ++t) {
-              float (&d)[kTileRegs] = *reinterpret_cast<float(*)[kTileRegs]>(&acc[t * kTileRegs]);
-              const uint32_t a_t = a_lo + (ROWS ? (uint32_t)t * wp8 : (uint32_t)(t * 1024));
+              for (int k = 0; k < 4; ++k)       // +2 sixteen-byte units per 32-byte k-step; A = weights, B = activation rows
+                wgmma_bf16<128, 0, 0>(acc, desc_from_lo(w_lo + k * 2), desc_from_lo(a_lo + k * 2), (first && k == 0) ? 0u : 1u);
+            } else {
 #pragma unroll
-              for (int k = 0; k < 4; ++k) {     // +2 sixteen-byte units per 32-byte k-step
-                const uint32_t accum = (first && k == 0) ? 0u : 1u;
-                if constexpr (WIDE) {
-                  if (ph == 0) wgmma_bf16_head<2 * N_OUT, 0, 0>(d, desc_from_lo(a_t + k * 2), desc_from_lo(w_lo + k * 2), accum);
-                  else wgmma_bf16_head<N_OUT, 0, 0>(d, desc_from_lo(a_t + k * 2), desc_from_lo(w_lo + k * 2), accum);
-                } else {
-                  wgmma_bf16_head<N_OUT, 0, 0>(d, desc_from_lo(a_t + k * 2), desc_from_lo(w_lo + k * 2), accum);
-                }
+              for (int t = 0; t < T; ++t) {
+                float (&d)[kTileRegs] = *reinterpret_cast<float(*)[kTileRegs]>(&acc[t * kTileRegs]);
+                const uint32_t a_t = a_lo + (uint32_t)(t * 1024);
+#pragma unroll
+                for (int k = 0; k < 4; ++k)     // +2 sixteen-byte units per 32-byte k-step
+                  wgmma_bf16_head<N_OUT, 0, 0>(d, desc_from_lo(a_t + k * 2), desc_from_lo(w_lo + k * 2), (first && k == 0) ? 0u : 1u);
               }
             }
             wg_commit();
@@ -230,7 +264,8 @@ tc_conv_x3_kernel(const __grid_constant__ CUtensorMap tmA128, const __grid_const
       acc_fence(acc);
       // ===================================== epilogue =====================================
       if constexpr (POOL) {
-        // thread = image column x (W == 128 == tile rows); warps of parity eg pool the 32-channel chunk eg
+        // thread = image column x (W == 128 == tile rows); warps of parity eg pool the 32-channel chunk eg.  Warpgroup cw holds
+        // image row 2y + cw: in round r both stage quarter r of their row and the warps with ew == r read both blocks.
         const int OH = g.H >> 1, OW = g.W >> 1;
         const int x = ew * 32 + lane;
         const int px = x >> 1, odd = x & 1;
@@ -239,33 +274,36 @@ tc_conv_x3_kernel(const __grid_constant__ CUtensorMap tmA128, const __grid_const
         uint16_t* prow = out_pool + (((size_t)n * (OH + 2) + yy + 1) * (OW + 2) + px + 1) * 128;
         uint32_t* crow = mask_out + (((size_t)n * OH + yy) * OW + px) * 8;
         const int c = eg;
-        float v0[32], v1[32], u[32];
-        fetch(0, v0);                                             // tile 0 (+ AUX)
-        if (WIDE) {
-          fetch(2, u);
+        // scan order of the 2x2 window: (row 0, x even)=0, (row 0, x odd)=1, (row 1, even)=2, (row 1, odd)=3; the first
+        // maximum wins: larger value, ties to the smaller index.  The reader takes the vertical maximum of bias + ReLU as it
+        // reads (vs, and bit j of `lower` when row 1 is strictly larger), so only 32 values stay live next to the accumulators.
+        float vs[32];
+        uint32_t lower = 0u;
+        const uint32_t row0 = smem_u32(sStg) + (uint32_t)(lane * kStgStride + 32 * eg) * 4;
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v0[j] += u[j];
-        }
-        fetch(kTileCols / 32, v1);                                // tile 1 (+ AUX)
-        if (WIDE) {
-          fetch(kTileCols / 32 + 2, u);
+        for (int r = 0; r < 4; ++r) {
+          named_sync(7, 256); stage_acc_tr(acc, r, stg); named_sync(7, 256);
+          if (r == ew) {
+            float v0[32], v1[32];
+            lds_read32(row0, v0); lds_read32(row0 + kStg32Bytes, v1);
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v1[j] += u[j];
+            for (int j = 0; j < 32; ++j) {
+              const float bj = __ldg(bias + c * 32 + j);
+              const float a = fmaxf(v0[j] + bj, 0.f), d = fmaxf(v1[j] + bj, 0.f);
+              vs[j] = a;
+              if (d > a) { vs[j] = d; lower |= 1u << j; }
+            }
+          }
         }
         uint32_t code[4] = {0u, 0u, 0u, 0u};
         float m[32];
 #pragma unroll
         for (int j = 0; j < 32; ++j) {
-          const float bj = __ldg(bias + c * 32 + j);
-          const float a = fmaxf(v0[j] + bj, 0.f), d = fmaxf(v1[j] + bj, 0.f);
-          // scan order of the 2x2 window: (row 0, x even)=0, (row 0, x odd)=1, (row 1, even)=2, (row 1, odd)=3;
-          // the first maximum wins: larger value, ties to the smaller index
-          float vs = a; uint32_t ks = (uint32_t)odd;
-          if (d > a) { vs = d; ks = 2u + (uint32_t)odd; }
-          const float vo = __shfl_xor_sync(0xffffffffu, vs, 1);
+          const uint32_t ks = ((lower >> j) & 1u) * 2u + (uint32_t)odd;
+          const float vo = __shfl_xor_sync(0xffffffffu, vs[j], 1);
           const uint32_t ko = __shfl_xor_sync(0xffffffffu, ks, 1);
-          const bool other = vo > vs || (vo == vs && ko < ks);
-          const float mv = other ? vo : vs;
+          const bool other = vo > vs[j] || (vo == vs[j] && ko < ks);
+          const float mv = other ? vo : vs[j];
           const uint32_t mk = other ? ko : ks;
           m[j] = mv;
           code[j >> 3] |= (mv > 0.f ? mk : 4u) << (3 * (j & 7));
@@ -284,7 +322,7 @@ tc_conv_x3_kernel(const __grid_constant__ CUtensorMap tmA128, const __grid_const
         // barrier, and one lane issues the TMA store; the hi block and the lo block of a half go through the same block.
 #pragma unroll 1
         for (int t = 0; t < T; ++t) {
-          const int q0w = q0w0 + t * tstep;
+          const int q0w = slot_q0(q0, t);
           const int q = q0w + lane;
           const int n = q / HpWp, rem = q - n * HpWp;
           const int yp = rem / g.Wp, xp = rem - yp * g.Wp;
@@ -295,13 +333,8 @@ tc_conv_x3_kernel(const __grid_constant__ CUtensorMap tmA128, const __grid_const
           for (int hf = 0; hf < N_OUT / 64; ++hf) {
             const int c = hf * 2 + eg;
             float v[32];
-            fetch(t * (kTileCols / 32) + hf * 2, v);
-            if (WIDE) {                                           // MAIN (A.W_hi terms) + AUX (A_hi.W_lo)
-              float u[32];
-              fetch(t * (kTileCols / 32) + N_OUT / 32 + hf * 2, u);
-#pragma unroll
-              for (int j = 0; j < 32; ++j) v[j] += u[j];
-            }
+            if constexpr (TR) fetch_tr(t, v);
+            else fetch(t * (N_OUT / 32) + hf * 2, v);
             if (out_scale != 1.0f) {
 #pragma unroll
               for (int j = 0; j < 32; ++j) v[j] *= out_scale;
