@@ -416,6 +416,16 @@ int udh_debug_x3_conv1(const float* I1, const float* I2, const float* w, const f
  * pooled [B,H/2,64,64] fp32 and routing codes [B,H/2,64,8] uint32 (3 bits per channel, 4 = no gradient). */
 int udh_debug_tc_conv_pool(const float* x, const float* w, const float* bias, float* pooled, uint32_t* codes, void* scratch,
                            int B, int H, int W, void* stream);
+/* fc1 (32768 -> 1024, the 128x128-patch regressor) through exactly the calls the step makes in `numeric_mode`:
+ * y[B,1024] = x[B,32768] . w[32768,1024] (no bias, no ReLU); with dy[B,1024] != NULL also dW[32768,1024] = x^T . dy and
+ * dx[B,32768] = dy . w^T, computed from the operand copies the forward made.  dW is STORED in the tensor-core modes and
+ * ACCUMULATED in UDH_NUMERIC_FP32, as in the step.  scratch: udh_debug_fc1_scratch_bytes(B, numeric_mode) bytes (0 and
+ * unused in UDH_NUMERIC_FP32; 0 also for B < 1 or an unknown mode); it receives, each at a 256-byte aligned offset, the
+ * 16-bit copies of x [B][32768 x limbs], w (fc1's weight mirror: bf16, or the hi plane then the lo plane in
+ * UDH_NUMERIC_BF16X3) and dy, which the forward casts from w itself (the step's mirror is not assumed current). */
+size_t udh_debug_fc1_scratch_bytes(int B, int numeric_mode);
+int udh_debug_fc1(int numeric_mode, const float* x, const float* w, const float* dy, float* y, float* dW, float* dx, void* scratch,
+                  int B, void* stream);
 
 #ifdef __cplusplus
 }

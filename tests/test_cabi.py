@@ -81,6 +81,37 @@ def test_x3_mask_and_row_tile_debug_entries_reject_bad_arguments():
     assert b"udh_debug_x3_conv_rows" in L.udh_last_error()
 
 
+def test_fc1_debug_entry_rejects_bad_arguments():
+    """udh_debug_fc1 / udh_debug_fc1_scratch_bytes are exported and check their arguments before touching the device."""
+    from unsuperviseddeephomographyral2018_b200 import _lib
+    L = _lib.lib
+    raw = ctypes.CDLL(_lib.LIB_PATH)
+    assert hasattr(raw, "udh_debug_fc1") and hasattr(raw, "udh_debug_fc1_scratch_bytes")
+    F = 32768
+    for B in (1, 129, 512):
+        x3, bf = L.udh_debug_fc1_scratch_bytes(B, _lib.NUMERIC_BF16X3), L.udh_debug_fc1_scratch_bytes(B, _lib.NUMERIC_BF16)
+        assert x3 >= 4 * (B * F + F * 1024 + B * 1024) and bf >= 2 * (B * F + F * 1024 + B * 1024), B
+        assert x3 < 4 * (B * F + F * 1024 + B * 1024) + 1024 and bf < 2 * (B * F + F * 1024 + B * 1024) + 1024, B
+    assert L.udh_debug_fc1_scratch_bytes(4, _lib.NUMERIC_FP32) == 0
+    assert L.udh_debug_fc1_scratch_bytes(0, _lib.NUMERIC_BF16X3) == 0
+    assert L.udh_debug_fc1_scratch_bytes(4, 3) == 0
+    p = ctypes.c_void_p(256)                          # never dereferenced: every call below fails its argument checks
+    for mode in (_lib.NUMERIC_FP32, _lib.NUMERIC_BF16, _lib.NUMERIC_BF16X3):
+        for i in (0, 1, 3, 4, 5, 6):                  # x, w, y; dW and dx when dy is given; scratch in the tensor-core modes
+            if i == 6 and mode == _lib.NUMERIC_FP32:
+                continue
+            a = [p, p, p, p, p, p, p]
+            a[i] = None
+            assert L.udh_debug_fc1(mode, *a, 4, None) == _lib.EINVAL, (mode, i)
+            assert b"udh_debug_fc1: null pointer" in L.udh_last_error()
+        assert L.udh_debug_fc1(mode, p, p, p, p, p, p, p, 0, None) == _lib.EINVAL
+        assert b"batch must be >= 1" in L.udh_last_error()
+        assert L.udh_debug_fc1(mode, p, p, p, p, p, p, p, -3, None) == _lib.EINVAL
+    for mode in (-1, 3):
+        assert L.udh_debug_fc1(mode, p, p, p, p, p, p, p, 4, None) == _lib.EINVAL
+        assert b"unknown numeric_mode" in L.udh_last_error()
+
+
 def test_schedule_matches_reference_constants():
     from unsuperviseddeephomographyral2018_b200 import engine
     assert engine.decay_steps(1e-4, 0.9e-4) == 58117 and engine.decay_steps(5e-4, 0.9e-4) == 3570

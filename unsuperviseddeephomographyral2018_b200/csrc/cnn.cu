@@ -158,6 +158,37 @@ extern "C" int udh_cnn_fc1_mirror(void* ws, size_t ws_bytes, int B, int P, int n
   return UDH_OK;
 }
 
+extern "C" size_t udh_debug_fc1_scratch_bytes(int B, int numeric_mode) {
+  if (B < 1) return 0;
+  if (numeric_mode == UDH_NUMERIC_BF16) return fc1_region_bytes(B, 128, 1);
+  if (numeric_mode == UDH_NUMERIC_BF16X3) return fc1_region_bytes(B, 128, 2);
+  return 0;
+}
+
+extern "C" int udh_debug_fc1(int numeric_mode, const float* x, const float* w, const float* dy, float* y, float* dW, float* dx,
+                             void* scratch, int B, void* stream) {
+  UDH_REQUIRE(numeric_mode == UDH_NUMERIC_FP32 || numeric_mode == UDH_NUMERIC_BF16 || numeric_mode == UDH_NUMERIC_BF16X3,
+              "udh_debug_fc1: unknown numeric_mode %d", numeric_mode);
+  UDH_REQUIRE(B >= 1, "udh_debug_fc1: batch must be >= 1 (got %d)", B);
+  UDH_REQUIRE(x && w && y && (dy == nullptr || (dW && dx)) && (numeric_mode == UDH_NUMERIC_FP32 || scratch),
+              "udh_debug_fc1: null pointer");
+  const int P = 128, feat = (P / 8) * (P / 8) * 128;
+  cudaStream_t st = as_stream(stream);
+  // the calls of udh_cnn_fwd_ex / udh_cnn_bwd_phase, with the tensor-core region at the start of `scratch`
+  UDH_CUDA(cudaMemsetAsync(y, 0, (size_t)B * 1024 * 4, st));
+  if (numeric_mode == UDH_NUMERIC_BF16) {
+    TRY(tc_fc1_fwd(x, w, y, scratch, 0, B, P, false, st));
+    if (dy) TRY(tc_fc1_bwd(dy, dW, dx, scratch, 0, B, P, st));
+  } else if (numeric_mode == UDH_NUMERIC_BF16X3) {
+    TRY(x3_fc1_fwd(x, w, y, scratch, 0, B, P, false, st));
+    if (dy) TRY(x3_fc1_bwd(dy, dW, dx, scratch, 0, B, P, st));
+  } else {
+    TRY(fc1_fwd_simt(x, w, y, B, feat, st));
+    if (dy) TRY(fc1_bwd_simt(x, w, dy, dW, dx, B, feat, st));
+  }
+  return UDH_OK;
+}
+
 extern "C" int udh_cnn_fwd(const float* params, const float* I1, const float* I2, float* h4p, void* ws, size_t ws_bytes,
                            int B, int P, int train, uint64_t seed, int numeric_mode, void* stream) {
   return udh_cnn_fwd_ex(params, I1, I2, h4p, ws, ws_bytes, B, P, train, seed, numeric_mode, 0, stream);
@@ -213,8 +244,7 @@ extern "C" int udh_cnn_fwd_ex(const float* params, const float* I1, const float*
   } else if (numeric_mode == UDH_NUMERIC_BF16X3) {
     TRY(x3_fc1_fwd(feat_in, params + PL.off[16], at<float>(ws, L.fc1_acc), ws, L.tc, B, P, (flags & UDH_FWD_FC1_MIRROR_CURRENT) != 0, st));
   } else {
-    TRY(sgemm_simt(feat_in, feat, 1, params + PL.off[16], 1024, 1, at<float>(ws, L.fc1_acc), 1024, B, 1024, feat,
-                   B <= 256 ? 16 : 4, 0, st));
+    TRY(fc1_fwd_simt(feat_in, params + PL.off[16], at<float>(ws, L.fc1_acc), B, feat, st));
   }
   TRY(bias_act_dropout(at<float>(ws, L.fc1_acc), params + PL.off[17], at<float>(ws, L.act[11]), at<float>(ws, L.fc1d),
                        train ? at<uint8_t>(ws, L.mask2) : nullptr, B, 1024, 1, 1, seed, 2, st));
@@ -260,8 +290,7 @@ extern "C" int udh_cnn_bwd_phase(const float* params, const float* I1, const flo
   } else if (numeric_mode == UDH_NUMERIC_BF16X3) {
     TRY(x3_fc1_bwd(dfc1, grads + PL.off[16], gA, ws, L.tc, B, P, st));
   } else {
-    TRY(sgemm_simt(feat_in, 1, feat, dfc1, 1024, 1, grads + PL.off[16], 1024, feat, 1024, B, 1, 1, st));  // dW1 += x^T . dfc1
-    TRY(sgemm_simt(dfc1, 1024, 1, params + PL.off[16], 1, 1024, gA, feat, B, feat, 1024, 1, 0, st));   // dx = dfc1 . W1^T
+    TRY(fc1_bwd_simt(feat_in, params + PL.off[16], dfc1, grads + PL.off[16], gA, B, feat, st));
   }
   TRY(colsum_accum(dfc1, grads + PL.off[17], B, 1024, st));
   TRY(drop_relu_bwd(gA, train ? at<uint8_t>(ws, L.mask1) : nullptr, at<float>(ws, L.act[7]), (size_t)B * feat, st));

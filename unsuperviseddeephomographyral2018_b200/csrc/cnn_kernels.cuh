@@ -30,6 +30,11 @@ int maxpool2x2_bwd(const float* in, const float* dout, float* din, int B, int H,
 int sgemm_simt(const float* A, int64_t a_rs, int64_t a_cs, const float* Bm, int64_t b_rs, int64_t b_cs, float* C,
                int64_t ldc, int M, int N, int K, int split_k, int accumulate, cudaStream_t st);
 
+// fc1 of UDH_NUMERIC_FP32 (F -> 1024): acc[B,1024] (zeroed by the caller) += x[B,F] . W[F,1024];
+// backward dW[F,1024] += x^T . dy, dx[B,F] = dy . W^T
+int fc1_fwd_simt(const float* x, const float* w, float* acc, int B, int F, cudaStream_t st);
+int fc1_bwd_simt(const float* x, const float* w, const float* dy, float* dW, float* dx, int B, int F, cudaStream_t st);
+
 // y = relu(x + bias) -> act (nullable) ; drop = act * keep * 2 (if mask != nullptr, mask generated from seed/salt)
 int bias_act_dropout(const float* x, const float* bias, float* act, float* drop, uint8_t* mask, int rows, int cols,
                      int relu, int gen_mask, uint64_t seed, uint64_t salt, cudaStream_t st);

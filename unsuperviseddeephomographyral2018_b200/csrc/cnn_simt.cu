@@ -448,6 +448,15 @@ int sgemm_simt(const float* A, int64_t a_rs, int64_t a_cs, const float* Bm, int6
   return slab_reduce(t, st);
 }
 
+int fc1_fwd_simt(const float* x, const float* w, float* acc, int B, int F, cudaStream_t st) {
+  return sgemm_simt(x, F, 1, w, 1024, 1, acc, 1024, B, 1024, F, B <= 256 ? 16 : 4, 0, st);
+}
+
+int fc1_bwd_simt(const float* x, const float* w, const float* dy, float* dW, float* dx, int B, int F, cudaStream_t st) {
+  if (int rc = sgemm_simt(x, 1, F, dy, 1024, 1, dW, 1024, F, 1024, B, 1, 1, st)) return rc;   // dW += x^T . dy
+  return sgemm_simt(dy, 1024, 1, w, 1, 1024, dx, F, B, F, 1024, 1, 0, st);                   // dx = dy . W^T
+}
+
 int bias_act_dropout(const float* x, const float* bias, float* act, float* drop, uint8_t* mask, int rows, int cols,
                      int relu, int gen_mask, uint64_t seed, uint64_t salt, cudaStream_t st) {
   const size_t total = (size_t)rows * cols;

@@ -591,6 +591,8 @@ int tc_cnn_bwd_convs(const float* params, const size_t* poff, const float* I1, c
   return UDH_OK;
 }
 
+size_t fc1_region_bytes(int B, int P, int limbs) { return TcLayout(B, P, limbs).fc_end; }
+
 // fc1 forward on tensor cores: acc[B,1024] (zeroed by the caller) += x[B,F] . W[F,1024]
 void* tc_fc1_mirror(void* ws, size_t tc_off, int B, int P) {
   TcLayout L(B, P);

@@ -23,6 +23,8 @@ int tc_cnn_bwd_convs(const float* params, const size_t* param_off, const float* 
 int tc_fc1_fwd(const float* x, const float* w, float* acc, void* ws, size_t tc_off, int B, int P, bool w_mirror_current, cudaStream_t st);
 void* tc_fc1_mirror(void* ws, size_t tc_off, int B, int P);
 int tc_fc1_bwd(const float* dy, float* dW, float* dx, void* ws, size_t tc_off, int B, int P, cudaStream_t st);
+// bytes at the start of the tensor-core region that fc1's forward / backward touch (limbs = 1: bf16 mode, 2: two-limb mode)
+size_t fc1_region_bytes(int B, int P, int limbs);
 
 // ---- UDH_NUMERIC_BF16X3 (conv_x3.cu): the same pipeline on two-limb streams, lo.hi + hi.hi + hi.lo per product ----------
 size_t x3_workspace_bytes(int B, int P);

@@ -22,12 +22,18 @@ struct TcLayout {
   size_t Mb[8];      // 1-bit ReLU masks [Q][C/32] uint32 of the conv outputs a dgrad needs (layers 0, 2, 4, 6)
   size_t Px[3];      // max-pool routing codes [B][H/2][W/2][C/8] uint32 (3 bits per channel), written by the forward
   size_t fc_x, fc_w, fc_dy;   // 16-bit copies for the fc1 GEMMs: x [B,F], W [F,1024], dy [B,1024] (x limbs)
+  size_t fc_end;     // end of the fc1 copies: they come first, so fc1 alone runs in a region of fc_end bytes (udh_debug_fc1)
   size_t total;
   int limbs;
   TcLayout(int B, int P_, int limbs_ = 1) : limbs(limbs_) {
     size_t o = 0;
     auto take = [&](size_t bytes) { size_t r = o; o += al256(bytes); return r; };
     const size_t eb = 2 * (size_t)limbs;                         // bytes per logical element
+    const size_t feat = (size_t)(P_ / 8) * (P_ / 8) * 128;
+    fc_x = take((size_t)B * feat * eb);
+    fc_w = take(feat * 1024 * eb);
+    fc_dy = take((size_t)B * 1024 * eb);
+    fc_end = o;
     for (int i = 0; i < 8; ++i) {
       const size_t s = P_ / kConv[i].div + 2;
       numel[i] = (size_t)B * s * s * kConv[i].cout;
@@ -40,10 +46,6 @@ struct TcLayout {
     for (int i = 0; i < 8; ++i) { wf[i] = take((size_t)9 * kConv[i].cin * kConv[i].cout * eb); wd[i] = take((size_t)9 * kConv[i].cin * kConv[i].cout * eb); }
     for (int i = 0; i < 8; ++i) Mb[i] = (i % 2 == 0) ? take(numel[i] / 8) : 0;
     for (int i = 0; i < 3; ++i) Px[i] = take((size_t)B * (P_ >> (i + 1)) * (P_ >> (i + 1)) * (i == 2 ? 16 : 8) * 4);
-    const size_t feat = (size_t)(P_ / 8) * (P_ / 8) * 128;
-    fc_x = take((size_t)B * feat * eb);
-    fc_w = take(feat * 1024 * eb);
-    fc_dy = take((size_t)B * 1024 * eb);
     total = o;
   }
 };
