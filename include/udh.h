@@ -270,6 +270,29 @@ int udh_ecc_homography(const uint8_t* tmpl, const uint8_t* input, const float* W
                        void* stream);
 int udh_ecc_h4p(const float* W, const int32_t* status, const float* pts1, const float* gt, float rho_clamp, float* pred_h4p,
                 float* h_loss, int32_t* fail, int B, void* stream);
+/* udh_ecc_corr_h4p: the real-data harness's metric (homography_conventional_real.py:213-246, return_h_inv = False).
+ *   gt [B,16] fp32: four correspondences clicked on 480x640 frames; corr1 = gt[0:8] / 2, corr2 = gt[8:16] / 2.
+ *   status == 0: pred_h4p [B,8] = perspectiveTransform(corr1, W) - corr1 (W NOT inverted), clamped to +-80;
+ *     h_loss [B] = RMSE(pred + corr1, corr2) in fp32; fail = 2 and h_loss = the identity RMSE when that is smaller.
+ *   status != 0: pred_h4p = 0, fail = 1, h_loss = the identity RMSE computed in float64 (no identity bound). */
+int udh_ecc_corr_h4p(const float* W, const int32_t* status, const float* gt, float* pred_h4p, double* h_loss, int32_t* fail, int B,
+                     void* stream);
+
+/* ---- real-data input pipeline (dataloader.py:146-200), bit-identical to the host's cv2 / NumPy arithmetic ----------------
+ * udh_resize_area_up_u8: cv2.resize(src, (dst_w, dst_h), INTER_AREA) on n uint8 [src_h,src_w,3] images, dst larger on both
+ *   axes.  tab (device, int32): xsrc[dst_w], xa0[dst_w], xa1[dst_w], ysrc[dst_h], ya0[dst_h], ya1[dst_h] — first source
+ *   index and the two 11-bit coefficients per output column / row, as OpenCV computes them (ops.linear_area_table).
+ * udh_real_prep: full-size uint8 I, I' [B,full_h,full_w,3] -> the loader's four network-size fp32 images [B,img_h,img_w,3]:
+ *   I_plain = T0[I], I_prime_plain = T1[I'], I_aug = T2[I], I_prime_aug = T3[I'], each AREA-downscaled when the sizes
+ *   differ.  luts (device) [B][4][256][3] fp32 are the per-value tables T0..T3 (augment + normalise).  tab (device, int32,
+ *   nullable when the sizes are equal): nx, ny, xofs[img_w+1], xsrc[nx], xw[nx], yofs[img_h+1], ysrc[ny], yw[ny] (weights
+ *   as fp32 bits): OpenCV's computeResizeAreaTab entries of each output column / row in table order (ops.area_table);
+ *   max_rows = the most entries of one output row.  The downscale is resizeArea's generic path: sequential fp32 sums, no FMA. */
+int udh_resize_area_up_u8(const uint8_t* src, const int32_t* tab, uint8_t* dst, int n, int src_h, int src_w, int dst_h, int dst_w,
+                          void* stream);
+size_t udh_real_prep_smem_bytes(int max_rows, int full_w);
+int udh_real_prep(const uint8_t* I, const uint8_t* I_prime, const float* luts, const int32_t* tab, int max_rows, int B, int full_h,
+                  int full_w, int img_h, int img_w, float* I_plain, float* I_prime_plain, float* I_aug, float* I_prime_aug, void* stream);
 
 /* ---- baseline-JPEG decode, bit-identical to cv2.imread(..., IMREAD_COLOR) + BGR->RGB (libjpeg-turbo defaults) --------
  * Accepted: baseline Huffman 8-bit (SOF0, SOF1), one interleaved scan, gray or YCbCr with luma sampling 1x1, 2x1 or 2x2 and

@@ -124,6 +124,11 @@ SIGNATURES = {
     "udh_ecc_homography": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_double, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                    c_size_t, c_int, c_int, c_int, c_void_p]),
     "udh_ecc_h4p": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
+    "udh_ecc_corr_h4p": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
+    "udh_resize_area_up_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "udh_real_prep_smem_bytes": (c_size_t, [c_int, c_int]),
+    "udh_real_prep": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                              c_void_p, c_void_p, c_void_p]),
     "udh_jpeg_parse": (c_int, [c_void_p, c_int64, POINTER(JpegInfo)]),
     "udh_jpeg_plan_bytes": (c_size_t, [c_void_p, c_void_p, c_int, c_int, c_int]),
     "udh_jpeg_plan": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_size_t]),

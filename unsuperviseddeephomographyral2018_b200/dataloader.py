@@ -4,7 +4,9 @@ Produces, per batch, the nine post-dataloader tensors the model consumes (`*_bat
 I1, I2, I1_aug, I2_aug [B,P,P,1]; I (=I_aug), I_prime (=I_prime_aug) [B,Hh,W,3]; pts1, gt [B,8]; patch_indices [B,P*P].
 JPEG decode runs on the device for the baseline files cv2.imwrite produces (bit-identical to cv2.imread; other files are
 decoded on the host); list parsing runs on the host; photometric augmentation, normalisation, gray conversion and patch
-gather run on the device.  `synthetic=N` replaces the on-disk set by N
+gather run on the device.  The real-data set (extended_dataloader_params) takes the same device path at its two file sizes,
+with its augment + normalise + AREA resize in one kernel, bit-identical to its host path (_disk_batch_extended_host).
+`synthetic=N` replaces the on-disk set by N
 on-device generated pairs (synthetic.make_batch) — MS-COCO is not available offline.
 """
 import os
@@ -66,6 +68,15 @@ def read_img_and_gt(filenames_file, pts1_file, gt_file):
     return names, pts1, gt
 
 
+def _value_table(g=None, br=None, c=None):
+    """[256, 3] fp32: the real-data host path's augment (g, br, c; none when g is None) and normalise expression evaluated
+    on the values 0..255.  Every step is elementwise in the uint8 value and the channel, so a lookup equals it bit for bit."""
+    v = np.repeat(np.arange(256, dtype=np.float32)[:, None], 3, axis=1)
+    if g is not None:
+        v = np.clip(v ** np.float32(g) * np.float32(br) * c, 0, 255)
+    return (v - np.array(synthetic.MEAN_I, np.float32)) / np.array(synthetic.STD_I, np.float32)
+
+
 class Dataloader(object):
     def __init__(self, params, shuffle=True, synthetic_pairs=0, seed=0, device="cuda", rho=45):
         self.params = params
@@ -92,15 +103,16 @@ class Dataloader(object):
         name = self.names[idx][1] if len(self.names[idx]) > 1 else self.names[idx][0]   # dataloader.py:143-144 (column 1 for both)
         return [os.path.join(self.params.data_path, sub, name) for sub in ("I", "I_prime")]
 
-    def _read_image(self, path):
-        """The host decode: cv2.imread + BGR -> RGB, INTER_AREA-resized to the network size when it differs."""
+    def _read_image(self, path, size=None):
+        """The host decode: cv2.imread + BGR -> RGB, INTER_AREA-resized to `size` (default: the network size) when it differs."""
         import cv2
+        h, w = size or (self.params.img_h, self.params.img_w)
         im = cv2.imread(path, cv2.IMREAD_COLOR)
         if im is None:
             raise IOError("cannot read %s" % path)
         im = cv2.cvtColor(im, cv2.COLOR_BGR2RGB)
-        if im.shape[0] != self.params.img_h or im.shape[1] != self.params.img_w:
-            im = cv2.resize(im, (self.params.img_w, self.params.img_h), interpolation=cv2.INTER_AREA)    # dataloader.py:245
+        if im.shape[0] != h or im.shape[1] != w:
+            im = cv2.resize(im, (w, h), interpolation=cv2.INTER_AREA)    # dataloader.py:245
         return im
 
     def _read_pair(self, idx):
@@ -116,10 +128,11 @@ class Dataloader(object):
             out.append(self._order[self._cursor]); self._cursor += 1
         return np.array(out)
 
-    def _disk_batch_extended(self):
+    def _disk_batch_extended_host(self):
         """Real-data samples (code/dataloader.py:146-200): FULL-size images are read, augmented and normalised at full
         size, then AREA-resized to the network size; the ground truth (test only) is four hand-picked correspondences
-        (16 numbers), not a 4-point displacement.  JPEG decode, augmentation and resize run on the host as in the reference."""
+        (16 numbers), not a 4-point displacement.  JPEG decode, augmentation and resize run on the host as in the reference.
+        _disk_batch_extended gives the same batches from the device; this path serves the geometries it does not restate."""
         import cv2
         p = self.params
         B, P, Hh, W, FH, FW = p.batch_size, p.patch_size, p.img_h, p.img_w, p.full_img_h, p.full_img_w
@@ -127,6 +140,7 @@ class Dataloader(object):
         mean, std = np.array(synthetic.MEAN_I, np.float32), np.array(synthetic.STD_I, np.float32)
         I_aug = np.empty((B, Hh, W, 3), np.float32); Ip_aug = np.empty_like(I_aug); I_pl = np.empty_like(I_aug); Ip_pl = np.empty_like(I_aug)
         full_I = np.empty((B, FH, FW, 3), np.uint8); full_Ip = np.empty_like(full_I)
+        aug_tab = np.zeros((B, 11), np.float32)
         for j, i in enumerate(idx):
             name = self.names[i][1] if len(self.names[i]) > 1 else self.names[i][0]
             pair = []
@@ -145,9 +159,11 @@ class Dataloader(object):
                 draw = lambda: (self._rng.uniform(0.8, 1.2), self._rng.uniform(0.5, 2.0), self._rng.uniform(0.8, 1.2, size=3).astype(np.float32))
                 g, br, c = draw()
                 aa = np.clip(a ** np.float32(g) * np.float32(br) * c, 0, 255)
+                aug_tab[j, :6] = [1.0, g, br, *c]
                 if self.mode != 'train':
                     g, br, c = draw()                                                             # disjoint noise in test
                 ba = np.clip(b ** np.float32(g) * np.float32(br) * c, 0, 255)
+                aug_tab[j, 6:] = [g, br, *c]
             rs = lambda t: cv2.resize((t - mean) / std, (W, Hh), interpolation=cv2.INTER_AREA) if (FH != Hh or FW != W) else (t - mean) / std
             I_pl[j], Ip_pl[j], I_aug[j], Ip_aug[j] = rs(a), rs(b), rs(aa), rs(ba)
         dev = self.device
@@ -159,11 +175,81 @@ class Dataloader(object):
         g = lambda a: torch.gather(t(a).mean(dim=3).reshape(B, -1), 1, pidx).reshape(B, P, P, 1).contiguous()
         out = dict(I1=g(I_pl), I2=g(Ip_pl), I1_aug=g(I_aug), I2_aug=g(Ip_aug), I_aug=t(I_aug).contiguous(), I_prime_aug=t(Ip_aug).contiguous(),
                    pts1=pts1, gt=None, patch_indices=pidx.to(torch.int32).contiguous(), full_I=full_I, full_I_prime=full_Ip)
+        out.update(I_u8=t(full_I), I_prime_u8=t(full_Ip), aug=t(aug_tab))
+        self._extended_gt(out, idx)
+        return out
+
+    def _extended_gt(self, out, idx):
         if self.gt is not None:
             if self.gt.shape[1] == 16:
                 out["gt_corr"] = self.gt[idx].astype(np.float32)                                  # four correspondences (test set)
             else:
-                out["gt"] = torch.tensor(self.gt[idx], dtype=torch.float32, device=dev)
+                out["gt"] = torch.tensor(self.gt[idx], dtype=torch.float32, device=self.device)
+
+    # The same batches from the device: the full-size uint8 images come from the decode groups below (files at the network
+    # size are decoded at that size and brought up to the full size by udh_resize_area_up_u8), and udh_real_prep turns them
+    # into the four network-size fp32 images through per-sample value tables.  The tables are the host path's augment +
+    # normalise expression evaluated on 0..255, drawn from the RNG in the host path's order.  The channel mean and the
+    # patch gather are the host path's torch calls on the same device tensors.
+    def _extended_on_device(self):
+        """Whether udh_real_prep restates this geometry's fp32 resize (else every batch takes the host path)."""
+        p = self.params
+        from . import ops
+        return (p.full_img_h, p.full_img_w) == (p.img_h, p.img_w) or ops.area_is_generic(p.full_img_h, p.full_img_w, p.img_h, p.img_w)
+
+    def _decode_sizes(self):
+        """File sizes the device decoder takes: the full size, and the network size when it can be upscaled on the device."""
+        p = self.params
+        if not hasattr(p, "full_img_h"):
+            return [(p.img_h, p.img_w)]
+        sizes = [(p.full_img_h, p.full_img_w)]
+        if p.img_h < p.full_img_h and p.img_w < p.full_img_w:
+            sizes.append((p.img_h, p.img_w))
+        return sizes
+
+    def _draw_batch_extended(self):
+        """Indices, value tables [B,4,256,3] (plain I, plain I', augmented I, augmented I') and the [B,11] augmentation
+        table, drawn as _disk_batch_extended_host draws: per sample uniform(0, 1), then (g, br, c[3]) when augmenting and
+        a second (g, br, c[3]) in test mode."""
+        p = self.params
+        B = p.batch_size
+        idx = self._next_indices(B)
+        plain = _value_table()
+        tables = np.empty((B, 4, 256, 3), np.float32)
+        tables[:] = plain[None, None]
+        aug = np.zeros((B, 11), np.float32)
+        for j in range(B):
+            if self._rng.uniform(0, 1) > (1 - p.do_augment):                                      # dataloader.py:163-169
+                draw = lambda: (self._rng.uniform(0.8, 1.2), self._rng.uniform(0.5, 2.0), self._rng.uniform(0.8, 1.2, size=3).astype(np.float32))
+                g, br, c = draw()
+                tables[j, 2] = _value_table(g, br, c)
+                aug[j, :6] = [1.0, g, br, *c]
+                if self.mode != 'train':
+                    g, br, c = draw()
+                tables[j, 3] = _value_table(g, br, c)
+                aug[j, 6:] = [g, br, *c]
+        return idx, tables, aug
+
+    def _disk_batch_extended(self):
+        if not self._extended_on_device():
+            return self._disk_batch_extended_host()
+        from . import ops
+        p = self.params
+        B, P, Hh, W = p.batch_size, p.patch_size, p.img_h, p.img_w
+        if not self._ready:
+            self._decode_group()
+        idx, tables, aug, I_u8, Ip_u8 = self._ready.pop(0)
+        dev = self.device
+        I_pl, Ip_pl, I_aug, Ip_aug = ops.real_prep(I_u8, Ip_u8, torch.from_numpy(tables).to(dev), Hh, W)
+        pts1 = torch.tensor(self.pts1[idx], dtype=torch.float32, device=dev)
+        x0 = pts1[:, 0].long(); y0 = pts1[:, 1].long()
+        yy, xx = torch.meshgrid(torch.arange(P, device=dev), torch.arange(P, device=dev), indexing="ij")
+        pidx = ((yy[None] + y0[:, None, None]) * W + (xx[None] + x0[:, None, None])).reshape(B, -1)
+        g = lambda a: torch.gather(a.mean(dim=3).reshape(B, -1), 1, pidx).reshape(B, P, P, 1).contiguous()
+        out = dict(I1=g(I_pl), I2=g(Ip_pl), I1_aug=g(I_aug), I2_aug=g(Ip_aug), I_aug=I_aug, I_prime_aug=Ip_aug,
+                   pts1=pts1, gt=None, patch_indices=pidx.to(torch.int32).contiguous(), full_I=I_u8.cpu().numpy(), full_I_prime=Ip_u8.cpu().numpy())
+        out.update(I_u8=I_u8, I_prime_u8=Ip_u8, aug=torch.from_numpy(aug).to(dev))
+        self._extended_gt(out, idx)
         return out
 
     def _synthetic_real_batch(self):
@@ -215,12 +301,12 @@ class Dataloader(object):
             aug[j, 6:11] = a if self.mode == 'train' else draw()                                   # joint (train) / disjoint (test)
         return idx, aug
 
-    def _read_group(self, paths):
-        """Background thread: file bytes -> (device-decodable file positions, JpegPlan or None).  File reads and the
-        ctypes parser calls release the GIL."""
+    def _read_group(self, paths, sizes):
+        """Background thread: file bytes -> ([(size, device-decodable file positions, JpegPlan)] per size in `sizes` that
+        has files).  File reads and the ctypes parser calls release the GIL."""
         from . import ops
         t0 = time.perf_counter()
-        blobs, take = [], []
+        blobs, take = {s: [] for s in sizes}, {s: [] for s in sizes}
         for k, path in enumerate(paths):
             try:
                 with open(path, "rb") as f:
@@ -228,18 +314,19 @@ class Dataloader(object):
             except OSError:
                 continue                                       # _read_image raises the host path's error
             info = ops.jpeg_parse(b)
-            if info.reason == 0 and info.height == self.params.img_h and info.width == self.params.img_w:
-                blobs.append(b); take.append(k)
-        plan = ops.JpegPlan(blobs, self.params.img_h, self.params.img_w) if blobs else None
-        return take, plan, time.perf_counter() - t0
+            if info.reason == 0 and (info.height, info.width) in blobs:
+                blobs[(info.height, info.width)].append(b); take[(info.height, info.width)].append(k)
+        plans = [(s, take[s], ops.JpegPlan(blobs[s], *s)) for s in sizes if blobs[s]]
+        return plans, time.perf_counter() - t0
 
     def _submit_group(self):
-        draws = [self._draw_batch() for _ in range(self.DECODE_BATCHES)]
-        paths = [path for idx, _ in draws for i in idx for path in self._pair_paths(i)]
+        extended = hasattr(self.params, "full_img_h")
+        draws = [self._draw_batch_extended() if extended else self._draw_batch() for _ in range(self.DECODE_BATCHES)]
+        paths = [path for d in draws for i in d[0] for path in self._pair_paths(i)]
         if self._reader is None:
             import concurrent.futures
             self._reader = concurrent.futures.ThreadPoolExecutor(max_workers=1, thread_name_prefix="udh-jpeg-reader")
-        return draws, paths, self._reader.submit(self._read_group, paths)
+        return draws, paths, self._reader.submit(self._read_group, paths, self._decode_sizes())
 
     def _decode_group(self):
         t_group = time.perf_counter()
@@ -248,24 +335,29 @@ class Dataloader(object):
         draws, paths, fut = self._pending
         self._pending = self._submit_group()                   # read the next group while this one is decoded and consumed
         t0 = time.perf_counter()
-        take, plan, read_s = fut.result()
+        plans, read_s = fut.result()
         st = self.decode_stats
         st["groups"] += 1; st["read_s"] += read_s; st["wait_s"] += time.perf_counter() - t0
         p, dev = self.params, self.device
-        imgs = torch.empty(len(paths), p.img_h, p.img_w, 3, dtype=torch.uint8, device=dev)
-        host = sorted(set(range(len(paths))) - set(take))
-        if plan is not None:
+        h, w = self._decode_sizes()[0]                          # the size the batch is assembled at
+        imgs = torch.empty(len(paths), h, w, 3, dtype=torch.uint8, device=dev)
+        host = set(range(len(paths)))
+        for size, take, plan in plans:
             out, status = plan.decode(dev)
+            if size != (h, w):
+                from . import ops
+                out = ops.resize_area_up_u8(out, h, w)           # network-size files of the real-data set
             imgs[torch.tensor(take, device=dev)] = out
             bad = [take[k] for k in np.flatnonzero(status.cpu().numpy())]
-            host = sorted(host + bad)
+            host = (host - set(take)) | set(bad)
             st["device_images"] += len(take) - len(bad); st["decode_errors"] += len(bad)
+        host = sorted(host)
         st["host_images"] += len(host)
         if host:
-            h = np.stack([self._read_image(paths[k]) for k in host])
-            imgs[torch.tensor(host, device=dev)] = torch.from_numpy(h).to(dev)
-        imgs = imgs.view(len(draws), p.batch_size, 2, p.img_h, p.img_w, 3)
-        self._ready = [(idx, aug, imgs[d, :, 0].contiguous(), imgs[d, :, 1].contiguous()) for d, (idx, aug) in enumerate(draws)]
+            hi = np.stack([self._read_image(paths[k], (h, w)) for k in host])
+            imgs[torch.tensor(host, device=dev)] = torch.from_numpy(hi).to(dev)
+        imgs = imgs.view(len(draws), p.batch_size, 2, h, w, 3)
+        self._ready = [tuple(d) + (imgs[k, :, 0].contiguous(), imgs[k, :, 1].contiguous()) for k, d in enumerate(draws)]
         st["group_s"] += time.perf_counter() - t_group
 
     def _disk_batch(self):

@@ -1,6 +1,7 @@
 """Torch-tensor wrappers over the C ABI (include/udh.h).  PyTorch is plumbing here: device memory, streams and
 autograd bookkeeping; all arithmetic happens in libudh's CUDA kernels.  Every function requires CUDA tensors."""
 import ctypes
+import functools
 
 import numpy as np
 import torch
@@ -221,6 +222,110 @@ def ecc_h4p(W, status, pts1, gt=None, rho=45.0):
     check(lib.udh_ecc_h4p(_ptr(W), _ptr(status), _ptr(pts1), _ptr(gt), float(rho), _ptr(pred), _ptr(h), _ptr(fail), B, _stream()),
           "udh_ecc_h4p")
     return pred, h, fail
+
+
+def ecc_corr_h4p(W, status, gt):
+    """The real-data harness's metric on clicked correspondences gt [B,16] (480x640 frame): -> (pred_h4p [B,8] fp32,
+    h_loss [B] float64, fail [B] int32: 0 ok, 1 not found, 2 worse than identity).  W is not inverted; see include/udh.h."""
+    W = W.reshape(-1, 9).contiguous()
+    _req(W, torch.float32, "W"); _req(status, torch.int32, "status"); _req(gt, torch.float32, "gt")
+    B = W.shape[0]
+    pred = torch.empty(B, 8, device=W.device, dtype=torch.float32)
+    h = torch.empty(B, device=W.device, dtype=torch.float64)
+    fail = torch.empty(B, device=W.device, dtype=torch.int32)
+    check(lib.udh_ecc_corr_h4p(_ptr(W), _ptr(status), _ptr(gt), _ptr(pred), _ptr(h), _ptr(fail), B, _stream()), "udh_ecc_corr_h4p")
+    return pred, h, fail
+
+
+# ------------------------------------------------------------------ real-data input pipeline (cv2.resize INTER_AREA)
+def area_is_generic(src_h, src_w, dst_h, dst_w):
+    """True when cv2.resize(INTER_AREA) downscales with its generic resizeArea (the path udh_real_prep restates): scale
+    >= 1 on both axes, and not an integer ratio on both (that takes resizeAreaFast, another summation order)."""
+    if dst_h > src_h or dst_w > src_w:
+        return False
+    eps = np.finfo(np.float64).eps
+    sx, sy = src_w / dst_w, src_h / dst_h
+    return not (abs(sx - round(sx)) < eps and abs(sy - round(sy)) < eps)
+
+
+def _area_entries(ssize, dsize):
+    """OpenCV's computeResizeAreaTab (imgproc/src/resize.cpp): (offsets [dsize+1], source index, fp32 weight) in table order."""
+    scale = 1.0 / (float(dsize) / float(ssize))
+    ofs, src, wt = [0], [], []
+    for d in range(dsize):
+        f1 = d * scale
+        f2 = f1 + scale
+        cell = min(scale, ssize - f1)
+        s1, s2 = int(np.ceil(f1)), int(np.floor(f2))
+        s2 = min(s2, ssize - 1)
+        s1 = min(s1, s2)
+        if s1 - f1 > 1e-3:
+            src.append(s1 - 1); wt.append((s1 - f1) / cell)
+        for s in range(s1, s2):
+            src.append(s); wt.append(1.0 / cell)
+        if f2 - s2 > 1e-3:
+            src.append(s2); wt.append(min(min(f2 - s2, 1.0), cell) / cell)
+        ofs.append(len(src))
+    return np.array(ofs, np.int32), np.array(src, np.int32), np.array(wt, np.float32)
+
+
+@functools.lru_cache(maxsize=8)
+def area_table(src_h, src_w, dst_h, dst_w):
+    """udh_real_prep's packed area table (int32) and its max_rows, for the generic resizeArea downscale."""
+    if not area_is_generic(src_h, src_w, dst_h, dst_w):
+        raise _lib.UdhError("INTER_AREA %dx%d -> %dx%d is not the generic resizeArea downscale" % (src_h, src_w, dst_h, dst_w))
+    xo, xs, xw = _area_entries(src_w, dst_w)
+    yo, ys, yw = _area_entries(src_h, dst_h)
+    tab = np.concatenate([[len(xs), len(ys)], xo, xs, xw.view(np.int32), yo, ys, yw.view(np.int32)]).astype(np.int32)
+    return tab, int(np.diff(yo).max())
+
+
+@functools.lru_cache(maxsize=8)
+def linear_area_table(src_h, src_w, dst_h, dst_w):
+    """udh_resize_area_up_u8's table (int32): INTER_AREA upscaling is linear interpolation with area coefficients —
+    fx = (d+1) - (s+1) inv_scale in float, fx - floor(fx), 11-bit fixed point (cvRound), both taps on the last pixel at
+    the right / bottom border."""
+    def axis(ssize, dsize):
+        inv = float(dsize) / float(ssize)
+        s_, a0, a1 = [], [], []
+        for d in range(dsize):
+            s = int(np.floor(d * (1.0 / inv)))
+            fx = np.float32((d + 1) - (s + 1) * inv)
+            fx = np.float32(0) if fx <= 0 else np.float32(fx - np.floor(fx))
+            c0, c1 = np.float32(1) - fx, fx
+            if s >= ssize - 1:
+                s, c0, c1 = ssize - 1, np.float32(1), np.float32(0)
+            s_.append(s); a0.append(np.rint(c0 * np.float32(2048))); a1.append(np.rint(c1 * np.float32(2048)))
+        return [s_, a0, a1]
+    if not (dst_h > src_h and dst_w > src_w):
+        raise _lib.UdhError("udh_resize_area_up_u8 upscales on both axes (got %dx%d -> %dx%d)" % (src_h, src_w, dst_h, dst_w))
+    return np.concatenate([np.array(a, np.float64) for a in axis(src_w, dst_w) + axis(src_h, dst_h)]).astype(np.int32)
+
+
+def resize_area_up_u8(src, dst_h, dst_w):
+    """uint8 [N,h,w,3] CUDA tensor -> [N,dst_h,dst_w,3]: cv2.resize(INTER_AREA) per image, bit for bit."""
+    _req(src, torch.uint8, "src")
+    n, h, w, _ = src.shape
+    tab = torch.from_numpy(linear_area_table(h, w, dst_h, dst_w)).to(src.device)
+    out = torch.empty(n, dst_h, dst_w, 3, device=src.device, dtype=torch.uint8)
+    check(lib.udh_resize_area_up_u8(_ptr(src), _ptr(tab), _ptr(out), n, h, w, dst_h, dst_w, _stream()), "udh_resize_area_up_u8")
+    return out
+
+
+def real_prep(I_u8, Ip_u8, luts, img_h, img_w):
+    """Full-size uint8 I, I' [B,FH,FW,3] and per-sample value tables luts [B,4,256,3] fp32 (plain I, plain I', augmented I,
+    augmented I') -> (I, I_prime, I_aug, I_prime_aug) [B,img_h,img_w,3] fp32: table lookup, then cv2's INTER_AREA
+    downscale when the sizes differ — the real-data loader's host arithmetic, bit for bit."""
+    _req(I_u8, torch.uint8, "I"); _req(Ip_u8, torch.uint8, "I_prime"); _req(luts, torch.float32, "luts")
+    B, FH, FW, _ = I_u8.shape
+    tab, max_rows = None, 0
+    if (FH, FW) != (img_h, img_w):
+        t, max_rows = area_table(FH, FW, img_h, img_w)
+        tab = torch.from_numpy(t).to(I_u8.device, non_blocking=True)
+    outs = [torch.empty(B, img_h, img_w, 3, device=I_u8.device, dtype=torch.float32) for _ in range(4)]
+    check(lib.udh_real_prep(_ptr(I_u8), _ptr(Ip_u8), _ptr(luts), _ptr(tab), max_rows, B, FH, FW, img_h, img_w, *[_ptr(o) for o in outs],
+                            _stream()), "udh_real_prep")
+    return outs
 
 
 # ------------------------------------------------------------------ baseline-JPEG decode
