@@ -290,6 +290,13 @@ int udh_ecc_corr_h4p(const float* W, const int32_t* status, const float* gt, flo
  *   max_rows = the most entries of one output row.  The downscale is resizeArea's generic path: sequential fp32 sums, no FMA. */
 int udh_resize_area_up_u8(const uint8_t* src, const int32_t* tab, uint8_t* dst, int n, int src_h, int src_w, int dst_h, int dst_w,
                           void* stream);
+/* udh_resize_linear_u8: cv2.resize(src, (dst_w, dst_h)) with the default INTER_LINEAR on n uint8 [src_h,src_w,3] images, any
+ *   sizes (down or up).  The kernel of udh_resize_area_up_u8 with OpenCV's INTER_LINEAR table (ops.linear_table):
+ *   f = (float)((d + 0.5) * scale - 0.5), floor, coefficients in float rounded to 11 bits; tab = xsrc[dst_w], xa0, xa1,
+ *   ysrc[dst_h], ya0, ya1, ysrc1[dst_h]: columns clamp index and coefficient at the borders, rows keep the coefficients
+ *   and give both (clamped) source rows. */
+int udh_resize_linear_u8(const uint8_t* src, const int32_t* tab, uint8_t* dst, int n, int src_h, int src_w, int dst_h, int dst_w,
+                         void* stream);
 size_t udh_real_prep_smem_bytes(int max_rows, int full_w);
 int udh_real_prep(const uint8_t* I, const uint8_t* I_prime, const float* luts, const int32_t* tab, int max_rows, int B, int full_h,
                   int full_w, int img_h, int img_w, float* I_plain, float* I_prime_plain, float* I_aug, float* I_prime_aug, void* stream);
@@ -334,6 +341,29 @@ int udh_jpeg_decode(const void* plan_host, const void* plan_dev, const uint8_t* 
 /* Lanes per image in the entropy-decode kernel (32: one warp per image, the default; 1: eight images share a warp).  For
  * the timing tool's comparison; process-wide. */
 int udh_debug_jpeg_set_lanes(int lanes);
+
+/* ---- baseline-JPEG encode, byte-identical to cv2.imencode('.jpg', img, [IMWRITE_JPEG_QUALITY, quality]) ------------------
+ * libjpeg-turbo's defaults: JFIF APP0, standard Huffman tables, ISLOW DCT, no restart markers; channels = 3 takes uint8 BGR
+ * [n,h,w,3] and writes YCbCr 4:2:0, channels = 1 takes gray [n,h,w] and writes one component.  quality 1..100.
+ * udh_jpeg_encode_capacity: the largest file an h x w image can encode to (every coefficient at its longest code, every
+ *   byte stuffed), 0 on bad dimensions; size each output row with it, no dry run needed.
+ * udh_jpeg_encode_workspace_bytes: device workspace of one call, 0 on bad dimensions.
+ * udh_jpeg_encode (device): img [n,h,w,channels] uint8; out [n][cap] with cap >= the capacity; nbytes [n] int64 = the file
+ *   length of each image (its bytes are out[k][0, nbytes[k])); status [n] int32 = 0, or nonzero when that image could not
+ *   be encoded (its output is then undefined, the other images are unaffected).  n <= 65535 per call.  The library
+ *   allocates nothing. */
+int64_t udh_jpeg_encode_capacity(int h, int w, int channels);
+size_t udh_jpeg_encode_workspace_bytes(int n, int h, int w, int channels);
+int udh_jpeg_encode(const uint8_t* img, int n, int h, int w, int channels, int quality, uint8_t* out, int64_t cap, int64_t* nbytes,
+                    int32_t* status, void* ws, size_t ws_bytes, void* stream);
+
+/* ---- the dataset generator's warp (gen_synthetic_data.py:63-64), bit-identical to the reference's NumPy ------------------
+ * udh_gen_warp_u8: bgr [n,h,w,3] uint8 (cv2's channel order), theta [n,9] float64 (row-major inv(M) inv(H_inverse) M on the
+ *   [-1,1] grid) -> gray [n,h,w] = cv2.cvtColor(bgr, COLOR_RGB2GRAY), warped [n,h,w,3] = numpy_transformer(bgr, H_inverse)
+ *   per channel, warped_gray [n,h,w] = numpy_transformer(gray, H_inverse): float64 throughout, astype(uint8) on the result.
+ *   n <= 65535. */
+int udh_gen_warp_u8(const uint8_t* bgr, const double* theta, int n, int h, int w, uint8_t* gray, uint8_t* warped,
+                    uint8_t* warped_gray, void* stream);
 
 /* ---- instrumentation read by bench.py -------------------------------------------------------------------------
  * udh_launch_count: kernels this library has launched in this process (monotonic).

@@ -126,6 +126,7 @@ SIGNATURES = {
     "udh_ecc_h4p": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "udh_ecc_corr_h4p": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "udh_resize_area_up_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "udh_resize_linear_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "udh_real_prep_smem_bytes": (c_size_t, [c_int, c_int]),
     "udh_real_prep": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                               c_void_p, c_void_p, c_void_p]),
@@ -135,6 +136,11 @@ SIGNATURES = {
     "udh_jpeg_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "udh_jpeg_decode": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "udh_debug_jpeg_set_lanes": (c_int, [c_int]),
+    "udh_jpeg_encode_capacity": (c_int64, [c_int, c_int, c_int]),
+    "udh_jpeg_encode_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "udh_jpeg_encode": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p, c_void_p,
+                                c_size_t, c_void_p]),
+    "udh_gen_warp_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "udh_launch_count": (c_ulonglong, []),
     "udh_set_sm_reserve": (c_int, [c_int]),
     "udh_set_sm_reserve_top": (c_int, [c_int]),

@@ -1,7 +1,8 @@
 // Real-data input pipeline (code/dataloader.py:146-200) and the real-data direct-method metric
 // (code/homography_conventional_real.py:213-246), bit-identical to the host arithmetic they replace.
 //   resize_up_u8_kernel      cv2.resize(uint8, INTER_AREA) to a larger size: linear interpolation with area coefficients,
-//                            11-bit fixed point, VResizeLinearVec_32s8u's rounding.  Integer arithmetic: exact.
+//                            11-bit fixed point, VResizeLinearVec_32s8u's rounding.  Integer arithmetic: exact.  With
+//                            INTER_LINEAR's table (udh_resize_linear_u8) it is cv2.resize(uint8, INTER_LINEAR), up or down.
 //   real_prep_kernel         full-size uint8 I, I' -> the four network-size fp32 images of the loader (plain and augmented,
 //                            normalised, INTER_AREA-downscaled).  Augment + normalise is a per-value table built on the host;
 //                            the downscale is OpenCV's generic resizeArea in its summation order, each step rounded (no FMA).
@@ -13,7 +14,10 @@
 namespace udh {
 
 // ---- uint8 upscale -------------------------------------------------------------------------------------------------------
-// tab (int32): xsrc[dw], xa0[dw], xa1[dw], ysrc[dh], ya0[dh], ya1[dh]; one thread per output pixel (3 channels)
+// tab (int32): xsrc[dw], xa0[dw], xa1[dw], ysrc[dh], ya0[dh], ya1[dh]; one thread per output pixel (3 channels).
+// ROW_PAIR: a further ysrc1[dh] gives the second source row.  INTER_LINEAR keeps the vertical coefficients at the borders
+// and clamps both rows (rows -1 and 0 at the top are row 0 twice), which "the row after ysrc" cannot express.
+template <bool ROW_PAIR>
 __global__ void __launch_bounds__(256) resize_up_u8_kernel(const uint8_t* __restrict__ src, const int32_t* __restrict__ tab,
                                                            uint8_t* __restrict__ dst, int sh, int sw, int dh, int dw) {
   const int n = blockIdx.y;
@@ -22,7 +26,7 @@ __global__ void __launch_bounds__(256) resize_up_u8_kernel(const uint8_t* __rest
   const int dy = o / dw, dx = o - dy * dw;
   const int32_t *xs = tab, *xa0 = tab + dw, *xa1 = tab + 2 * dw;
   const int32_t *ys = tab + 3 * dw, *ya0 = ys + dh, *ya1 = ys + 2 * dh;
-  const int sx = xs[dx], nx = min(sx + 1, sw - 1), sy = ys[dy], ny = min(sy + 1, sh - 1);
+  const int sx = xs[dx], nx = min(sx + 1, sw - 1), sy = ys[dy], ny = ROW_PAIR ? ys[3 * dh + dy] : min(sy + 1, sh - 1);
   const int a0 = xa0[dx], a1 = xa1[dx], b0 = ya0[dy], b1 = ya1[dy];
   const uint8_t* r0 = src + ((size_t)n * sh + sy) * sw * 3;
   const uint8_t* r1 = src + ((size_t)n * sh + ny) * sw * 3;
@@ -179,8 +183,20 @@ extern "C" int udh_resize_area_up_u8(const uint8_t* src, const int32_t* tab, uin
   if (n == 0) return UDH_OK;
   cudaStream_t st = as_stream(stream);
   ProfScope ps(PROF_ELTWISE, st);
-  resize_up_u8_kernel<<<dim3((dst_h * dst_w + 255) / 256, n), 256, 0, st>>>(src, tab, dst, src_h, src_w, dst_h, dst_w);
+  resize_up_u8_kernel<false><<<dim3((dst_h * dst_w + 255) / 256, n), 256, 0, st>>>(src, tab, dst, src_h, src_w, dst_h, dst_w);
   return check_launch("udh_resize_area_up_u8");
+}
+
+extern "C" int udh_resize_linear_u8(const uint8_t* src, const int32_t* tab, uint8_t* dst, int n, int src_h, int src_w, int dst_h,
+                                    int dst_w, void* stream) {
+  UDH_REQUIRE(src && tab && dst, "udh_resize_linear_u8: null pointer");
+  UDH_REQUIRE(n >= 0 && src_h >= 1 && src_w >= 1 && dst_h >= 1 && dst_w >= 1 && (int64_t)dst_h * dst_w < INT32_MAX,
+              "udh_resize_linear_u8: bad dimensions");
+  if (n == 0) return UDH_OK;
+  cudaStream_t st = as_stream(stream);
+  ProfScope ps(PROF_ELTWISE, st);
+  resize_up_u8_kernel<true><<<dim3((dst_h * dst_w + 255) / 256, n), 256, 0, st>>>(src, tab, dst, src_h, src_w, dst_h, dst_w);
+  return check_launch("udh_resize_linear_u8");
 }
 
 extern "C" size_t udh_real_prep_smem_bytes(int max_rows, int full_w) {

@@ -312,6 +312,43 @@ def resize_area_up_u8(src, dst_h, dst_w):
     return out
 
 
+@functools.lru_cache(maxsize=32)
+def linear_table(src_h, src_w, dst_h, dst_w):
+    """udh_resize_linear_u8's table (int32): xsrc, xa0, xa1, ysrc, ya0, ya1, ysrc1 — OpenCV's INTER_LINEAR tables:
+    f = (float)((d + 0.5) * scale - 0.5), s = floor(f), f -= s in float, coefficients cvRound((1 - f) * 2048) and
+    cvRound(f * 2048) in float.  Columns: s < 0 takes (0, f = 0) and s >= size - 1 takes (size - 1, f = 0).  Rows keep
+    their coefficients; the two source rows s and s + 1 are clamped to the image instead."""
+    def axis(ssize, dsize, rows):
+        scale = 1.0 / (float(dsize) / float(ssize))
+        f = ((np.arange(dsize, dtype=np.float64) + 0.5) * scale - 0.5).astype(np.float32)
+        s = np.floor(f).astype(np.int64)
+        f = (f - s.astype(np.float32)).astype(np.float32)
+        if rows:
+            s0, s1 = np.clip(s, 0, ssize - 1), np.clip(s + 1, 0, ssize - 1)
+        else:
+            lo, hi = s < 0, s >= ssize - 1
+            f[lo | hi] = 0
+            s0 = np.clip(s, 0, ssize - 1)
+        out = [s0, np.rint((np.float32(1) - f) * np.float32(2048)), np.rint(f * np.float32(2048))]
+        return out + [s1] if rows else out
+    if min(src_h, src_w, dst_h, dst_w) < 1:
+        raise _lib.UdhError("linear_table: sizes must be >= 1 (got %dx%d -> %dx%d)" % (src_h, src_w, dst_h, dst_w))
+    return np.concatenate([np.asarray(a, np.float64) for a in axis(src_w, dst_w, False) + axis(src_h, dst_h, True)]).astype(np.int32)
+
+
+def resize_linear_u8(src, dst_h, dst_w):
+    """uint8 [N,h,w,3] CUDA tensor -> [N,dst_h,dst_w,3]: cv2.resize(img, (dst_w, dst_h)) (INTER_LINEAR) per image, bit
+    for bit, downscales and upscales.  One launch per source size."""
+    _req(src, torch.uint8, "src")
+    if src.dim() != 4 or src.shape[3] != 3:
+        raise _lib.UdhError("resize_linear_u8: src must be [N,h,w,3] (got %s)" % (tuple(src.shape),))
+    n, h, w, _ = src.shape
+    tab = torch.from_numpy(linear_table(h, w, dst_h, dst_w)).to(src.device)
+    out = torch.empty(n, dst_h, dst_w, 3, device=src.device, dtype=torch.uint8)
+    check(lib.udh_resize_linear_u8(_ptr(src), _ptr(tab), _ptr(out), n, h, w, dst_h, dst_w, _stream()), "udh_resize_linear_u8")
+    return out
+
+
 def real_prep(I_u8, Ip_u8, luts, img_h, img_w):
     """Full-size uint8 I, I' [B,FH,FW,3] and per-sample value tables luts [B,4,256,3] fp32 (plain I, plain I', augmented I,
     augmented I') -> (I, I_prime, I_aug, I_prime_aug) [B,img_h,img_w,3] fp32: table lookup, then cv2's INTER_AREA
@@ -380,6 +417,64 @@ def decode_jpeg(blobs, h, w):
     if len(bad):
         raise _lib.UdhError("decode_jpeg: image %d failed with status %d (%d of %d images failed)" % (bad[0], st[bad[0]], len(bad), len(st)))
     return out, status
+
+
+# ------------------------------------------------------------------ baseline-JPEG encode
+def encode_jpeg_device(imgs, quality=95):
+    """uint8 CUDA tensor [N,h,w,3] (BGR) or [N,h,w] (gray) -> (out uint8 [N,cap], nbytes int64 [N], status int32 [N]) on the
+    current stream: image k's file is out[k, :nbytes[k]]; nonzero status = that image failed."""
+    _req(imgs, torch.uint8, "imgs")
+    if imgs.dim() not in (3, 4) or (imgs.dim() == 4 and imgs.shape[3] != 3):
+        raise _lib.UdhError("encode_jpeg: images must be [N,h,w,3] BGR or [N,h,w] gray (got %s)" % (tuple(imgs.shape),))
+    n, h, w = imgs.shape[:3]
+    ch = 3 if imgs.dim() == 4 else 1
+    cap = lib.udh_jpeg_encode_capacity(h, w, ch)
+    nb = lib.udh_jpeg_encode_workspace_bytes(max(n, 1), h, w, ch)
+    if cap == 0 or nb == 0:
+        raise _lib.UdhError("encode_jpeg: unsupported size %dx%d" % (h, w))
+    out = torch.empty(n, cap, device=imgs.device, dtype=torch.uint8)
+    nbytes = torch.empty(n, device=imgs.device, dtype=torch.int64)
+    status = torch.empty(n, device=imgs.device, dtype=torch.int32)
+    if n == 0:
+        return out, nbytes, status
+    ws = torch.empty(nb, device=imgs.device, dtype=torch.uint8)
+    check(lib.udh_jpeg_encode(_ptr(imgs), n, h, w, ch, int(quality), _ptr(out), cap, _ptr(nbytes), _ptr(status), _ptr(ws), nb,
+                              _stream()), "udh_jpeg_encode")
+    return out, nbytes, status
+
+
+def encode_jpeg(imgs, quality=95):
+    """uint8 images [N,h,w,3] in cv2's BGR order or [N,h,w] gray (CUDA tensor, or anything torch.as_tensor takes) -> one
+    JPEG file (bytes) per image, each byte-identical to cv2.imencode('.jpg', img, [cv2.IMWRITE_JPEG_QUALITY, quality]).
+    Raises UdhError naming the first image that could not be encoded."""
+    _lib.require_device()
+    t = torch.as_tensor(imgs)
+    if not t.is_cuda:
+        t = t.cuda()
+    out, nbytes, status = encode_jpeg_device(t.contiguous(), quality)
+    st = status.cpu().numpy()
+    bad = np.flatnonzero(st)
+    if len(bad):
+        raise _lib.UdhError("encode_jpeg: image %d failed with status %d (%d of %d images failed)" % (bad[0], st[bad[0]], len(bad), len(st)))
+    nb = nbytes.cpu().numpy()
+    buf = out[:, :int(nb.max())].cpu().numpy() if len(nb) else None
+    return [buf[k, :nb[k]].tobytes() for k in range(len(nb))]
+
+
+# ------------------------------------------------------------------ the dataset generator's warp
+def gen_warp_u8(bgr, theta):
+    """uint8 [N,h,w,3] CUDA tensor in cv2's BGR order, float64 theta [N,3,3] (CUDA, the generator's
+    inv(M) inv(H_inverse) M) -> (gray [N,h,w], warped [N,h,w,3], warped_gray [N,h,w]): cv2.cvtColor(bgr, COLOR_RGB2GRAY) and
+    the reference's numpy_transformer of the colour image and of the gray image, bit for bit."""
+    _req(bgr, torch.uint8, "bgr"); _req(theta, torch.float64, "theta")
+    if bgr.dim() != 4 or bgr.shape[3] != 3 or tuple(theta.shape) != (bgr.shape[0], 3, 3):
+        raise _lib.UdhError("gen_warp_u8: bgr must be [N,h,w,3] and theta [N,3,3] (got %s and %s)" % (tuple(bgr.shape), tuple(theta.shape)))
+    n, h, w, _ = bgr.shape
+    gray = torch.empty(n, h, w, device=bgr.device, dtype=torch.uint8)
+    warped = torch.empty_like(bgr)
+    warped_gray = torch.empty_like(gray)
+    check(lib.udh_gen_warp_u8(_ptr(bgr), _ptr(theta), n, h, w, _ptr(gray), _ptr(warped), _ptr(warped_gray), _stream()), "udh_gen_warp_u8")
+    return gray, warped, warped_gray
 
 
 # ------------------------------------------------------------------ Adam
