@@ -80,8 +80,11 @@ __device__ __forceinline__ void sample_setup(const Homog& hm, float xt, float yt
 }
 
 // ((wa*Ia + wb*Ib) + wc*Ic) + wd*Id with every product and sum rounded separately — the reference evaluates
-// four tf.multiply and one add_n (tf_spatial_transformer.py:134-138), and the "black border" of out-of-range
-// samples relies on wa*Ia == -(wc*Ic) cancelling exactly; a fused multiply-add would leave ulp(w*I) residues.
+// four tf.multiply and one add_n (tf_spatial_transformer.py:134-138).  The "black border" cancels exactly only when y
+// clips (alone or with x): then Ia == Ib, Ic == Id, wb == -wa and wd == -wc, so wa*Ia + wb*Ib == 0 and the sum is
+// exactly 0.  Where only x clips, wa*Ia == -(wc*Ic) and wb*Ib == -(wd*Id), but fl(wa*Ia + wb*Ib) - wa*Ia need not
+// equal wb*Ib, so a residue of the blend's rounding, ulp(w*I), can remain (tests/test_gpu_photometric.py bounds it).  A fused multiply-add would leave
+// such residues everywhere.
 __device__ __forceinline__ float bilinear_rn(const Tap& t, float Ia, float Ib, float Ic, float Id) {
   return __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(t.wa, Ia), __fmul_rn(t.wb, Ib)), __fmul_rn(t.wc, Ic)), __fmul_rn(t.wd, Id));
 }

@@ -252,6 +252,7 @@ class HomographyEngine(object):
             dH = ops.warp_loss_backward(batch["I_aug"], out["H_mat"], batch["I2_aug"], batch.get("patch_indices"), self.Pz,
                                         self.Pz, _PHOTO_BWD[lt], out["_sums"], 1.0, dpred=dpm)
             dpred = ops.dlt_backward(batch["pts1"], out["pred_h4p"], out["H_mat"], dH)
+            out["_dH"] = dH
         else:
             raise _lib.UdhError("unknown loss_type %s" % lt)
         out["_dh4p"] = dpred
