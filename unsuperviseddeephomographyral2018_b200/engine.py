@@ -33,6 +33,15 @@ def learning_rate(step, lr, min_lr, num_total_steps=150000, decay_rate=0.96):
     return lr * decay_rate ** (step // decay_steps(lr, min_lr, num_total_steps, decay_rate))
 
 
+def adam_alpha(global_step, lr, min_lr):
+    """(lr_t, alpha_t) of the update that takes global_step to global_step + 1, t = global_step + 1.  Evaluated in float64
+    with exact powers of beta; the kernel receives alpha_t as float32.  TF forms the same quantity in float32 from its
+    running beta-power variables: the two alpha_t differ by at most 1.4e-5 relative (DESIGN section 2)."""
+    t = global_step + 1
+    lr_t = learning_rate(global_step, lr, min_lr)
+    return lr_t, lr_t * math.sqrt(1.0 - 0.999 ** t) / (1.0 - 0.9 ** t)
+
+
 def dp_slices(specs):
     """Row G (utils/utils.py:380-403) as two slices of the flat gradient buffer: (head, convs).  `head` = fc1 w/b + fc2 w/b
     (98 % of the bytes, complete after the head phase of the backward, reduced under the conv backward); `convs` = the eight
@@ -377,9 +386,7 @@ class HomographyEngine(object):
                                     1.0 / self.world_size, 1, ops._stream()), "udh_adam_step")
 
     def _alpha(self):
-        t = self.global_step + 1
-        lr_t = learning_rate(self.global_step, self.lr, self.min_lr)
-        return lr_t, lr_t * math.sqrt(1.0 - 0.999 ** t) / (1.0 - 0.9 ** t)
+        return adam_alpha(self.global_step, self.lr, self.min_lr)
 
     def update(self):
         self.sync_optimizer_state()          # no-op unless sharded steps (train_step on the multicast path) came before
