@@ -8,7 +8,10 @@
     those points on the full-size images, bounded by the identity error (:578-612; real_metrics.correspondence_errors).
 Images are 142 x 190 at the network (AREA-resized from 240 x 320 "full" images), patches 128 x 128, RHO = 24 (:17-23).
 The arithmetic runs in libudh's sm_90a kernels exactly as for the synthetic path (same engine, one process per GPU).
-The classical baselines (RANSAC / direct, --do_report) and the visualisations are out of scope (DESIGN.md §8).
+The classical baselines (RANSAC / direct, --do_report) and --visual (matplotlib windows) are out of scope (DESIGN.md §8).
+--mode test --save_visual True (the default) writes the reference's report image of every test sample to results_dir,
+named <k>_Unsupervised__loss_<h_loss>.jpg with k global over the ranks, drawn and encoded on the device byte-identical
+to cv2 (report.py); the reference's scratch copy /tmp/tmp.jpg is not written.
 
 New flags: --synthetic N (on-device stand-in pairs at the real-data geometry: the aerial set is private), --seed,
 --numeric {bf16x3,bf16,fp32}, --max_iterations is the reference's own flag.
@@ -60,7 +63,8 @@ def build_parser():
     p.add_argument('--filenames_file', type=str, default=None)
     p.add_argument('--test_filenames_file', type=str, default=None)
     p.add_argument('--visual', type=s2b, default='false')
-    p.add_argument('--save_visual', type=s2b, default='True')
+    p.add_argument('--save_visual', type=s2b, default='True',
+                   help='--mode test: write every sample\'s report image (JPEG, as the reference\'s) to results_dir')
     p.add_argument('--do_report', type=s2b, default='False')
     p.add_argument('--img_w', type=int, default=WIDTH)
     p.add_argument('--img_h', type=int, default=HEIGHT)
@@ -173,7 +177,7 @@ def train(args):
 
 def test_homography(args):
     import torch
-    from unsuperviseddeephomographyral2018_b200 import dataloader as dl, engine as en, real_metrics as rm
+    from unsuperviseddeephomographyral2018_b200 import dataloader as dl, engine as en, real_metrics as rm, report
     rank, world, local, pg = syn.setup(args)
     if rank == 0:
         for d in (args.log_dir, args.results_dir):
@@ -199,12 +203,20 @@ def test_homography(args):
         out = eng.eval_step(b)
         d = eng.losses_dict(out)
         rec += d["rec_loss"]; l1 += d["l1_loss"]
-        for h, ident, failed in rm.correspondence_errors(out["pred_h4p"].cpu().numpy(), b["pts1"].cpu().numpy(), b["gt_corr"],
-                                                         full_img_h=args.full_img_h, img_h=args.img_h):
+        errs = rm.correspondence_errors(out["pred_h4p"].cpu().numpy(), b["pts1"].cpu().numpy(), b["gt_corr"],
+                                        full_img_h=args.full_img_h, img_h=args.img_h, with_points=True)
+        for h, ident, failed, _ in errs:
             if failed:
                 print("===> Found error > %.3f = RMSE_identity" % ident)
                 fails += 1
             h_losses.append(h)
+        if args.save_visual:
+            # :614-619: every sample, the full-size I on the left, the clicked points and their predicted matches; each
+            # rank writes its own samples under their global index
+            corr1, corr2 = report.clicked_points(b["gt_corr"])
+            n = len(errs)
+            names = [report.real_cnn_name(report.global_index(rank, per_gpu, step, args.batch_size, i), errs[i][0]) for i in range(n)]
+            report.write(report.render(b, range(n), corr1, corr2, [e[3] for e in errs], prime_left=False), names, args.results_dir)
         if rank == 0:
             syn.progress('Test, h_loss %4.3f, rec_loss %4.3f, l1_loss %4.3f, fail_percent %4.4f'
                          % (float(np.mean(h_losses)), rec / (step + 1), l1 / (step + 1), fails / (step + 1) / per_gpu))

@@ -6,6 +6,10 @@ sm_90a CUDA kernels, one process per GPU (torchrun) with one NCCL gradient allre
 New flags: --synthetic N (generate N pairs on the device instead of reading <data_path>/I, I_prime — MS-COCO is not
 available offline), --seed, --numeric {bf16x3,bf16,fp32} (default bf16x3: the parity-certified tensor-core mode),
 --num_total_steps (the reference hard-codes 150000, :161).
+
+--mode test --save_visual True (the default) writes the reference's report image of each batch's sample 0 to
+results_dir, drawn and encoded on the device byte-identical to cv2 (report.py); the reference's scratch copy
+/tmp/tmp.jpg is not written.  --visual (matplotlib windows) is accepted and does nothing.
 """
 from __future__ import absolute_import, division, print_function
 
@@ -56,7 +60,8 @@ def build_parser():
     p.add_argument('--filenames_file', type=str, default=None)
     p.add_argument('--test_filenames_file', type=str, default=None)
     p.add_argument('--visual', type=str2bool, default='false')
-    p.add_argument('--save_visual', type=str2bool, default='True')
+    p.add_argument('--save_visual', type=str2bool, default='True',
+                   help='--mode test: write each batch\'s sample-0 report image (JPEG, as the reference\'s) to results_dir')
     p.add_argument('--img_w', type=int, default=WIDTH)
     p.add_argument('--img_h', type=int, default=HEIGHT)
     p.add_argument('--patch_size', type=int, default=PATCH_SIZE)
@@ -188,7 +193,7 @@ def progress(msg):
 
 def train(args):
     import torch
-    from unsuperviseddeephomographyral2018_b200 import dataloader as dl, engine as en
+    from unsuperviseddeephomographyral2018_b200 import dataloader as dl, engine as en, report
     rank, world, local, pg = setup(args)
     make_dirs(args, rank)
     per_gpu = int(args.batch_size / world)                               # :219 batch_size / num_gpus per tower
@@ -269,7 +274,7 @@ def find_percentile(values):
 
 def test_homography(args):
     import torch
-    from unsuperviseddeephomographyral2018_b200 import dataloader as dl, engine as en
+    from unsuperviseddeephomographyral2018_b200 import dataloader as dl, engine as en, report
     rank, world, local, pg = setup(args)
     make_dirs(args, rank)
     num_data = args.synthetic if args.synthetic else dl.count_text_lines(args.test_filenames_file)
@@ -295,7 +300,8 @@ def test_homography(args):
     h_losses_array = []
     step = 0
     for step in range(steps):
-        out = eng.eval_step(loader.next_batch())
+        b = loader.next_batch()
+        out = eng.eval_step(b)
         d = eng.losses_dict(out)
         vals = torch.tensor([d["bounded_h_loss"], d["rec_loss"], d["ssim_loss"], d["l1_loss"], d["num_fail"]], device="cuda", dtype=torch.float64)
         if world > 1:
@@ -303,6 +309,11 @@ def test_homography(args):
         h, rec, ssim, l1, fail = vals.tolist()
         tot["h"] += h; tot["rec"] += rec; tot["ssim"] += ssim; tot["l1"] += l1; tot["fail"] += fail
         h_losses_array.append(h)
+        if args.save_visual and rank == 0:
+            # :539-552: sample 0 of the batch, I' on the left, named after the batch's h_loss
+            pts = report.synthetic_points(b["pts1"][:1].cpu().numpy(), b["gt"][:1].cpu().numpy(), out["pred_h4p"][:1].cpu().numpy())
+            report.write(report.render(b, [0], *pts, prime_left=True), [report.synthetic_name(step, args.batch_size, args.loss_type, h)],
+                         args.results_dir)
         if step % 10 == 0 and rank == 0:
             print('===> This iteration num Fail: %d \n' % fail)
             progress('Test, h_loss %4.3f, rec_loss %4.3f, ssim_loss %4.3f, l1_loss %4.3f, fail_percent %4.4f'

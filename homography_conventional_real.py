@@ -9,8 +9,10 @@ loader reads and prepares the batch on the device.  --method identity predicts W
 (udh_ecc_corr_h4p) follows the reference: the clicked points are halved onto the full-size images, mapped through W (not
 inverted), clamped to +-80 px and scored by their RMSE; a sample fails when ECC raised (1) or when the identity does
 better (2, scored with the identity error).  SIFT and ORB (feature matching + RANSAC) are not built and exit with an
-error, as does --mode train.  --visual, --save_visual and --artifact_mode noise are accepted and do nothing: no images are
-drawn or written.  The running time is the batch's GPU time (CUDA events around input preparation, ECC and the metric)
+error, as does --mode train.  --save_visual True (the default) writes the reference's report image of every pair to
+results_dir as <k>_loss_<h_loss>.jpg: the full-size images, the clicked points and pred_h4p + corr1 with the clamped
+pred_h4p, drawn and encoded on the device byte-identical to cv2 (report.py); the reference's scratch copy tmp.jpg is not
+written.  --visual and --artifact_mode noise are accepted and do nothing.  The running time is the batch's GPU time (CUDA events around input preparation, ECC and the metric)
 divided by the batch size: a batched figure, not one pair at a time.
 
 New flags: --synthetic N (N full-size pairs generated on the device instead of reading <data_path>, with four
@@ -60,7 +62,7 @@ def build_parser():
     p.add_argument('--filenames_file', type=str, default=os.path.join(d, 'train_real.txt'))
     p.add_argument('--test_filenames_file', type=str, default=None)
     p.add_argument('--visual', type=str2bool, default='false', help='Visualize obtained images to debug (not built)')
-    p.add_argument('--save_visual', type=str2bool, default='True', help='Save images for report (not built)')
+    p.add_argument('--save_visual', type=str2bool, default='True', help='Save images for report')
     p.add_argument('--artifact_mode', type=str, default='None', help='Add aftifacts to the images (not built)', choices=['noise', 'None'])
     p.add_argument('--img_w', type=int, default=WIDTH)
     p.add_argument('--img_h', type=int, default=HEIGHT)
@@ -131,7 +133,8 @@ def write_results_txt(args, line):
 
 
 def run_batch(method, batch, num_iterations):
-    """-> (h_loss [B] float64, fail [B] int, GPU seconds) for one extended Dataloader batch."""
+    """-> (h_loss [B] float64, fail [B] int, GPU seconds, pred_h4p [B,8] float32 clamped to +-80) for one extended
+    Dataloader batch."""
     import torch
     from unsuperviseddeephomographyral2018_b200 import ops
     gt = torch.from_numpy(np.ascontiguousarray(batch["gt_corr"], np.float32)).cuda()
@@ -144,10 +147,10 @@ def run_batch(method, batch, num_iterations):
         B = gt.shape[0]
         W = torch.eye(3, device=gt.device).repeat(B, 1, 1).contiguous()
         status = torch.zeros(B, device=gt.device, dtype=torch.int32)
-    _, h, fail = ops.ecc_corr_h4p(W, status, gt)
+    pred, h, fail = ops.ecc_corr_h4p(W, status, gt)
     e1.record()
     torch.cuda.synchronize()
-    return h.cpu().numpy(), fail.cpu().numpy(), e0.elapsed_time(e1) * 1e-3
+    return h.cpu().numpy(), fail.cpu().numpy(), e0.elapsed_time(e1) * 1e-3, pred.cpu().numpy()
 
 
 def make_loader(args, batch_size):
@@ -165,7 +168,7 @@ def make_loader(args, batch_size):
 
 def test(args):
     from unsuperviseddeephomographyral2018_b200 import _lib
-    from unsuperviseddeephomographyral2018_b200 import dataloader as dl
+    from unsuperviseddeephomographyral2018_b200 import dataloader as dl, report
     _lib.require_device()
     print('Save mean, std values to ', args.log_dir)
     print('Save images to', args.results_dir)
@@ -181,7 +184,7 @@ def test(args):
     h_losses, num_fail, total_time, num_samples = [], 0, 0.0, 0
     for step in range(steps):
         b = loader.next_batch()
-        h, f, secs = run_batch(args.method, b, args.num_iterations)
+        h, f, secs, pred = run_batch(args.method, b, args.num_iterations)
         total_time += secs
         for i in range(len(h)):
             num_samples += 1
@@ -191,6 +194,12 @@ def test(args):
                 print('===> Fail case 2:  error > identity')
             num_fail += int(f[i] != 0)
             h_losses.append(float(h[i]))
+        if args.save_visual:
+            # :250-267: the same drawing inline, pred_corr2 = pred_h4p + corr1 (h_loss after the failure substitution)
+            corr1, corr2 = report.clicked_points(b["gt_corr"])
+            names = [report.conventional_name(step * args.batch_size + i, float(h[i])) for i in range(len(h))]
+            report.write(report.render(b, range(len(h)), corr1, corr2, pred.reshape(-1, 4, 2) + corr1, prime_left=False), names,
+                         args.results_dir)
         print(' Test| image %d, h_loss %.3f, h_loss_average %.3f, fail %d/%d, time %.4f (batched)'
               % (num_samples - 1, h_losses[-1], np.mean(h_losses), num_fail, num_samples, secs / len(h)), flush=True)
     line = summarise(h_losses, num_fail, total_time, num_samples)

@@ -245,6 +245,16 @@ int udh_prep_inputs_u8_ex(const uint8_t* I, const uint8_t* I_prime, const float*
 int udh_synth_scene_u8(uint8_t* I, float* pts1, float* gt, int B, int img_h, int img_w, int P, int rho, uint64_t seed, void* stream);
 int udh_warp_image_u8(const uint8_t* U, const float* H, uint8_t* out, int B, int img_h, int img_w, void* stream);
 
+/* ---- report image of the test harnesses (utils/utils.py:209-307, save_correspondences_img) -----------------------------
+ * udh_draw_report_u8: out [B,img_h,2*img_w,3] = [left | right], left = denorm(I') and right = denorm(I) when prime_left,
+ *   else the other way round (denorm as in udh_ecc_prep_u8, aug nullable), with cv2's drawing on it byte for byte:
+ *   verts [B,20,2] int32 = the prediction polygon (right-image coordinates, drawn on the right image alone), kp2 and kp1
+ *   (thick-3 closed polylines, colour (2,10,240)), and 4 match lines start -> end (LINE_AA, each end circled, r = 7).
+ *   Any int32 vertex is accepted; nothing outside the canvas is touched.  workspace: udh_draw_report_workspace_bytes. */
+size_t udh_draw_report_workspace_bytes(int B);
+int udh_draw_report_u8(const uint8_t* I, const uint8_t* I_prime, const float* aug, int prime_left, const int32_t* verts, uint8_t* out,
+                       void* ws, size_t ws_bytes, int B, int img_h, int img_w, void* stream);
+
 /* ---- direct-method baseline: cv2.findTransformECC, MOTION_HOMOGRAPHY (utils/direct_homography.py:8-57) ----------------
  * as homography_conventional_synthetic.py:186-223 runs it on the test set, batched.  Images are uint8 planes
  * [B,img_h,img_w]; W [B,9] row-major fp32 maps template pixels into the input image (WARP_INVERSE_MAP).

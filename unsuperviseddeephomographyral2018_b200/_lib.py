@@ -141,6 +141,9 @@ SIGNATURES = {
     "udh_jpeg_encode": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p, c_void_p,
                                 c_size_t, c_void_p]),
     "udh_gen_warp_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "udh_draw_report_workspace_bytes": (c_size_t, [c_int]),
+    "udh_draw_report_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_int, c_int, c_int,
+                                   c_void_p]),
     "udh_launch_count": (c_ulonglong, []),
     "udh_set_sm_reserve": (c_int, [c_int]),
     "udh_set_sm_reserve_top": (c_int, [c_int]),

@@ -113,6 +113,30 @@ inline void launch_chain(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t s
   cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);     // errors surface through check_launch()
 }
 
+// ---- the uint8 image the reference hands to cv2 ------------------------------------------------------------------------
+// denorm_img(normalised augmented image).astype(uint8) of one uint8 value x of channel c (utils/utils.py:406-413), with
+// a = the image's 5 augmentation parameters of udh_prep_inputs_u8_ex (gamma, brightness, 3 colour gains) or null.
+// gamma: pow in fp64 rounded once to fp32 (a correctly rounded powf, reproducible on the host); the rest is the fp32
+// arithmetic of udh_prep_inputs_u8_ex.  denorm_img multiplies the fp32 value by a float64 std and adds a float64 mean in
+// two roundings (no FMA), and astype(uint8) truncates.  Callers tabulate it per (sample, image, channel).
+__device__ __forceinline__ uint8_t denorm_u8(int x, int c, const float* a) {
+  const float mean = c == 0 ? 118.93f : (c == 1 ? 113.97f : 102.60f);
+  const float sd = c == 0 ? 69.85f : (c == 1 ? 68.81f : 72.45f);
+  const double mean64 = c == 0 ? 118.93 : (c == 1 ? 113.97 : 102.60);    // float64 numpy arrays
+  const double sd64 = c == 0 ? 69.85 : (c == 1 ? 68.81 : 72.45);
+  float v = (float)x;
+  if (a) {
+    v = (float)pow((double)v, (double)a[0]);
+    v = __fmul_rn(v, a[1]);
+    v = __fmul_rn(v, a[2 + c]);
+    v = fminf(fmaxf(v, 0.0f), 255.0f);
+  }
+  const float n = __fdiv_rn(__fsub_rn(v, mean), sd);
+  const double d = __dadd_rn(__dmul_rn((double)n, sd64), mean64);
+  const int t = (int)d;                                                  // truncation toward zero
+  return (uint8_t)(t < 0 ? 0 : (t > 255 ? 255 : t));
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

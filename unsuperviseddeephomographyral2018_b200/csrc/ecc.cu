@@ -14,16 +14,8 @@
 
 namespace udh {
 
-__constant__ float kEccMean[3] = {118.93f, 113.97f, 102.60f};
-__constant__ float kEccStd[3] = {69.85f, 68.81f, 72.45f};
-__constant__ double kEccMean64[3] = {118.93, 113.97, 102.60};      // utils/utils.py:406-413 (float64 numpy arrays)
-__constant__ double kEccStd64[3] = {69.85, 68.81, 72.45};
-
 // ---- input preparation ------------------------------------------------------------------------------------------------
-// Every step is a function of one uint8 value per (sample, image, channel), so it is tabulated once per CTA.
-// gamma: pow in fp64 rounded once to fp32 (a correctly rounded powf, reproducible on the host); the rest is the fp32
-// arithmetic of udh_prep_inputs_u8_ex.  denorm_img multiplies the fp32 value by a float64 std and adds a float64 mean in
-// two roundings (no FMA), and astype(uint8) truncates.
+// Every step is a function of one uint8 value per (sample, image, channel), so it is tabulated once per CTA (denorm_u8).
 __global__ void __launch_bounds__(256) ecc_prep_kernel(const uint8_t* __restrict__ I, const uint8_t* __restrict__ Ip,
                                                        const float* __restrict__ aug, uint8_t* __restrict__ gI,
                                                        uint8_t* __restrict__ gIp, int npx) {
@@ -32,18 +24,7 @@ __global__ void __launch_bounds__(256) ecc_prep_kernel(const uint8_t* __restrict
   const bool on = aug && aug[b * 11] != 0.0f;
   for (int i = threadIdx.x; i < 2 * 3 * 256; i += blockDim.x) {
     const int im = i / 768, c = (i / 256) % 3, x = i & 255;
-    float v = (float)x;
-    if (on) {
-      const float* a = aug + b * 11 + 1 + im * 5;
-      v = (float)pow((double)v, (double)a[0]);
-      v = __fmul_rn(v, a[1]);
-      v = __fmul_rn(v, a[2 + c]);
-      v = fminf(fmaxf(v, 0.0f), 255.0f);
-    }
-    const float n = __fdiv_rn(__fsub_rn(v, kEccMean[c]), kEccStd[c]);
-    const double d = __dadd_rn(__dmul_rn((double)n, kEccStd64[c]), kEccMean64[c]);
-    const int t = (int)d;                                                  // truncation toward zero
-    lut[im][c][x] = (uint8_t)(t < 0 ? 0 : (t > 255 ? 255 : t));
+    lut[im][c][x] = denorm_u8(x, c, on ? aug + b * 11 + 1 + im * 5 : nullptr);
   }
   __syncthreads();
   for (int o = blockIdx.x * blockDim.x + threadIdx.x; o < npx; o += gridDim.x * blockDim.x) {

@@ -461,6 +461,28 @@ def encode_jpeg(imgs, quality=95):
     return [buf[k, :nb[k]].tobytes() for k in range(len(nb))]
 
 
+# ------------------------------------------------------------------ report image of the test harnesses
+def draw_report_u8(I_u8, Ip_u8, aug, verts, prime_left):
+    """Decoded I, I' [B,h,w,3] uint8 (+ the [B,11] augmentation table or None) and the report's int32 vertices verts
+    [B,20,2] (report.report_vertices) -> the report canvases [B,h,2w,3] uint8 as cv2 draws them: denorm(I') | denorm(I)
+    when prime_left, else denorm(I) | denorm(I')."""
+    _req(I_u8, torch.uint8, "I"); _req(Ip_u8, torch.uint8, "I_prime"); _req(verts, torch.int32, "verts")
+    if aug is not None:
+        _req(aug, torch.float32, "aug")
+    if I_u8.dim() != 4 or I_u8.shape[3] != 3:
+        raise _lib.UdhError("draw_report_u8: I must be [B,h,w,3] (got %s)" % (tuple(I_u8.shape),))
+    B, Hh, W, _ = I_u8.shape
+    if tuple(Ip_u8.shape) != tuple(I_u8.shape) or tuple(verts.shape) != (B, 20, 2) or (aug is not None and tuple(aug.shape) != (B, 11)):
+        raise _lib.UdhError("draw_report_u8: I' must be shaped like I, verts [B,20,2] and aug [B,11] (got %s, %s, %s, %s)"
+                            % (tuple(I_u8.shape), tuple(Ip_u8.shape), tuple(verts.shape), None if aug is None else tuple(aug.shape)))
+    out = torch.empty(B, Hh, 2 * W, 3, device=I_u8.device, dtype=torch.uint8)
+    nb = lib.udh_draw_report_workspace_bytes(B)
+    ws = torch.empty(nb, device=I_u8.device, dtype=torch.uint8)
+    check(lib.udh_draw_report_u8(_ptr(I_u8), _ptr(Ip_u8), _ptr(aug), int(bool(prime_left)), _ptr(verts), _ptr(out), _ptr(ws), nb,
+                                 B, Hh, W, _stream()), "udh_draw_report_u8")
+    return out
+
+
 # ------------------------------------------------------------------ the dataset generator's warp
 def gen_warp_u8(bgr, theta):
     """uint8 [N,h,w,3] CUDA tensor in cv2's BGR order, float64 theta [N,3,3] (CUDA, the generator's

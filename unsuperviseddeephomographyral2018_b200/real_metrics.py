@@ -27,10 +27,11 @@ def perspective_transform(pts, H):
     return p[:, :2] / p[:, 2:3]
 
 
-def correspondence_errors(pred_h4p, pts1, gt_corr, full_img_h=240, img_h=142, corr_scale=0.5):
+def correspondence_errors(pred_h4p, pts1, gt_corr, full_img_h=240, img_h=142, corr_scale=0.5, with_points=False):
     """Per-sample (h_loss, identity_loss, failed) as the reference's test loop computes them.  pred_h4p, pts1: [B,8];
     gt_corr: [B,16] = corr1 (4 x (x,y)) then corr2, in the frame the points were clicked on (corr_scale maps it onto the
-    full images: 1/2 in the reference)."""
+    full images: 1/2 in the reference).  with_points: each tuple also carries pred_corr2 [4,2] (float64), the predicted
+    matches of corr1 that the report image draws."""
     r = float(full_img_h) / float(img_h)
     out = []
     for h4p, p1, gc in zip(np.asarray(pred_h4p, np.float64), np.asarray(pts1, np.float64), np.asarray(gt_corr, np.float64)):
@@ -42,5 +43,6 @@ def correspondence_errors(pred_h4p, pts1, gt_corr, full_img_h=240, img_h=142, co
         h_loss = float(np.sqrt(np.mean(np.square(pred_corr2 - corr2))))
         ident = float(np.sqrt(np.mean(np.square(corr1 - corr2))))
         failed = h_loss > ident
-        out.append((ident if failed else h_loss, ident, bool(failed)))
+        res = (ident if failed else h_loss, ident, bool(failed))
+        out.append(res + (pred_corr2,) if with_points else res)
     return out
