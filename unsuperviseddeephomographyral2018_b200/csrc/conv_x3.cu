@@ -228,14 +228,34 @@ __global__ void pool_bwd_x3_kernel(const uint32_t* __restrict__ codes, const uin
 }
 
 // ---------------------------------------------------------------------------------------------------- launchers
-template <int N_OUT, int CB, int T, int FA, int FW, int FO>
-int launch_conv_x3_impl(const CUtensorMap& tmA128, const CUtensorMap& tmAhh, const CUtensorMap& tmW, const CUtensorMap& tmOut, const tc::ConvGeom& g,
-                        int stages, size_t smem, const float* bias, const uint32_t* mask_bits, uint32_t* mask_out, float* out_f32, int relu,
-                        float out_scale, cudaStream_t st) {
-  auto kern = tc::tc_conv_x3_kernel<N_OUT, CB, T, FA, FW, FO>;
-  UDH_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+// The two-limb convs hand each item's accumulators to a dedicated epilogue warpgroup (tc_conv_x3_epiwg_kernel) by default;
+// UDH_X3_EPI_WG=0 / udh_debug_x3_set_epi_wg(0) select tc_conv_x3_kernel, which drains them in the MMA warpgroups (tests
+// compare the two bit for bit)
+int g_x3_epi_wg = [] { const char* e = getenv("UDH_X3_EPI_WG"); return (e && e[0] == '0') ? 0 : 1; }();
+
+// one launch of either kernel of the instance <N_OUT, CB, T, ..., ROWS>: weight-ring depth and shared memory for that kernel
+template <int N_OUT, int CB, int T, int FA, int FW, int FO, int ROWS>
+int launch_conv_x3_kernel(const CUtensorMap& tmA128, const CUtensorMap& tmAhh, const CUtensorMap& tmW, const CUtensorMap& tmOut,
+                          const tc::ConvGeom& g, const float* bias, const uint32_t* mask_bits, uint32_t* mask_out, float* out_f32,
+                          int relu, float out_scale, cudaStream_t st) {
   const int sms = persistent_ctas();
   const int grid = g.num_items < sms ? g.num_items : sms;
+  if (g_x3_epi_wg) {
+    using S = tc::ConvX3EpiSmem<N_OUT, CB, T>;
+    const int stages = S::stages(g.abuf_rows);        // weight-ring depth: as many stages as shared memory holds (<= 6)
+    UDH_REQUIRE(stages >= 2, "tc conv x3: activation rows (%d x %d blocks) leave no room for the weight ring", g.abuf_rows, 2 * CB);
+    const size_t smem = S::fixed_bytes(g.abuf_rows) + (size_t)stages * S::kWStageBytes;
+    auto kern = tc::tc_conv_x3_epiwg_kernel<N_OUT, CB, T, FA, FW, FO, ROWS>;
+    UDH_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    launch_chain(kern, dim3(grid), dim3(512), smem, st, tmA128, tmAhh, tmW, tmOut, g, stages, bias, mask_bits, mask_out, out_f32, relu, out_scale);
+    return check_launch("tc_conv_x3_epiwg_kernel");
+  }
+  using S = tc::ConvX3Smem<N_OUT, CB, T>;
+  const int stages = S::stages(g.abuf_rows);
+  UDH_REQUIRE(stages >= 2, "tc conv x3: activation rows (%d x %d blocks) leave no room for the weight ring", g.abuf_rows, 2 * CB);
+  const size_t smem = S::fixed_bytes(g.abuf_rows) + (size_t)stages * S::kWStageBytes;
+  auto kern = tc::tc_conv_x3_kernel<N_OUT, CB, T, FA, FW, FO, ROWS>;
+  UDH_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   launch_chain(kern, dim3(grid), dim3(384), smem, st, tmA128, tmAhh, tmW, tmOut, g, stages, bias, mask_bits, mask_out, out_f32, relu, out_scale);
   return check_launch("tc_conv_x3_kernel");
 }
@@ -262,11 +282,7 @@ int launch_conv_x3(const uint16_t* x, const uint16_t* wpk, const float* bias, co
   uint64_t dimsO[2] = {(uint64_t)2 * N_OUT, (uint64_t)g.Q}, strO[2] = {2, (uint64_t)2 * N_OUT * 2};
   uint32_t boxO[2] = {64, 32};
   TRY(tc::make_tmap_bf16(&tmOut, out_limbs, 2, dimsO, strO, boxO));
-  using S = tc::ConvX3Smem<N_OUT, CB, T>;
-  const int stages = S::stages(g.abuf_rows);          // weight-ring depth: as many stages as shared memory holds (<= 6)
-  UDH_REQUIRE(stages >= 2, "tc conv x3: activation rows (%d x %d blocks) leave no room for the weight ring", g.abuf_rows, 2 * CB);
-  return launch_conv_x3_impl<N_OUT, CB, T, FA, FW, FO>(tmA128, tmAhh, tmW, tmOut, g, stages, S::fixed_bytes(g.abuf_rows) + (size_t)stages * S::kWStageBytes,
-                                                             bias, mask_bits, mask_out, out_f32, relu, out_scale, st);
+  return launch_conv_x3_kernel<N_OUT, CB, T, FA, FW, FO, 0>(tmA128, tmAhh, tmW, tmOut, g, bias, mask_bits, mask_out, out_f32, relu, out_scale, st);
 }
 
 // conv1_2 on row tiles (64 -> 64 channels, 128-wide images): ROWS = 1 forward fused with pool1 (writes the pooled two-limb
@@ -292,18 +308,9 @@ int launch_conv_x3_rows(const uint16_t* x, const uint16_t* wpk, const float* bia
   TRY(tc::make_tmap_bf16(&tmW, wpk, 2, dimsW, strW, boxW));
   // ROWS = 1 stores the pooled stream with plain vector stores (the map is only a placeholder there)
   TRY(tc::make_tmap_bf16(&tmOut, ROWS == 2 ? out_limbs : const_cast<uint16_t*>(x), 2, dimsA, strA, boxO));
-  using S = tc::ConvX3Smem<64, 1, 2>;
-  const int stages = S::stages(g.abuf_rows);          // weight-ring depth: as many stages as shared memory holds (<= kX3MaxStages)
-  UDH_REQUIRE(stages >= 2, "tc conv x3 rows: activation rows (%d) leave no room for the weight ring", g.abuf_rows);
-  const size_t smem = S::fixed_bytes(g.abuf_rows) + (size_t)stages * S::kWStageBytes;
-  auto kern = tc::tc_conv_x3_kernel<64, 1, 2, FA, FW, FO, ROWS>;
-  UDH_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const int sms = persistent_ctas();
-  const int grid = g.num_items < sms ? g.num_items : sms;
   // ROWS = 1: `out_f32` carries the pooled stream pointer and `mask_out` the routing codes
-  launch_chain(kern, dim3(grid), dim3(384), smem, st, tmA128, tmAhh, tmW, tmOut, g, stages, bias, mask_bits, codes_or_mask,
-               ROWS == 1 ? reinterpret_cast<float*>(out_limbs) : (float*)nullptr, relu, 1.0f);
-  return check_launch("tc_conv_x3_kernel(rows)");
+  return launch_conv_x3_kernel<64, 1, 2, FA, FW, FO, ROWS>(tmA128, tmAhh, tmW, tmOut, g, bias, mask_bits, codes_or_mask,
+                                                           ROWS == 1 ? reinterpret_cast<float*>(out_limbs) : (float*)nullptr, relu, 1.0f, st);
 }
 
 // one 3x3 conv on limb streams; (cin -> cout, image width) selects the kernel instance.  FA/FW/FO: limb formats.
@@ -749,6 +756,11 @@ int x3_debug_conv1(const float* I1, const float* I2, const float* w, const float
 
 extern "C" int udh_debug_x3_set_rows(int on) {
   udh::g_x3_rows = on != 0;
+  return UDH_OK;
+}
+
+extern "C" int udh_debug_x3_set_epi_wg(int on) {
+  udh::g_x3_epi_wg = on != 0;
   return UDH_OK;
 }
 
