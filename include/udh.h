@@ -321,7 +321,9 @@ int udh_real_prep(const uint8_t* I, const uint8_t* I_prime, const float* luts, c
  * udh_jpeg_decode (device): plan_host is the plan as udh_jpeg_plan wrote it, plan_dev a 16-byte aligned device copy,
  *   data the same concatenated bytes on the device; writes out [N,h,w,3] uint8 RGB and status [N] (0, or a
  *   UDH_JPEG_E_* code: that image's output is undefined, the other images are unaffected).
- *   workspace: udh_jpeg_workspace_bytes(N, h, w), 16-byte aligned. */
+ *   workspace: udh_jpeg_plan_workspace_bytes(plan_host), 16-byte aligned.  It equals udh_jpeg_workspace_bytes(N, h, w)
+ *   unless the plan has a long segment (128 kB or more of entropy-coded data: a camera frame without restart markers);
+ *   those are decoded by the parallel path, many threads per segment, with the same output and status codes. */
 #define UDH_JPEG_R_OK 0
 #define UDH_JPEG_R_NOT_JPEG 1      /* no SOI marker (PNG, ...)                                         */
 #define UDH_JPEG_R_TRUNCATED 2     /* malformed or truncated header                                     */
@@ -351,6 +353,14 @@ int udh_jpeg_decode(const void* plan_host, const void* plan_dev, const uint8_t* 
 /* Lanes per image in the entropy-decode kernel (32: one warp per image, the default; 1: eight images share a warp).  For
  * the timing tool's comparison; process-wide. */
 int udh_debug_jpeg_set_lanes(int lanes);
+size_t udh_jpeg_plan_workspace_bytes(const void* plan_host);
+/* Which segments plans made from now on send to the parallel entropy path (-1: those of 128 kB or more, the default;
+ * 0: none; 1: all), and how many synchronisation rounds a segment gets before it falls back to the serial path
+ * (0..16, default 16).  udh_debug_jpeg_parallel_segments: after udh_jpeg_decode (synchronises), how many of the plan's
+ * segments the parallel path decoded (the others went to the serial path).  For tests and the timing tool; process-wide. */
+int udh_debug_jpeg_set_parallel(int mode);
+int udh_debug_jpeg_set_sync_rounds(int rounds);
+int udh_debug_jpeg_parallel_segments(const void* plan_host, const void* ws, int32_t* count);
 
 /* ---- baseline-JPEG encode, byte-identical to cv2.imencode('.jpg', img, [IMWRITE_JPEG_QUALITY, quality]) ------------------
  * libjpeg-turbo's defaults: JFIF APP0, standard Huffman tables, ISLOW DCT, no restart markers; channels = 3 takes uint8 BGR
@@ -374,6 +384,8 @@ int udh_jpeg_encode(const uint8_t* img, int n, int h, int w, int channels, int q
  *   n <= 65535. */
 int udh_gen_warp_u8(const uint8_t* bgr, const double* theta, int n, int h, int w, uint8_t* gray, uint8_t* warped,
                     uint8_t* warped_gray, void* stream);
+/* udh_gray_u8: bgr [npx,3] uint8 -> gray [npx] with udh_gen_warp_u8's gray rule (cv2.cvtColor(bgr, COLOR_RGB2GRAY)). */
+int udh_gray_u8(const uint8_t* bgr, int64_t npx, uint8_t* gray, void* stream);
 
 /* ---- instrumentation read by bench.py -------------------------------------------------------------------------
  * udh_launch_count: kernels this library has launched in this process (monotonic).

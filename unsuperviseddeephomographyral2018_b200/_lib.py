@@ -137,11 +137,16 @@ SIGNATURES = {
     "udh_jpeg_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "udh_jpeg_decode": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "udh_debug_jpeg_set_lanes": (c_int, [c_int]),
+    "udh_jpeg_plan_workspace_bytes": (c_size_t, [c_void_p]),
+    "udh_debug_jpeg_set_parallel": (c_int, [c_int]),
+    "udh_debug_jpeg_set_sync_rounds": (c_int, [c_int]),
+    "udh_debug_jpeg_parallel_segments": (c_int, [c_void_p, c_void_p, POINTER(c_int)]),
     "udh_jpeg_encode_capacity": (c_int64, [c_int, c_int, c_int]),
     "udh_jpeg_encode_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "udh_jpeg_encode": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p, c_void_p,
                                 c_size_t, c_void_p]),
     "udh_gen_warp_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "udh_gray_u8": (c_int, [c_void_p, c_int64, c_void_p, c_void_p]),
     "udh_draw_report_workspace_bytes": (c_size_t, [c_int]),
     "udh_draw_report_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_int, c_int, c_int,
                                    c_void_p]),

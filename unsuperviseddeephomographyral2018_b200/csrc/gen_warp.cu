@@ -7,6 +7,8 @@
 //             truncation toward zero, wrapped modulo 256 (NaN and values outside int32 give 0).
 // One thread per output pixel writes the gray plane, the warped BGR image and the warp of the gray plane (the gray of the
 // four source pixels, not the gray of the warped colour).  oracle/gen_data.py restates it.
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace udh {
@@ -63,6 +65,11 @@ __global__ void __launch_bounds__(256) gen_warp_u8_kernel(const uint8_t* __restr
   warped_gray[(int64_t)n * h * w + o] = blend(gen_gray(pa), gen_gray(pb), gen_gray(pc), gen_gray(pd));
 }
 
+__global__ void __launch_bounds__(256) gray_u8_kernel(const uint8_t* __restrict__ bgr, int64_t npx, uint8_t* __restrict__ gray) {
+  for (int64_t o = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; o < npx; o += (int64_t)gridDim.x * blockDim.x)
+    gray[o] = (uint8_t)gen_gray(bgr + o * 3);
+}
+
 }  // namespace udh
 
 using namespace udh;
@@ -74,4 +81,11 @@ extern "C" int udh_gen_warp_u8(const uint8_t* bgr, const double* theta, int n, i
   if (n == 0) return UDH_OK;
   gen_warp_u8_kernel<<<dim3((h * w + 255) / 256, n), 256, 0, as_stream(stream)>>>(bgr, theta, h, w, gray, warped, warped_gray);
   return check_launch("udh_gen_warp_u8");
+}
+
+extern "C" int udh_gray_u8(const uint8_t* bgr, int64_t npx, uint8_t* gray, void* stream) {
+  UDH_REQUIRE(bgr && gray && npx >= 0, "udh_gray_u8: bad argument");
+  if (npx == 0) return UDH_OK;
+  gray_u8_kernel<<<(int)std::min<int64_t>((npx + 255) / 256, 8192), 256, 0, as_stream(stream)>>>(bgr, npx, gray);
+  return check_launch("udh_gray_u8");
 }

@@ -5,11 +5,16 @@
 //                      interval; one for the whole scan without DRI).  Anything else is rejected with a reason code.
 //   jpeg_entropy_kernel one thread per segment, serial within it; the Huffman tables of the CTA's images in shared memory.
 //                      Writes the quantised coefficients (int16, natural order) of every block into the workspace.
+//   jpeg_sync_kernel / jpeg_scan_kernel / jpeg_write_kernel  the parallel path for long segments (camera frames without
+//                      restart markers): self-synchronising Huffman decode, one thread per kJpegSubBytes subsequence
+//                      (Weissenberger & Schmidt, ICPP 2018).  Bit-identical to the serial path; a segment whose
+//                      subsequences do not synchronise within the round limit goes to jpeg_entropy_kernel instead.
 //   jpeg_idct_kernel   one thread per 8x8 block: dequantise + ISLOW IDCT into component sample planes.
 //   jpeg_color_kernel  one thread per output pixel: fancy upsampling of the chroma planes + YCbCr -> RGB (gray: Y to R=G=B).
 #include <stddef.h>
 #include <string.h>
 
+#include <algorithm>
 #include <vector>
 
 #include "common.cuh"
@@ -37,11 +42,42 @@ struct JpegSeg {
   int32_t image, mcu0, nmcu, pad;
 };
 
+// A segment on the parallel path.  dend: the first byte the serial reader would treat as a marker (or end), so the
+// subsequences' readers see no marker and every bit position below 8 * dend is a file bit position.
+struct JpegLong {
+  int64_t begin, dend;
+  int32_t seg, image, sub0, nsub;   // subsequences sub0 .. sub0 + nsub - 1 of the plan's flat list
+};
+
 struct JpegPlanHeader {
   uint32_t magic;
-  int32_t n, h, w, nseg, pad;
+  int32_t n, h, w, nseg, nlong;
   int64_t bytes, plane;   // total plan bytes; coefficients per component plane (stride of the workspace planes)
 };
+
+// Parallel-path scratch, per subsequence.  A decoder state sits at a block boundary: the bit position of the block's DC
+// code (file bits from the start of the concatenated data; -1 = none, the decode before it failed) and its block slot
+// within the MCU (luma blocks in raster order, then Cb, then Cr).
+struct JpegPState {
+  int64_t pos;
+  int32_t slot, pad;
+};
+struct JpegSubRes {        // what one decode of a subsequence found
+  int64_t exit_pos;        // state at the first block boundary at or past the next subsequence's start
+  int32_t exit_slot;
+  int32_t cnt;             // blocks decoded
+  int32_t dc[3];           // sum of the DC differences per component
+  int32_t err, errblk;     // first error (UDH_JPEG_E_*, 0 = none) and the local block it hit
+};
+struct JpegSubOut {        // exclusive scan over the segment's subsequences
+  int32_t first;           // first block (in decode order within the segment)
+  int32_t pred[3];         // DC predictors on entry
+};
+
+constexpr int kJpegSubBytes = 256;            // subsequence length; longer than the longest possible block (< 1800 bits)
+constexpr int64_t kJpegParallelMin = 1 << 17; // segments this long or longer take the parallel path
+constexpr int kJpegMaxRounds = 16;            // synchronisation rounds before a segment goes to the serial path
+constexpr int kJpegWarmSubs = 3;              // round 0 decodes this many subsequences before its own (not counted)
 
 // the entropy kernel copies each image's tables into shared memory as int4 words
 static_assert(sizeof(JpegHuff) % 16 == 0 && sizeof(JpegImage) % 16 == 0 && offsetof(JpegImage, huff) == 0,
@@ -93,8 +129,63 @@ struct BitReader {
 
 __device__ __forceinline__ int jpeg_extend(uint32_t v, int s) { return (s && v < (1u << (s - 1))) ? (int)v - (1 << s) + 1 : (int)v; }
 
+// BitReader that also knows the file bit position of its next bit: pos counts the bits consumed plus 8 for every
+// stuffed 00 passed (marked in `mask` at the last bit of its FF, aligned with acc).
+struct PosReader {
+  const uint8_t* p;
+  const uint8_t* end;
+  uint64_t acc, mask;
+  int nbits, fake;
+  int64_t pos;
+
+  // reader whose next bit is file bit `bitpos` of `data` (bit 0 = MSB of byte 0); bytes at or past `end` read as fake
+  __device__ __forceinline__ void init(const uint8_t* data, const uint8_t* e, int64_t bitpos) {
+    p = data + (bitpos >> 3);
+    end = e;
+    if (p > end) p = end;
+    acc = mask = 0;
+    nbits = fake = 0;
+    pos = bitpos & ~(int64_t)7;
+    fill();
+    skip((int)(bitpos & 7));
+  }
+  __device__ __forceinline__ void fill() {
+    while (nbits <= 56) {
+      uint32_t b = 0;
+      if (p < end) {
+        b = *p++;
+        if (b == 0xFF) {
+          if (p < end && *p == 0x00) {
+            ++p;
+            mask |= 1ull << (56 - nbits);
+          } else {
+            p = end;
+            b = 0;
+            fake += 8;
+          }
+        }
+      } else {
+        fake += 8;
+      }
+      acc |= (uint64_t)b << (56 - nbits);
+      nbits += 8;
+    }
+  }
+  __device__ __forceinline__ uint32_t peek(int n) const { return (uint32_t)(acc >> (64 - n)); }
+  __device__ __forceinline__ bool skip(int n) {
+    if (n) {
+      pos += n + 8 * __popcll(mask >> (64 - n));
+      mask <<= n;
+    }
+    acc <<= n;
+    nbits -= n;
+    return nbits >= fake;
+  }
+};
+
 // -1 on an invalid code; otherwise the symbol (the bits are consumed even when they run past the data; the caller checks)
-__device__ __forceinline__ int huff_decode(BitReader& br, const JpegHuff& t, bool& ok) {
+template <class R>
+__device__ __forceinline__ int huff_decode(R& br, const JpegHuff& t, bool& ok) {
   const uint32_t e = t.look[br.peek(9)];
   if (e) {
     ok = br.skip(e >> 8);
@@ -121,7 +212,8 @@ template <int L>
 __global__ void __launch_bounds__(kJpegImgsPerCta * L, 1) jpeg_entropy_kernel(const JpegImage* __restrict__ imgs,
                                                                            const JpegSeg* __restrict__ segs,
                                                                            const uint8_t* __restrict__ data, int16_t* __restrict__ coef,
-                                                                           int64_t plane, int32_t* __restrict__ status, int n) {
+                                                                           int64_t plane, int32_t* __restrict__ status, int n,
+                                                                           const uint8_t* __restrict__ parallel_done) {
   __shared__ __align__(16) JpegHuff tabs[kJpegImgsPerCta][4];
   const int img0 = blockIdx.x * kJpegImgsPerCta;
   const int nimg = min(kJpegImgsPerCta, n - img0);
@@ -139,6 +231,7 @@ __global__ void __launch_bounds__(kJpegImgsPerCta * L, 1) jpeg_entropy_kernel(co
   const JpegImage& im = imgs[img];
   const int ncomp = im.ncomp, mcus_x = im.mcus_x;
   for (int s = lane; s < im.nseg; s += L) {
+    if (parallel_done && parallel_done[im.seg0 + s]) continue;   // decoded by the parallel path
     const JpegSeg sg = segs[im.seg0 + s];
     BitReader br{data + sg.begin, data + sg.end, 0, 0, 0};
     int pred0 = 0, pred1 = 0, pred2 = 0;   // DC predictors (scalars: a dynamically indexed array would live in local memory)
@@ -188,6 +281,250 @@ __global__ void __launch_bounds__(kJpegImgsPerCta * L, 1) jpeg_entropy_kernel(co
       }
     }
     if (err) atomicCAS(&status[img], 0, err);
+  }
+}
+
+// ---- device: parallel entropy decode of long segments -----------------------------------------------------------------
+// 1. jpeg_sync_kernel, round 0: thread i decodes from the start of subsequence i - kJpegWarmSubs (byte begin +
+//    k * kJpegSubBytes, one byte later when that byte is the 00 of a stuffed FF 00; block slot 0) up to its own
+//    subsequence and takes the block boundary it reaches there as its start; threads i <= kJpegWarmSubs thereby start in
+//    the true state.  A decode that begins at a guessed bit position soon meets the true codeword boundaries, but it
+//    needs the true block slot too (luma and chroma tables differ), which one subsequence is often too short to find.
+//    Each thread then decodes whole blocks until the first block boundary at or past the next subsequence's start and
+//    records that exit state, its block count, its DC difference sums and its first error.
+// 2. Rounds 1..R: subsequence i restarts from i-1's exit state (its own assumed start when i-1 failed); a thread whose
+//    start did not change copies its previous result.  A round in which no exit state changes proves every start state
+//    true by induction from subsequence 0.  A segment still changing after R rounds goes to the serial kernel.
+// 3. jpeg_scan_kernel: exclusive scan of the block counts and DC sums -> each subsequence's first block and its DC
+//    predictors; the first error before the segment's last block becomes the image's status (as the serial path would).
+// 4. jpeg_write_kernel: each subsequence decodes again from its synchronised start and stores its blocks.
+// Errors met before synchronisation are speculative and never reach `status`.
+
+struct JpegSlotMap {   // block slot -> component and block offset within the MCU
+  int bpm, ny, hs0;
+  __device__ __forceinline__ JpegSlotMap(const JpegImage& im)
+      : bpm(im.ncomp == 1 ? 1 : im.hs[0] * im.vs[0] + 2), ny(im.hs[0] * im.vs[0]), hs0(im.hs[0]) {}
+  __device__ __forceinline__ int comp(int slot) const { return slot < ny ? 0 : slot - ny + 1; }
+};
+
+// One block as jpeg_entropy_kernel decodes it (same checks, same order, same codes); blk == nullptr: count only.
+// Returns 0 or the UDH_JPEG_E_* code; *dcdiff = the DC difference.
+__device__ __forceinline__ int jpeg_block(PosReader& br, const JpegHuff& dct, const JpegHuff& act, int* dcdiff, int16_t* blk) {
+  if (blk) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) reinterpret_cast<int4*>(blk)[k] = make_int4(0, 0, 0, 0);
+  }
+  br.fill();
+  bool ok = true;
+  const int t = huff_decode(br, dct, ok);
+  if (t < 0 || t > 15) return 2;
+  const uint32_t bits = t ? br.peek(t) : 0u;
+  ok = br.skip(t) && ok;
+  if (!ok) return 1;
+  *dcdiff = jpeg_extend(bits, t);
+  for (int k = 1; k < 64;) {
+    br.fill();
+    const int rs = huff_decode(br, act, ok);
+    if (rs < 0) return 2;
+    if (!ok) return 1;
+    const int r = rs >> 4, sz = rs & 15;
+    if (sz) {
+      k += r;
+      if (k > 63) return 3;
+      const uint32_t b = br.peek(sz);
+      if (!br.skip(sz)) return 1;
+      if (blk) blk[kZigzag[k]] = (int16_t)jpeg_extend(b, sz);
+      ++k;
+    } else if (r == 15) {
+      k += 16;
+    } else {
+      break;
+    }
+  }
+  return 0;
+}
+
+// first byte of subsequence i (the byte after a stuffed pair's FF rather than its 00)
+__device__ __forceinline__ int64_t jpeg_sub_start(const JpegLong& L, const uint8_t* data, int i) {
+  int64_t b = L.begin + (int64_t)i * kJpegSubBytes;
+  if (i > 0 && b < L.dend && data[b - 1] == 0xFF) ++b;
+  return b;
+}
+
+__device__ __forceinline__ void jpeg_load_tables(JpegHuff (&tabs)[4], const JpegImage& im) {
+  constexpr int kWords = (int)(sizeof(JpegHuff) * 4 / 16);
+  for (int i = threadIdx.x; i < kWords; i += blockDim.x)
+    reinterpret_cast<int4*>(&tabs[0])[i] = reinterpret_cast<const int4*>(&im.huff[0])[i];
+  __syncthreads();
+}
+
+// grid (subsequence chunks, long segments); round 0 seeds every state, round r >= 1 synchronises
+__global__ void __launch_bounds__(128) jpeg_sync_kernel(const JpegImage* __restrict__ imgs, const JpegSeg* __restrict__ segs,
+                                                        const JpegLong* __restrict__ longs, const uint8_t* __restrict__ data,
+                                                        JpegSubRes* __restrict__ res, JpegPState* __restrict__ used,
+                                                        int32_t* __restrict__ changed, int64_t nsub_all, int round) {
+  const JpegLong L = longs[blockIdx.y];
+  if (blockIdx.x * blockDim.x >= L.nsub) return;
+  int32_t* chg = changed + (int64_t)blockIdx.y * (kJpegMaxRounds + 1);
+  if (round >= 2 && chg[round - 1] == 0) return;   // converged in an earlier round
+  __shared__ __align__(16) JpegHuff tabs[4];
+  const JpegImage& im = imgs[L.image];
+  jpeg_load_tables(tabs, im);
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= L.nsub) return;
+  const int64_t g = L.sub0 + i;
+  const JpegSubRes* prev = res + (int64_t)((round + 1) & 1) * nsub_all;
+  JpegSubRes* cur = res + (int64_t)(round & 1) * nsub_all;
+  const JpegSeg sg = segs[L.seg];
+  const JpegSlotMap sm(im);
+  const int64_t total = (int64_t)sg.nmcu * sm.bpm;
+  JpegPState st{8 * jpeg_sub_start(L, data, i), 0, 0};
+  PosReader br;
+  bool positioned = false;
+  if (round == 0 && i > 0) {
+    br.init(data, data + L.dend, 8 * jpeg_sub_start(L, data, max(0, i - kJpegWarmSubs)));
+    int slot = 0, werr = 0, d = 0;
+    for (int64_t n = 0; br.pos < st.pos && n < total && !werr; ++n) {
+      werr = jpeg_block(br, tabs[im.dc[sm.comp(slot)]], tabs[2 + im.ac[sm.comp(slot)]], &d, nullptr);
+      if (++slot == sm.bpm) slot = 0;
+    }
+    if (!werr) {
+      st = JpegPState{br.pos, slot, 0};
+      positioned = true;
+    }
+  }
+  if (round > 0 && i > 0 && prev[g - 1].exit_pos >= 0) st = JpegPState{prev[g - 1].exit_pos, prev[g - 1].exit_slot, 0};
+  if (round > 0 && st.pos == used[g].pos && st.slot == used[g].slot) {
+    cur[g] = prev[g];
+    return;
+  }
+  used[g] = st;
+  const int64_t limit = i + 1 < L.nsub ? 8 * jpeg_sub_start(L, data, i + 1) : INT64_MAX;
+  if (!positioned) br.init(data, data + L.dend, st.pos);
+  int slot = st.slot, cnt = 0, err = 0, dc[3] = {0, 0, 0};
+  while (br.pos < limit && cnt < total) {
+    const int c = sm.comp(slot);
+    int d = 0;
+    err = jpeg_block(br, tabs[im.dc[c]], tabs[2 + im.ac[c]], &d, nullptr);
+    if (err) break;
+    dc[0] += c == 0 ? d : 0; dc[1] += c == 1 ? d : 0; dc[2] += c == 2 ? d : 0;
+    ++cnt;
+    if (++slot == sm.bpm) slot = 0;
+  }
+  JpegSubRes r;
+  r.exit_pos = err ? -1 : br.pos;
+  r.exit_slot = err ? 0 : slot;
+  r.cnt = cnt;
+  r.dc[0] = dc[0]; r.dc[1] = dc[1]; r.dc[2] = dc[2];
+  r.err = err;
+  r.errblk = cnt;
+  cur[g] = r;
+  if (round > 0 && (r.exit_pos != prev[g].exit_pos || r.exit_slot != prev[g].exit_slot)) chg[round] = 1;
+}
+
+// inclusive warp scan of four ints
+__device__ __forceinline__ void warp_scan4(int4& v) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int a = __shfl_up_sync(0xffffffffu, v.x, o), b = __shfl_up_sync(0xffffffffu, v.y, o);
+    const int c = __shfl_up_sync(0xffffffffu, v.z, o), d = __shfl_up_sync(0xffffffffu, v.w, o);
+    if (lane >= o) { v.x += a; v.y += b; v.z += c; v.w += d; }
+  }
+}
+
+// one CTA of 1024 threads per long segment
+__global__ void __launch_bounds__(1024) jpeg_scan_kernel(const JpegImage* __restrict__ imgs, const JpegSeg* __restrict__ segs,
+                                                         const JpegLong* __restrict__ longs, const JpegSubRes* __restrict__ res,
+                                                         const int32_t* __restrict__ changed, JpegSubOut* __restrict__ outp,
+                                                         uint8_t* __restrict__ parallel_done, int32_t* __restrict__ status,
+                                                         int64_t nsub_all, int rounds) {
+  const JpegLong L = longs[blockIdx.x];
+  const int32_t* chg = changed + (int64_t)blockIdx.x * (kJpegMaxRounds + 1);
+  int conv = 0;
+  for (int r = 1; r <= rounds && !conv; ++r)
+    if (chg[r] == 0) conv = r;
+  if (!conv) return;   // not synchronised: the serial kernel decodes this segment
+  const JpegSubRes* rs = res + (int64_t)(conv & 1) * nsub_all + L.sub0;
+  const int64_t total = (int64_t)segs[L.seg].nmcu * JpegSlotMap(imgs[L.image]).bpm;
+  __shared__ int4 wsum[32];
+  __shared__ int4 carry;
+  __shared__ int first_err;
+  if (threadIdx.x == 0) { carry = make_int4(0, 0, 0, 0); first_err = INT32_MAX; }
+  __syncthreads();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int base = 0; base < L.nsub; base += blockDim.x) {
+    const int i = base + threadIdx.x;
+    int4 v = make_int4(0, 0, 0, 0);
+    if (i < L.nsub) v = make_int4(rs[i].cnt, rs[i].dc[0], rs[i].dc[1], rs[i].dc[2]);
+    const int4 own = v;
+    warp_scan4(v);
+    if (lane == 31) wsum[warp] = v;
+    __syncthreads();
+    if (warp == 0) {
+      int4 w = wsum[lane];
+      warp_scan4(w);
+      wsum[lane] = w;
+    }
+    __syncthreads();
+    const int4 c0 = carry;
+    int4 ex = make_int4(c0.x + v.x - own.x, c0.y + v.y - own.y, c0.z + v.z - own.z, c0.w + v.w - own.w);
+    if (warp > 0) { const int4 p = wsum[warp - 1]; ex.x += p.x; ex.y += p.y; ex.z += p.z; ex.w += p.w; }
+    if (i < L.nsub) {
+      JpegSubOut o;
+      o.first = ex.x;
+      o.pred[0] = ex.y; o.pred[1] = ex.z; o.pred[2] = ex.w;
+      outp[L.sub0 + i] = o;
+      if (rs[i].err && (int64_t)ex.x + rs[i].errblk < total) atomicMin(&first_err, i);
+    }
+    __syncthreads();
+    if (threadIdx.x == blockDim.x - 1) {
+      const int4 t = wsum[31];
+      carry = make_int4(c0.x + t.x, c0.y + t.y, c0.z + t.z, c0.w + t.w);
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    parallel_done[L.seg] = 1;
+    if (first_err != INT32_MAX) atomicCAS(&status[L.image], 0, rs[first_err].err);
+  }
+}
+
+__global__ void __launch_bounds__(128) jpeg_write_kernel(const JpegImage* __restrict__ imgs, const JpegSeg* __restrict__ segs,
+                                                         const JpegLong* __restrict__ longs, const uint8_t* __restrict__ data,
+                                                         const JpegPState* __restrict__ used, const JpegSubOut* __restrict__ outp,
+                                                         const uint8_t* __restrict__ parallel_done, int16_t* __restrict__ coef,
+                                                         int64_t plane) {
+  const JpegLong L = longs[blockIdx.y];
+  if (blockIdx.x * blockDim.x >= L.nsub || !parallel_done[L.seg]) return;
+  __shared__ __align__(16) JpegHuff tabs[4];
+  const JpegImage& im = imgs[L.image];
+  jpeg_load_tables(tabs, im);
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= L.nsub) return;
+  const int64_t g = L.sub0 + i;
+  const JpegSeg sg = segs[L.seg];
+  const JpegSlotMap sm(im);
+  const int64_t total = (int64_t)sg.nmcu * sm.bpm;
+  const JpegSubOut o = outp[g];
+  if (o.first >= total) return;
+  const int64_t limit = i + 1 < L.nsub ? 8 * jpeg_sub_start(L, data, i + 1) : INT64_MAX;
+  PosReader br;
+  br.init(data, data + L.dend, used[g].pos);
+  int pred0 = o.pred[0], pred1 = o.pred[1], pred2 = o.pred[2];
+  const int mcus_x = im.mcus_x;
+  int m = sg.mcu0 + o.first / sm.bpm, slot = o.first % sm.bpm;
+  for (int64_t b = o.first; b < total && br.pos < limit; ++b) {
+    const int c = sm.comp(slot);
+    const int my = m / mcus_x, mx = m - my * mcus_x;
+    const int v = c ? 0 : slot / sm.hs0, u = c ? 0 : slot - v * sm.hs0;
+    int16_t* blk = coef + ((int64_t)L.image * 3 + c) * plane + ((int64_t)(my * im.vs[c] + v) * im.bw[c] + mx * im.hs[c] + u) * 64;
+    int d = 0;
+    if (jpeg_block(br, tabs[im.dc[c]], tabs[2 + im.ac[c]], &d, blk)) return;   // reported by jpeg_scan_kernel
+    const int dc = (c == 0 ? pred0 : c == 1 ? pred1 : pred2) + d;
+    if (c == 0) pred0 = dc; else if (c == 1) pred1 = dc; else pred2 = dc;
+    blk[0] = (int16_t)dc;
+    if (++slot == sm.bpm) { slot = 0; ++m; }
   }
 }
 
@@ -519,10 +856,44 @@ static void jpeg_segments(const uint8_t* d, int64_t n, const JpegParsed& P, std:
   }
 }
 
+// -1: segments of kJpegParallelMin bytes or more take the parallel path; 0: none does; 1: every segment does
+static int g_jpeg_parallel = -1;
+
+// The serial reader's end of a segment's data: the first FF not followed by a stuffed 00 (a marker), or end.
+static int64_t jpeg_data_end(const uint8_t* d, int64_t begin, int64_t end) {
+  for (int64_t j = begin; j < end;) {
+    const uint8_t* f = static_cast<const uint8_t*>(memchr(d + j, 0xFF, (size_t)(end - j)));
+    if (!f) break;
+    j = f - d;
+    if (j + 1 < end && d[j + 1] == 0x00) j += 2;
+    else return j;
+  }
+  return end;
+}
+
+static void jpeg_long_segments(const uint8_t* data, const std::vector<JpegSeg>& segs, std::vector<JpegLong>& longs) {
+  longs.clear();
+  int64_t sub = 0;
+  for (size_t s = 0; s < segs.size(); ++s) {
+    const JpegSeg& g = segs[s];
+    if (!(g_jpeg_parallel == 1 || (g_jpeg_parallel < 0 && g.end - g.begin >= kJpegParallelMin))) continue;
+    JpegLong L{};
+    L.begin = g.begin;
+    L.dend = jpeg_data_end(data, g.begin, g.end);
+    L.seg = (int)s;
+    L.image = g.image;
+    L.sub0 = (int)sub;
+    L.nsub = (int)std::max<int64_t>(1, (L.dend - L.begin + kJpegSubBytes - 1) / kJpegSubBytes);
+    sub += L.nsub;
+    longs.push_back(L);
+  }
+}
+
 static int jpeg_build_plan(const uint8_t* data, const int64_t* offsets, int n, int h, int w, std::vector<JpegImage>& imgs,
-                           std::vector<JpegSeg>& segs) {
+                           std::vector<JpegSeg>& segs, std::vector<JpegLong>& longs) {
   imgs.resize(n);
   segs.clear();
+  longs.clear();
   JpegParsed P;
   for (int k = 0; k < n; ++k) {
     const int64_t b = offsets[k], len = offsets[k + 1] - offsets[k];
@@ -544,11 +915,35 @@ static int jpeg_build_plan(const uint8_t* data, const int64_t* offsets, int n, i
     P.img.nseg = (int)segs.size() - P.img.seg0;
     imgs[k] = P.img;
   }
+  jpeg_long_segments(data, segs, longs);
+  if (!longs.empty() && (int64_t)longs.back().sub0 + longs.back().nsub > INT32_MAX / 2) {
+    set_error("udh_jpeg_plan: too much entropy-coded data for one plan");
+    return UDH_EINVAL;
+  }
   return UDH_OK;
 }
 
-static size_t plan_size(int n, size_t nseg) {
+// header | images | segments | long segments (none: the plan is laid out as it was before the parallel path existed)
+static_assert(sizeof(JpegSeg) % 16 == 0 && sizeof(JpegLong) % 16 == 0, "plan sections must stay 16-byte aligned");
+static size_t plan_longs_offset(int n, size_t nseg) {
   return align_up(sizeof(JpegPlanHeader), 16) + align_up((size_t)n * sizeof(JpegImage), 16) + nseg * sizeof(JpegSeg);
+}
+static size_t plan_size(int n, size_t nseg, size_t nlong) { return plan_longs_offset(n, nseg) + nlong * sizeof(JpegLong); }
+
+// Parallel-path workspace after the coefficient and sample planes: per subsequence two JpegSubRes (ping-pong rounds), a
+// JpegPState and a JpegSubOut; per long segment kJpegMaxRounds + 1 change flags; per segment one done byte.
+struct JpegParWs {
+  size_t res, used, outp, changed, done, end;
+};
+static JpegParWs jpeg_par_ws(size_t base, int64_t nsub, int nlong, int nseg) {
+  JpegParWs o;
+  o.res = align_up(base, 16);
+  o.used = o.res + align_up(2 * (size_t)nsub * sizeof(JpegSubRes), 16);
+  o.outp = o.used + align_up((size_t)nsub * sizeof(JpegPState), 16);
+  o.changed = o.outp + align_up((size_t)nsub * sizeof(JpegSubOut), 16);
+  o.done = o.changed + align_up((size_t)nlong * (kJpegMaxRounds + 1) * sizeof(int32_t), 16);
+  o.end = o.done + align_up((size_t)nseg, 16);
+  return o;
 }
 
 }  // namespace udh
@@ -556,6 +951,7 @@ static size_t plan_size(int n, size_t nseg) {
 using namespace udh;
 
 static int g_jpeg_lanes = 32;
+static int g_jpeg_rounds = kJpegMaxRounds;
 
 extern "C" int udh_jpeg_parse(const uint8_t* data, int64_t nbytes, udh_jpeg_info* info) {
   UDH_REQUIRE(info && (data || nbytes == 0) && nbytes >= 0, "udh_jpeg_parse: bad argument");
@@ -570,8 +966,9 @@ extern "C" size_t udh_jpeg_plan_bytes(const uint8_t* data, const int64_t* offset
   if (!data || !offsets || n < 1 || h < 1 || w < 1) return 0;
   std::vector<JpegImage> imgs;
   std::vector<JpegSeg> segs;
-  if (jpeg_build_plan(data, offsets, n, h, w, imgs, segs) != UDH_OK) return 0;
-  return plan_size(n, segs.size());
+  std::vector<JpegLong> longs;
+  if (jpeg_build_plan(data, offsets, n, h, w, imgs, segs, longs) != UDH_OK) return 0;
+  return plan_size(n, segs.size(), longs.size());
 }
 
 extern "C" int udh_jpeg_plan(const uint8_t* data, const int64_t* offsets, int n, int h, int w, void* plan, size_t plan_bytes) {
@@ -579,9 +976,10 @@ extern "C" int udh_jpeg_plan(const uint8_t* data, const int64_t* offsets, int n,
   UDH_REQUIRE(n >= 1 && h >= 1 && w >= 1 && h <= 65535 && w <= 65535, "udh_jpeg_plan: bad dimensions");
   std::vector<JpegImage> imgs;
   std::vector<JpegSeg> segs;
-  const int rc = jpeg_build_plan(data, offsets, n, h, w, imgs, segs);
+  std::vector<JpegLong> longs;
+  const int rc = jpeg_build_plan(data, offsets, n, h, w, imgs, segs, longs);
   if (rc != UDH_OK) return rc;
-  const size_t need = plan_size(n, segs.size());
+  const size_t need = plan_size(n, segs.size(), longs.size());
   if (plan_bytes < need) {
     set_error("udh_jpeg_plan: plan buffer of %zu bytes, %zu needed", plan_bytes, need);
     return UDH_EWS;
@@ -589,7 +987,7 @@ extern "C" int udh_jpeg_plan(const uint8_t* data, const int64_t* offsets, int n,
   uint8_t* p = static_cast<uint8_t*>(plan);
   JpegPlanHeader hd{};
   hd.magic = kJpegMagic;
-  hd.n = n; hd.h = h; hd.w = w; hd.nseg = (int)segs.size();
+  hd.n = n; hd.h = h; hd.w = w; hd.nseg = (int)segs.size(); hd.nlong = (int)longs.size();
   hd.bytes = (int64_t)need;
   hd.plane = jpeg_plane_coefs(h, w);
   memcpy(p, &hd, sizeof(hd));
@@ -597,6 +995,8 @@ extern "C" int udh_jpeg_plan(const uint8_t* data, const int64_t* offsets, int n,
   memcpy(p, imgs.data(), (size_t)n * sizeof(JpegImage));
   p += align_up((size_t)n * sizeof(JpegImage), 16);
   memcpy(p, segs.data(), segs.size() * sizeof(JpegSeg));
+  p += segs.size() * sizeof(JpegSeg);
+  if (!longs.empty()) memcpy(p, longs.data(), longs.size() * sizeof(JpegLong));
   return UDH_OK;
 }
 
@@ -605,13 +1005,35 @@ extern "C" size_t udh_jpeg_workspace_bytes(int n, int h, int w) {
   return (size_t)n * 3 * (size_t)jpeg_plane_coefs(h, w) * (sizeof(int16_t) + sizeof(uint8_t));
 }
 
+// the plan's long segments and their subsequence count (host copy of the plan)
+static const JpegLong* plan_longs(const JpegPlanHeader& hd, const void* plan, int64_t* nsub, int* max_nsub) {
+  const JpegLong* L = reinterpret_cast<const JpegLong*>(static_cast<const uint8_t*>(plan) + plan_longs_offset(hd.n, hd.nseg));
+  *nsub = hd.nlong ? (int64_t)L[hd.nlong - 1].sub0 + L[hd.nlong - 1].nsub : 0;
+  *max_nsub = 0;
+  for (int k = 0; k < hd.nlong; ++k) *max_nsub = std::max(*max_nsub, L[k].nsub);
+  return L;
+}
+
+extern "C" size_t udh_jpeg_plan_workspace_bytes(const void* plan_host) {
+  if (!plan_host) return 0;
+  JpegPlanHeader hd;
+  memcpy(&hd, plan_host, sizeof(hd));
+  if (hd.magic != kJpegMagic || hd.n < 1) return 0;
+  const size_t base = udh_jpeg_workspace_bytes(hd.n, hd.h, hd.w);
+  if (hd.nlong == 0) return base;
+  int64_t nsub;
+  int max_nsub;
+  plan_longs(hd, plan_host, &nsub, &max_nsub);
+  return jpeg_par_ws(base, nsub, hd.nlong, hd.nseg).end;
+}
+
 extern "C" int udh_jpeg_decode(const void* plan_host, const void* plan_dev, const uint8_t* data, uint8_t* out, int32_t* status,
                                void* ws, size_t ws_bytes, void* stream) {
   UDH_REQUIRE(plan_host && plan_dev && data && out && status && ws, "udh_jpeg_decode: null pointer");
   JpegPlanHeader hd;
   memcpy(&hd, plan_host, sizeof(hd));
   UDH_REQUIRE(hd.magic == kJpegMagic && hd.n >= 1, "udh_jpeg_decode: not a plan made by udh_jpeg_plan");
-  const size_t need = udh_jpeg_workspace_bytes(hd.n, hd.h, hd.w);
+  const size_t need = udh_jpeg_plan_workspace_bytes(plan_host);
   if (ws_bytes < need) {
     set_error("udh_jpeg_decode: workspace of %zu bytes, %zu needed", ws_bytes, need);
     return UDH_EWS;
@@ -624,13 +1046,44 @@ extern "C" int udh_jpeg_decode(const void* plan_host, const void* plan_dev, cons
   int16_t* coef = static_cast<int16_t*>(ws);
   uint8_t* samples = reinterpret_cast<uint8_t*>(coef + (size_t)hd.n * 3 * hd.plane);
   UDH_CUDA(cudaMemsetAsync(status, 0, sizeof(int32_t) * hd.n, st));
+  int rc;
+  uint8_t* done = nullptr;
+  JpegSubRes* res = nullptr;
+  JpegPState* used = nullptr;
+  JpegSubOut* outp = nullptr;
+  const JpegLong* longs_d = nullptr;
+  int64_t nsub = 0;
+  int max_nsub = 0;
+  if (hd.nlong) {   // parallel path: rounds, scan (segments that synchronised are marked done for the serial kernel)
+    plan_longs(hd, plan_host, &nsub, &max_nsub);
+    const JpegParWs o = jpeg_par_ws(udh_jpeg_workspace_bytes(hd.n, hd.h, hd.w), nsub, hd.nlong, hd.nseg);
+    uint8_t* w8 = static_cast<uint8_t*>(ws);
+    res = reinterpret_cast<JpegSubRes*>(w8 + o.res);
+    used = reinterpret_cast<JpegPState*>(w8 + o.used);
+    outp = reinterpret_cast<JpegSubOut*>(w8 + o.outp);
+    int32_t* changed = reinterpret_cast<int32_t*>(w8 + o.changed);
+    done = w8 + o.done;
+    longs_d = reinterpret_cast<const JpegLong*>(pd + plan_longs_offset(hd.n, hd.nseg));
+    UDH_CUDA(cudaMemsetAsync(w8 + o.changed, 0, o.end - o.changed, st));
+    const dim3 grid((max_nsub + 127) / 128, hd.nlong);
+    for (int r = 0; r <= g_jpeg_rounds; ++r) {
+      jpeg_sync_kernel<<<grid, 128, 0, st>>>(imgs, segs, longs_d, data, res, used, changed, nsub, r);
+      if ((rc = check_launch("jpeg_sync"))) return rc;
+    }
+    jpeg_scan_kernel<<<hd.nlong, 1024, 0, st>>>(imgs, segs, longs_d, res, changed, outp, done, status, nsub, g_jpeg_rounds);
+    if ((rc = check_launch("jpeg_scan"))) return rc;
+  }
   const int ctas = (hd.n + kJpegImgsPerCta - 1) / kJpegImgsPerCta;
   if (g_jpeg_lanes == 1)
-    jpeg_entropy_kernel<1><<<ctas, kJpegImgsPerCta * 1, 0, st>>>(imgs, segs, data, coef, hd.plane, status, hd.n);
+    jpeg_entropy_kernel<1><<<ctas, kJpegImgsPerCta * 1, 0, st>>>(imgs, segs, data, coef, hd.plane, status, hd.n, done);
   else
-    jpeg_entropy_kernel<32><<<ctas, kJpegImgsPerCta * 32, 0, st>>>(imgs, segs, data, coef, hd.plane, status, hd.n);
-  int rc = check_launch("jpeg_entropy");
-  if (rc) return rc;
+    jpeg_entropy_kernel<32><<<ctas, kJpegImgsPerCta * 32, 0, st>>>(imgs, segs, data, coef, hd.plane, status, hd.n, done);
+  if ((rc = check_launch("jpeg_entropy"))) return rc;
+  if (hd.nlong) {
+    jpeg_write_kernel<<<dim3((max_nsub + 127) / 128, hd.nlong), 128, 0, st>>>(imgs, segs, longs_d, data, used, outp, done, coef,
+                                                                               hd.plane);
+    if ((rc = check_launch("jpeg_write"))) return rc;
+  }
   const int maxblk = (int)(3 * hd.plane / 64);
   jpeg_idct_kernel<<<dim3((maxblk + 127) / 128, hd.n), 128, 0, st>>>(imgs, coef, samples, hd.plane);
   rc = check_launch("jpeg_idct");
@@ -638,6 +1091,35 @@ extern "C" int udh_jpeg_decode(const void* plan_host, const void* plan_dev, cons
   const int npx = hd.h * hd.w;
   jpeg_color_kernel<<<dim3(min((npx + 255) / 256, 64), hd.n), 256, 0, st>>>(imgs, samples, hd.plane, out, hd.h, hd.w);
   return check_launch("udh_jpeg_decode");
+}
+
+extern "C" int udh_debug_jpeg_set_parallel(int mode) {
+  UDH_REQUIRE(mode >= -1 && mode <= 1, "udh_debug_jpeg_set_parallel: mode must be -1 (by segment length), 0 (off) or 1 (on)");
+  g_jpeg_parallel = mode;
+  return UDH_OK;
+}
+
+extern "C" int udh_debug_jpeg_set_sync_rounds(int rounds) {
+  UDH_REQUIRE(rounds >= 0 && rounds <= kJpegMaxRounds, "udh_debug_jpeg_set_sync_rounds: rounds must be 0..16");
+  g_jpeg_rounds = rounds;
+  return UDH_OK;
+}
+
+extern "C" int udh_debug_jpeg_parallel_segments(const void* plan_host, const void* ws, int32_t* count) {
+  UDH_REQUIRE(plan_host && ws && count, "udh_debug_jpeg_parallel_segments: null pointer");
+  JpegPlanHeader hd;
+  memcpy(&hd, plan_host, sizeof(hd));
+  UDH_REQUIRE(hd.magic == kJpegMagic && hd.n >= 1, "udh_debug_jpeg_parallel_segments: not a plan made by udh_jpeg_plan");
+  *count = 0;
+  if (!hd.nlong) return UDH_OK;
+  int64_t nsub;
+  int max_nsub;
+  plan_longs(hd, plan_host, &nsub, &max_nsub);
+  const JpegParWs o = jpeg_par_ws(udh_jpeg_workspace_bytes(hd.n, hd.h, hd.w), nsub, hd.nlong, hd.nseg);
+  std::vector<uint8_t> done(hd.nseg);
+  UDH_CUDA(cudaMemcpy(done.data(), static_cast<const uint8_t*>(ws) + o.done, hd.nseg, cudaMemcpyDeviceToHost));
+  for (uint8_t d : done) *count += d;
+  return UDH_OK;
 }
 
 extern "C" int udh_debug_jpeg_set_lanes(int lanes) {

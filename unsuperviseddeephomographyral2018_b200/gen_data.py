@@ -18,12 +18,11 @@ is accepted and draws nothing.
 """
 import concurrent.futures
 import os
-import queue
 import random
-import shutil
-import threading
 
 import numpy as np
+
+from . import gen_io
 
 CHUNK = 64                     # raw images per device round
 
@@ -64,71 +63,17 @@ def read_raw(path):
     return cv2.imread(path)
 
 
-def _prepare(args):
-    """dataCollection's deletions and directories."""
-    if args.resume in ("N", "n") and args.start_index == 0 and args.mode == "train" and not args.debug:
-        try:
-            os.remove(args.gt_file)
-            os.remove(args.pts1_file)
-            os.remove(args.filenames_file)
-            shutil.rmtree(args.I_dir, ignore_errors=True)
-            if args.I_prime_dir is not None:
-                shutil.rmtree(args.I_prime_dir, ignore_errors=True)
-        except OSError:
-            pass
-    if args.resume in ("N", "n") and args.mode == "test" and not args.debug:
-        try:
-            os.remove(args.test_gt_file)
-            os.remove(args.test_pts1_file)
-            os.remove(args.test_filenames_file)
-        except OSError:
-            pass
-    if not args.debug:
-        os.makedirs(args.I_dir, exist_ok=True)
-        if args.I_prime_dir is not None:
-            os.makedirs(args.I_prime_dir, exist_ok=True)
-
-
-class _Writer:
-    """Writes (path, bytes) on a background thread; close() waits for every file and re-raises a write error."""
-
-    def __init__(self):
-        self.q, self.err = queue.Queue(maxsize=4096), None
-        self.t = threading.Thread(target=self._run, daemon=True)
-        self.t.start()
-
-    def _run(self):
-        while True:
-            item = self.q.get()
-            if item is None:
-                return
-            try:
-                with open(item[0], "wb") as f:
-                    f.write(item[1])
-            except OSError as e:
-                self.err = self.err or e
-
-    def put(self, path, data):
-        self.q.put((path, data))
-
-    def close(self):
-        self.q.put(None)
-        self.t.join()
-        if self.err:
-            raise self.err
-
-
 def generate(args, backend, seed=0):
     """Run the generator with `backend` (DeviceBackend or oracle.gen_data.HostBackend); returns the next free index."""
     rnd = random.Random(seed)
-    _prepare(args)
+    gen_io.prepare(args, (args.I_dir, args.I_prime_dir))
     names = raw_list(args.raw_data_path)
     end = args.num_data + args.start_index
     index = args.start_index
     train = args.mode == "train"
     gray_files = train and not args.color
     files = None
-    writer = None if args.debug else _Writer()
+    writer = None if args.debug else gen_io.Writer()
     pool = concurrent.futures.ThreadPoolExecutor(min(16, os.cpu_count() or 1))
     paths = [os.path.join(args.raw_data_path, n) for n in names]
     chunks = [paths[i:i + CHUNK] for i in range(0, len(paths), CHUNK)]

@@ -400,8 +400,8 @@ class JpegPlan:
         data_d = self.data.to(dev, non_blocking=True)
         out = torch.empty(self.n, self.h, self.w, 3, device=dev, dtype=torch.uint8)
         status = torch.empty(self.n, device=dev, dtype=torch.int32)
-        nbytes = lib.udh_jpeg_workspace_bytes(self.n, self.h, self.w)
-        ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+        nbytes = lib.udh_jpeg_plan_workspace_bytes(self.plan.data_ptr())
+        ws = self.ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)     # kept for udh_debug_jpeg_parallel_segments
         check(lib.udh_jpeg_decode(self.plan.data_ptr(), _ptr(plan_d), _ptr(data_d), _ptr(out), _ptr(status), _ptr(ws), nbytes,
                                   _stream()), "udh_jpeg_decode")
         return out, status
@@ -497,6 +497,17 @@ def gen_warp_u8(bgr, theta):
     warped_gray = torch.empty_like(gray)
     check(lib.udh_gen_warp_u8(_ptr(bgr), _ptr(theta), n, h, w, _ptr(gray), _ptr(warped), _ptr(warped_gray), _stream()), "udh_gen_warp_u8")
     return gray, warped, warped_gray
+
+
+def gray_u8(bgr):
+    """uint8 [..., 3] CUDA tensor in cv2's BGR order -> uint8 [...]: cv2.cvtColor(bgr, COLOR_RGB2GRAY) as the reference
+    calls it on BGR data, with gen_warp_u8's gray rule."""
+    _req(bgr, torch.uint8, "bgr")
+    if bgr.dim() < 1 or bgr.shape[-1] != 3:
+        raise _lib.UdhError("gray_u8: bgr must be [..., 3] (got %s)" % (tuple(bgr.shape),))
+    gray = torch.empty(bgr.shape[:-1], device=bgr.device, dtype=torch.uint8)
+    check(lib.udh_gray_u8(_ptr(bgr), gray.numel(), _ptr(gray), _stream()), "udh_gray_u8")
+    return gray
 
 
 # ------------------------------------------------------------------ Adam
