@@ -377,6 +377,58 @@ size_t udh_jpeg_encode_workspace_bytes(int n, int h, int w, int channels);
 int udh_jpeg_encode(const uint8_t* img, int n, int h, int w, int channels, int quality, uint8_t* out, int64_t cap, int64_t* nbytes,
                     int32_t* status, void* ws, size_t ws_bytes, void* stream);
 
+/* ---- PNG decode, bit-identical to cv2.imread(..., IMREAD_COLOR) ------------------------------------------------------------
+ * Accepted: non-interlaced, bit depth 8, colour type 0 (gray: replicated to 3 channels), 2 (RGB) or 6 (RGBA: alpha dropped),
+ * every chunk's CRC correct, IEND present.  Ancillary chunks that do not change what cv2 returns are skipped: tEXt, zTXt,
+ * iTXt, tIME and pHYs.  Any other chunk (gAMA, sBIT, tRNS, cHRM, sRGB, iCCP, eXIf, PLTE, APNG frames, ...) is rejected
+ * with UDH_PNG_R_CHUNK, and everything else out of scope with its own UDH_PNG_R_* reason.
+ * udh_png_parse (host): one file -> info; returns UDH_OK with info->reason set, or UDH_EINVAL on a null pointer.
+ * udh_png_plan_bytes / udh_png_plan (host): N files, concatenated in `data` with file k at [offsets[k], offsets[k+1]), all
+ *   h x w and supported -> the descriptor (plan) and the files' IDAT payloads, concatenated per file into `idat`
+ *   (*idat_bytes of them; file k's zlib stream is contiguous).  plan_bytes returns 0 when the plan cannot be built;
+ *   udh_png_plan then returns UDH_ENOSUP (a file is not supported) or UDH_EINVAL (wrong size).
+ * udh_png_decode (device): plan_host as udh_png_plan wrote it, plan_dev a 16-byte aligned device copy, idat the payloads on
+ *   the device; writes out [N,h,w,3] uint8 (BGR as cv2 returns it; RGB when rgb != 0) and status [N] (0, or a
+ *   UDH_PNG_E_* code: that image's output is undefined, the other images are unaffected).  Workspace:
+ *   udh_png_workspace_bytes(plan_host) (the filtered scanlines), 16-byte aligned. */
+#define UDH_PNG_R_OK 0
+#define UDH_PNG_R_NOT_PNG 1         /* no PNG signature                                               */
+#define UDH_PNG_R_JPEG 2            /* a JPEG file (SOI marker)                                       */
+#define UDH_PNG_R_TRUNCATED 3       /* a chunk other than IDAT runs past the end of the file         */
+#define UDH_PNG_R_IDAT_TRUNCATED 4  /* an IDAT chunk runs past the end of the file                    */
+#define UDH_PNG_R_CRC 5             /* a chunk's CRC does not match                                   */
+#define UDH_PNG_R_NO_IEND 6         /* the chunks end without IEND                                    */
+#define UDH_PNG_R_MALFORMED 7       /* no or invalid IHDR, IDAT chunks not consecutive, no IDAT       */
+#define UDH_PNG_R_PALETTE 8         /* colour type 3                                                  */
+#define UDH_PNG_R_DEPTH16 9         /* bit depth 16                                                   */
+#define UDH_PNG_R_DEPTH_SUB8 10     /* bit depth 1, 2 or 4                                            */
+#define UDH_PNG_R_INTERLACED 11     /* Adam7                                                          */
+#define UDH_PNG_R_GRAY_ALPHA 12     /* colour type 4                                                  */
+#define UDH_PNG_R_CHUNK 13          /* a chunk that may change what cv2 returns (see above)           */
+#define UDH_PNG_E_TRUNCATED 1       /* the zlib stream ran out                                        */
+#define UDH_PNG_E_ZLIB 2            /* bad zlib header (method, window, check bits, preset dictionary) */
+#define UDH_PNG_E_BLOCK 3           /* bad block: type 3, stored length check, invalid code lengths   */
+#define UDH_PNG_E_CODE 4            /* invalid literal/length or distance code                        */
+#define UDH_PNG_E_DISTANCE 5        /* a distance beyond the output or the window                     */
+#define UDH_PNG_E_ADLER 6           /* Adler-32 mismatch                                              */
+#define UDH_PNG_E_SHORT 7           /* fewer bytes than h * (1 + w * channels)                        */
+#define UDH_PNG_E_LONG 8            /* more bytes than h * (1 + w * channels)                         */
+#define UDH_PNG_E_FILTER 9          /* a row's filter type above 4                                    */
+typedef struct udh_png_info {
+  int32_t width, height, bit_depth, color_type, interlace;
+  int32_t channels;         /* samples per pixel in the file (1, 2, 3 or 4; 1 for a palette)    */
+  int64_t idat_bytes;       /* the zlib stream's length (all IDAT payloads)                      */
+  int32_t reason;           /* UDH_PNG_R_*                                                        */
+  int32_t pad;
+} udh_png_info;
+int udh_png_parse(const uint8_t* data, int64_t nbytes, udh_png_info* info);
+size_t udh_png_plan_bytes(const uint8_t* data, const int64_t* offsets, int n, int h, int w, int64_t* idat_bytes);
+int udh_png_plan(const uint8_t* data, const int64_t* offsets, int n, int h, int w, void* plan, size_t plan_bytes, uint8_t* idat,
+                 int64_t idat_bytes);
+size_t udh_png_workspace_bytes(const void* plan_host);
+int udh_png_decode(const void* plan_host, const void* plan_dev, const uint8_t* idat, uint8_t* out, int32_t* status, int rgb,
+                   void* ws, size_t ws_bytes, void* stream);
+
 /* ---- the dataset generator's warp (gen_synthetic_data.py:63-64), bit-identical to the reference's NumPy ------------------
  * udh_gen_warp_u8: bgr [n,h,w,3] uint8 (cv2's channel order), theta [n,9] float64 (row-major inv(M) inv(H_inverse) M on the
  *   [-1,1] grid) -> gray [n,h,w] = cv2.cvtColor(bgr, COLOR_RGB2GRAY), warped [n,h,w,3] = numpy_transformer(bgr, H_inverse)

@@ -45,6 +45,18 @@ JPEG_R = dict(OK=0, NOT_JPEG=1, TRUNCATED=2, NOT_BASELINE=3, PRECISION=4, COMPON
 JPEG_E = dict(TRUNCATED=1, HUFFMAN=2, COEF=3)
 
 
+class PngInfo(ctypes.Structure):
+    """udh_png_info (include/udh.h)."""
+    _fields_ = [("width", c_int), ("height", c_int), ("bit_depth", c_int), ("color_type", c_int), ("interlace", c_int),
+                ("channels", c_int), ("idat_bytes", c_int64), ("reason", c_int), ("pad", c_int)]
+
+
+# udh_png_parse reasons (UDH_PNG_R_*) and udh_png_decode statuses (UDH_PNG_E_*)
+PNG_R = dict(OK=0, NOT_PNG=1, JPEG=2, TRUNCATED=3, IDAT_TRUNCATED=4, CRC=5, NO_IEND=6, MALFORMED=7, PALETTE=8, DEPTH16=9,
+             DEPTH_SUB8=10, INTERLACED=11, GRAY_ALPHA=12, CHUNK=13)
+PNG_E = dict(TRUNCATED=1, ZLIB=2, BLOCK=3, CODE=4, DISTANCE=5, ADLER=6, SHORT=7, LONG=8, FILTER=9)
+
+
 STEP_ALL, STEP_FWD_HEAD, STEP_CONVS, STEP_FWD_ONLY = 0, 1, 2, 3
 STEP_LOSS = {"h_loss": 0, "l1_loss": 1, "rec_loss": 2, "l1_smooth_loss": 3, "ncc_loss": 4, "ssim_loss": 5}
 
@@ -141,6 +153,11 @@ SIGNATURES = {
     "udh_debug_jpeg_set_parallel": (c_int, [c_int]),
     "udh_debug_jpeg_set_sync_rounds": (c_int, [c_int]),
     "udh_debug_jpeg_parallel_segments": (c_int, [c_void_p, c_void_p, POINTER(c_int)]),
+    "udh_png_parse": (c_int, [c_void_p, c_int64, POINTER(PngInfo)]),
+    "udh_png_plan_bytes": (c_size_t, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_int64)]),
+    "udh_png_plan": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_size_t, c_void_p, c_int64]),
+    "udh_png_workspace_bytes": (c_size_t, [c_void_p]),
+    "udh_png_decode": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_size_t, c_void_p]),
     "udh_jpeg_encode_capacity": (c_int64, [c_int, c_int, c_int]),
     "udh_jpeg_encode_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "udh_jpeg_encode": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p, c_void_p,

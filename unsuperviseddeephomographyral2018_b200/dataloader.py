@@ -2,8 +2,8 @@
 
 Produces, per batch, the nine post-dataloader tensors the model consumes (`*_batch` attributes / dict keys):
 I1, I2, I1_aug, I2_aug [B,P,P,1]; I (=I_aug), I_prime (=I_prime_aug) [B,Hh,W,3]; pts1, gt [B,8]; patch_indices [B,P*P].
-JPEG decode runs on the device for the baseline files cv2.imwrite produces (bit-identical to cv2.imread; other files are
-decoded on the host); list parsing runs on the host; photometric augmentation, normalisation, gray conversion and patch
+JPEG decode runs on the device for the baseline files cv2.imwrite produces, and PNG decode for 8-bit non-interlaced gray,
+RGB and RGBA files (both bit-identical to cv2.imread; other files are decoded on the host); list parsing runs on the host; photometric augmentation, normalisation, gray conversion and patch
 gather run on the device.  The real-data set (extended_dataloader_params) takes the same device path at its two file sizes,
 with its augment + normalise + AREA resize in one kernel, bit-identical to its host path (_disk_batch_extended_host).
 `synthetic=N` replaces the on-disk set by N
@@ -89,7 +89,7 @@ class Dataloader(object):
         self._rng = np.random.default_rng(seed)
         self._step = 0
         self._reader, self._pending, self._ready = None, None, []
-        self.decode_stats = dict(groups=0, read_s=0.0, wait_s=0.0, group_s=0.0, device_images=0, host_images=0, decode_errors=0)
+        self.decode_stats = dict(groups=0, read_s=0.0, wait_s=0.0, group_s=0.0, device_images=0, host_images=0, decode_errors=0, png_images=0)
         if not self.synthetic_pairs:
             self.names, self.pts1, self.gt = read_img_and_gt(params.filenames_file, params.pts1_file, params.gt_file)
             self.num_samples = len(self.names)
@@ -279,11 +279,13 @@ class Dataloader(object):
     # Device decode of the on-disk set.  A group of DECODE_BATCHES batches is decoded in one launch: the indices and the
     # augmentation table of each batch are drawn from the host RNG batch after batch, exactly as the host path draws them,
     # so the batches are the same whichever decoder ran.  A background thread reads (and parses) the next group's files
-    # while the current group is being consumed.  Files the device decoder does not take (progressive, PNG, another size,
-    # a decode error, ...) go through _read_image.  Because a group is built at once, a missing or unreadable file raises
+    # while the current group is being consumed.  Baseline JPEG and 8-bit PNG files of a decode size go to a JpegPlan or a
+    # PngPlan per size; the files neither device decoder takes (progressive, palette PNG, another size, a decode error, ...)
+    # go through _read_image.  Because a group is built at once, a missing or unreadable file raises
     # its IOError when the first batch of its group is requested (up to DECODE_BATCHES - 1 batches before its own).
     # decode_stats counts, over the loader's life, the groups, the reader thread's seconds, the seconds next_batch spent
-    # waiting for it, the seconds next_batch spent building groups (wait included), and the images decoded on the device, on the host, and sent to the host after a device decode error.
+    # waiting for it, the seconds next_batch spent building groups (wait included), and the images decoded on the device, on the host, and sent to the host after a device decode error;
+    # png_images counts the device-decoded images that were PNG files.
     # DECODE_BATCHES: see DESIGN §4.
     DECODE_BATCHES = 4
 
@@ -302,21 +304,26 @@ class Dataloader(object):
         return idx, aug
 
     def _read_group(self, paths, sizes):
-        """Background thread: file bytes -> ([(size, device-decodable file positions, JpegPlan)] per size in `sizes` that
-        has files).  File reads and the ctypes parser calls release the GIL."""
+        """Background thread: file bytes -> ([(size, device-decodable file positions, JpegPlan or PngPlan)] per format and
+        size in `sizes` that has files).  File reads and the ctypes parser calls release the GIL."""
         from . import ops
         t0 = time.perf_counter()
-        blobs, take = {s: [] for s in sizes}, {s: [] for s in sizes}
+        kinds = ((ops.jpeg_parse, ops.JpegPlan), (ops.png_parse, ops.PngPlan))
+        blobs = [{s: [] for s in sizes} for _ in kinds]
+        take = [{s: [] for s in sizes} for _ in kinds]
         for k, path in enumerate(paths):
             try:
                 with open(path, "rb") as f:
                     b = f.read()
             except OSError:
                 continue                                       # _read_image raises the host path's error
-            info = ops.jpeg_parse(b)
-            if info.reason == 0 and (info.height, info.width) in blobs:
-                blobs[(info.height, info.width)].append(b); take[(info.height, info.width)].append(k)
-        plans = [(s, take[s], ops.JpegPlan(blobs[s], *s)) for s in sizes if blobs[s]]
+            for j, (parse, _) in enumerate(kinds):
+                info = parse(b)
+                if info.reason == 0:
+                    if (info.height, info.width) in blobs[j]:
+                        blobs[j][(info.height, info.width)].append(b); take[j][(info.height, info.width)].append(k)
+                    break
+        plans = [(s, take[j][s], plan(blobs[j][s], *s)) for j, (_, plan) in enumerate(kinds) for s in sizes if blobs[j][s]]
         return plans, time.perf_counter() - t0
 
     def _submit_group(self):
@@ -342,15 +349,18 @@ class Dataloader(object):
         h, w = self._decode_sizes()[0]                          # the size the batch is assembled at
         imgs = torch.empty(len(paths), h, w, 3, dtype=torch.uint8, device=dev)
         host = set(range(len(paths)))
+        from . import ops
         for size, take, plan in plans:
-            out, status = plan.decode(dev)
+            png = isinstance(plan, ops.PngPlan)
+            out, status = plan.decode(dev, rgb=True) if png else plan.decode(dev)      # RGB, as _read_image returns
             if size != (h, w):
-                from . import ops
                 out = ops.resize_area_up_u8(out, h, w)           # network-size files of the real-data set
             imgs[torch.tensor(take, device=dev)] = out
             bad = [take[k] for k in np.flatnonzero(status.cpu().numpy())]
             host = (host - set(take)) | set(bad)
             st["device_images"] += len(take) - len(bad); st["decode_errors"] += len(bad)
+            if png:
+                st["png_images"] += len(take) - len(bad)
         host = sorted(host)
         st["host_images"] += len(host)
         if host:

@@ -419,6 +419,64 @@ def decode_jpeg(blobs, h, w):
     return out, status
 
 
+# ------------------------------------------------------------------ PNG decode
+def png_parse(blob):
+    """One file's bytes -> _lib.PngInfo (host only): size, bit depth, colour type, interlace, the zlib stream's length
+    and `reason`, 0 when the device decoder takes the file, else one of _lib.PNG_R."""
+    info = _lib.PngInfo()
+    buf = np.frombuffer(blob, np.uint8) if len(blob) else np.zeros(1, np.uint8)
+    check(lib.udh_png_parse(buf.ctypes.data, len(blob), ctypes.byref(info)), "udh_png_parse")
+    return info
+
+
+class PngPlan:
+    """Host side of one PNG decode launch: the files' IDAT payloads concatenated in pinned memory (each file's zlib stream
+    contiguous) and the per-file descriptor."""
+
+    def __init__(self, blobs, h, w):
+        offs = np.zeros(len(blobs) + 1, np.int64)
+        offs[1:] = np.cumsum([len(b) for b in blobs])
+        self.n, self.h, self.w = len(blobs), h, w
+        pin = torch.cuda.is_available()                  # the plan itself is host-only; pinning needs a device
+        files = np.zeros(max(int(offs[-1]), 1), np.uint8)
+        for k, b in enumerate(blobs):
+            files[offs[k]:offs[k + 1]] = np.frombuffer(b, np.uint8)
+        nidat = ctypes.c_int64(0)
+        nb = lib.udh_png_plan_bytes(files.ctypes.data, offs.ctypes.data, self.n, h, w, ctypes.byref(nidat))
+        if nb == 0:
+            raise _lib.UdhError("udh_png_plan_bytes: %s" % lib.udh_last_error().decode())
+        self.idat = torch.empty(max(nidat.value, 1), dtype=torch.uint8, pin_memory=pin)
+        self.plan = torch.empty(nb, dtype=torch.uint8, pin_memory=pin)
+        check(lib.udh_png_plan(files.ctypes.data, offs.ctypes.data, self.n, h, w, self.plan.data_ptr(), nb, self.idat.data_ptr(),
+                               self.idat.numel()), "udh_png_plan")
+
+    def decode(self, device=None, rgb=False):
+        """-> (uint8 [N,h,w,3], int32 [N] status) on the current stream: BGR as cv2.imread returns it (RGB when rgb);
+        nonzero status = that image failed (one of _lib.PNG_E) and its output is undefined."""
+        dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        plan_d = self.plan.to(dev, non_blocking=True)
+        idat_d = self.idat.to(dev, non_blocking=True)
+        out = torch.empty(self.n, self.h, self.w, 3, device=dev, dtype=torch.uint8)
+        status = torch.empty(self.n, device=dev, dtype=torch.int32)
+        nbytes = lib.udh_png_workspace_bytes(self.plan.data_ptr())
+        ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+        check(lib.udh_png_decode(self.plan.data_ptr(), _ptr(plan_d), _ptr(idat_d), _ptr(out), _ptr(status), int(bool(rgb)), _ptr(ws),
+                                 nbytes, _stream()), "udh_png_decode")
+        return out, status
+
+
+def decode_png(blobs, h, w, rgb=False):
+    """PNG files (bytes) the parser accepts, all h x w -> (uint8 [N,h,w,3] CUDA tensor, int32 [N] status): bit-identical to
+    cv2.imread(..., IMREAD_COLOR) (BGR; RGB when rgb).  Raises UdhError naming the first file the device could not decode."""
+    _lib.require_device()
+    out, status = PngPlan(blobs, h, w).decode(rgb=rgb)
+    st = status.cpu().numpy()
+    bad = np.flatnonzero(st)
+    if len(bad):
+        raise _lib.UdhError("decode_png: image %d failed with status %d (%d of %d images failed)" % (bad[0], st[bad[0]], len(bad), len(st)))
+    return out, status
+
+
 # ------------------------------------------------------------------ baseline-JPEG encode
 def encode_jpeg_device(imgs, quality=95):
     """uint8 CUDA tensor [N,h,w,3] (BGR) or [N,h,w] (gray) -> (out uint8 [N,cap], nbytes int64 [N], status int32 [N]) on the
