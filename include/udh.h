@@ -516,10 +516,6 @@ int udh_debug_x3_materialize(void* ws, size_t ws_bytes, int B, int P, size_t* fp
  * activation is never stored; row-tile dgrad).  on = 0 selects the generic flattened-tile kernels + the separate pool kernel —
  * tests compare the two paths and need the un-fused one to read conv1_2's activation. */
 int udh_debug_x3_set_rows(int on);
-/* The UDH_NUMERIC_BF16X3 3x3 convolutions hand each work item's accumulators to a dedicated epilogue warpgroup by default, so
- * the tensor cores start the next item while the previous one is stored.  on = 0 selects the kernel whose MMA warpgroups run
- * the epilogue themselves; both produce bit-identical results (tests compare them).  Also set by UDH_X3_EPI_WG=0. */
-int udh_debug_x3_set_epi_wg(int on);
 size_t udh_debug_x3_scratch_bytes(int B, int H, int W, int cin, int cout);
 int udh_debug_x3_conv(const float* x, const float* w, const float* bias, float* out, void* scratch, int B, int H, int W, int cin,
                       int cout, int relu, int dgrad, void* stream);

@@ -107,7 +107,6 @@ SIGNATURES = {
                                     c_int, c_float, c_float, c_float, c_float, c_float, c_int, c_void_p]),
     "udh_debug_x3_materialize": (c_int, [c_void_p, c_size_t, c_int, c_int, POINTER(c_size_t), c_void_p]),
     "udh_debug_x3_set_rows": (c_int, [c_int]),
-    "udh_debug_x3_set_epi_wg": (c_int, [c_int]),
     "udh_debug_x3_scratch_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
     "udh_debug_x3_conv": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
                                   c_void_p]),

@@ -228,35 +228,20 @@ __global__ void pool_bwd_x3_kernel(const uint32_t* __restrict__ codes, const uin
 }
 
 // ---------------------------------------------------------------------------------------------------- launchers
-// The two-limb convs hand each item's accumulators to a dedicated epilogue warpgroup (tc_conv_x3_epiwg_kernel) by default;
-// UDH_X3_EPI_WG=0 / udh_debug_x3_set_epi_wg(0) select tc_conv_x3_kernel, which drains them in the MMA warpgroups (tests
-// compare the two bit for bit)
-int g_x3_epi_wg = [] { const char* e = getenv("UDH_X3_EPI_WG"); return (e && e[0] == '0') ? 0 : 1; }();
-
-// one launch of either kernel of the instance <N_OUT, CB, T, ..., ROWS>: weight-ring depth and shared memory for that kernel
+// one launch of the instance <N_OUT, CB, T, ..., ROWS>: weight-ring depth and shared memory for its geometry
 template <int N_OUT, int CB, int T, int FA, int FW, int FO, int ROWS>
 int launch_conv_x3_kernel(const CUtensorMap& tmA128, const CUtensorMap& tmAhh, const CUtensorMap& tmW, const CUtensorMap& tmOut,
                           const tc::ConvGeom& g, const float* bias, const uint32_t* mask_bits, uint32_t* mask_out, float* out_f32,
                           int relu, float out_scale, cudaStream_t st) {
   const int sms = persistent_ctas();
   const int grid = g.num_items < sms ? g.num_items : sms;
-  if (g_x3_epi_wg) {
-    using S = tc::ConvX3EpiSmem<N_OUT, CB, T>;
-    const int stages = S::stages(g.abuf_rows);        // weight-ring depth: as many stages as shared memory holds (<= 6)
-    UDH_REQUIRE(stages >= 2, "tc conv x3: activation rows (%d x %d blocks) leave no room for the weight ring", g.abuf_rows, 2 * CB);
-    const size_t smem = S::fixed_bytes(g.abuf_rows) + (size_t)stages * S::kWStageBytes;
-    auto kern = tc::tc_conv_x3_epiwg_kernel<N_OUT, CB, T, FA, FW, FO, ROWS>;
-    UDH_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    launch_chain(kern, dim3(grid), dim3(512), smem, st, tmA128, tmAhh, tmW, tmOut, g, stages, bias, mask_bits, mask_out, out_f32, relu, out_scale);
-    return check_launch("tc_conv_x3_epiwg_kernel");
-  }
   using S = tc::ConvX3Smem<N_OUT, CB, T>;
-  const int stages = S::stages(g.abuf_rows);
+  const int stages = S::stages(g.abuf_rows);          // weight-ring depth: as many stages as shared memory holds (<= 6)
   UDH_REQUIRE(stages >= 2, "tc conv x3: activation rows (%d x %d blocks) leave no room for the weight ring", g.abuf_rows, 2 * CB);
   const size_t smem = S::fixed_bytes(g.abuf_rows) + (size_t)stages * S::kWStageBytes;
   auto kern = tc::tc_conv_x3_kernel<N_OUT, CB, T, FA, FW, FO, ROWS>;
   UDH_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  launch_chain(kern, dim3(grid), dim3(384), smem, st, tmA128, tmAhh, tmW, tmOut, g, stages, bias, mask_bits, mask_out, out_f32, relu, out_scale);
+  launch_chain(kern, dim3(grid), dim3(512), smem, st, tmA128, tmAhh, tmW, tmOut, g, stages, bias, mask_bits, mask_out, out_f32, relu, out_scale);
   return check_launch("tc_conv_x3_kernel");
 }
 
@@ -756,11 +741,6 @@ int x3_debug_conv1(const float* I1, const float* I2, const float* w, const float
 
 extern "C" int udh_debug_x3_set_rows(int on) {
   udh::g_x3_rows = on != 0;
-  return UDH_OK;
-}
-
-extern "C" int udh_debug_x3_set_epi_wg(int on) {
-  udh::g_x3_epi_wg = on != 0;
   return UDH_OK;
 }
 

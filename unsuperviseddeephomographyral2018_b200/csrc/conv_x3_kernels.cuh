@@ -12,18 +12,17 @@
 // next item's phase LO — each limb buffer has its own full/empty mbarrier pair, and a dedicated producer warp so that the
 // weight ring (a second producer warp) never waits behind an activation buffer.  Weights always stream through a TMA ring
 // (hi + lo of all 9 taps do not fit next to the activations); each ring block is reused by the T tiles of the item.
-//   warpgroup 0: weight-ring producer (warp 0), activation producer (warp 3) | warpgroups 1-2: MMA | warpgroup 3: epilogue
-//   (tc_conv_x3_epiwg_kernel, below; tc_conv_x3_kernel keeps the epilogue in the MMA warpgroups).
+//   warpgroup 0: weight-ring producer (warp 0), activation producer (warp 3) | warpgroups 1-2: MMA | warpgroup 3: epilogue.
 // Phase order: HI first (its first MMA initialises the accumulators), then LO.
 // 128 output channels: each MMA warpgroup owns 64 of the 128 rows of every tile, D[pos][co] = X . W with the activation
-// rows as A and the ring stage as B (m64n128k16), drained through stage_acc32 as in the bf16 kernel.
+// rows as A and the ring stage as B (m64n128k16).
 // 64 output channels (TR): the tile is transposed, D^T[co][pos] = W . X^T: the ring stage [64 co][64 ci] is the A operand
 // and 128 activation rows are the B operand, so each MMA is an m64n128k16 (2 KB + 4 KB of shared memory per 131 072 MACs)
 // instead of two m64n64k16 (4 KB + 4 KB); at N = 64 the operand reads alone would need all 128 B/clk of shared memory at
 // tensor peak.  MMA warpgroup cw owns the whole tile t = cw.  Every output element sees the same chain of k16 partial
 // products as in the untransposed tile (same stages, same k-step order, same first / accumulate flags).  The epilogue
-// transposes the fragment back through shared memory (stage_acc_tr) so that, as for 128 channels, one thread works on 32
-// channels of one position.
+// warpgroup reads the fragment column-wise out of the shared-memory handoff so that, as for 128 channels, one thread works
+// on 32 channels of one position.
 #pragma once
 #include "conv_tc_kernels.cuh"
 
@@ -32,40 +31,13 @@ namespace tc {
 
 constexpr int kX3MaxStages = 6;
 
-template <int N_OUT, int CB, int T>
-struct ConvX3Smem {
-  static constexpr int kWStageBytes = N_OUT * 128;
-  // fixed part: alignment slack + both limbs of the A rows + epilogue staging + accumulator transpose blocks + barriers
-  static size_t fixed_bytes(int abuf_rows) { return 1024 + (size_t)2 * CB * abuf_rows * 128 + kEpiStageBytes + 2 * kStg32Bytes + 256; }
-  static int stages(int abuf_rows) {
-    const long long left = 232448ll - (long long)fixed_bytes(abuf_rows);
-    const int s = (int)(left / kWStageBytes);
-    return s > kX3MaxStages ? kX3MaxStages : s;
-  }
-};
-
-// Transposed fragment (TR: rows = 64 channels, columns = 128 positions) -> positions [32 r, 32 r + 32), all 64 channels, as a
-// [32 positions][kStgStride] fp32 block (r may be a runtime value: every register index stays static).  The bank of element
-// (pos, co) is 4 pos + co mod 32, so a warp's stores are conflict-free, and so are lds_read32's row reads.
-// Stores go through a 32-bit shared address: the 16 offsets then fold into immediates instead of 16 generic pointers.
-__device__ __forceinline__ void stage_acc_tr(const float (&d)[64], int r, float* stg) {
-  const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
-  const uint32_t p0 = smem_u32(stg) + (uint32_t)(2 * (lane & 3) * kStgStride + 16 * w + (lane >> 2)) * 4;
-#pragma unroll
-  for (int i = 0; i < 64; ++i) {
-    if ((i >> 4) != r) continue;
-    const uint32_t off = (uint32_t)((8 * ((i >> 2) & 3) + (i & 1)) * kStgStride + 8 * ((i >> 1) & 1)) * 4;
-    asm volatile("st.shared.f32 [%0], %1;" ::"r"(p0 + off), "f"(d[i]) : "memory");
-  }
-}
-// v[j] = 32 consecutive fp32 at shared address addr (a row of a stage_acc_tr block)
+// v[j] = 32 consecutive fp32 at shared address addr (part of a handoff row)
 __device__ __forceinline__ void lds_read32(uint32_t addr, float (&v)[32]) {
 #pragma unroll
   for (int j = 0; j < 8; ++j)
     asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v[4 * j]), "=f"(v[4 * j + 1]), "=f"(v[4 * j + 2]), "=f"(v[4 * j + 3])
                  : "r"(addr + 16 * j) : "memory");
 }
-static_assert(32 * kStgStride * 4 <= kStg32Bytes, "a transposed quarter tile fits a warpgroup's staging block");
 
 // The weight ring has `stages` slots (a runtime value: as many as shared memory holds next to the activation rows).
 // ROWS (W == 128 images, 64 -> 64 channels, T == 2: conv1_2).  An item is the interior of two consecutive image rows
@@ -76,9 +48,6 @@ static_assert(32 * kStgStride * 4 <= kStg32Bytes, "a transposed quarter tile fit
 //              the 3-bit routing codes of the max-pool backward are written; the full-resolution activation (554 MB in this
 //              mode) is never written or re-read;
 //   ROWS == 2: the ordinary epilogue (bias / ReLU-backward mask / limb split / TMA store) on row tiles (the dgrad).
-// Two kernels share the producers and the MMA main loop below: tc_conv_x3_epiwg_kernel (the default) hands every item's
-// fragment to a dedicated epilogue warpgroup and goes straight on to the next item's MMAs; tc_conv_x3_kernel drains its own
-// accumulators between items.  Both sum the same chain of k16 products, so they produce bit-identical results.
 
 // first position of an item and distance between its tiles (in positions)
 template <int T, int ROWS>
@@ -87,7 +56,9 @@ __device__ __forceinline__ int x3_item_q0(const ConvGeom& g, int item) {
 }
 
 // activation producer (one thread): both limbs of the A rows of every item, hi limb first (the consumption order).
-// lo_free (nullable): a second barrier whose phase must also complete before the lo buffer of the next item is loaded.
+// lo_free: the epilogue's h_empty, whose phase must also complete before the lo buffer of the next item is loaded (the
+// handoff lives in that buffer).  The kernel always passes it; the null test stays because without it ptxas allocates
+// registers differently in every instance.
 template <int CB, int T, int ROWS>
 __device__ __forceinline__ void x3_produce_acts(const CUtensorMap* tmA128, const CUtensorMap* tmAhh, const ConvGeom& g, int my_items,
                                                 uint8_t* sA, uint64_t* a_full, uint64_t* a_empty, uint64_t* lo_free) {
@@ -191,261 +162,12 @@ __device__ __forceinline__ void x3_mma_item(float (&acc)[T * N_OUT / 2], int it,
   acc_fence(acc);
 }
 
-// Drains its accumulators in the MMA warpgroups (the in-warpgroup epilogue; UDH_X3_EPI_WG=0 selects it).
-//   warpgroup 0: weight-ring producer (warp 0), activation producer (warp 3) | warpgroups 1-2: MMA + epilogue.
-template <int N_OUT, int CB, int T, int FMT_A, int FMT_W, int FMT_O, int ROWS = 0>
-__global__ void __launch_bounds__(384, 1)
-tc_conv_x3_kernel(const __grid_constant__ CUtensorMap tmA128, const __grid_constant__ CUtensorMap tmAhh,
-                  const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmOut, const ConvGeom g,
-                  const int stages, const float* __restrict__ bias, const uint32_t* __restrict__ mask_bits,
-                  uint32_t* __restrict__ mask_out, float* __restrict__ out_f32, const int relu, const float out_scale) {
-  static_assert(FMT_A == kFmtBF16 && FMT_W == kFmtBF16, "wgmma multiplies limbs of one format");
-  extern __shared__ uint8_t raw[];
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw) + 1023) & ~(uintptr_t)1023);
-  const int abuf_bytes = g.abuf_rows * 128;                       // one 64-channel block of one limb
-  uint8_t* sA = base;                                             // [2 limbs][CB][abuf_rows][128]
-  uint8_t* sW = base + (size_t)2 * CB * abuf_bytes;               // [stages][N_OUT][128]
-  constexpr bool TR = N_OUT == 64;                                // transposed tile (see the top of this file)
-  static_assert(!TR || T == 2, "transposed tile: one 128-position tile per MMA warpgroup");
-  static_assert(ROWS == 0 || (N_OUT == 64 && CB == 1 && T == 2), "row tiles: the 64-channel instance with two tiles");
-  constexpr bool POOL = ROWS == 1;
-  const int tstep = ROWS ? g.Wp : 128;
-  constexpr int kTileRegs = N_OUT / 2;                            // fragment registers per tile
-  constexpr int kStageBytes = N_OUT * 128;                        // one ring stage: [N_OUT][64] of one limb
-  uint8_t* sEpi = sW + (size_t)stages * kStageBytes;              // [4 quarters][32 rows][128 B]
-  float* sStg = reinterpret_cast<float*>(sEpi + kEpiStageBytes);  // [2 warpgroups][kStg32Bytes]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(sStg) + 2 * kStg32Bytes);
-  uint64_t* a_full = bars;            // [2] per limb (0 = hi, 1 = lo)
-  uint64_t* a_empty = bars + 2;       // [2]
-  uint64_t* w_full = bars + 4;        // [kX3MaxStages]
-  uint64_t* w_empty = bars + 4 + kX3MaxStages;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  static_assert(T <= 4, "mask prefetch registers are sized for T <= 4");
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < 2; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 256); }
-    for (int i = 0; i < kX3MaxStages; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], 256); }
-    fence_barrier_init();
-  }
-  if (warp == 0 && lane == 0) { prefetch_tmap(&tmW); prefetch_tmap(&tmOut); }
-  if (warp == 3 && lane == 0) { prefetch_tmap(&tmA128); prefetch_tmap(&tmAhh); }
-  __syncthreads();
-  const int my_items = (g.num_items - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;   // items blockIdx.x + i*gridDim.x
-  pdl_wait();                  // predecessor grid complete: global memory may be touched from here on
-  pdl_trigger();
-
-  if (warp < 4) {
-    regs_dec<40>();
-    if (warp == 3 && lane == 0) x3_produce_acts<CB, T, ROWS>(&tmA128, &tmAhh, g, my_items, sA, a_full, a_empty, nullptr);
-    else if (warp == 0 && lane == 0) x3_produce_weights<N_OUT, CB>(&tmW, my_items, stages, sW, w_full, w_empty);
-  } else {
-    regs_inc<232>();
-    const int cw = (warp - 4) >> 2;               // MMA warpgroup: TR: tile cw; else rows [64 cw, 64 cw + 64) of every tile
-    const int wi = warp & 3;
-    const int ew = 2 * cw + (wi & 1);             // staging block (pair of warps) this warp drains through
-    const int eg = wi >> 1;                       // 32-channel chunk this warp drains
-    const int erow = 32 * (wi & 1) + lane;
-    float* stg = sStg + cw * (kStg32Bytes / 4);
-    auto wg_sync = [&]() { named_sync(5 + cw, 128); };
-    // first position of the 32 this warp drains in epilogue slot s (a tile of the item; TR: a half of the warpgroup's tile)
-    auto slot_q0 = [&](int q0, int s) { return TR ? q0 + cw * tstep + (2 * s + (wi & 1)) * 32 : q0 + ew * 32 + s * tstep; };
-    const uint32_t a_addr0 = smem_u32(sA) + (uint32_t)(TR ? cw * tstep : 64 * cw) * 128;
-    const uint32_t w_lo0 = desc_lo(smem_u32(sW), 16);
-    uint32_t ws = 0, wpar = 0;
-    float acc[T * kTileRegs];
-    // 32 columns (block b32 of the fragment) of row erow of the warpgroup, for the warps of chunk parity eg; every warp
-    // of the warpgroup takes part (two transpose rounds, one per parity)
-    auto fetch = [&](int b32, float (&v)[32]) {
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        wg_sync(); stage_acc32(acc, b32 + e, stg); wg_sync();
-        if (e == eg) stg32_read32(stg, erow, v);
-      }
-    };
-    // TR: channel chunk eg of position 32 (2 s + (wi & 1)) + lane of the warpgroup's tile (two quarter rounds)
-    const uint32_t my_stg_row = smem_u32(stg) + (uint32_t)(lane * kStgStride + 32 * eg) * 4;
-    auto fetch_tr = [&](int s, float (&v)[32]) {
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        wg_sync(); stage_acc_tr(acc, 2 * s + e, stg); wg_sync();
-        if (e == (wi & 1)) lds_read32(my_stg_row, v);
-      }
-    };
-    const int HpWp = g.Hp * g.Wp;
-    uint8_t* estg = sEpi + ew * 4096;
-    const uint32_t my_row = smem_u32(estg) + lane * 128;
-    const int sw = lane & 7;
-    const bool issuer = eg == 0 && lane == 0;
-    auto pair_sync = [&]() { named_sync(1 + ew, 64); };
-    bool store_pending = false;
-    for (int it = 0; it < my_items; ++it) {
-      const int item = (int)blockIdx.x + it * (int)gridDim.x;
-      const int q0 = x3_item_q0<T, ROWS>(g, item);
-      // ReLU-backward mask words (1 bit / element) of all T epilogue slots, requested before the MMAs
-      uint32_t mbt[T][2];
-      if (!POOL) {
-#pragma unroll
-        for (int t = 0; t < T; ++t) {
-          const int qt = slot_q0(q0, t) + lane;
-          const bool ok = mask_bits && qt < g.Q;
-          if (N_OUT == 64) {
-            mbt[t][0] = ok ? __ldg(mask_bits + (size_t)qt * 2 + eg) : 0u; mbt[t][1] = 0u;
-          } else {
-            mbt[t][0] = ok ? __ldg(mask_bits + (size_t)qt * 4 + eg) : 0u;
-            mbt[t][1] = ok ? __ldg(mask_bits + (size_t)qt * 4 + 2 + eg) : 0u;
-          }
-        }
-      }
-      // ===================================== MMA =====================================
-      x3_mma_item<N_OUT, CB, T>(acc, it, g, stages, a_addr0, w_lo0, a_full, a_empty, w_full, w_empty, ws, wpar);
-      // ===================================== epilogue =====================================
-      if constexpr (POOL) {
-        // thread = image column x (W == 128 == tile rows); warps of parity eg pool the 32-channel chunk eg.  Warpgroup cw holds
-        // image row 2y + cw: in round r both stage quarter r of their row and the warps with ew == r read both blocks.
-        const int OH = g.H >> 1, OW = g.W >> 1;
-        const int x = ew * 32 + lane;
-        const int px = x >> 1, odd = x & 1;
-        uint16_t* out_pool = reinterpret_cast<uint16_t*>(out_f32);             // pooled two-limb stream [B][OH+2][OW+2][hi 64 | lo 64]
-        const int n = item / OH, yy = item - n * OH;
-        uint16_t* prow = out_pool + (((size_t)n * (OH + 2) + yy + 1) * (OW + 2) + px + 1) * 128;
-        uint32_t* crow = mask_out + (((size_t)n * OH + yy) * OW + px) * 8;
-        const int c = eg;
-        // scan order of the 2x2 window: (row 0, x even)=0, (row 0, x odd)=1, (row 1, even)=2, (row 1, odd)=3; the first
-        // maximum wins: larger value, ties to the smaller index.  The reader takes the vertical maximum of bias + ReLU as it
-        // reads (vs, and bit j of `lower` when row 1 is strictly larger), so only 32 values stay live next to the accumulators.
-        float vs[32];
-        uint32_t lower = 0u;
-        const uint32_t row0 = smem_u32(sStg) + (uint32_t)(lane * kStgStride + 32 * eg) * 4;
-#pragma unroll
-        for (int r = 0; r < 4; ++r) {
-          named_sync(7, 256); stage_acc_tr(acc, r, stg); named_sync(7, 256);
-          if (r == ew) {
-            float v0[32], v1[32];
-            lds_read32(row0, v0); lds_read32(row0 + kStg32Bytes, v1);
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const float bj = __ldg(bias + c * 32 + j);
-              const float a = fmaxf(v0[j] + bj, 0.f), d = fmaxf(v1[j] + bj, 0.f);
-              vs[j] = a;
-              if (d > a) { vs[j] = d; lower |= 1u << j; }
-            }
-          }
-        }
-        uint32_t code[4] = {0u, 0u, 0u, 0u};
-        float m[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const uint32_t ks = ((lower >> j) & 1u) * 2u + (uint32_t)odd;
-          const float vo = __shfl_xor_sync(0xffffffffu, vs[j], 1);
-          const uint32_t ko = __shfl_xor_sync(0xffffffffu, ks, 1);
-          const bool other = vo > vs[j] || (vo == vs[j] && ko < ks);
-          const float mv = other ? vo : vs[j];
-          const uint32_t mk = other ? ko : ks;
-          m[j] = mv;
-          code[j >> 3] |= (mv > 0.f ? mk : 4u) << (3 * (j & 7));
-        }
-        // both lanes of a pair hold the pooled pixel: the even lane stores channels 0-15 of this chunk, the odd 16-31
-        uint32_t ph_[8], pl_[8];
-#pragma unroll
-        for (int h = 0; h < 8; ++h) split2<FMT_O>(odd ? m[16 + 2 * h] : m[2 * h], odd ? m[17 + 2 * h] : m[2 * h + 1], ph_[h], pl_[h]);
-        uint4* oh = reinterpret_cast<uint4*>(prow + c * 32 + odd * 16);
-        oh[0] = make_uint4(ph_[0], ph_[1], ph_[2], ph_[3]); oh[1] = make_uint4(ph_[4], ph_[5], ph_[6], ph_[7]);
-        uint4* ol = reinterpret_cast<uint4*>(prow + 64 + c * 32 + odd * 16);
-        ol[0] = make_uint4(pl_[0], pl_[1], pl_[2], pl_[3]); ol[1] = make_uint4(pl_[4], pl_[5], pl_[6], pl_[7]);
-        *reinterpret_cast<uint2*>(crow + c * 4 + odd * 2) = odd ? make_uint2(code[2], code[3]) : make_uint2(code[0], code[1]);
-      } else {
-        // Both warps of a quarter fill their halves of the quarter's 32 x 128 B staging block, meet at a 64-thread named
-        // barrier, and one lane issues the TMA store; the hi block and the lo block of a half go through the same block.
-#pragma unroll 1
-        for (int t = 0; t < T; ++t) {
-          const int q0w = slot_q0(q0, t);
-          const int q = q0w + lane;
-          const int n = q / HpWp, rem = q - n * HpWp;
-          const int yp = rem / g.Wp, xp = rem - yp * g.Wp;
-          const bool valid = q < g.Q && xp >= 1 && xp <= g.W && yp >= 1 && yp <= g.H;
-          const size_t o_f32 = (((size_t)n * g.H + (yp - 1)) * g.W + (xp - 1)) * N_OUT;
-          uint32_t mo[N_OUT / 64];
-#pragma unroll
-          for (int hf = 0; hf < N_OUT / 64; ++hf) {
-            const int c = hf * 2 + eg;
-            float v[32];
-            if constexpr (TR) fetch_tr(t, v);
-            else fetch(t * (N_OUT / 32) + hf * 2, v);
-            if (out_scale != 1.0f) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) v[j] *= out_scale;
-            }
-            if (bias) {
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                const float4 bv = __ldg(reinterpret_cast<const float4*>(bias + c * 32 + j));
-                v[j] += bv.x; v[j + 1] += bv.y; v[j + 2] += bv.z; v[j + 3] += bv.w;
-              }
-            }
-            if (relu) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-            }
-            if (mask_bits) {
-              const uint32_t w = mbt[t][hf];
-#pragma unroll
-              for (int j = 0; j < 32; ++j) v[j] = ((w >> j) & 1u) ? v[j] : 0.f;
-            }
-            mo[hf] = 0u;
-            if (mask_out) {
-              uint32_t w = 0;
-#pragma unroll
-              for (int j = 0; j < 32; ++j) w |= (v[j] > 0.f ? 1u : 0u) << j;
-              mo[hf] = w;
-            }
-            uint32_t hi[16], lo[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              if (valid) split2<FMT_O>(v[2 * j], v[2 * j + 1], hi[j], lo[j]);
-              else { hi[j] = 0u; lo[j] = 0u; }                       // border / out-of-range positions store zeros
-            }
-#pragma unroll
-            for (int limb = 0; limb < 2; ++limb) {
-              // the staging block may still be read by the previous TMA store
-              if (store_pending) { if (issuer) bulk_wait_read0(); pair_sync(); }
-#pragma unroll
-              for (int j4 = 0; j4 < 4; ++j4) {
-                const uint32_t addr = my_row + (uint32_t)(((eg * 4 + j4) ^ sw) << 4);
-                const uint32_t* src = limb ? lo : hi;
-                asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(src[j4 * 4]), "r"(src[j4 * 4 + 1]),
-                             "r"(src[j4 * 4 + 2]), "r"(src[j4 * 4 + 3]) : "memory");
-              }
-              fence_proxy_async();                    // generic-proxy smem writes -> visible to the TMA engine
-              pair_sync();                            // both 64-byte halves of every row are in place
-              if (issuer && q0w < g.Q) { tma_store_2d(&tmOut, estg, limb * N_OUT + hf * 64, q0w); bulk_commit(); }
-              store_pending = true;
-            }
-            if (out_f32 && valid) {
-              float4* fp = reinterpret_cast<float4*>(out_f32 + o_f32 + c * 32);
-#pragma unroll
-              for (int j = 0; j < 8; ++j) fp[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-            }
-          }
-          if (mask_out && q < g.Q) {
-#pragma unroll
-            for (int hf = 0; hf < N_OUT / 64; ++hf) mask_out[(size_t)q * (N_OUT / 32) + hf * 2 + eg] = valid ? mo[hf] : 0u;
-          }
-        }
-      }
-    }
-    if (!POOL && issuer) bulk_wait0();
-    __syncwarp();
-  }
-}
-
 // ---- warp-specialised epilogue ---------------------------------------------------------------------------------------
-// tc_conv_x3_epiwg_kernel: a fourth warpgroup owns the epilogue, so the tensor pipe is not idle while an item drains.
-//   warpgroup 0: weight-ring producer (warp 0), activation producer (warp 3) | warpgroups 1-2: MMA | warpgroup 3: epilogue.
+// tc_conv_x3_kernel: a fourth warpgroup owns the epilogue, so the tensor pipe is not idle while an item drains.
 // After an item's last MMA (phase LO), each MMA warpgroup writes its raw fp32 fragment (64 rows x 128 columns) into the
 // HANDOFF, arrives on h_full and goes straight on to the next item; the epilogue warpgroup reads the handoff, arrives on
-// h_empty, and applies bias / ReLU / masks / limb split / TMA stores (or, ROWS == 1, the fused pool1) exactly as the
-// in-warpgroup epilogue does.  The handoff is 128 rows of kHandRowBytes: fragment row i of MMA warpgroup cw is handoff row
+// h_empty, and applies bias / ReLU / masks / limb split / TMA stores (or, ROWS == 1, the fused pool1).
+// The handoff is 128 rows of kHandRowBytes: fragment row i of MMA warpgroup cw is handoff row
 // 64 cw + i (positions x channels; TR: channels x positions).  It lives in the lo-limb A buffer, whose rows are no longer
 // read once phase LO is complete and which is refilled only for the next item's phase LO: the rows that do not fit there
 // take a dedicated tail block.  Protocol, per item it:
@@ -461,7 +183,7 @@ constexpr int kX3EpiRegsProducer = 40, kX3EpiRegsMma = 176, kX3EpiRegsEpi = 112;
 static_assert(128 * (kX3EpiRegsProducer + kX3EpiRegsEpi) + 256 * kX3EpiRegsMma <= 65536, "register file of a 512-thread CTA");
 
 template <int N_OUT, int CB, int T>
-struct ConvX3EpiSmem {
+struct ConvX3Smem {
   static constexpr int kWStageBytes = N_OUT * 128;
   // handoff rows held by the lo-limb A buffer; the rest take the tail block
   __host__ __device__ static int alo_rows(int abuf_rows) { const int r = CB * abuf_rows * 128 / kHandRowBytes; return r < 128 ? r : 128; }
@@ -483,17 +205,17 @@ __device__ __forceinline__ float lds_f32(uint32_t addr) {
 
 template <int N_OUT, int CB, int T, int FMT_A, int FMT_W, int FMT_O, int ROWS = 0>
 __global__ void __launch_bounds__(512, 1)
-tc_conv_x3_epiwg_kernel(const __grid_constant__ CUtensorMap tmA128, const __grid_constant__ CUtensorMap tmAhh,
-                        const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmOut, const ConvGeom g,
-                        const int stages, const float* __restrict__ bias, const uint32_t* __restrict__ mask_bits,
-                        uint32_t* __restrict__ mask_out, float* __restrict__ out_f32, const int relu, const float out_scale) {
+tc_conv_x3_kernel(const __grid_constant__ CUtensorMap tmA128, const __grid_constant__ CUtensorMap tmAhh,
+                  const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmOut, const ConvGeom g,
+                  const int stages, const float* __restrict__ bias, const uint32_t* __restrict__ mask_bits,
+                  uint32_t* __restrict__ mask_out, float* __restrict__ out_f32, const int relu, const float out_scale) {
   static_assert(FMT_A == kFmtBF16 && FMT_W == kFmtBF16, "wgmma multiplies limbs of one format");
   constexpr bool TR = N_OUT == 64;
   static_assert(!TR || T == 2, "transposed tile: one 128-position tile per MMA warpgroup");
   static_assert(TR || T == 1, "128 output channels: one tile per item (64 rows of it per MMA warpgroup)");
   static_assert(ROWS == 0 || (N_OUT == 64 && CB == 1 && T == 2), "row tiles: the 64-channel instance with two tiles");
   constexpr bool POOL = ROWS == 1;
-  using S = ConvX3EpiSmem<N_OUT, CB, T>;
+  using S = ConvX3Smem<N_OUT, CB, T>;
   extern __shared__ uint8_t raw[];
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw) + 1023) & ~(uintptr_t)1023);
   const int abuf_bytes = g.abuf_rows * 128;

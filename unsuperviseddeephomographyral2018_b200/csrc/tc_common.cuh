@@ -319,29 +319,6 @@ __device__ __forceinline__ void stage_acc64(const float (&d)[K], int blk, float*
     *reinterpret_cast<float2*>(r0 + 8 * kStgStride + c) = make_float2(d[4 * j + 2], d[4 * j + 3]);
   }
 }
-// 32-column variant for kernels short of shared memory: columns [32 blk, 32 blk + 32) into a [64][kStg32Stride] block
-constexpr int kStg32Stride = 36;
-constexpr int kStg32Bytes = 64 * kStg32Stride * 4;
-template <int K>
-__device__ __forceinline__ void stage_acc32(const float (&d)[K], int blk, float* stg) {
-  const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
-  float* r0 = stg + (16 * w + (lane >> 2)) * kStg32Stride + 2 * (lane & 3);
-#pragma unroll
-  for (int j = 0; j < K / 4; ++j) {
-    if ((j >> 2) != blk) continue;
-    const int c = 8 * (j & 3);
-    *reinterpret_cast<float2*>(r0 + c) = make_float2(d[4 * j], d[4 * j + 1]);
-    *reinterpret_cast<float2*>(r0 + 8 * kStg32Stride + c) = make_float2(d[4 * j + 2], d[4 * j + 3]);
-  }
-}
-__device__ __forceinline__ void stg32_read32(const float* stg, int row, float (&v)[32]) {
-  const float4* p = reinterpret_cast<const float4*>(stg + row * kStg32Stride);
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const float4 x = p[j];
-    v[4 * j] = x.x; v[4 * j + 1] = x.y; v[4 * j + 2] = x.z; v[4 * j + 3] = x.w;
-  }
-}
 // every (row, column pair) of this warpgroup's 64-row fragment d to off(row, column) (nullptr: not stored); column is even
 template <int K, typename Off>
 __device__ __forceinline__ void store_acc(const float (&d)[K], Off off) {
