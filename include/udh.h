@@ -297,7 +297,9 @@ int udh_ecc_corr_h4p(const float* W, const int32_t* status, const float* gt, flo
  *   differ.  luts (device) [B][4][256][3] fp32 are the per-value tables T0..T3 (augment + normalise).  tab (device, int32,
  *   nullable when the sizes are equal): nx, ny, xofs[img_w+1], xsrc[nx], xw[nx], yofs[img_h+1], ysrc[ny], yw[ny] (weights
  *   as fp32 bits): OpenCV's computeResizeAreaTab entries of each output column / row in table order (ops.area_table);
- *   max_rows = the most entries of one output row.  The downscale is resizeArea's generic path: sequential fp32 sums, no FMA. */
+ *   max_rows = the most entries of one output row.  The downscale is resizeArea's generic path: sequential fp32 sums, no FMA.
+ *   Any full size: an output row's source rows are staged in shared memory (udh_real_prep_smem_bytes(max_rows, full_w))
+ *   when that fits in 227 KB, and read from global memory otherwise, with the same sums in the same order. */
 int udh_resize_area_up_u8(const uint8_t* src, const int32_t* tab, uint8_t* dst, int n, int src_h, int src_w, int dst_h, int dst_w,
                           void* stream);
 /* udh_resize_linear_u8: cv2.resize(src, (dst_w, dst_h)) with the default INTER_LINEAR on n uint8 [src_h,src_w,3] images, any
@@ -438,6 +440,15 @@ int udh_gen_warp_u8(const uint8_t* bgr, const double* theta, int n, int h, int w
                     uint8_t* warped_gray, void* stream);
 /* udh_gray_u8: bgr [npx,3] uint8 -> gray [npx] with udh_gen_warp_u8's gray rule (cv2.cvtColor(bgr, COLOR_RGB2GRAY)). */
 int udh_gray_u8(const uint8_t* bgr, int64_t npx, uint8_t* gray, void* stream);
+
+/* ---- image alignment's warp -----------------------------------------------------------------------------------------
+ * udh_warp_perspective_u8: cv2.warpPerspective(src, M, (dst_w, dst_h)) with its defaults (INTER_LINEAR, BORDER_CONSTANT,
+ *   border value 0), bit for bit: src [n,h,w,c] uint8 (c = 1 or 3), M [n,9] float64 row-major (device), dst [n,dst_h,dst_w,c].
+ *   M is inverted in float64 by cv2's 3x3 cofactor rule; source positions are rounded to 1/32 pixel in float64 (a zero
+ *   denominator lands on source pixel (0, 0), as in cv2); 15-bit bilinear weights; taps outside the source read 0.
+ *   n <= 65535, all sides < 32767.  oracle/warp_perspective.py restates it. */
+int udh_warp_perspective_u8(const uint8_t* src, const double* M, uint8_t* dst, int n, int h, int w, int c, int dst_h, int dst_w,
+                            void* stream);
 
 /* ---- instrumentation read by bench.py -------------------------------------------------------------------------
  * udh_launch_count: kernels this library has launched in this process (monotonic).

@@ -163,6 +163,7 @@ SIGNATURES = {
                                 c_size_t, c_void_p]),
     "udh_gen_warp_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "udh_gray_u8": (c_int, [c_void_p, c_int64, c_void_p, c_void_p]),
+    "udh_warp_perspective_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "udh_draw_report_workspace_bytes": (c_size_t, [c_int]),
     "udh_draw_report_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_int, c_int, c_int,
                                    c_void_p]),

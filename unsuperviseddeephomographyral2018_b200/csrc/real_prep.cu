@@ -44,9 +44,14 @@ __global__ void __launch_bounds__(256) resize_up_u8_kernel(const uint8_t* __rest
 // luts [B][4][256][3]: plain I, plain I', augmented I, augmented I' (output t reads image t & 1 through table t).
 // tab (int32, nullable = same size): nx, ny, then xofs[W+1], xsrc[nx], xw[nx] (fp32 bits), yofs[Hh+1], ysrc[ny], yw[ny]
 // (fp32 bits): the entries of output column dx are [xofs[dx], xofs[dx+1]), in OpenCV's table order.
-// One CTA per band of output rows of one sample; the source rows of the current output row are staged in shared memory.
+// One CTA per band of output rows of one sample.  STAGED: the source rows of the current output row are staged in shared
+// memory; otherwise (they do not fit: camera frames, e.g. 14 rows of 4000 px at 3000x4000 -> 240x320) they are read from
+// global memory through the read-only cache.  The two variants differ only in where the bytes come from: the same table
+// entries are summed in the same order.
 constexpr int kRealRowsPerCta = 16;
+constexpr size_t kRealPrepSmemMax = 227 * 1024;
 
+template <bool STAGED>
 __global__ void __launch_bounds__(256) real_prep_kernel(const uint8_t* __restrict__ I, const uint8_t* __restrict__ Ip,
                                                         const float* __restrict__ luts, const int32_t* __restrict__ tab,
                                                         int max_rows, int FH, int FW, int Hh, int W, float* __restrict__ oI,
@@ -80,11 +85,18 @@ __global__ void __launch_bounds__(256) real_prep_kernel(const uint8_t* __restric
   for (int dy = dy0; dy < dy1; ++dy) {
     const int k0 = yofs[dy], nk = yofs[dy + 1] - k0;
     __syncthreads();                                                   // previous row's readers are done (and the tables)
-    for (int i = threadIdx.x; i < nk * 2 * srclen; i += blockDim.x) {
-      const int k = i / (2 * srclen), r = i - k * 2 * srclen, im = r / srclen, x = r - im * srclen;
-      rows[(k * 2 + im) * srclen + x] = (im ? srcs[1] : srcs[0])[(size_t)ysrc[k0 + k] * srclen + x];
+    if (STAGED) {
+      for (int i = threadIdx.x; i < nk * 2 * srclen; i += blockDim.x) {
+        const int k = i / (2 * srclen), r = i - k * 2 * srclen, im = r / srclen, x = r - im * srclen;
+        rows[(k * 2 + im) * srclen + x] = (im ? srcs[1] : srcs[0])[(size_t)ysrc[k0 + k] * srclen + x];
+      }
+      __syncthreads();
     }
-    __syncthreads();
+    // byte s of source row k (of this output row) of image im
+    auto src_at = [&](int k, int im, int s) -> int {
+      if (STAGED) return rows[(k * 2 + im) * srclen + s];
+      return __ldg(srcs[im] + (size_t)ysrc[k0 + k] * srclen + s);
+    };
     for (int o = threadIdx.x; o < rowlen; o += blockDim.x) {
       const int dx = o / 3, c = o - dx * 3, j0 = xofs[dx], j1 = xofs[dx + 1];
       float sum[4];
@@ -96,7 +108,7 @@ __global__ void __launch_bounds__(256) real_prep_kernel(const uint8_t* __restric
           const int s = xsrc[j] * 3 + c;
 #pragma unroll
           for (int t = 0; t < 4; ++t)
-            buf[t] = __fadd_rn(buf[t], __fmul_rn(lut[t * 768 + rows[(k * 2 + (t & 1)) * srclen + s] * 3 + c], alpha));
+            buf[t] = __fadd_rn(buf[t], __fmul_rn(lut[t * 768 + src_at(k, t & 1, s) * 3 + c], alpha));
         }
 #pragma unroll
         for (int t = 0; t < 4; ++t) sum[t] = k == 0 ? __fmul_rn(beta, buf[t]) : __fadd_rn(sum[t], __fmul_rn(beta, buf[t]));
@@ -210,18 +222,19 @@ extern "C" int udh_real_prep(const uint8_t* I, const uint8_t* I_prime, const flo
   UDH_REQUIRE(B >= 1 && img_h >= 1 && img_w >= 1 && full_h >= img_h && full_w >= img_w, "udh_real_prep: bad dimensions");
   UDH_REQUIRE(tab || (full_h == img_h && full_w == img_w), "udh_real_prep: a resize needs the area tables");
   UDH_REQUIRE(!tab || max_rows >= 1, "udh_real_prep: max_rows must be >= 1");
-  const size_t smem = udh_real_prep_smem_bytes(tab ? max_rows : 0, full_w);
-  UDH_REQUIRE(smem <= 227 * 1024, "udh_real_prep: %zu bytes of shared memory needed (227 KB available)", smem);
+  const bool staged = udh_real_prep_smem_bytes(tab ? max_rows : 0, full_w) <= kRealPrepSmemMax;
+  const size_t smem = udh_real_prep_smem_bytes(staged && tab ? max_rows : 0, full_w);
   cudaStream_t st = as_stream(stream);
   ProfScope ps(PROF_ELTWISE, st);
+  auto kern = staged ? real_prep_kernel<true> : real_prep_kernel<false>;
   if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(real_prep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) {
       set_error("udh_real_prep: %s", cudaGetErrorString(e));
       return UDH_ECUDA;
     }
   }
-  real_prep_kernel<<<dim3((img_h + kRealRowsPerCta - 1) / kRealRowsPerCta, B), 256, smem, st>>>(
+  kern<<<dim3((img_h + kRealRowsPerCta - 1) / kRealRowsPerCta, B), 256, smem, st>>>(
       I, I_prime, luts, tab, max_rows, full_h, full_w, img_h, img_w, I_plain, I_prime_plain, I_aug, I_prime_aug);
   return check_launch("udh_real_prep");
 }

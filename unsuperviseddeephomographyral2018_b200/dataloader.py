@@ -77,6 +77,25 @@ def _value_table(g=None, br=None, c=None):
     return (v - np.array(synthetic.MEAN_I, np.float32)) / np.array(synthetic.STD_I, np.float32)
 
 
+def normalise_resize_host(t, img_h, img_w):
+    """The real-data host path's normalise + cv2 INTER_AREA resize of one fp32 [h,w,3] RGB image to the network size."""
+    import cv2
+    n = (t - np.array(synthetic.MEAN_I, np.float32)) / np.array(synthetic.STD_I, np.float32)
+    return cv2.resize(n, (img_w, img_h), interpolation=cv2.INTER_AREA) if t.shape[:2] != (img_h, img_w) else n
+
+
+def gather_patches(I_pl, Ip_pl, I_aug, Ip_aug, pts1, P, W):
+    """The real-data device path's patch step: patch_indices from each sample's first corner of pts1 [B,8] (CUDA fp32) and
+    the gray (channel-mean) P x P patches of the four network-size planes [B,Hh,W,3]."""
+    B, dev = pts1.shape[0], pts1.device
+    x0 = pts1[:, 0].long(); y0 = pts1[:, 1].long()
+    yy, xx = torch.meshgrid(torch.arange(P, device=dev), torch.arange(P, device=dev), indexing="ij")
+    pidx = ((yy[None] + y0[:, None, None]) * W + (xx[None] + x0[:, None, None])).reshape(B, -1)
+    g = lambda a: torch.gather(a.mean(dim=3).reshape(B, -1), 1, pidx).reshape(B, P, P, 1).contiguous()
+    return dict(I1=g(I_pl), I2=g(Ip_pl), I1_aug=g(I_aug), I2_aug=g(Ip_aug), I_aug=I_aug, I_prime_aug=Ip_aug,
+                pts1=pts1, gt=None, patch_indices=pidx.to(torch.int32).contiguous())
+
+
 class Dataloader(object):
     def __init__(self, params, shuffle=True, synthetic_pairs=0, seed=0, device="cuda", rho=45):
         self.params = params
@@ -137,7 +156,6 @@ class Dataloader(object):
         p = self.params
         B, P, Hh, W, FH, FW = p.batch_size, p.patch_size, p.img_h, p.img_w, p.full_img_h, p.full_img_w
         idx = self._next_indices(B)
-        mean, std = np.array(synthetic.MEAN_I, np.float32), np.array(synthetic.STD_I, np.float32)
         I_aug = np.empty((B, Hh, W, 3), np.float32); Ip_aug = np.empty_like(I_aug); I_pl = np.empty_like(I_aug); Ip_pl = np.empty_like(I_aug)
         full_I = np.empty((B, FH, FW, 3), np.uint8); full_Ip = np.empty_like(full_I)
         aug_tab = np.zeros((B, 11), np.float32)
@@ -164,7 +182,7 @@ class Dataloader(object):
                     g, br, c = draw()                                                             # disjoint noise in test
                 ba = np.clip(b ** np.float32(g) * np.float32(br) * c, 0, 255)
                 aug_tab[j, 6:] = [g, br, *c]
-            rs = lambda t: cv2.resize((t - mean) / std, (W, Hh), interpolation=cv2.INTER_AREA) if (FH != Hh or FW != W) else (t - mean) / std
+            rs = lambda t: normalise_resize_host(t, Hh, W)
             I_pl[j], Ip_pl[j], I_aug[j], Ip_aug[j] = rs(a), rs(b), rs(aa), rs(ba)
         dev = self.device
         pts1 = torch.tensor(self.pts1[idx], dtype=torch.float32, device=dev)
@@ -242,12 +260,8 @@ class Dataloader(object):
         dev = self.device
         I_pl, Ip_pl, I_aug, Ip_aug = ops.real_prep(I_u8, Ip_u8, torch.from_numpy(tables).to(dev), Hh, W)
         pts1 = torch.tensor(self.pts1[idx], dtype=torch.float32, device=dev)
-        x0 = pts1[:, 0].long(); y0 = pts1[:, 1].long()
-        yy, xx = torch.meshgrid(torch.arange(P, device=dev), torch.arange(P, device=dev), indexing="ij")
-        pidx = ((yy[None] + y0[:, None, None]) * W + (xx[None] + x0[:, None, None])).reshape(B, -1)
-        g = lambda a: torch.gather(a.mean(dim=3).reshape(B, -1), 1, pidx).reshape(B, P, P, 1).contiguous()
-        out = dict(I1=g(I_pl), I2=g(Ip_pl), I1_aug=g(I_aug), I2_aug=g(Ip_aug), I_aug=I_aug, I_prime_aug=Ip_aug,
-                   pts1=pts1, gt=None, patch_indices=pidx.to(torch.int32).contiguous(), full_I=I_u8.cpu().numpy(), full_I_prime=Ip_u8.cpu().numpy())
+        out = gather_patches(I_pl, Ip_pl, I_aug, Ip_aug, pts1, P, W)
+        out.update(full_I=I_u8.cpu().numpy(), full_I_prime=Ip_u8.cpu().numpy())
         out.update(I_u8=I_u8, I_prime_u8=Ip_u8, aug=torch.from_numpy(aug).to(dev))
         self._extended_gt(out, idx)
         return out

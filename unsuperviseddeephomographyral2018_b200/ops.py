@@ -568,6 +568,24 @@ def gray_u8(bgr):
     return gray
 
 
+# ------------------------------------------------------------------ image alignment's warp
+def warp_perspective_u8(src, M, dst_h, dst_w):
+    """uint8 [B,h,w,C] CUDA tensor (C = 1 or 3, any channel order), float64 M [B,3,3] (CUDA) -> uint8 [B,dst_h,dst_w,C]:
+    cv2.warpPerspective(src[b], M[b], (dst_w, dst_h)) per item (INTER_LINEAR, BORDER_CONSTANT 0), bit for bit."""
+    _req(src, torch.uint8, "src")
+    if src.dim() != 4 or src.shape[3] not in (1, 3):
+        raise _lib.UdhError("warp_perspective_u8: src must be [B,h,w,1] or [B,h,w,3] (got %s)" % (tuple(src.shape),))
+    B, h, w, C = src.shape
+    M = M.reshape(-1, 9).contiguous()
+    _req(M, torch.float64, "M")
+    if M.shape[0] != B:
+        raise _lib.UdhError("warp_perspective_u8: %d matrices for %d images" % (M.shape[0], B))
+    out = torch.empty(B, int(dst_h), int(dst_w), C, device=src.device, dtype=torch.uint8)
+    check(lib.udh_warp_perspective_u8(_ptr(src), _ptr(M), _ptr(out), B, h, w, C, int(dst_h), int(dst_w), _stream()),
+          "udh_warp_perspective_u8")
+    return out
+
+
 # ------------------------------------------------------------------ Adam
 def adam_step(p, g, m, v, alpha_t, beta1=0.9, beta2=0.999, eps=1e-8, grad_scale=1.0, zero_grad=True):
     for t, n in ((p, "p"), (g, "g"), (m, "m"), (v, "v")):
