@@ -13,6 +13,11 @@ with cv2.imread for the rest.  Writes out_dir/homographies.txt (`img1 img2` and 
 their float32 values) and, with --save_warped, out_dir/<k>_warped.jpg: image 1 warped by H as written into image 2's
 size, JPEG quality 95, byte-identical to cv2.imencode of cv2.warpPerspective.  Prints one line per pair and each batch's
 GPU time per pair (CUDA events around prep, forward and warp).
+
+--refine_levels N (N > 0, or -1 for levels down to a 320 px long side; default 0: off) refines each H with coarse-to-fine
+ECC on the images' own pixels (align.HomographyEstimator.refine, with --refine_iters, --refine_eps, --refine_max_side):
+homographies.txt and the warped files then hold the refined H, out_dir/refine.txt holds `img1 img2 rho status levels`
+per pair (status 0, or the ECC failure that stopped the pair; levels: how many succeeded), and the timing line a refine term.
 """
 from __future__ import absolute_import, division, print_function
 
@@ -43,6 +48,12 @@ def build_parser():
     p.add_argument('--seeded_weights', type=syn.str2bool, default='False',
                    help='without a checkpoint, use the seeded initial weights instead of stopping with an error')
     p.add_argument('--seed', type=int, default=0, help='seed of the initial weights (--seeded_weights True)')
+    p.add_argument('--refine_levels', type=int, default=0,
+                   help='refine H with coarse-to-fine ECC on this many levels (0: off; -1: halve down to a 320 px long side)')
+    p.add_argument('--refine_iters', type=int, default=50, help='ECC iterations per refinement level')
+    p.add_argument('--refine_eps', type=float, default=1e-6, help='ECC stops a level when rho changes by less than this')
+    p.add_argument('--refine_max_side', type=int, default=None,
+                   help='refine on images scaled to this long side at most (default: the images\' own size)')
     return p
 
 
@@ -85,19 +96,26 @@ def run(args, est, decode, encode):
     from unsuperviseddeephomographyral2018_b200 import align
     names, paths = pair_list(args)
     os.makedirs(args.out_dir, exist_ok=True)
-    lines, written = [], np.empty((len(names), 9), np.float32)
+    lines, written, refine_lines = [], np.empty((len(names), 9), np.float32), []
+    refining = args.refine_levels != 0
     for c0 in range(0, len(names), args.batch_size):
         chunk = range(c0, min(c0 + args.batch_size, len(names)))
         imgs = decode([p for k in chunk for p in paths[k]])
         I1, I2 = imgs[0::2], imgs[1::2]
         H, _, _ = est.estimate(I1, I2)
         ms = dict(est.last_ms)
+        if refining:
+            H, rho, status, level = est.refine(I1, I2, H, None if args.refine_levels < 0 else args.refine_levels, args.refine_iters,
+                                               args.refine_eps, args.refine_max_side)
+            ms["refine"] = est.last_ms["refine"]
         ms["warp"] = 0.0
         n = len(chunk)
         written[c0:c0 + n] = align.homography_as_written(H)
         for j, k in enumerate(chunk):
             lines.append(align.format_line(names[k][0], names[k][1], H[j]))
             print("%s %s  H = %s" % (names[k][0], names[k][1], " ".join("%.6g" % v for v in written[k])))
+            if refining:
+                refine_lines.append("%s %s %.9g %d %d" % (names[k][0], names[k][1], rho[j], status[j], level[j]))
         if args.save_warped:
             import torch
             groups = {}
@@ -110,10 +128,14 @@ def run(args, est, decode, encode):
                 for j, blob in zip(js, encode(warped.flip(-1))):            # RGB -> cv2's BGR for the encoder
                     with open(os.path.join(args.out_dir, "%d_warped.jpg" % (c0 + j)), "wb") as f:
                         f.write(blob)
-        print("===> batch of %d pairs: GPU %.3f ms/pair (prep %.3f, forward %.3f, warp %.3f)"
-              % (n, sum(ms.values()) / n, ms["prep"] / n, ms["forward"] / n, ms["warp"] / n), flush=True)
+        print("===> batch of %d pairs: GPU %.3f ms/pair (prep %.3f, forward %.3f, %swarp %.3f)"
+              % (n, sum(ms.values()) / n, ms["prep"] / n, ms["forward"] / n,
+                 "refine %.3f, " % (ms["refine"] / n) if refining else "", ms["warp"] / n), flush=True)
     with open(os.path.join(args.out_dir, "homographies.txt"), "w") as f:
         f.write("".join(ln + "\n" for ln in lines))
+    if refining:
+        with open(os.path.join(args.out_dir, "refine.txt"), "w") as f:
+            f.write("".join(ln + "\n" for ln in refine_lines))
     return written
 
 

@@ -278,6 +278,14 @@ int udh_ecc_prep_u8(const uint8_t* I, const uint8_t* I_prime, const float* aug, 
 int udh_ecc_homography(const uint8_t* tmpl, const uint8_t* input, const float* W_init, int max_iters, double eps, float* W,
                        double* rho, int32_t* iters, int32_t* status, void* ws, size_t ws_bytes, int B, int img_h, int img_w,
                        void* stream);
+/* udh_ecc_homography_split: udh_ecc_homography's contract (arguments, outputs, statuses, cv2 semantics) with each pair's
+ *   pixel sums split over many CTAs, for a few large pairs.  The tiling depends on img_h x img_w only: a pair's result is
+ *   bit-identical alone or in any batch.  Sums are added in a fixed order (no atomics); the call enqueues max_iters
+ *   iterations of three launches each and returns without synchronising.  workspace: udh_ecc_split_workspace_bytes. */
+size_t udh_ecc_split_workspace_bytes(int B, int img_h, int img_w);
+int udh_ecc_homography_split(const uint8_t* tmpl, const uint8_t* input, const float* W_init, int max_iters, double eps, float* W,
+                             double* rho, int32_t* iters, int32_t* status, void* ws, size_t ws_bytes, int B, int img_h, int img_w,
+                             void* stream);
 int udh_ecc_h4p(const float* W, const int32_t* status, const float* pts1, const float* gt, float rho_clamp, float* pred_h4p,
                 float* h_loss, int32_t* fail, int B, void* stream);
 /* udh_ecc_corr_h4p: the real-data harness's metric (homography_conventional_real.py:213-246, return_h_inv = False).

@@ -135,6 +135,9 @@ SIGNATURES = {
     "udh_ecc_prep_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "udh_ecc_homography": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_double, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                    c_size_t, c_int, c_int, c_int, c_void_p]),
+    "udh_ecc_split_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "udh_ecc_homography_split": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_double, c_void_p, c_void_p, c_void_p, c_void_p,
+                                         c_void_p, c_size_t, c_int, c_int, c_int, c_void_p]),
     "udh_ecc_h4p": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "udh_ecc_corr_h4p": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "udh_resize_area_up_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),

@@ -33,8 +33,25 @@ so that x2 ~ H x1 in original pixels, and cv2.warpPerspective(I1, H, (w2, h2)) l
 images have the metric's full size and the resize keeps the aspect ratio (S_1 = S_2 = r I), H x1 is the metric's
 pred_corr2; the metric scales both axes by full_img_h / img_h, which differs from S_k where the aspect ratio changes
 (240 x 320 -> 142 x 190 by 0.35 % in x).
+
+Refinement.  est.refine(I1, I2, H, levels, iters, eps, max_side) improves H on the images' own pixels with coarse-to-fine
+ECC (cv2.findTransformECC, MOTION_HOMOGRAPHY, on the split-pair kernel udh_ecc_homography_split):
+  * levels     refine_level_sizes: the finest level is image 2's size, or that size scaled to a long side of max_side;
+               each coarser level is ((h + 1) // 2, (w + 1) // 2), and levels whose short side would fall below
+               MIN_LEVEL_SIDE are not made.  levels=None (the default) halves until the long side is at most 320 px,
+               about the network frame the estimate came from.  Both images of a pair are resized to the level's size;
+  * planes     cvtColor(cv2.resize(img, (w_k, h_k)), RGB2GRAY) (ops.resize_linear_u8, ops.gray_u8; no resize at the
+               image's own size);
+  * coordinates  cv2.resize's pixel-centre map x_k = (x + 0.5) s - 0.5 per axis (level_transform), so
+               W_k = inv(T2k H T1k^-1) (template: image 2's plane, input: image 1's; to_level) and back
+               H = T2k^-1 inv(W_k) T1k (from_level), all in float64 with W_k rounded to float32 as cv2 takes it;
+  * per level  findTransformECC(template, input, W_k, MOTION_HOMOGRAPHY, (COUNT | EPS, iters, eps), None, 5);
+  * failures   a pair whose level ends with a non-zero status (where cv2 raises) keeps the H it had before that level
+               and runs no finer level; status is that level's, level_reached counts the levels that succeeded.
+oracle/ecc_refine.py restates the schedule with cv2 calls.
 """
 import collections
+import math
 import os
 
 import numpy as np
@@ -95,6 +112,67 @@ def check_corners(corners, n, img_h, img_w, patch_size):
         raise ValueError("corners[%d] = %s is not an integer %dx%d square inside the %dx%d network frame"
                          % (k, c[k].tolist(), P, P, img_h, img_w))
     return c.astype(np.float32)
+
+
+# ---- refinement schedule (the module docstring's "Refinement") --------------------------------------------------------
+MIN_LEVEL_SIDE = 16
+# levels=None: halve until the long side is at most AUTO_COARSEST_SIDE, about the network frame the estimate came from
+# (its error there is a few px); coarser levels can lose what the estimate had on textures with little coarse detail
+AUTO_COARSEST_SIDE = 320
+REFINE_LEVELS, REFINE_ITERS, REFINE_EPS = None, 50, 1e-6
+REFINE_PIXELS = 1 << 28          # pixels of the finest level per split-kernel batch (2 GB of workspace)
+
+
+def refine_level_sizes(h, w, levels=None, max_side=None):
+    """[(h_k, w_k)] coarsest first, for image 2 of size h x w: the finest h x w or scaled to a long side of max_side
+    (rounded half up), each coarser one ((h + 1) // 2, (w + 1) // 2), none with a short side below MIN_LEVEL_SIDE except
+    the finest; at most `levels` levels, or with levels=None until the long side is at most AUTO_COARSEST_SIDE."""
+    if levels is not None and levels < 1:
+        raise ValueError("levels must be >= 1 (got %d)" % levels)
+    if max_side is not None:
+        if max_side < 2:
+            raise ValueError("max_side must be >= 2 (got %d)" % max_side)
+        if max(h, w) > max_side:
+            s = max_side / float(max(h, w))
+            h, w = max(1, int(math.floor(h * s + 0.5))), max(1, int(math.floor(w * s + 0.5)))
+    if min(h, w) < 2:
+        raise ValueError("the finest level %dx%d is smaller than 2x2" % (h, w))
+    sizes = [(h, w)]
+    while len(sizes) < levels if levels is not None else max(h, w) > AUTO_COARSEST_SIDE:
+        h, w = (h + 1) // 2, (w + 1) // 2
+        if min(h, w) < MIN_LEVEL_SIDE:
+            break
+        sizes.append((h, w))
+    return sizes[::-1]
+
+
+def level_transform(size, size_k):
+    """3x3 float64 taking pixel coordinates of an image of size (h, w) to those of its cv2.resize to size_k = (h_k, w_k):
+    x_k = (x + 0.5) w_k / w - 0.5, y_k likewise."""
+    sx, sy = size_k[1] / float(size[1]), size_k[0] / float(size[0])
+    return np.array([[sx, 0.0, 0.5 * sx - 0.5], [0.0, sy, 0.5 * sy - 0.5], [0.0, 0.0, 1.0]])
+
+
+def to_level(H, size1, size2, size_k):
+    """H [n,3,3] (image 1 -> image 2, original pixels) -> ECC's W_k float32 [n,3,3] at level size_k: inv(T2k H T1k^-1),
+    normalised to W_k[2,2] = 1 (template: image 2's plane, input: image 1's)."""
+    T1, T2 = level_transform(size1, size_k), level_transform(size2, size_k)
+    W = np.linalg.inv(T2 @ np.asarray(H, np.float64).reshape(-1, 3, 3) @ np.linalg.inv(T1))
+    return (W / W[:, 2:3, 2:3]).astype(np.float32)
+
+
+def from_level(W, size1, size2, size_k):
+    """ECC's W_k [n,3,3] at level size_k -> H float64 [n,3,3] = T2k^-1 inv(W_k) T1k, normalised to H[2,2] = 1."""
+    T1, T2 = level_transform(size1, size_k), level_transform(size2, size_k)
+    H = np.linalg.inv(T2) @ np.linalg.inv(np.asarray(W, np.float32).astype(np.float64).reshape(-1, 3, 3)) @ T1
+    return H / H[:, 2:3, 2:3]
+
+
+def _level_plane(I, size_k):
+    """uint8 RGB [n,h,w,3] CUDA -> the level's gray planes [n,h_k,w_k]."""
+    if tuple(I.shape[1:3]) != tuple(size_k):
+        I = ops.resize_linear_u8(I.contiguous(), size_k[0], size_k[1])
+    return ops.gray_u8(I.contiguous())
 
 
 def _as_list(I):
@@ -213,6 +291,49 @@ class HomographyEstimator(object):
         e1.synchronize()
         self.last_ms["warp"] = e0.elapsed_time(e1)
         return out
+
+    def refine(self, I1, I2, H, levels=REFINE_LEVELS, iters=REFINE_ITERS, eps=REFINE_EPS, max_side=None):
+        """Coarse-to-fine ECC from H (the module docstring's "Refinement").  I1, I2 as for estimate, H [B,3,3] (image 1 ->
+        image 2, original pixels) -> (H float64 [B,3,3] with H[2,2] = 1, rho float64 [B] (the last level run; NaN before
+        any), status int32 [B] (_lib.ECC_*), level_reached int32 [B]) as numpy arrays.  Pairs are grouped by
+        (size1, size2); the host reads each level's result before the next.  last_ms['refine'] is its CUDA-event time."""
+        L1, L2 = _as_list(I1), _as_list(I2)
+        if len(L1) != len(L2):
+            raise ValueError("%d images 1 for %d images 2" % (len(L1), len(L2)))
+        n = len(L1)
+        H = np.array(H, np.float64).reshape(n, 3, 3)
+        H = H / H[:, 2:3, 2:3]
+        rho = np.full(n, np.nan); status = np.zeros(n, np.int32); reached = np.zeros(n, np.int32)
+        groups = collections.OrderedDict()
+        for k in range(n):
+            groups.setdefault((tuple(L1[k].shape[:2]), tuple(L2[k].shape[:2])), []).append(k)
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for (s1, s2), idx in groups.items():
+            sizes = refine_level_sizes(s2[0], s2[1], levels, max_side)
+            step = max(1, REFINE_PIXELS // (sizes[-1][0] * sizes[-1][1]))
+            for c0 in range(0, len(idx), step):
+                chunk = np.array(idx[c0:c0 + step])
+                live = np.arange(len(chunk))
+                for lv, sk in enumerate(sizes):
+                    A = torch.stack([L1[k] for k in chunk[live]])
+                    B = torch.stack([L2[k] for k in chunk[live]])
+                    Wk = torch.from_numpy(to_level(H[chunk[live]], s1, s2, sk)).to(A.device)
+                    W, r, _, st = ops.find_homography_ecc_split(_level_plane(B, sk), _level_plane(A, sk), Wk, iters, eps)
+                    W, r, st = W.cpu().numpy(), r.cpu().numpy(), st.cpu().numpy()
+                    ok = st == 0
+                    ks = chunk[live]
+                    rho[ks] = r
+                    H[ks[ok]] = from_level(W[ok], s1, s2, sk)
+                    reached[ks[ok]] = lv + 1
+                    status[ks[~ok]] = st[~ok]
+                    live = live[ok]
+                    if not len(live):
+                        break
+        e1.record()
+        e1.synchronize()
+        self.last_ms["refine"] = e0.elapsed_time(e1)
+        return H, rho, status, reached
 
 
 # ---- files --------------------------------------------------------------------------------------------------------------

@@ -189,6 +189,16 @@ def ecc_prep_u8(I_u8, Ip_u8, aug=None):
 def find_homography_ecc(template, image, W_init=None, max_iters=8, eps=1e-10):
     """Batched cv2.findTransformECC(template, image, W, MOTION_HOMOGRAPHY, (COUNT|EPS, max_iters, eps)) on uint8 planes
     [B,H,W].  Returns (W [B,3,3] fp32, rho [B] fp64, iterations [B] int32, status [B] int32 in _lib.ECC_*)."""
+    return _ecc_call("udh_ecc_homography", "udh_ecc_workspace_bytes", template, image, W_init, max_iters, eps)
+
+
+def find_homography_ecc_split(template, image, W_init=None, max_iters=8, eps=1e-10):
+    """find_homography_ecc with each pair's pixel sums split over many CTAs (udh_ecc_homography_split): for a few large
+    pairs.  Same arguments and outputs; a pair's result does not depend on the rest of the batch."""
+    return _ecc_call("udh_ecc_homography_split", "udh_ecc_split_workspace_bytes", template, image, W_init, max_iters, eps)
+
+
+def _ecc_call(fn, ws_fn, template, image, W_init, max_iters, eps):
     _req(template, torch.uint8, "template"); _req(image, torch.uint8, "image")
     if template.shape != image.shape or template.dim() != 3:
         raise _lib.UdhError("template and image must both be [B,H,W] (got %s and %s)" % (tuple(template.shape), tuple(image.shape)))
@@ -201,10 +211,10 @@ def find_homography_ecc(template, image, W_init=None, max_iters=8, eps=1e-10):
     rho = torch.empty(B, device=dev, dtype=torch.float64)
     iters = torch.empty(B, device=dev, dtype=torch.int32)
     status = torch.empty(B, device=dev, dtype=torch.int32)
-    nbytes = lib.udh_ecc_workspace_bytes(B, Hh, W)
+    nbytes = getattr(lib, ws_fn)(B, Hh, W)
     ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
-    check(lib.udh_ecc_homography(_ptr(template), _ptr(image), _ptr(W_init), int(max_iters), float(eps), _ptr(Wout), _ptr(rho),
-                                 _ptr(iters), _ptr(status), _ptr(ws), nbytes, B, Hh, W, _stream()), "udh_ecc_homography")
+    check(getattr(lib, fn)(_ptr(template), _ptr(image), _ptr(W_init), int(max_iters), float(eps), _ptr(Wout), _ptr(rho),
+                           _ptr(iters), _ptr(status), _ptr(ws), nbytes, B, Hh, W, _stream()), fn)
     return Wout, rho, iters, status
 
 
