@@ -34,6 +34,15 @@ def build_parser():
     p.add_argument('--pairs', type=str, default=None, help='file of "img1 img2" lines, paths relative to the file')
     p.add_argument('--img1', type=str, default=None)
     p.add_argument('--img2', type=str, default=None)
+    add_model_options(p)
+    p.add_argument('--out_dir', type=str, default='aligned')
+    p.add_argument('--save_warped', type=syn.str2bool, default='True')
+    add_weights_and_refine_options(p)
+    return p
+
+
+def add_model_options(p):
+    """The model's options, shared with mosaic_images.py: checkpoint lookup, network size, numeric mode, batch size."""
     p.add_argument('--model_dir', type=str, default=syn.MODEL_DIR)
     p.add_argument('--model_name', type=str, default='model.ckpt')
     p.add_argument('--loss_type', type=str, default='l1_loss', help='the loss the model was trained with (its subdirectory)',
@@ -43,8 +52,10 @@ def build_parser():
     p.add_argument('--patch_size', type=int, default=syn.PATCH_SIZE)
     p.add_argument('--numeric', type=str, default='bf16x3', choices=['fp32', 'bf16', 'bf16x3'])
     p.add_argument('--batch_size', type=int, default=128)
-    p.add_argument('--out_dir', type=str, default='aligned')
-    p.add_argument('--save_warped', type=syn.str2bool, default='True')
+
+
+def add_weights_and_refine_options(p):
+    """The seeded-weights fallback and the refinement options, shared with mosaic_images.py."""
     p.add_argument('--seeded_weights', type=syn.str2bool, default='False',
                    help='without a checkpoint, use the seeded initial weights instead of stopping with an error')
     p.add_argument('--seed', type=int, default=0, help='seed of the initial weights (--seeded_weights True)')
@@ -54,7 +65,6 @@ def build_parser():
     p.add_argument('--refine_eps', type=float, default=1e-6, help='ECC stops a level when rho changes by less than this')
     p.add_argument('--refine_max_side', type=int, default=None,
                    help='refine on images scaled to this long side at most (default: the images\' own size)')
-    return p
 
 
 def pair_list(args):

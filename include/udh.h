@@ -458,6 +458,26 @@ int udh_gray_u8(const uint8_t* bgr, int64_t npx, uint8_t* gray, void* stream);
 int udh_warp_perspective_u8(const uint8_t* src, const double* M, uint8_t* dst, int n, int h, int w, int c, int dst_h, int dst_w,
                             void* stream);
 
+/* ---- sequence mosaic ---------------------------------------------------------------------------------------------------
+ * udh_mosaic_blend_u8: n frames warped onto one dst_h x dst_w canvas and blended with feathered integer weights
+ *   (oracle/mosaic.py restates the rule).  Per canvas pixel and frame k, (X, Y) is the source position in 1/32 pixel that
+ *   udh_warp_perspective_u8(frame k, M_k, dst_h, dst_w) computes, W its denominator before 32 / W; the pixel is valid for k
+ *   iff W != 0, 0 <= X <= 32 (w_k - 1) and 0 <= Y <= 32 (h_k - 1).  v_k is that warp's output value and
+ *   wt_k = 1 + min(min(X, 32 (w_k - 1) - X, Y, 32 (h_k - 1) - Y), 32 feather).  Per channel S = sum wt_k v_k, D = sum wt_k
+ *   over the valid frames (64-bit integers); dst = (S + (D >> 1)) / D and mask = 255, or 0 and 0 where D = 0.
+ *   frames [n] (host array of device pointers), frame k uint8 [h_k,w_k,c] (c = 1 or 3); sizes [n,2] int32 (host, h_k w_k);
+ *   M [n,9] float64 row-major (device), frame k -> canvas; dst [dst_h,dst_w,c], mask [dst_h,dst_w] uint8 (device).
+ *   tile_ptr [ntiles + 1] and tile_frames [tile_ptr[ntiles]] int32 (device, CSR): the frames whose footprint can reach each
+ *   UDH_MOSAIC_TILE_H x UDH_MOSAIC_TILE_W canvas tile, tiles row-major, ceil(dst_w / UDH_MOSAIC_TILE_W) per row.  The lists
+ *   must be conservative (a frame valid at a pixel is listed for its tile); a frame listed twice counts twice.
+ *   ws: udh_mosaic_workspace_bytes(n) bytes of device memory.  n <= 65535, all sides < 32767, 0 <= feather <= 1024. */
+#define UDH_MOSAIC_TILE_H 16
+#define UDH_MOSAIC_TILE_W 64
+size_t udh_mosaic_workspace_bytes(int n);
+int udh_mosaic_blend_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, int n, int c, const int32_t* tile_ptr,
+                        const int32_t* tile_frames, int dst_h, int dst_w, int feather, uint8_t* dst, uint8_t* mask, void* ws,
+                        size_t ws_bytes, void* stream);
+
 /* ---- instrumentation read by bench.py -------------------------------------------------------------------------
  * udh_launch_count: kernels this library has launched in this process (monotonic).
  * udh_prof_*: when enabled, every tagged phase is bracketed by CUDA events recorded on the launching stream;

@@ -1,0 +1,124 @@
+#!/usr/bin/env python
+"""Stitch an image sequence into one mosaic with a trained model: the homography of every consecutive pair (frame k ->
+frame k + 1, as align_images.py computes it), chained to a reference frame, and every frame blended onto one canvas on the
+GPU (unsuperviseddeephomographyral2018_b200.mosaic states the chaining, the canvas and the blend rule).
+
+    python mosaic_images.py --frames raw/ --model_dir ../models/real_models/ --img_h 142 --img_w 190
+    python mosaic_images.py --frames frames.txt --seeded_weights True --refine_levels -1 --out_dir mosaic/
+
+--frames takes a list file (one path per line, relative to the file, in sequence order) or a directory, read as
+sorted(glob(dir/--glob)) (default *.JPG, gen_real_data.py's rule).  The model, refinement and batch options are
+align_images.py's.  --ref_frame picks the reference frame (-1: the middle one, N // 2); --feather is the blend's ramp in
+source pixels (0: a plain average of the overlapping frames).
+
+Writes in --out_dir:
+  pairs.txt    `frame_k frame_k+1` and H's nine entries per consecutive pair, as align_images.py's homographies.txt;
+  refine.txt   with refinement, `frame_k frame_k+1 rho status levels` per pair, as align_images.py writes it;
+  mosaic.txt   `canvas Hc Wc ref r`, then `name kept|dropped` and the nine entries of M_k (frame k -> canvas) per frame,
+               '%.9g' of their float32 values; the blend uses those float32 values, so the file reproduces mosaic.jpg;
+  mosaic.jpg   the mosaic (BGR, JPEG quality 95, byte-identical to cv2.imencode of the same pixels).
+A frame whose grown corners map behind the reference camera is dropped.  The canvas must be one the JPEG encoder takes
+(about 110 MP in colour); a larger one stops with an error naming the frame that reaches farthest.  Prints the GPU time
+of each phase (CUDA events: prep, forward, refine, blend, encode).
+"""
+from __future__ import absolute_import, division, print_function
+
+import argparse
+import glob
+import os
+import sys
+
+import numpy as np
+
+import align_images
+
+
+def build_parser():
+    p = argparse.ArgumentParser(description="Stitch an image sequence into one mosaic with a trained model")
+    p.add_argument('--frames', type=str, required=True, help='list file (one path per line, relative to it) or directory')
+    p.add_argument('--glob', type=str, default='*.JPG', help='the frames of a --frames directory: sorted(glob(dir/GLOB))')
+    align_images.add_model_options(p)
+    align_images.add_weights_and_refine_options(p)
+    p.add_argument('--ref_frame', type=int, default=-1, help='reference frame (-1: the middle one)')
+    p.add_argument('--feather', type=int, default=64, help='blend ramp in source pixels, 0..1024 (0: plain average)')
+    p.add_argument('--out_dir', type=str, default='mosaic')
+    return p
+
+
+def frame_list(args):
+    """-> (names as written in mosaic.txt, paths) in sequence order."""
+    if os.path.isdir(args.frames):
+        paths = sorted(glob.glob(os.path.join(args.frames, args.glob)))
+        names = [os.path.basename(p) for p in paths]
+    else:
+        base = os.path.dirname(os.path.abspath(args.frames))
+        with open(args.frames) as f:
+            names = [ln.strip() for ln in f if ln.strip()]
+        paths = [os.path.join(base, nm) for nm in names]
+    if len(paths) < 2:
+        raise SystemExit("%s: a mosaic needs at least two frames (found %d)" % (args.frames, len(paths)))
+    return names, paths
+
+
+def run(args, est, decode, encode):
+    """Mosaic the frames of `args`: est is an align.HomographyEstimator, decode(paths) -> CUDA RGB images, encode(images
+    BGR [n,h,w,3]) -> JPEG bytes.  Returns build_mosaic's result."""
+    import torch
+    from unsuperviseddeephomographyral2018_b200 import align, mosaic
+    if not 0 <= args.feather <= 1024:
+        raise SystemExit("--feather must be in 0..1024 (got %d)" % args.feather)
+    names, paths = frame_list(args)
+    os.makedirs(args.out_dir, exist_ok=True)
+    refining = args.refine_levels != 0
+    refine = dict(levels=None if args.refine_levels < 0 else args.refine_levels, iters=args.refine_iters, eps=args.refine_eps,
+                  max_side=args.refine_max_side) if refining else None
+    imgs = decode(paths)
+    try:
+        out = mosaic.build_mosaic(est, imgs, None if args.ref_frame < 0 else args.ref_frame, refine, args.feather,
+                                  float32_M=True)
+    except ValueError as e:
+        raise SystemExit(str(e))
+    H = out["H_pairs"]
+    with open(os.path.join(args.out_dir, "pairs.txt"), "w") as f:
+        f.write("".join(align.format_line(names[k], names[k + 1], H[k]) + "\n" for k in range(len(H))))
+    if refining:
+        rho, status, level = out["refine"]
+        with open(os.path.join(args.out_dir, "refine.txt"), "w") as f:
+            f.write("".join("%s %s %.9g %d %d\n" % (names[k], names[k + 1], rho[k], status[k], level[k]) for k in range(len(H))))
+    Hc, Wc = out["mask"].shape
+    lines = ["canvas %d %d ref %d" % (Hc, Wc, out["ref"])]
+    for k, nm in enumerate(names):
+        lines.append(" ".join([nm, "kept" if out["kept"][k] else "dropped"] +
+                              ["%.9g" % v for v in align.homography_as_written(out["M"][k])[0]]))
+        if not out["kept"][k]:
+            print("===> dropped %s: it maps behind the reference frame's camera" % nm)
+    with open(os.path.join(args.out_dir, "mosaic.txt"), "w") as f:
+        f.write("\n".join(lines) + "\n")
+    ms = out["last_ms"]
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    blob = encode(out["mosaic"].flip(-1)[None])[0]                       # RGB -> cv2's BGR for the encoder
+    e1.record()
+    e1.synchronize()
+    ms["encode"] = e0.elapsed_time(e1)
+    with open(os.path.join(args.out_dir, "mosaic.jpg"), "wb") as f:
+        f.write(blob)
+    cover = float((out["mask"] != 0).float().mean())
+    print("===> %d frames (%d kept) on a %dx%d canvas (ref %s, %.1f %% covered): GPU %.3f ms (prep %.3f, forward %.3f, %s"
+          "blend %.3f, encode %.3f)" % (len(names), int(np.sum(out["kept"])), Hc, Wc, names[out["ref"]], 100 * cover,
+                                        sum(ms.values()), ms["prep"], ms["forward"],
+                                        "refine %.3f, " % ms["refine"] if refining else "", ms["blend"], ms["encode"]), flush=True)
+    return out
+
+
+def main(argv=None):
+    args = build_parser().parse_args(argv)
+    import torch
+    from unsuperviseddeephomographyral2018_b200 import align, ops
+    torch.cuda.set_device(0)
+    run(args, align_images.make_estimator(args), align.decode_images, ops.encode_jpeg)
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())

@@ -1,0 +1,144 @@
+"""Sequence-mosaic timing, in one run on the GPU:
+  * udh_mosaic_blend_u8 alone (tile lists built once, CUDA events over repeated launches) on synthetic camera sweeps of
+    32 x 1080x1920 and 16 x 3000x4000 RGB frames with about 60 % overlap between neighbours, placed with their true
+    homographies: ms per mosaic and bytes/s against the H100 SXM's 3.35 TB/s.  Bytes: the canvas write, (C + 1) per pixel,
+    plus C source bytes per covered frame-pixel (each frame's mapped area); candidate frame-pixels (tile pixels times
+    candidates, ~12 fp64 operations and one fp64 division each) are printed beside them;
+  * the host path, oracle/mosaic.py (cv2.warpPerspective per frame + a NumPy int64 blend), with cv2.setNumThreads(1) and
+    (16), against the kernel on the same 8 x 1080x1920 sweep (the oracle evaluates every frame at every canvas pixel);
+  * mosaic_images.py end to end (device decode, estimate, chain, blend, JPEG encode, files written) with seeded weights on
+    8 quality-95 JPEGs of 1080x1920, ms per frame.
+Prints one JSON line with the card name and power limit read in the same run.
+
+    python tools/mosaic_time.py
+"""
+import json
+import os
+import shutil
+import sys
+import tempfile
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
+
+import _mosaic_sweep as SW  # noqa: E402
+from tools import jpeg_time  # noqa: E402
+from unsuperviseddeephomographyral2018_b200 import _lib, mosaic, ops  # noqa: E402
+
+HBM_TBS = 3.35
+
+
+def placed_sweep(n, h, w, seed=0):
+    """Frames (seeded noise: content does not change the kernel's work) on the canvas of their true homographies."""
+    A, _ = SW.sweep_cameras(n, h, w, 0.6, seed)
+    G, ref = mosaic.chain_to_reference(SW.true_pairs(A))
+    M, (Hc, Wc), kept = mosaic.canvas([(h, w)] * n, G, ref)
+    assert kept.all()
+    rng = np.random.default_rng(seed)
+    frames = [rng.integers(0, 256, (h, w, 3), np.uint8) for _ in range(n)]
+    return frames, M, (Hc, Wc)
+
+
+def mapped_area(M, h, w):
+    x, y, _ = mosaic._map(M, mosaic.centre_corners(h, w))
+    return 0.5 * abs(np.dot(x, np.roll(y, -1)) - np.dot(y, np.roll(x, -1)))
+
+
+def kernel_time(frames, M, canvas, feather=64, reps=10):
+    import ctypes
+    Hc, Wc = canvas
+    n, (h, w, C) = len(frames), frames[0].shape
+    dev = [torch.from_numpy(f).cuda() for f in frames]
+    ptr, idx = ops.mosaic_tile_lists(M, [(h, w)] * n, Hc, Wc)
+    ptr_d, idx_d = torch.from_numpy(ptr).cuda(), torch.from_numpy(idx).cuda()
+    M_d = torch.from_numpy(np.ascontiguousarray(M.reshape(n, 9))).cuda()
+    out = torch.empty(Hc, Wc, C, dtype=torch.uint8, device="cuda")
+    mask = torch.empty(Hc, Wc, dtype=torch.uint8, device="cuda")
+    nb = _lib.lib.udh_mosaic_workspace_bytes(n)
+    ws = torch.empty(nb, dtype=torch.uint8, device="cuda")
+    ptrs = (ctypes.c_void_p * n)(*[t.data_ptr() for t in dev])
+    sz = np.array([(h, w)] * n, np.int32)
+    p = lambda t: ctypes.c_void_p(t.data_ptr())
+    st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+    call = lambda: _lib.check(_lib.lib.udh_mosaic_blend_u8(ptrs, sz.ctypes.data, p(M_d), n, C, p(ptr_d), p(idx_d), Hc, Wc, feather,
+                                                           p(out), p(mask), p(ws), nb, st), "udh_mosaic_blend_u8")
+    call()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(reps):
+        call()
+    e1.record()
+    e1.synchronize()
+    ms = e0.elapsed_time(e1) / reps
+    # the same bytes as ops.mosaic_blend_u8 (its own lists) gives: check the direct call's output once
+    ref, ref_mask = ops.mosaic_blend_u8(dev, M, Hc, Wc, feather)
+    assert torch.equal(ref, out) and torch.equal(ref_mask, mask)
+    covered = sum(mapped_area(M[k], h, w) for k in range(n))
+    nbytes = (C + 1) * Hc * Wc + C * covered
+    cand = float(np.diff(ptr).astype(np.int64).sum()) * _lib.MOSAIC_TILE_H * _lib.MOSAIC_TILE_W
+    return {"frames": n, "frame": [h, w], "canvas": [Hc, Wc], "canvas_mp": Hc * Wc / 1e6, "ms": ms, "GB_per_s": nbytes / ms / 1e6,
+            "pct_of_hbm": 100.0 * nbytes / ms / 1e9 / HBM_TBS, "bytes": nbytes, "candidate_frame_pixels": cand,
+            "covered_frame_pixels": covered, "coverage": float((mask != 0).float().mean())}
+
+
+def host_time(frames, M, canvas, threads):
+    import cv2
+    from oracle import mosaic as OM
+    cv2.setNumThreads(threads)
+    t0 = time.perf_counter()
+    OM.blend(frames, M, canvas[0], canvas[1], 64)
+    return (time.perf_counter() - t0) * 1e3
+
+
+def cli_time(root, n=8, h=1080, w=1920):
+    import cv2
+    import mosaic_images as cli
+    _, frames, _, _ = SW.sweep(n, h, w, seed=4)
+    raw = os.path.join(root, "raw")
+    os.makedirs(raw)
+    for k, f in enumerate(frames):
+        cv2.imwrite(os.path.join(raw, "F_%03d.JPG" % k), f[..., ::-1], [cv2.IMWRITE_JPEG_QUALITY, 95])
+    argv = ["--frames", raw, "--seeded_weights", "True", "--model_dir", os.path.join(root, "none")]
+    res = {}
+    for run in ("warm", "timed"):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        try:
+            cli.main(argv + ["--out_dir", os.path.join(root, run)])
+        except SystemExit as e:                               # e.g. seeded weights chaining to a canvas the encoder rejects
+            return {"error": str(e)}
+        torch.cuda.synchronize()
+        res[run] = (time.perf_counter() - t0) * 1e3
+    return {"frames": n, "frame": [h, w], "ms_per_frame": res["timed"] / n}
+
+
+def main():
+    torch.cuda.set_device(0)
+    out = {"gpu": torch.cuda.get_device_name(0), "card": jpeg_time.card(), "feather": 64}
+    for n, h, w in ((32, 1080, 1920), (16, 3000, 4000)):
+        frames, M, canvas = placed_sweep(n, h, w)
+        out["kernel_%dx%dx%d" % (n, h, w)] = r = kernel_time(frames, M, canvas)
+        print(json.dumps(r), flush=True)
+        del frames
+    frames, M, canvas = placed_sweep(8, 1080, 1920)
+    host = {"kernel_ms": kernel_time(frames, M, canvas)["ms"], "canvas": list(canvas)}
+    for t in (1, 16):
+        host["host_ms_threads_%d" % t] = host_time(frames, M, canvas, t)
+    out["host_8x1080x1920"] = host
+    print(json.dumps(host), flush=True)
+    root = tempfile.mkdtemp(prefix="mosaic_time_")
+    try:
+        out["cli_8x1080x1920"] = cli_time(root)
+    finally:
+        shutil.rmtree(root, ignore_errors=True)
+    print(json.dumps(out))
+
+
+if __name__ == "__main__":
+    main()

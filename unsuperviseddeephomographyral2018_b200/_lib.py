@@ -17,6 +17,7 @@ NSUMS, NLOSSES, NMETRICS = 8, 8, 4
 L_REC, L_SSIM, L_L1, L_L1_SMOOTH, L_NCC = 0, 1, 2, 3, 4
 M_H_LOSS, M_BOUNDED_H_LOSS, M_NUM_FAIL, M_ACE = 0, 1, 2, 3
 ECC_OK, ECC_NAN, ECC_NOCONV = 0, 1, 2
+MOSAIC_TILE_H, MOSAIC_TILE_W = 16, 64            # UDH_MOSAIC_TILE_H / _W
 
 class StepArgs(ctypes.Structure):
     """udh_step_args (include/udh.h)."""
@@ -167,6 +168,9 @@ SIGNATURES = {
     "udh_gen_warp_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "udh_gray_u8": (c_int, [c_void_p, c_int64, c_void_p, c_void_p]),
     "udh_warp_perspective_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "udh_mosaic_workspace_bytes": (c_size_t, [c_int]),
+    "udh_mosaic_blend_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p,
+                                    c_void_p, c_void_p, c_size_t, c_void_p]),
     "udh_draw_report_workspace_bytes": (c_size_t, [c_int]),
     "udh_draw_report_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_int, c_int, c_int,
                                    c_void_p]),

@@ -1,0 +1,148 @@
+"""Stitch an image sequence into one mosaic: chain the learned pairwise homographies to a reference frame, lay out a
+canvas, and blend every frame onto it on the GPU (udh_mosaic_blend_u8).
+
+    out = build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None)
+    out["mosaic"], out["mask"], out["M"], out["kept"], out["H_pairs"], out["last_ms"]
+
+frames are CUDA uint8 RGB [h_k,w_k,3] tensors in sequence order (sizes may differ); est is an align.HomographyEstimator.
+
+Chaining.  H_k maps frame k to frame k + 1 (align's image 1 -> image 2).  chain_to_reference gives G_k, frame k -> the
+reference frame: G_ref = I, G_k = n(G_{k+1} H_k) below the reference and G_k = n(G_{k-1} inv(H_{k-1})) above it, with n
+normalising [2,2] to 1.  The default reference is the middle frame N // 2, which halves the longest chain.  Errors of the
+pairwise H's accumulate along the chain (drift); nothing here closes loops or adjusts the chain globally.
+
+Canvas.  canvas() drops a frame (never the reference) when a corner of its source rectangle grown by 1 px, (-1, -1) ..
+(w, h), maps with a denominator <= 0: such a frame reaches the line at infinity.  Over the kept frames' mapped pixel-centre
+corners (0, 0), (w - 1, 0), (w - 1, h - 1), (0, h - 1): x0 = floor(min x), Wc = ceil(max x) - x0 + 1, likewise in y, and
+M_k = T G_k with T the translation by (-x0, -y0).
+
+Blend.  oracle/mosaic.py states the rule: per canvas pixel, the integer feathered average of every frame's
+cv2.warpPerspective(F_k, M_k, (Wc, Hc)) value where the frame is valid, with weights 1 + min(distance to the frame's edge in
+1/32 px, 32 feather).
+"""
+import numpy as np
+
+MAX_SIDE = 32766                 # udh_mosaic_blend_u8 takes canvas sides below 32767
+
+
+def _normalise(G):
+    return G / G[2, 2]
+
+
+def chain_to_reference(H_pairs, ref=None):
+    """H_pairs [N-1,3,3] (frame k -> frame k + 1) -> (G float64 [N,3,3] frame k -> frame ref with G[k][2,2] = 1, ref)."""
+    H = np.asarray(H_pairs, np.float64).reshape(-1, 3, 3)
+    N = len(H) + 1
+    ref = N // 2 if ref is None or ref < 0 else int(ref)
+    if ref >= N:
+        raise ValueError("reference frame %d of a %d-frame sequence" % (ref, N))
+    G = np.empty((N, 3, 3))
+    G[ref] = np.eye(3)
+    for k in range(ref - 1, -1, -1):
+        G[k] = _normalise(G[k + 1] @ H[k])
+    for k in range(ref + 1, N):
+        G[k] = _normalise(G[k - 1] @ np.linalg.inv(H[k - 1]))
+    return G, ref
+
+
+def _map(G, pts):
+    p = np.asarray(pts, np.float64) @ np.asarray(G, np.float64).T
+    return p[:, 0] / p[:, 2], p[:, 1] / p[:, 2], p[:, 2]
+
+
+def grown_corners(h, w):
+    return np.array([[-1.0, -1.0, 1.0], [w, -1.0, 1.0], [w, h, 1.0], [-1.0, h, 1.0]])
+
+
+def centre_corners(h, w):
+    return np.array([[0.0, 0.0, 1.0], [w - 1.0, 0.0, 1.0], [w - 1.0, h - 1.0, 1.0], [0.0, h - 1.0, 1.0]])
+
+
+def canvas(sizes, G, ref, max_pixels=None):
+    """sizes [(h_k, w_k)], G [N,3,3] (frame k -> reference) -> (M float64 [N,3,3] frame k -> canvas, (Hc, Wc), kept bool
+    [N]).  ValueError naming the frame with the corner farthest from the reference frame's centre when a side exceeds
+    MAX_SIDE or, with max_pixels, Hc Wc > max_pixels."""
+    G = np.asarray(G, np.float64).reshape(-1, 3, 3)
+    kept = np.ones(len(G), bool)
+    xs, ys = [], []
+    for k, (h, w) in enumerate(sizes):
+        with np.errstate(all="ignore"):
+            _, _, den = _map(G[k], grown_corners(h, w))
+            x, y, _ = _map(G[k], centre_corners(h, w))
+        if k != ref and not ((den > 0).all() and np.isfinite(x).all() and np.isfinite(y).all()):
+            kept[k] = False
+            continue
+        xs.append(x); ys.append(y)
+    xs, ys = np.concatenate(xs), np.concatenate(ys)
+    x0, y0 = np.floor(xs.min()), np.floor(ys.min())
+    Wc, Hc = int(np.ceil(xs.max()) - x0) + 1, int(np.ceil(ys.max()) - y0) + 1
+    if max(Hc, Wc) > MAX_SIDE or (max_pixels is not None and Hc * Wc > max_pixels):
+        raise ValueError("the %dx%d canvas exceeds %s; frame %d reaches farthest from the reference frame (drop it or pick "
+                         "another --ref_frame)" % (Hc, Wc, "%d px a side" % MAX_SIDE if max(Hc, Wc) > MAX_SIDE else
+                                                   "%d pixels" % max_pixels, farthest_frame(sizes, G, kept, ref)))
+    T = np.array([[1.0, 0.0, -x0], [0.0, 1.0, -y0], [0.0, 0.0, 1.0]])
+    return T @ G, (Hc, Wc), kept
+
+
+def farthest_frame(sizes, G, kept, ref):
+    """The kept frame whose mapped pixel-centre corner lies farthest from the reference frame's centre."""
+    h, w = sizes[ref]
+    cx, cy = (w - 1) / 2.0, (h - 1) / 2.0
+    best, far = -1.0, ref
+    for k, (h, w) in enumerate(sizes):
+        if kept[k]:
+            x, y, _ = _map(G[k], centre_corners(h, w))
+            d = np.hypot(x - cx, y - cy).max()
+            if d > best:
+                best, far = d, k
+    return far
+
+
+def build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None, float32_M=False):
+    """est: align.HomographyEstimator; frames: CUDA uint8 RGB [h_k,w_k,3] tensors in sequence order.  refine: None, or a
+    dict of est.refine's keyword arguments (levels, iters, eps, max_side) to refine each pair's H.  max_pixels: the canvas
+    limit (None: the JPEG encoder's, udh_jpeg_encode_capacity(Hc, Wc, 3) != 0).  float32_M: blend with each M_k rounded to
+    float32, the values a text file of '%.9g' float32 entries gives back.
+    -> dict(mosaic uint8 [Hc,Wc,3] RGB, mask uint8 [Hc,Wc], M [N,3,3] frame k -> canvas (float64, float32 values with
+    float32_M), kept bool [N], ref, H_pairs [N-1,3,3], refine (rho, status, level_reached) or None, last_ms {prep, forward,
+    refine, blend} of CUDA-event time)."""
+    frames = list(frames)
+    if len(frames) < 2:
+        raise ValueError("a mosaic needs at least two frames (got %d)" % len(frames))
+    H, _, _ = est.estimate(frames[:-1], frames[1:])
+    ms = dict(est.last_ms)
+    refined = None
+    if refine is not None:
+        H, rho, status, reached = est.refine(frames[:-1], frames[1:], H, **refine)
+        refined = (rho, status, reached)
+        ms["refine"] = est.last_ms["refine"]
+    G, ref = chain_to_reference(H, ref)
+    sizes = [tuple(int(v) for v in f.shape[:2]) for f in frames]
+    M, (Hc, Wc), kept = canvas(sizes, G, ref, max_pixels)
+    if float32_M:
+        M = M.astype(np.float32).astype(np.float64)
+    if max_pixels is None:
+        check_encodable(Hc, Wc, sizes, G, kept, ref)
+    mosaic, mask, ms["blend"] = blend(frames, M, kept, Hc, Wc, feather)
+    return dict(mosaic=mosaic, mask=mask, M=M, kept=kept, ref=ref, H_pairs=H, refine=refined, last_ms=ms)
+
+
+def check_encodable(Hc, Wc, sizes, G, kept, ref):
+    """ValueError unless the JPEG encoder takes an Hc x Wc colour image, naming the frame that reaches farthest."""
+    from . import _lib
+    if _lib.lib.udh_jpeg_encode_capacity(Hc, Wc, 3) == 0:
+        raise ValueError("the %dx%d canvas is larger than the JPEG encoder takes; frame %d reaches farthest from the reference "
+                         "frame (drop it or pick another --ref_frame)" % (Hc, Wc, farthest_frame(sizes, G, kept, ref)))
+
+
+def blend(frames, M, kept, Hc, Wc, feather):
+    """The kept frames through ops.mosaic_blend_u8 -> (mosaic, mask, CUDA-event ms)."""
+    import torch
+    from . import ops
+    take = [k for k in range(len(frames)) if kept[k]]
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    mosaic, mask = ops.mosaic_blend_u8([frames[k].contiguous() for k in take], np.asarray(M)[take], Hc, Wc, feather)
+    e1.record()
+    e1.synchronize()
+    return mosaic, mask, e0.elapsed_time(e1)

@@ -596,6 +596,79 @@ def warp_perspective_u8(src, M, dst_h, dst_w):
     return out
 
 
+# ------------------------------------------------------------------ sequence mosaic
+def mosaic_tile_lists(M, sizes, dst_h, dst_w):
+    """float64 M [n,3,3] (frame k -> canvas), sizes [(h_k, w_k)] -> udh_mosaic_blend_u8's CSR candidate lists (tile_ptr int32
+    [ntiles + 1], tile_frames int32): per _lib.MOSAIC_TILE_H x MOSAIC_TILE_W canvas tile (row-major), the frames whose
+    footprint can reach it, in frame order.  The footprint is the source rectangle grown by 1 px, corners (-1, -1) ..
+    (w, h): when all four map with a positive denominator its image is a convex quad and the tiles meeting the quad's
+    floor / ceil bounding box are listed; otherwise every tile is.  A valid pixel's source position lies within 1/64 px
+    (rounding) of the frame, so the lists are conservative."""
+    M = np.asarray(M, np.float64).reshape(-1, 3, 3)
+    TH, TW = _lib.MOSAIC_TILE_H, _lib.MOSAIC_TILE_W
+    gy, gx = -(-dst_h // TH), -(-dst_w // TW)
+    tiles, frames = [], []
+    for k, (h, w) in enumerate(sizes):
+        p = np.array([[-1.0, -1.0, 1.0], [w, -1.0, 1.0], [w, h, 1.0], [-1.0, h, 1.0]]) @ M[k].T
+        if np.isfinite(p).all() and (p[:, 2] > 0).all():
+            x, y = p[:, 0] / p[:, 2], p[:, 1] / p[:, 2]
+            if not (np.isfinite(x).all() and np.isfinite(y).all()):
+                tx, ty = np.arange(gx), np.arange(gy)
+            else:
+                x0, x1 = max(np.floor(x.min()), 0.0), min(np.ceil(x.max()), dst_w - 1.0)
+                y0, y1 = max(np.floor(y.min()), 0.0), min(np.ceil(y.max()), dst_h - 1.0)
+                if x0 > x1 or y0 > y1:
+                    continue
+                tx = np.arange(int(x0) // TW, int(x1) // TW + 1)
+                ty = np.arange(int(y0) // TH, int(y1) // TH + 1)
+        else:
+            tx, ty = np.arange(gx), np.arange(gy)
+        ids = (ty[:, None] * gx + tx[None, :]).ravel()
+        tiles.append(ids)
+        frames.append(np.full(len(ids), k, np.int64))
+    tiles = np.concatenate(tiles) if tiles else np.zeros(0, np.int64)
+    frames = np.concatenate(frames) if frames else np.zeros(0, np.int64)
+    if len(tiles) >= 2 ** 31:
+        raise _lib.UdhError("mosaic_tile_lists: %d candidate entries do not fit int32" % len(tiles))
+    order = np.lexsort((frames, tiles))
+    ptr = np.zeros(gy * gx + 1, np.int64)
+    ptr[1:] = np.cumsum(np.bincount(tiles, minlength=gy * gx))
+    return ptr.astype(np.int32), frames[order].astype(np.int32)
+
+
+def mosaic_blend_u8(frames, M, dst_h, dst_w, feather):
+    """frames: n CUDA uint8 tensors [h_k,w_k,C] (C = 1 or 3, sizes may differ; or one [n,h,w,C] tensor), M float64 [n,3,3]
+    (frame k -> canvas; numpy or tensor) -> (mosaic uint8 [dst_h,dst_w,C], mask uint8 [dst_h,dst_w]): udh_mosaic_blend_u8's
+    feathered blend of cv2.warpPerspective(frame k, M_k, (dst_w, dst_h)), bit for bit with oracle/mosaic.py.  The tile
+    lists are built on the host (mosaic_tile_lists); the frames are read where they are."""
+    frames = list(frames.unbind(0)) if isinstance(frames, torch.Tensor) else list(frames)
+    Mh = (M.detach().cpu().numpy() if isinstance(M, torch.Tensor) else np.asarray(M)).astype(np.float64).reshape(-1, 3, 3)
+    n = len(frames)
+    if Mh.shape[0] != n:
+        raise _lib.UdhError("mosaic_blend_u8: %d matrices for %d frames" % (Mh.shape[0], n))
+    if n == 0:
+        raise _lib.UdhError("mosaic_blend_u8: no frames")
+    for k, f in enumerate(frames):
+        _req(f, torch.uint8, "frames[%d]" % k)
+        if f.dim() != 3 or f.shape[2] not in (1, 3) or f.shape[2] != frames[0].shape[2]:
+            raise _lib.UdhError("mosaic_blend_u8: frames must all be [h,w,1] or all [h,w,3] (frame %d is %s)" % (k, tuple(f.shape)))
+    C, dev = frames[0].shape[2], frames[0].device
+    sizes = [(int(f.shape[0]), int(f.shape[1])) for f in frames]
+    ptr, idx = mosaic_tile_lists(Mh, sizes, int(dst_h), int(dst_w))
+    ptr_d = torch.from_numpy(ptr).to(dev)
+    idx_d = torch.from_numpy(idx if len(idx) else np.zeros(1, np.int32)).to(dev)
+    M_d = torch.from_numpy(np.ascontiguousarray(Mh.reshape(n, 9))).to(dev)
+    out = torch.empty(int(dst_h), int(dst_w), C, device=dev, dtype=torch.uint8)
+    mask = torch.empty(int(dst_h), int(dst_w), device=dev, dtype=torch.uint8)
+    nb = lib.udh_mosaic_workspace_bytes(n)
+    ws = torch.empty(max(nb, 1), device=dev, dtype=torch.uint8)
+    ptrs = (ctypes.c_void_p * n)(*[f.data_ptr() for f in frames])
+    sz = np.ascontiguousarray(np.array(sizes, np.int32).reshape(n, 2))
+    check(lib.udh_mosaic_blend_u8(ptrs, sz.ctypes.data, _ptr(M_d), n, C, _ptr(ptr_d), _ptr(idx_d), int(dst_h), int(dst_w),
+                                  int(feather), _ptr(out), _ptr(mask), _ptr(ws), nb, _stream()), "udh_mosaic_blend_u8")
+    return out, mask
+
+
 # ------------------------------------------------------------------ Adam
 def adam_step(p, g, m, v, alpha_t, beta1=0.9, beta2=0.999, eps=1e-8, grad_scale=1.0, zero_grad=True):
     for t, n in ((p, "p"), (g, "g"), (m, "m"), (v, "v")):
