@@ -286,6 +286,14 @@ size_t udh_ecc_split_workspace_bytes(int B, int img_h, int img_w);
 int udh_ecc_homography_split(const uint8_t* tmpl, const uint8_t* input, const float* W_init, int max_iters, double eps, float* W,
                              double* rho, int32_t* iters, int32_t* status, void* ws, size_t ws_bytes, int B, int img_h, int img_w,
                              void* stream);
+/* udh_debug_ecc_layout: where the ECC workspaces keep their intermediates, for tests that read them (byte offsets).
+ *   off[0]: the blurred fp32 planes [2][B][img_h][img_w], template planes then input planes — the whole of
+ *     udh_ecc_homography's workspace, and the first part of udh_ecc_homography_split's;
+ *   split kernel only: off[1] the per-pair states, off[2] slab1 fp64 [B][tiles][5] (per tile: mask count n, sum Iw,
+ *     sum Iw^2, sum T, sum T^2), off[3] slab2 fp64 [B][tiles][53] (per tile: the Hessian's upper triangle row by row,
+ *     the 8 image projections, the 8 template projections, the correlation).  *tiles = the tiles of 16384 row-major
+ *     pixels.  After the call the slabs hold the last iteration's sums (with max_iters = 1: the first one's). */
+int udh_debug_ecc_layout(int B, int img_h, int img_w, size_t off[4], int* tiles);
 int udh_ecc_h4p(const float* W, const int32_t* status, const float* pts1, const float* gt, float rho_clamp, float* pred_h4p,
                 float* h_loss, int32_t* fail, int B, void* stream);
 /* udh_ecc_corr_h4p: the real-data harness's metric (homography_conventional_real.py:213-246, return_h_inv = False).

@@ -137,7 +137,7 @@ def _lu_inv_f32(A):
 
 def ecc(template_u8, image_u8, W_init=None, max_iters=8, eps=1e-10, solve="fp64", trace=None):
     """-> dict(W [3,3] float32, rho, iters, status) for one pair.  `trace` (a list) receives per iteration the quantities
-    that decide the outcome: rho and lambda_d."""
+    that decide the outcome: rho and lambda_d, and the sums they come from (correlation, Hessian, projections)."""
     H, Wd = template_u8.shape
     T = blur(template_u8); Ib = blur(image_u8)
     gx, gy = gradients(Ib)
@@ -187,7 +187,7 @@ def ecc(template_u8, image_u8, W_init=None, max_iters=8, eps=1e-10, solve="fp64"
             lambda_n = imgNorm * imgNorm - float(ip @ sol[:, 0])
             lambda_d = corr - float(tp @ sol[:, 0])
         if trace is not None:
-            trace.append(dict(rho=rho, lambda_d=lambda_d, corr=corr))
+            trace.append(dict(rho=rho, lambda_d=lambda_d, corr=corr, hessian=Hs, ip=ip, tp=tp))
         if np.isnan(rho):
             status = ECC_NAN; break
         if lambda_d <= 0.0:

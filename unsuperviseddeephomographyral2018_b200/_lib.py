@@ -139,6 +139,7 @@ SIGNATURES = {
     "udh_ecc_split_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "udh_ecc_homography_split": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_double, c_void_p, c_void_p, c_void_p, c_void_p,
                                          c_void_p, c_size_t, c_int, c_int, c_int, c_void_p]),
+    "udh_debug_ecc_layout": (c_int, [c_int, c_int, c_int, POINTER(c_size_t), POINTER(c_int)]),
     "udh_ecc_h4p": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "udh_ecc_corr_h4p": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "udh_resize_area_up_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),

@@ -137,6 +137,16 @@ __device__ __forceinline__ uint8_t denorm_u8(int x, int c, const float* a) {
   return (uint8_t)(t < 0 ? 0 : (t > 255 ? 255 : t));
 }
 
+// OpenCV's BORDER_REFLECT_101 (gfedcb|abcdefgh|gfedcba): the index in [0, n) that i reads, for any n >= 2 and any i.  The
+// pattern has period 2n - 2, so |i| is folded into one period and its upper half mirrored; reflecting once is not enough
+// when the reach exceeds n - 1 (a 5-tap filter on a side of 2).
+__host__ __device__ __forceinline__ int reflect101(int i, int n) {
+  if (i >= 0 && i < n) return i;
+  const int p = 2 * n - 2;
+  const int r = (i < 0 ? -i : i) % p;
+  return r < n ? r : p - r;
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

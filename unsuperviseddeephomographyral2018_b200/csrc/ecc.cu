@@ -38,8 +38,6 @@ __global__ void __launch_bounds__(256) ecc_prep_kernel(const uint8_t* __restrict
 }
 
 // ---- pre-pass ---------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ int reflect101(int i, int n) { return i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i); }
-
 // plane z = 0: template, z = 1: input image
 __global__ void __launch_bounds__(256) ecc_blur_kernel(const uint8_t* __restrict__ tmpl, const uint8_t* __restrict__ input,
                                                        float* __restrict__ out, int H, int W) {
@@ -632,6 +630,14 @@ extern "C" size_t udh_ecc_split_workspace_bytes(int B, int img_h, int img_w) {
   if (B < 1 || img_h < 2 || img_w < 2) return 0;
   size_t off[4];
   return ecc_split_offsets(B, img_h, img_w, off);
+}
+
+extern "C" int udh_debug_ecc_layout(int B, int img_h, int img_w, size_t off[4], int* tiles) {
+  UDH_REQUIRE(off && tiles, "udh_debug_ecc_layout: null pointer");
+  UDH_REQUIRE(B >= 1 && img_h >= 2 && img_w >= 2 && img_h < 32768 && img_w < 32768, "udh_debug_ecc_layout: bad dimensions");
+  ecc_split_offsets(B, img_h, img_w, off);
+  *tiles = ecc_split_tiles(img_h, img_w);
+  return UDH_OK;
 }
 
 extern "C" int udh_ecc_homography_split(const uint8_t* tmpl, const uint8_t* input, const float* W_init, int max_iters, double eps,
