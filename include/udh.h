@@ -485,6 +485,29 @@ size_t udh_mosaic_workspace_bytes(int n);
 int udh_mosaic_blend_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, int n, int c, const int32_t* tile_ptr,
                         const int32_t* tile_frames, int dst_h, int dst_w, int feather, uint8_t* dst, uint8_t* mask, void* ws,
                         size_t ws_bytes, void* stream);
+/* udh_mosaic_multiband_u8: n frames blended onto one dst_h x dst_w canvas across frequency bands, byte for byte
+ *   cv2.detail_MultiBandBlender(0, bands, CV_16S) on the CPU (oracle/multiband.py restates the rule).  Frame k is fed as
+ *   udh_warp_perspective_u8(frame k, M_k, roi_h, roi_w) at the ROI's top-left (x_lo, y_lo), with mask 255 where that warp is
+ *   valid (udh_mosaic_blend_u8's rule: W != 0 and the source position inside the frame) and 0 elsewhere.  Then, with
+ *   B' = min(bands, ceil(log2(max(dst_h, dst_w)))) and the canvas padded to multiples of 2^B': each frame's rectangle is its
+ *   ROI grown by 3 2^B' per side and aligned as cv2 does; the image is bordered BORDER_REFLECT, the weight (256 where the
+ *   mask is set) a constant 0; G_{i+1} = pyrDown(G_i) in uint8 and W_{i+1} = pyrDown(W_i) in int16; L_i = G_i - pyrUp(G_{i+1})
+ *   (L_B' = G_B'); per level acc += (int16)((L W) >> 8), wacc += W with wrapping int16 adds.  The blend normalises each level
+ *   to (int16)((acc << 8) / (wacc + 1)) (0 where wacc = -1, where cv2 divides by zero), collapses from the top with
+ *   pyrUp and saturating int16 adds, and crops; dst = saturate_u8 of that and mask = 255 where wacc_0 > 0, else both 0.
+ *   frames [n] (host array of device pointers), frame k uint8 [h_k,w_k,3]; sizes [n,2] int32 (host); M [n,9] float64
+ *   (device) frame k -> its ROI (M_canvas translated by (-x_lo, -y_lo)); rois [n,4] int32 (host) x_lo, y_lo, x_hi, y_hi
+ *   (exclusive), non-empty and inside the canvas; dst [dst_h,dst_w,3] and mask [dst_h,dst_w] uint8 (device).  The sums are
+ *   gathered per canvas pixel in int32 and stored once, so the bytes do not depend on the frames' order.  Only c = 3 (the
+ *   blender takes 3 channels).  n <= 65535, sides < 32767, 0 <= bands <= 10.
+ *   ws: udh_mosaic_multiband_workspace_bytes(rois, n, dst_h, dst_w, bands) bytes of device memory (0: bad arguments). */
+size_t udh_mosaic_multiband_workspace_bytes(const int32_t* rois, int n, int dst_h, int dst_w, int bands);
+int udh_mosaic_multiband_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const int32_t* rois, int n, int c,
+                            int dst_h, int dst_w, int bands, uint8_t* dst, uint8_t* mask, void* ws, size_t ws_bytes, void* stream);
+/* udh_debug_multiband_layout: where udh_mosaic_multiband_u8's workspace keeps the canvas pyramid, for tests that read it.
+ *   off[i] (i <= B'): byte offset of level i, int16 [Hp >> i][Wp >> i][4] (acc's three channels, then wacc), as the feeds
+ *   left it (the blend does not overwrite it); dims = {B', Hp, Wp}, the padded canvas. */
+int udh_debug_multiband_layout(const int32_t* rois, int n, int dst_h, int dst_w, int bands, size_t off[11], int dims[3]);
 
 /* ---- instrumentation read by bench.py -------------------------------------------------------------------------
  * udh_launch_count: kernels this library has launched in this process (monotonic).

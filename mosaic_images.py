@@ -9,17 +9,19 @@ GPU (unsuperviseddeephomographyral2018_b200.mosaic states the chaining, the canv
 --frames takes a list file (one path per line, relative to the file, in sequence order) or a directory, read as
 sorted(glob(dir/--glob)) (default *.JPG, gen_real_data.py's rule).  The model, refinement and batch options are
 align_images.py's.  --ref_frame picks the reference frame (-1: the middle one, N // 2); --feather is the blend's ramp in
-source pixels (0: a plain average of the overlapping frames).
+source pixels (0: a plain average of the overlapping frames).  --blend multiband blends across --bands frequency bands
+instead (cv2.detail_MultiBandBlender's rule, byte for byte): low frequencies over a wide region, high ones over a narrow
+one, which hides the seams a drifting chain or an exposure change leaves.
 
 Writes in --out_dir:
   pairs.txt    `frame_k frame_k+1` and H's nine entries per consecutive pair, as align_images.py's homographies.txt;
   refine.txt   with refinement, `frame_k frame_k+1 rho status levels` per pair, as align_images.py writes it;
-  mosaic.txt   `canvas Hc Wc ref r`, then `name kept|dropped` and the nine entries of M_k (frame k -> canvas) per frame,
+  mosaic.txt   `canvas Hc Wc ref r` (` blend multiband B` appended with --blend multiband), then `name kept|dropped` and the nine entries of M_k (frame k -> canvas) per frame,
                '%.9g' of their float32 values; the blend uses those float32 values, so the file reproduces mosaic.jpg;
   mosaic.jpg   the mosaic (BGR, JPEG quality 95, byte-identical to cv2.imencode of the same pixels).
 A frame whose grown corners map behind the reference camera is dropped.  The canvas must be one the JPEG encoder takes
 (about 110 MP in colour); a larger one stops with an error naming the frame that reaches farthest.  Prints the GPU time
-of each phase (CUDA events: prep, forward, refine, blend, encode).
+of each phase (CUDA events: prep, forward, refine, blend, encode; the blend named when it is multi-band).
 """
 from __future__ import absolute_import, division, print_function
 
@@ -41,6 +43,9 @@ def build_parser():
     align_images.add_weights_and_refine_options(p)
     p.add_argument('--ref_frame', type=int, default=-1, help='reference frame (-1: the middle one)')
     p.add_argument('--feather', type=int, default=64, help='blend ramp in source pixels, 0..1024 (0: plain average)')
+    p.add_argument('--blend', type=str, default='feather', choices=['feather', 'multiband'],
+                   help='feather: feathered average; multiband: blend across frequency bands')
+    p.add_argument('--bands', type=int, default=5, help='frequency bands of --blend multiband, 0..10')
     p.add_argument('--out_dir', type=str, default='mosaic')
     return p
 
@@ -67,6 +72,8 @@ def run(args, est, decode, encode):
     from unsuperviseddeephomographyral2018_b200 import align, mosaic
     if not 0 <= args.feather <= 1024:
         raise SystemExit("--feather must be in 0..1024 (got %d)" % args.feather)
+    if not 0 <= args.bands <= 10:
+        raise SystemExit("--bands must be in 0..10 (got %d)" % args.bands)
     names, paths = frame_list(args)
     os.makedirs(args.out_dir, exist_ok=True)
     refining = args.refine_levels != 0
@@ -75,7 +82,7 @@ def run(args, est, decode, encode):
     imgs = decode(paths)
     try:
         out = mosaic.build_mosaic(est, imgs, None if args.ref_frame < 0 else args.ref_frame, refine, args.feather,
-                                  float32_M=True)
+                                  float32_M=True, blend=args.blend, bands=args.bands)
     except ValueError as e:
         raise SystemExit(str(e))
     H = out["H_pairs"]
@@ -86,7 +93,7 @@ def run(args, est, decode, encode):
         with open(os.path.join(args.out_dir, "refine.txt"), "w") as f:
             f.write("".join("%s %s %.9g %d %d\n" % (names[k], names[k + 1], rho[k], status[k], level[k]) for k in range(len(H))))
     Hc, Wc = out["mask"].shape
-    lines = ["canvas %d %d ref %d" % (Hc, Wc, out["ref"])]
+    lines = ["canvas %d %d ref %d" % (Hc, Wc, out["ref"]) + (" blend multiband %d" % args.bands if args.blend == "multiband" else "")]
     for k, nm in enumerate(names):
         lines.append(" ".join([nm, "kept" if out["kept"][k] else "dropped"] +
                               ["%.9g" % v for v in align.homography_as_written(out["M"][k])[0]]))
@@ -105,9 +112,11 @@ def run(args, est, decode, encode):
         f.write(blob)
     cover = float((out["mask"] != 0).float().mean())
     print("===> %d frames (%d kept) on a %dx%d canvas (ref %s, %.1f %% covered): GPU %.3f ms (prep %.3f, forward %.3f, %s"
-          "blend %.3f, encode %.3f)" % (len(names), int(np.sum(out["kept"])), Hc, Wc, names[out["ref"]], 100 * cover,
-                                        sum(ms.values()), ms["prep"], ms["forward"],
-                                        "refine %.3f, " % ms["refine"] if refining else "", ms["blend"], ms["encode"]), flush=True)
+          "%sblend %.3f, encode %.3f)" % (len(names), int(np.sum(out["kept"])), Hc, Wc, names[out["ref"]], 100 * cover,
+                                          sum(ms.values()), ms["prep"], ms["forward"],
+                                          "refine %.3f, " % ms["refine"] if refining else "",
+                                          "multiband %d " % args.bands if args.blend == "multiband" else "", ms["blend"],
+                                          ms["encode"]), flush=True)
     return out
 
 

@@ -7,11 +7,16 @@
   * the host path, oracle/mosaic.py (cv2.warpPerspective per frame + a NumPy int64 blend), with cv2.setNumThreads(1) and
     (16), against the kernel on the same 8 x 1080x1920 sweep (the oracle evaluates every frame at every canvas pixel);
   * mosaic_images.py end to end (device decode, estimate, chain, blend, JPEG encode, files written) with seeded weights on
-    8 quality-95 JPEGs of 1080x1920, ms per frame.
+    8 quality-95 JPEGs of 1080x1920, ms per frame;
+  * the multi-band blend (udh_mosaic_multiband_u8) on the same two sweeps at 5 and 8 bands: CUDA-event ms per mosaic, per
+    phase through the library's phase timers (base level, pyramids, accumulate, collapse), bytes moved computed from the
+    shapes against 3.35 TB/s, and cv2.detail_MultiBandBlender (the oracle, CPU) on the same frames with 1 and 16 threads
+    (the ROI warps and the blender timed apart).
 Prints one JSON line with the card name and power limit read in the same run.
 
-    python tools/mosaic_time.py
+    python tools/mosaic_time.py [--legs feather,multiband]
 """
+import argparse
 import json
 import os
 import shutil
@@ -118,9 +123,86 @@ def cli_time(root, n=8, h=1080, w=1920):
     return {"frames": n, "frame": [h, w], "ms_per_frame": res["timed"] / n}
 
 
+def multiband_bytes(M, h, w, canvas, bands):
+    """Bytes the multi-band kernels move at least, from the shapes: per frame element of level i, G (4) and W (2) written
+    once (base level or pyrDown) and read by pyrDown and accumulate, G_{i+1} read again for pyrUp; per canvas element of
+    level i, (acc, wacc) written (8) and read (8), R_i written and read (8, i >= 1); the source pixels (3 per covered
+    frame pixel) and the uint8 mosaic and mask (4 per canvas pixel)."""
+    from oracle import multiband as MB
+    Hc, Wc = canvas
+    rois, _ = mosaic.multiband_rois(M, [(h, w)] * len(M), Hc, Wc)
+    B = MB.num_bands(Hc, Wc, bands)
+    a = 1 << B
+    Hp, Wp = Hc + (-Hc) % a, Wc + (-Wc) % a
+    frame_el = [0] * (B + 1)
+    for x0, y0, x1, y1 in rois:
+        r = MB.padded_rect(int(x0), int(y0), int(x1 - x0), int(y1 - y0), Hp, Wp, B)
+        for i in range(B + 1):
+            frame_el[i] += ((r[2] - r[0]) >> i) * ((r[3] - r[1]) >> i)
+    canvas_el = [(Hp >> i) * (Wp >> i) for i in range(B + 1)]
+    nbytes = 3 * sum(mapped_area(M[k], h, w) for k in range(len(M))) + 4 * Hc * Wc
+    for i in range(B + 1):
+        nbytes += 6 * frame_el[i] * (3 if i < B else 2) + (4 * frame_el[i + 1] if i < B else 0)
+        nbytes += 16 * canvas_el[i] + (16 if i >= 1 else 0) * canvas_el[i]
+    return nbytes, B, frame_el, canvas_el
+
+
+def multiband_time(frames, M, canvas, bands, reps=5):
+    Hc, Wc = canvas
+    dev = [torch.from_numpy(f).cuda() for f in frames]
+    ops.mosaic_multiband_u8(dev, M, Hc, Wc, bands)
+    torch.cuda.synchronize()
+    _lib.lib.udh_prof_enable(1)
+    _lib.lib.udh_prof_reset()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(reps):
+        ops.mosaic_multiband_u8(dev, M, Hc, Wc, bands)
+    e1.record()
+    e1.synchronize()
+    ph = _lib.prof_read_all()
+    _lib.lib.udh_prof_enable(0)
+    ms = e0.elapsed_time(e1) / reps
+    nbytes, B, frame_el, canvas_el = multiband_bytes(M, frames[0].shape[0], frames[0].shape[1], canvas, bands)
+    phases = {k.split(".")[1]: v[0] / reps for k, v in ph.items() if k.startswith("multiband.")}
+    return {"frames": len(frames), "frame": list(frames[0].shape[:2]), "canvas": [Hc, Wc], "canvas_mp": Hc * Wc / 1e6,
+            "bands": bands, "bands_used": B, "ms": ms, "phase_ms": phases, "bytes": nbytes, "GB_per_s": nbytes / ms / 1e6,
+            "pct_of_hbm": 100.0 * nbytes / ms / 1e9 / HBM_TBS, "frame_elements": frame_el, "canvas_elements": canvas_el}
+
+
+def multiband_host_time(frames, M, canvas, bands, threads):
+    import cv2
+    from oracle import multiband as MB
+    cv2.setNumThreads(threads)
+    t0 = time.perf_counter()
+    fed = MB.fed(frames, M, canvas[0], canvas[1])
+    t1 = time.perf_counter()
+    MB.cv2_blend(*fed, canvas[0], canvas[1], bands)
+    t2 = time.perf_counter()
+    return {"rois_ms": (t1 - t0) * 1e3, "blender_ms": (t2 - t1) * 1e3}
+
+
 def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--legs", default="feather,multiband")
+    legs = ap.parse_args().legs.split(",")
     torch.cuda.set_device(0)
     out = {"gpu": torch.cuda.get_device_name(0), "card": jpeg_time.card(), "feather": 64}
+    if "multiband" in legs:
+        for n, h, w in ((32, 1080, 1920), (16, 3000, 4000)):
+            frames, M, canvas = placed_sweep(n, h, w)
+            for bands in (5, 8):
+                out["multiband_%dx%dx%d_b%d" % (n, h, w, bands)] = r = multiband_time(frames, M, canvas, bands)
+                print(json.dumps(r), flush=True)
+            host = {"bands": 5}
+            for t in (1, 16):
+                host["threads_%d" % t] = multiband_host_time(frames, M, canvas, 5, t)
+            out["multiband_host_%dx%dx%d" % (n, h, w)] = host
+            print(json.dumps(host), flush=True)
+            del frames
+    if "feather" not in legs:
+        print(json.dumps(out))
+        return
     for n, h, w in ((32, 1080, 1920), (16, 3000, 4000)):
         frames, M, canvas = placed_sweep(n, h, w)
         out["kernel_%dx%dx%d" % (n, h, w)] = r = kernel_time(frames, M, canvas)

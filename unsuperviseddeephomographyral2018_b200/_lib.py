@@ -172,6 +172,10 @@ SIGNATURES = {
     "udh_mosaic_workspace_bytes": (c_size_t, [c_int]),
     "udh_mosaic_blend_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p,
                                     c_void_p, c_void_p, c_size_t, c_void_p]),
+    "udh_mosaic_multiband_workspace_bytes": (c_size_t, [c_void_p, c_int, c_int, c_int, c_int]),
+    "udh_mosaic_multiband_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                        c_void_p, c_size_t, c_void_p]),
+    "udh_debug_multiband_layout": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(c_size_t), POINTER(c_int)]),
     "udh_draw_report_workspace_bytes": (c_size_t, [c_int]),
     "udh_draw_report_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_int, c_int, c_int,
                                    c_void_p]),

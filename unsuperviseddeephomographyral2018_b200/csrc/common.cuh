@@ -18,7 +18,9 @@ enum ProfTag {
   PROF_CONV_DGRAD0 = 8,  // +layer
   PROF_CONV_WGRAD0 = 16, // +layer
   PROF_POOL_FWD = 24, PROF_POOL_BWD, PROF_FC_FWD, PROF_FC_BWD, PROF_DLT, PROF_WARP_FWD, PROF_WARP_BWD, PROF_SSIM,
-  PROF_H4P_LOSS, PROF_ADAM, PROF_ELTWISE, PROF_TC_PREP, PROF_NUM_TAGS
+  PROF_H4P_LOSS, PROF_ADAM, PROF_ELTWISE, PROF_TC_PREP,
+  PROF_MB_BASE, PROF_MB_DOWN, PROF_MB_ACC, PROF_MB_COLLAPSE,   // the mosaic's multi-band blend, by phase
+  PROF_NUM_TAGS
 };
 extern unsigned long long g_launches;
 extern int g_sm_reserve;      // SMs the persistent tensor-core kernels leave free (udh_set_sm_reserve)

@@ -30,7 +30,8 @@ const char* kTagNames[PROF_NUM_TAGS] = {
     "conv1_1.fwd", "conv1_2.fwd", "conv2_1.fwd", "conv2_2.fwd", "conv3_1.fwd", "conv3_2.fwd", "conv4_1.fwd", "conv4_2.fwd",
     "conv1_1.dgrad", "conv1_2.dgrad", "conv2_1.dgrad", "conv2_2.dgrad", "conv3_1.dgrad", "conv3_2.dgrad", "conv4_1.dgrad", "conv4_2.dgrad",
     "conv1_1.wgrad", "conv1_2.wgrad", "conv2_1.wgrad", "conv2_2.wgrad", "conv3_1.wgrad", "conv3_2.wgrad", "conv4_1.wgrad", "conv4_2.wgrad",
-    "pool.fwd", "pool.bwd", "fc.fwd", "fc.bwd", "dlt", "warp_loss.fwd", "warp_loss.bwd", "ssim", "h4p_loss", "adam", "eltwise", "tc_prep"};
+    "pool.fwd", "pool.bwd", "fc.fwd", "fc.bwd", "dlt", "warp_loss.fwd", "warp_loss.bwd", "ssim", "h4p_loss", "adam", "eltwise", "tc_prep",
+    "multiband.base", "multiband.pyramids", "multiband.accumulate", "multiband.collapse"};
 constexpr int kMaxPairs = 2048;
 struct TagState { cudaEvent_t ev[kMaxPairs][2]; int created = 0, used = 0; bool open = false; };
 bool g_prof_on = false;

@@ -10,7 +10,9 @@
 // (4 C bytes), so a warp writes 128 C contiguous bytes; the 4 C taps of a pixel are read through the read-only data cache,
 // where neighbouring output pixels share them.  It does not reach HBM's bound (DESIGN section 5): the float64 coordinate
 // arithmetic, one IEEE division per pixel, is part of the rounding contract.
-// The sequence mosaic's blend (udh_mosaic_blend_u8, below) samples every frame with the same coordinate and tap helpers.
+// The sequence mosaic's blends (udh_mosaic_blend_u8 and udh_mosaic_multiband_u8, below) sample every frame with the same
+// coordinate and tap helpers.
+#include <cmath>
 #include <cstdint>
 #include <vector>
 
@@ -202,6 +204,297 @@ __global__ void __launch_bounds__(256) mosaic_blend_u8_kernel(const MosaicFrame*
   }
 }
 
+// ---- multi-band blend: cv2.detail_MultiBandBlender with CV_16S weights (the rule: oracle/multiband.py) ----------------
+// Per frame k, its fed rectangle (ROI grown by the gap, aligned to 2^B) holds the image pyramid G_i (uchar4, RGB + pad)
+// and the weight pyramid W_i (int16) in two pools; the canvas pyramid keeps (acc, wacc) as short4 per pixel, and the
+// collapsed levels R_i (i >= 1) as short4 in a second pyramid, so acc and wacc survive the blend.
+constexpr int MB_MAX_BANDS = 10;
+
+struct MultibandFrame {
+  const uint8_t* src;
+  int h, w;                        // the frame
+  int rx, ry, rw, rh, bw;          // its ROI on the canvas, and the ROI warp's tile width
+  int x0, y0, pw, ph;              // the fed rectangle at level 0 (canvas coordinates; multiples of 2^B)
+  int64_t off[MB_MAX_BANDS + 1];   // element offset of level i in the G and W pools
+};
+
+// BORDER_REFLECT (fedcba|abcdef|fedcba) for any n >= 1, folding as often as needed.
+__device__ __forceinline__ int mb_reflect(int i, int n) {
+  if (n == 1) return 0;
+  int p = i % (2 * n);
+  if (p < 0) p += 2 * n;
+  return p < n ? p : 2 * n - 1 - p;
+}
+
+// cv2.pyrUp's taps along one axis at output o of a source of n: -1 reads 1 (reflect-101), n reads n - 1 (reflect).
+__device__ __forceinline__ void mb_up_taps(int o, int n, int* t, int* wt) {
+  const int j = o >> 1;
+  if (o & 1) {
+    t[0] = j; t[1] = j + 1; t[2] = j + 1;
+    wt[0] = 4; wt[1] = 4; wt[2] = 0;
+  } else {
+    t[0] = j - 1; t[1] = j; t[2] = j + 1;
+    wt[0] = 1; wt[1] = 6; wt[2] = 1;
+  }
+#pragma unroll
+  for (int k = 0; k < 3; ++k) t[k] = t[k] < 0 ? min(1, n - 1) : min(t[k], n - 1);
+}
+
+__device__ __forceinline__ int mb_sat16(int v) { return min(max(v, -32768), 32767); }
+
+// Level 0 of every frame: the ROI warp bordered with BORDER_REFLECT, and the 0 / 256 weight with a constant 0 border.
+__global__ void __launch_bounds__(256) multiband_base_kernel(const MultibandFrame* __restrict__ fr, const double* __restrict__ M,
+                                                             uchar4* __restrict__ G, int16_t* __restrict__ Wt) {
+  __shared__ double mi[9];
+  const int k = blockIdx.y;
+  if (threadIdx.x == 0) cv_invert3(M + (int64_t)k * 9, mi);
+  __syncthreads();
+  const MultibandFrame* F = fr + k;
+  const uint8_t* s = reinterpret_cast<const uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&F->src)));
+  const int h = __ldg(&F->h), w = __ldg(&F->w), rx = __ldg(&F->rx), ry = __ldg(&F->ry), rw = __ldg(&F->rw), rh = __ldg(&F->rh);
+  const int bw = __ldg(&F->bw), ox = __ldg(&F->x0) - rx, oy = __ldg(&F->y0) - ry, pw = __ldg(&F->pw);
+  const int npx = pw * __ldg(&F->ph);                                 // < 2^31: padded sides < 32767 + 1024
+  const int64_t off = __ldg(&F->off[0]);
+  const int xm = 32 * (w - 1), ym = 32 * (h - 1);
+  for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < npx; e += gridDim.x * blockDim.x) {
+    const int y = e / pw, x = e - y * pw;
+    const int ix = x + ox, iy = y + oy;
+    const int sx = mb_reflect(ix, rw), sy = mb_reflect(iy, rh);
+    int X, Y, v[3];
+    const double Wd = wp_coords(mi, sx, sy, bw, X, Y);
+    wp_sample<3>(s, h, w, X, Y, v);
+    const bool valid = ix == sx && iy == sy && Wd != 0.0 && X >= 0 && X <= xm && Y >= 0 && Y <= ym;
+    G[off + e] = make_uchar4((unsigned char)v[0], (unsigned char)v[1], (unsigned char)v[2], 0);
+    Wt[off + e] = valid ? 256 : 0;
+  }
+}
+
+// Level lvl -> lvl + 1 of every frame's G and W: cv2.pyrDown (taps 1 4 6 4 1, BORDER_REFLECT_101, (sum + 128) >> 8).
+__global__ void __launch_bounds__(256) multiband_down_kernel(const MultibandFrame* __restrict__ fr, uchar4* __restrict__ G,
+                                                             int16_t* __restrict__ Wt, int lvl) {
+  const MultibandFrame* F = fr + blockIdx.y;
+  const int sw = __ldg(&F->pw) >> lvl, sh = __ldg(&F->ph) >> lvl, dw = sw >> 1, npx = dw * (sh >> 1);
+  const int64_t si = __ldg(&F->off[lvl]), di = __ldg(&F->off[lvl + 1]);
+  const int kw[5] = {1, 4, 6, 4, 1};
+  for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < npx; e += gridDim.x * blockDim.x) {
+    const int y = e / dw, x = e - y * dw;
+    int tx[5];
+#pragma unroll
+    for (int j = 0; j < 5; ++j) tx[j] = reflect101(2 * x + j - 2, sw);
+    int a0 = 0, a1 = 0, a2 = 0, aw = 0;
+#pragma unroll
+    for (int i = 0; i < 5; ++i) {
+      const int64_t row = si + (int64_t)reflect101(2 * y + i - 2, sh) * sw;
+      int r0 = 0, r1 = 0, r2 = 0, rw = 0;
+#pragma unroll
+      for (int j = 0; j < 5; ++j) {
+        const uchar4 g = G[row + tx[j]];
+        r0 += kw[j] * g.x; r1 += kw[j] * g.y; r2 += kw[j] * g.z;
+        rw += kw[j] * Wt[row + tx[j]];
+      }
+      a0 += kw[i] * r0; a1 += kw[i] * r1; a2 += kw[i] * r2; aw += kw[i] * rw;
+    }
+    G[di + e] = make_uchar4((unsigned char)((a0 + 128) >> 8), (unsigned char)((a1 + 128) >> 8), (unsigned char)((a2 + 128) >> 8), 0);
+    Wt[di + e] = (int16_t)mb_sat16((aw + 128) >> 8);
+  }
+}
+
+// Gather form, level lvl of the canvas pyramid: one thread per pixel of a MB_TILE_W x MB_TILE_H tile.  The CTA collects the
+// frames whose rectangle at this level meets its tile (256 at a time), and each thread sums (L W) >> 8 and W of every such
+// frame in int32 and stores them once, truncated to int16: the same bytes as cv2's wrapping int16 adds, in any frame order.
+// L = G_lvl - pyrUp(G_lvl+1), formed on the fly (G_B at the top).
+constexpr int MB_TILE_W = 32, MB_TILE_H = 8;
+
+__global__ void __launch_bounds__(256) multiband_accumulate_kernel(const MultibandFrame* __restrict__ fr, int n,
+                                                                   const uchar4* __restrict__ G, const int16_t* __restrict__ Wt,
+                                                                   int lvl, int top, int cw, int ch, short4* __restrict__ acc) {
+  __shared__ int cand[256];
+  __shared__ int ncand;
+  const int tx0 = blockIdx.x * MB_TILE_W, ty0 = blockIdx.y * MB_TILE_H;
+  const int x = tx0 + threadIdx.x % MB_TILE_W, y = ty0 + threadIdx.x / MB_TILE_W;
+  int a0 = 0, a1 = 0, a2 = 0, aw = 0;
+  for (int c0 = 0; c0 < n; c0 += 256) {
+    if (threadIdx.x == 0) ncand = 0;
+    __syncthreads();
+    const int k = c0 + threadIdx.x;
+    if (k < n) {
+      const MultibandFrame* F = fr + k;
+      const int fx0 = __ldg(&F->x0) >> lvl, fy0 = __ldg(&F->y0) >> lvl;
+      const int fx1 = fx0 + (__ldg(&F->pw) >> lvl), fy1 = fy0 + (__ldg(&F->ph) >> lvl);
+      if (fx0 < tx0 + MB_TILE_W && fx1 > tx0 && fy0 < ty0 + MB_TILE_H && fy1 > ty0) cand[atomicAdd(&ncand, 1)] = k;
+    }
+    __syncthreads();
+    const int nc = ncand;
+    for (int j = 0; j < nc; ++j) {
+      const MultibandFrame* F = fr + cand[j];
+      const int fw = __ldg(&F->pw) >> lvl, fh = __ldg(&F->ph) >> lvl;
+      const int lx = x - (__ldg(&F->x0) >> lvl), ly = y - (__ldg(&F->y0) >> lvl);
+      if ((unsigned)lx >= (unsigned)fw || (unsigned)ly >= (unsigned)fh) continue;
+      const int64_t p = __ldg(&F->off[lvl]) + (int64_t)ly * fw + lx;
+      const int wt = Wt[p];
+      if (wt == 0) continue;                                            // adds 0 to both sums
+      const uchar4 g = G[p];
+      int l0 = g.x, l1 = g.y, l2 = g.z;
+      if (!top) {
+        const int uw = fw >> 1, uh = fh >> 1;
+        const int64_t u0 = __ldg(&F->off[lvl + 1]);
+        int txs[3], wxs[3], tys[3], wys[3];
+        mb_up_taps(lx, uw, txs, wxs);
+        mb_up_taps(ly, uh, tys, wys);
+        int s0 = 0, s1 = 0, s2 = 0;
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+          if (wys[i] == 0) continue;
+          int r0 = 0, r1 = 0, r2 = 0;
+#pragma unroll
+          for (int q = 0; q < 3; ++q) {
+            if (wxs[q] == 0) continue;
+            const uchar4 u = G[u0 + (int64_t)tys[i] * uw + txs[q]];
+            r0 += wxs[q] * u.x; r1 += wxs[q] * u.y; r2 += wxs[q] * u.z;
+          }
+          s0 += wys[i] * r0; s1 += wys[i] * r1; s2 += wys[i] * r2;
+        }
+        l0 -= (s0 + 32) >> 6; l1 -= (s1 + 32) >> 6; l2 -= (s2 + 32) >> 6;
+      }
+      a0 += (l0 * wt) >> 8; a1 += (l1 * wt) >> 8; a2 += (l2 * wt) >> 8;
+      aw += wt;
+    }
+    __syncthreads();
+  }
+  if (x < cw && y < ch) acc[(int64_t)y * cw + x] = make_short4((short)a0, (short)a1, (short)a2, (short)aw);
+}
+
+// cv2's normalisation: (int16)((acc << 8) / (wacc + 1)), truncating.  cv2 divides by zero where wacc = -1; this writes 0.
+__device__ __forceinline__ int mb_norm(int a, int wacc) {
+  const int d = wacc + 1;
+  return d ? (short)((a * 256) / d) : 0;
+}
+
+// Level lvl of the collapse: R = sat16(pyrUp(R_lvl+1) + N) (N alone at the top).  FINAL (level 0) writes the cropped
+// uint8 RGB mosaic and the 0 / 255 mask (wacc > 0) instead of R.
+template <bool FINAL>
+__global__ void __launch_bounds__(256) multiband_collapse_kernel(const short4* __restrict__ acc, const short4* __restrict__ up,
+                                                                 int cw, int ch, short4* __restrict__ R, int dh, int dw,
+                                                                 uint8_t* __restrict__ dst, uint8_t* __restrict__ mask) {
+  const int ow = FINAL ? dw : cw, npx = FINAL ? dh * dw : cw * ch;
+  for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < npx; e += gridDim.x * blockDim.x) {
+    const int y = e / ow, x = e - y * ow;
+    const short4 a = acc[(int64_t)y * cw + x];
+    int v0 = mb_norm(a.x, a.w), v1 = mb_norm(a.y, a.w), v2 = mb_norm(a.z, a.w);
+    if (up) {
+      const int uw = cw >> 1, uh = ch >> 1;
+      int txs[3], wxs[3], tys[3], wys[3];
+      mb_up_taps(x, uw, txs, wxs);
+      mb_up_taps(y, uh, tys, wys);
+      int s0 = 0, s1 = 0, s2 = 0;
+#pragma unroll
+      for (int i = 0; i < 3; ++i) {
+        if (wys[i] == 0) continue;
+        int r0 = 0, r1 = 0, r2 = 0;
+#pragma unroll
+        for (int q = 0; q < 3; ++q) {
+          if (wxs[q] == 0) continue;
+          const short4 u = up[(int64_t)tys[i] * uw + txs[q]];
+          r0 += wxs[q] * u.x; r1 += wxs[q] * u.y; r2 += wxs[q] * u.z;
+        }
+        s0 += wys[i] * r0; s1 += wys[i] * r1; s2 += wys[i] * r2;
+      }
+      v0 = mb_sat16(mb_sat16((s0 + 32) >> 6) + v0);
+      v1 = mb_sat16(mb_sat16((s1 + 32) >> 6) + v1);
+      v2 = mb_sat16(mb_sat16((s2 + 32) >> 6) + v2);
+    }
+    if (FINAL) {
+      const bool m = a.w > 0;
+      uint8_t* d = dst + ((int64_t)y * dw + x) * 3;
+      d[0] = m ? (uint8_t)min(max(v0, 0), 255) : 0;
+      d[1] = m ? (uint8_t)min(max(v1, 0), 255) : 0;
+      d[2] = m ? (uint8_t)min(max(v2, 0), 255) : 0;
+      mask[(int64_t)y * dw + x] = m ? 255 : 0;
+    } else {
+      R[(int64_t)y * cw + x] = make_short4((short)v0, (short)v1, (short)v2, 0);
+    }
+  }
+}
+
+// The host's plan of one multi-band call: bands, padded canvas, frame table and workspace layout.
+struct MultibandPlan {
+  int B, Hp, Wp, max_px[MB_MAX_BANDS + 1];
+  int64_t E;                                                          // elements per pool
+  size_t off_g, off_w, off_acc[MB_MAX_BANDS + 1], off_r[MB_MAX_BANDS + 1], total;
+  std::vector<MultibandFrame> fr;
+};
+
+static size_t mb_align(size_t v) { return (v + 255) & ~(size_t)255; }
+
+// rois [n,4] (x_lo, y_lo, x_hi, y_hi) -> plan (sizes may be null: the frame fields are left unset).  0 or an error.
+static int mb_plan(const int32_t* rois, const int32_t* sizes, int n, int Hc, int Wc, int bands, MultibandPlan& p) {
+  UDH_REQUIRE(n >= 1 && n <= 65535 && Hc >= 1 && Wc >= 1 && Hc < 32767 && Wc < 32767,
+              "udh_mosaic_multiband_u8: bad dimensions (n %d, canvas %dx%d)", n, Hc, Wc);
+  UDH_REQUIRE(bands >= 0 && bands <= MB_MAX_BANDS, "udh_mosaic_multiband_u8: bands must be in [0, %d] (got %d)", MB_MAX_BANDS, bands);
+  UDH_REQUIRE(rois, "udh_mosaic_multiband_u8: null rois");
+  // cv2's band count: min(B, ceil(log(max side) / log 2)) in double
+  const int lg = (int)std::ceil(std::log((double)(Hc > Wc ? Hc : Wc)) / std::log(2.0));
+  p.B = bands < lg ? bands : lg;
+  const int a = 1 << p.B, gap = 3 << p.B;
+  p.Hp = Hc + (a - Hc % a) % a;
+  p.Wp = Wc + (a - Wc % a) % a;
+  p.fr.assign((size_t)n, MultibandFrame{});
+  for (int i = 0; i <= MB_MAX_BANDS; ++i) p.max_px[i] = 0;
+  int64_t E = 0;
+  for (int k = 0; k < n; ++k) {
+    const int* r = rois + 4 * k;
+    UDH_REQUIRE(r[0] >= 0 && r[1] >= 0 && r[0] < r[2] && r[1] < r[3] && r[2] <= Wc && r[3] <= Hc,
+                "udh_mosaic_multiband_u8: frame %d's ROI (%d, %d)..(%d, %d) is empty or leaves the %dx%d canvas", k, r[0], r[1],
+                r[2], r[3], Hc, Wc);
+    MultibandFrame& F = p.fr[k];
+    F.rx = r[0]; F.ry = r[1]; F.rw = r[2] - r[0]; F.rh = r[3] - r[1];
+    const int bh = F.rh < 16 ? F.rh : 16;
+    F.bw = 1024 / bh < F.rw ? 1024 / bh : F.rw;
+    // cv2's tl_new / br_new: grow by the gap, clip, align to 2^B, shift back inside the padded canvas
+    int x0 = F.rx - gap > 0 ? F.rx - gap : 0, y0 = F.ry - gap > 0 ? F.ry - gap : 0;
+    int x1 = r[2] + gap < p.Wp ? r[2] + gap : p.Wp, y1 = r[3] + gap < p.Hp ? r[3] + gap : p.Hp;
+    x0 = (x0 >> p.B) << p.B;
+    y0 = (y0 >> p.B) << p.B;
+    x1 = x0 + (x1 - x0) + (a - (x1 - x0) % a) % a;
+    y1 = y0 + (y1 - y0) + (a - (y1 - y0) % a) % a;
+    const int dx = x1 - p.Wp > 0 ? x1 - p.Wp : 0, dy = y1 - p.Hp > 0 ? y1 - p.Hp : 0;
+    F.x0 = x0 - dx; F.y0 = y0 - dy; F.pw = x1 - x0; F.ph = y1 - y0;
+    for (int i = 0; i <= p.B; ++i) {
+      const int px = (F.pw >> i) * (F.ph >> i);
+      F.off[i] = E;
+      E += px;
+      if (px > p.max_px[i]) p.max_px[i] = px;
+    }
+    if (sizes) {
+      F.h = sizes[2 * k];
+      F.w = sizes[2 * k + 1];
+      UDH_REQUIRE(F.h >= 1 && F.w >= 1 && F.h < 32767 && F.w < 32767, "udh_mosaic_multiband_u8: frame %d is %dx%d", k, F.h, F.w);
+    }
+  }
+  p.E = E;
+  size_t o = mb_align((size_t)n * sizeof(MultibandFrame));
+  p.off_g = o;
+  o = mb_align(o + (size_t)E * sizeof(uchar4));
+  p.off_w = o;
+  o = mb_align(o + (size_t)E * sizeof(int16_t));
+  for (int i = 0; i <= p.B; ++i) {
+    p.off_acc[i] = o;
+    o = mb_align(o + (size_t)(p.Hp >> i) * (size_t)(p.Wp >> i) * sizeof(short4));
+  }
+  p.off_r[0] = 0;
+  for (int i = 1; i <= p.B; ++i) {
+    p.off_r[i] = o;
+    o = mb_align(o + (size_t)(p.Hp >> i) * (size_t)(p.Wp >> i) * sizeof(short4));
+  }
+  p.total = o;
+  return UDH_OK;
+}
+
+static unsigned mb_blocks(int64_t px) {
+  const int64_t b = (px + 255) / 256;
+  return (unsigned)(b < 1 ? 1 : b > 4096 ? 4096 : b);
+}
+
 }  // namespace udh
 
 using namespace udh;
@@ -271,4 +564,84 @@ extern "C" int udh_mosaic_blend_u8(const uint8_t* const* frames, const int32_t* 
   else
     mosaic_blend_u8_kernel<1><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, 32 * feather, dst, mask);
   return check_launch("udh_mosaic_blend_u8");
+}
+
+extern "C" size_t udh_mosaic_multiband_workspace_bytes(const int32_t* rois, int n, int dst_h, int dst_w, int bands) {
+  MultibandPlan p;
+  return mb_plan(rois, nullptr, n, dst_h, dst_w, bands, p) == UDH_OK ? p.total : 0;
+}
+
+extern "C" int udh_debug_multiband_layout(const int32_t* rois, int n, int dst_h, int dst_w, int bands, size_t off[MB_MAX_BANDS + 1],
+                                          int dims[3]) {
+  UDH_REQUIRE(off && dims, "udh_debug_multiband_layout: null pointer");
+  MultibandPlan p;
+  const int rc = mb_plan(rois, nullptr, n, dst_h, dst_w, bands, p);
+  if (rc != UDH_OK) return rc;
+  for (int i = 0; i <= MB_MAX_BANDS; ++i) off[i] = i <= p.B ? p.off_acc[i] : 0;
+  dims[0] = p.B;
+  dims[1] = p.Hp;
+  dims[2] = p.Wp;
+  return UDH_OK;
+}
+
+extern "C" int udh_mosaic_multiband_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const int32_t* rois, int n,
+                                       int c, int dst_h, int dst_w, int bands, uint8_t* dst, uint8_t* mask, void* ws, size_t ws_bytes,
+                                       void* stream) {
+  UDH_REQUIRE(frames && sizes && M && rois && dst && mask && ws, "udh_mosaic_multiband_u8: null pointer");
+  UDH_REQUIRE(c == 3, "udh_mosaic_multiband_u8: channels must be 3 (got %d)", c);
+  MultibandPlan p;
+  int rc = mb_plan(rois, sizes, n, dst_h, dst_w, bands, p);
+  if (rc != UDH_OK) return rc;
+  if (ws_bytes < p.total) {
+    set_error("udh_mosaic_multiband_u8: workspace of %zu bytes, %zu needed", ws_bytes, p.total);
+    return UDH_EWS;
+  }
+  for (int k = 0; k < n; ++k) {
+    UDH_REQUIRE(frames[k], "udh_mosaic_multiband_u8: frame %d is a null pointer", k);
+    p.fr[k].src = frames[k];
+  }
+  const cudaStream_t st = as_stream(stream);
+  char* base = static_cast<char*>(ws);
+  // pageable source: the copy is staged before this call returns, so `p` may go
+  const cudaError_t e = cudaMemcpyAsync(base, p.fr.data(), (size_t)n * sizeof(MultibandFrame), cudaMemcpyHostToDevice, st);
+  if (e != cudaSuccess) {
+    set_error("udh_mosaic_multiband_u8: frame table copy: %s", cudaGetErrorString(e));
+    return UDH_ECUDA;
+  }
+  const MultibandFrame* fr = reinterpret_cast<const MultibandFrame*>(base);
+  uchar4* G = reinterpret_cast<uchar4*>(base + p.off_g);
+  int16_t* Wt = reinterpret_cast<int16_t*>(base + p.off_w);
+  auto acc = [&](int i) { return reinterpret_cast<short4*>(base + p.off_acc[i]); };
+  auto R = [&](int i) { return reinterpret_cast<short4*>(base + p.off_r[i]); };
+  {
+    ProfScope ps(PROF_MB_BASE, st);
+    multiband_base_kernel<<<dim3(mb_blocks(p.max_px[0]), (unsigned)n), 256, 0, st>>>(fr, M, G, Wt);
+    if ((rc = check_launch("udh_mosaic_multiband_u8 (base)")) != UDH_OK) return rc;
+  }
+  {
+    ProfScope ps(PROF_MB_DOWN, st);
+    for (int i = 0; i < p.B; ++i) {
+      multiband_down_kernel<<<dim3(mb_blocks(p.max_px[i + 1]), (unsigned)n), 256, 0, st>>>(fr, G, Wt, i);
+      if ((rc = check_launch("udh_mosaic_multiband_u8 (pyrDown)")) != UDH_OK) return rc;
+    }
+  }
+  {
+    ProfScope ps(PROF_MB_ACC, st);
+    for (int i = 0; i <= p.B; ++i) {
+      const int cw = p.Wp >> i, ch = p.Hp >> i;
+      const dim3 grid((unsigned)((cw + MB_TILE_W - 1) / MB_TILE_W), (unsigned)((ch + MB_TILE_H - 1) / MB_TILE_H));
+      multiband_accumulate_kernel<<<grid, 256, 0, st>>>(fr, n, G, Wt, i, i == p.B, cw, ch, acc(i));
+      if ((rc = check_launch("udh_mosaic_multiband_u8 (accumulate)")) != UDH_OK) return rc;
+    }
+  }
+  ProfScope ps(PROF_MB_COLLAPSE, st);
+  for (int i = p.B; i >= 1; --i) {
+    const int cw = p.Wp >> i, ch = p.Hp >> i;
+    multiband_collapse_kernel<false><<<mb_blocks((int64_t)cw * ch), 256, 0, st>>>(acc(i), i < p.B ? R(i + 1) : nullptr, cw, ch, R(i),
+                                                                                 0, 0, nullptr, nullptr);
+    if ((rc = check_launch("udh_mosaic_multiband_u8 (collapse)")) != UDH_OK) return rc;
+  }
+  multiband_collapse_kernel<true><<<mb_blocks((int64_t)dst_h * dst_w), 256, 0, st>>>(acc(0), p.B ? R(1) : nullptr, p.Wp, p.Hp, nullptr,
+                                                                                     dst_h, dst_w, dst, mask);
+  return check_launch("udh_mosaic_multiband_u8");
 }

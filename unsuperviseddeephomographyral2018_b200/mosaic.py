@@ -1,7 +1,7 @@
 """Stitch an image sequence into one mosaic: chain the learned pairwise homographies to a reference frame, lay out a
-canvas, and blend every frame onto it on the GPU (udh_mosaic_blend_u8).
+canvas, and blend every frame onto it on the GPU (udh_mosaic_blend_u8, or udh_mosaic_multiband_u8 across frequency bands).
 
-    out = build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None)
+    out = build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None, blend="feather", bands=5)
     out["mosaic"], out["mask"], out["M"], out["kept"], out["H_pairs"], out["last_ms"]
 
 frames are CUDA uint8 RGB [h_k,w_k,3] tensors in sequence order (sizes may differ); est is an align.HomographyEstimator.
@@ -16,9 +16,14 @@ Canvas.  canvas() drops a frame (never the reference) when a corner of its sourc
 corners (0, 0), (w - 1, 0), (w - 1, h - 1), (0, h - 1): x0 = floor(min x), Wc = ceil(max x) - x0 + 1, likewise in y, and
 M_k = T G_k with T the translation by (-x0, -y0).
 
-Blend.  oracle/mosaic.py states the rule: per canvas pixel, the integer feathered average of every frame's
-cv2.warpPerspective(F_k, M_k, (Wc, Hc)) value where the frame is valid, with weights 1 + min(distance to the frame's edge in
-1/32 px, 32 feather).
+Blend, blend="feather" (the default).  oracle/mosaic.py states the rule: per canvas pixel, the integer feathered average of
+every frame's cv2.warpPerspective(F_k, M_k, (Wc, Hc)) value where the frame is valid, with weights 1 + min(distance to the
+frame's edge in 1/32 px, 32 feather).
+
+Blend, blend="multiband".  oracle/multiband.py states the rule: cv2.detail_MultiBandBlender(0, bands, CV_16S) (Burt-Adelson:
+low frequencies blended over a wide region, high ones over a narrow one), fed each frame's warp on its ROI
+(multiband_rois) with the feathered blend's validity as its mask.  It hides the steps a drifting chain or an exposure
+change leaves where a feathered average would ghost or band.
 """
 import numpy as np
 
@@ -84,6 +89,29 @@ def canvas(sizes, G, ref, max_pixels=None):
     return T @ G, (Hc, Wc), kept
 
 
+def multiband_rois(M, sizes, Hc, Wc):
+    """M [n,3,3] (frame k -> canvas), sizes [(h_k, w_k)] -> (rois int64 [n,4] (x_lo, y_lo, x_hi, y_hi), M' float64 [n,3,3]
+    frame k -> its ROI): the canvas rectangle the multi-band blend warps frame k onto.  Over the mapped pixel-centre corners,
+    x_lo = max(0, floor(min x) - 1), x_hi = min(Wc, ceil(max x) + 2) (exclusive), likewise in y; M'_k = T(-x_lo, -y_lo) M_k.
+    The margin holds every pixel whose warp is valid (its source position rounds to within 1/64 px of the frame).  An ROI
+    that misses the canvas is empty (x_hi <= x_lo or y_hi <= y_lo).  ValueError for a frame whose grown corners map with a
+    denominator <= 0 or whose corners do not map to finite points: canvas() drops such frames."""
+    M = np.asarray(M, np.float64).reshape(-1, 3, 3)
+    rois = np.zeros((len(M), 4), np.int64)
+    Mr = np.empty_like(M)
+    for k, (h, w) in enumerate(sizes):
+        with np.errstate(all="ignore"):
+            _, _, den = _map(M[k], grown_corners(h, w))
+            x, y, _ = _map(M[k], centre_corners(h, w))
+        if not ((den > 0).all() and np.isfinite(x).all() and np.isfinite(y).all()):
+            raise ValueError("frame %d: its corners do not map to finite points in front of the canvas's camera" % k)
+        x0, y0 = max(0, int(np.floor(x.min())) - 1), max(0, int(np.floor(y.min())) - 1)
+        x1, y1 = min(int(Wc), int(np.ceil(x.max())) + 2), min(int(Hc), int(np.ceil(y.max())) + 2)
+        rois[k] = (x0, y0, x1, y1)
+        Mr[k] = np.array([[1.0, 0.0, -x0], [0.0, 1.0, -y0], [0.0, 0.0, 1.0]]) @ M[k]
+    return rois, Mr
+
+
 def farthest_frame(sizes, G, kept, ref):
     """The kept frame whose mapped pixel-centre corner lies farthest from the reference frame's centre."""
     h, w = sizes[ref]
@@ -98,8 +126,9 @@ def farthest_frame(sizes, G, kept, ref):
     return far
 
 
-def build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None, float32_M=False):
-    """est: align.HomographyEstimator; frames: CUDA uint8 RGB [h_k,w_k,3] tensors in sequence order.  refine: None, or a
+def build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None, float32_M=False, blend="feather", bands=5):
+    """est: align.HomographyEstimator; frames: CUDA uint8 RGB [h_k,w_k,3] tensors in sequence order.  blend: "feather"
+    (udh_mosaic_blend_u8 with `feather`) or "multiband" (udh_mosaic_multiband_u8 with `bands`).  refine: None, or a
     dict of est.refine's keyword arguments (levels, iters, eps, max_side) to refine each pair's H.  max_pixels: the canvas
     limit (None: the JPEG encoder's, udh_jpeg_encode_capacity(Hc, Wc, 3) != 0).  float32_M: blend with each M_k rounded to
     float32, the values a text file of '%.9g' float32 entries gives back.
@@ -123,7 +152,9 @@ def build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None
         M = M.astype(np.float32).astype(np.float64)
     if max_pixels is None:
         check_encodable(Hc, Wc, sizes, G, kept, ref)
-    mosaic, mask, ms["blend"] = blend(frames, M, kept, Hc, Wc, feather)
+    if blend not in ("feather", "multiband"):
+        raise ValueError("blend must be 'feather' or 'multiband' (got %r)" % (blend,))
+    mosaic, mask, ms["blend"] = blend_kept(frames, M, kept, Hc, Wc, feather, blend, bands)
     return dict(mosaic=mosaic, mask=mask, M=M, kept=kept, ref=ref, H_pairs=H, refine=refined, last_ms=ms)
 
 
@@ -135,14 +166,18 @@ def check_encodable(Hc, Wc, sizes, G, kept, ref):
                          "frame (drop it or pick another --ref_frame)" % (Hc, Wc, farthest_frame(sizes, G, kept, ref)))
 
 
-def blend(frames, M, kept, Hc, Wc, feather):
-    """The kept frames through ops.mosaic_blend_u8 -> (mosaic, mask, CUDA-event ms)."""
+def blend_kept(frames, M, kept, Hc, Wc, feather, mode="feather", bands=5):
+    """The kept frames through ops.mosaic_blend_u8 (mode "feather") or ops.mosaic_multiband_u8 ("multiband") -> (mosaic,
+    mask, CUDA-event ms)."""
     import torch
     from . import ops
     take = [k for k in range(len(frames)) if kept[k]]
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
-    mosaic, mask = ops.mosaic_blend_u8([frames[k].contiguous() for k in take], np.asarray(M)[take], Hc, Wc, feather)
+    if mode == "multiband":
+        mosaic, mask = ops.mosaic_multiband_u8([frames[k].contiguous() for k in take], np.asarray(M)[take], Hc, Wc, bands)
+    else:
+        mosaic, mask = ops.mosaic_blend_u8([frames[k].contiguous() for k in take], np.asarray(M)[take], Hc, Wc, feather)
     e1.record()
     e1.synchronize()
     return mosaic, mask, e0.elapsed_time(e1)

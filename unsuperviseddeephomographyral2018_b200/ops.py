@@ -669,6 +669,57 @@ def mosaic_blend_u8(frames, M, dst_h, dst_w, feather):
     return out, mask
 
 
+def mosaic_multiband_u8(frames, M, dst_h, dst_w, bands, levels=False):
+    """frames: n CUDA uint8 RGB tensors [h_k,w_k,3] (sizes may differ), M float64 [n,3,3] (frame k -> canvas; numpy or
+    tensor) -> (mosaic uint8 [dst_h,dst_w,3], mask uint8 [dst_h,dst_w]): udh_mosaic_multiband_u8, byte for byte
+    cv2.detail_MultiBandBlender(0, bands, CV_16S) fed each frame's warp on its ROI (oracle/multiband.py).  The ROIs and the
+    frame -> ROI maps are formed on the host (mosaic.multiband_rois, which raises ValueError for a frame whose corners do not
+    map to finite points with a positive denominator); a frame whose ROI misses the canvas is left out.  levels=True also
+    returns the canvas pyramid as the feeds left it: [B' + 1] int16 CUDA tensors [Hp >> i, Wp >> i, 4] (acc, then wacc)."""
+    from . import mosaic
+    frames = list(frames.unbind(0)) if isinstance(frames, torch.Tensor) else list(frames)
+    Mh = (M.detach().cpu().numpy() if isinstance(M, torch.Tensor) else np.asarray(M)).astype(np.float64).reshape(-1, 3, 3)
+    n = len(frames)
+    if Mh.shape[0] != n:
+        raise _lib.UdhError("mosaic_multiband_u8: %d matrices for %d frames" % (Mh.shape[0], n))
+    if n == 0:
+        raise _lib.UdhError("mosaic_multiband_u8: no frames")
+    for k, f in enumerate(frames):
+        _req(f, torch.uint8, "frames[%d]" % k)
+        if f.dim() != 3 or f.shape[2] != 3:
+            raise _lib.UdhError("mosaic_multiband_u8: frames must be [h,w,3] (frame %d is %s)" % (k, tuple(f.shape)))
+    sizes = [(int(f.shape[0]), int(f.shape[1])) for f in frames]
+    rois, Mr = mosaic.multiband_rois(Mh, sizes, int(dst_h), int(dst_w))
+    take = [k for k in range(n) if rois[k, 2] > rois[k, 0] and rois[k, 3] > rois[k, 1]]
+    dev = frames[0].device
+    out = torch.zeros(int(dst_h), int(dst_w), 3, device=dev, dtype=torch.uint8)
+    mask = torch.zeros(int(dst_h), int(dst_w), device=dev, dtype=torch.uint8)
+    if not take:
+        return (out, mask, []) if levels else (out, mask)
+    m = len(take)
+    rr = np.ascontiguousarray(rois[take].astype(np.int32))
+    M_d = torch.from_numpy(np.ascontiguousarray(Mr[take].reshape(m, 9))).to(dev)
+    sz = np.ascontiguousarray(np.array([sizes[k] for k in take], np.int32).reshape(m, 2))
+    ptrs = (ctypes.c_void_p * m)(*[frames[k].data_ptr() for k in take])
+    nb = lib.udh_mosaic_multiband_workspace_bytes(rr.ctypes.data, m, int(dst_h), int(dst_w), int(bands))
+    if nb == 0:
+        raise _lib.UdhError("mosaic_multiband_u8: bad arguments (%d frames, canvas %dx%d, %d bands)" % (m, dst_h, dst_w, bands))
+    ws = torch.empty(nb, device=dev, dtype=torch.uint8)
+    check(lib.udh_mosaic_multiband_u8(ptrs, sz.ctypes.data, _ptr(M_d), rr.ctypes.data, m, 3, int(dst_h), int(dst_w), int(bands),
+                                      _ptr(out), _ptr(mask), _ptr(ws), nb, _stream()), "udh_mosaic_multiband_u8")
+    if not levels:
+        return out, mask
+    off, dims = (ctypes.c_size_t * 11)(), (ctypes.c_int * 3)()
+    check(lib.udh_debug_multiband_layout(rr.ctypes.data, m, int(dst_h), int(dst_w), int(bands), off, dims),
+          "udh_debug_multiband_layout")
+    B, Hp, Wp = dims
+    pyr = []
+    for i in range(B + 1):
+        cnt = (Hp >> i) * (Wp >> i) * 4
+        pyr.append(ws[off[i]:off[i] + 2 * cnt].view(torch.int16).reshape(Hp >> i, Wp >> i, 4))
+    return out, mask, pyr
+
+
 # ------------------------------------------------------------------ Adam
 def adam_step(p, g, m, v, alpha_t, beta1=0.9, beta2=0.999, eps=1e-8, grad_scale=1.0, zero_grad=True):
     for t, n in ((p, "p"), (g, "g"), (m, "m"), (v, "v")):
