@@ -509,6 +509,37 @@ int udh_mosaic_multiband_u8(const uint8_t* const* frames, const int32_t* sizes, 
  *   left it (the blend does not overwrite it); dims = {B', Hp, Wp}, the padded canvas. */
 int udh_debug_multiband_layout(const int32_t* rois, int n, int dst_h, int dst_w, int bands, size_t off[11], int dims[3]);
 
+/* ---- exposure compensation (cv2.detail_GainCompensator / ChannelsCompensator; oracle/exposure.py restates the rule) ----
+ * apply: v' = saturate_u8(rint(v g)) in float64, ties to even, per channel (cv2.multiply(uint8, double)).
+ * udh_mosaic_blend_gain_u8: udh_mosaic_blend_u8 with each frame's warp value compensated before it is weighted, v' with
+ *   g = gains[k][c] (gains [n][3] float64, device; channel 0's gain when c = 1).  Same arguments and limits otherwise.
+ * udh_mosaic_multiband_gain_u8: udh_mosaic_multiband_u8 fed each frame's compensated ROI warp (v' with gains[k][c] on every
+ *   pixel of the ROI warp, valid or not), as cv2's stitcher applies the compensator before the blender.
+ * udh_mosaic_exposure_stats_u8: the compensators' per-pair statistics of the frames' ROI warps (udh_mosaic_multiband_u8's
+ *   frames, M (frame -> ROI, device) and rois (host)), in one pass over the canvas.  For each listed pair p = (i, j), i <= j,
+ *   over the canvas pixels where both ROI warps are valid, stats[p] (uint64, device) holds UDH_EXPOSURE_STATS sums: [0] the
+ *   count; [1..3] frame i's channel sums; [4..6] frame j's; with norms, [7..9] and [10..12] frame i's and j's sums of
+ *   q = sqrt(double(r^2 + g^2 + b^2)) 2^52 (an integer below 2^61) as three 21-bit limbs, sum q = [7] + [8] 2^21 + [9] 2^42:
+ *   exact, rounded to double by the caller (without norms those six are 0).  Before the sums, frame k's values are
+ *   compensated by history[0][k][c], then history[1][k][c], ... up to history[feeds - 1] ([feeds][n][3] float64, device):
+ *   the images cv2's feed number `feeds` sees.  pair_ptr [n + 1] and pair_j [npairs] int32 (device): the CSR list of pairs
+ *   (row i, ascending j >= i); list every pair whose ROIs intersect, the diagonal included.  Integer sums: the result does
+ *   not depend on the frames' order or the run.  n <= UDH_EXPOSURE_MAX_FRAMES, feeds <= UDH_EXPOSURE_MAX_FEEDS, canvas
+ *   sides < 32767 (so a pair's count stays below 2^31).  ws: udh_mosaic_exposure_workspace_bytes(n) bytes of device memory. */
+#define UDH_EXPOSURE_MAX_FRAMES 1024
+#define UDH_EXPOSURE_MAX_FEEDS 16
+#define UDH_EXPOSURE_STATS 13
+int udh_mosaic_blend_gain_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains, int n, int c,
+                             const int32_t* tile_ptr, const int32_t* tile_frames, int dst_h, int dst_w, int feather, uint8_t* dst,
+                             uint8_t* mask, void* ws, size_t ws_bytes, void* stream);
+int udh_mosaic_multiband_gain_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains,
+                                 const int32_t* rois, int n, int c, int dst_h, int dst_w, int bands, uint8_t* dst, uint8_t* mask,
+                                 void* ws, size_t ws_bytes, void* stream);
+size_t udh_mosaic_exposure_workspace_bytes(int n);
+int udh_mosaic_exposure_stats_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const int32_t* rois, int n,
+                                 const int32_t* pair_ptr, const int32_t* pair_j, int npairs, const double* history, int feeds,
+                                 int norms, int dst_h, int dst_w, uint64_t* stats, void* ws, size_t ws_bytes, void* stream);
+
 /* ---- instrumentation read by bench.py -------------------------------------------------------------------------
  * udh_launch_count: kernels this library has launched in this process (monotonic).
  * udh_prof_*: when enabled, every tagged phase is bracketed by CUDA events recorded on the launching stream;

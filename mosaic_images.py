@@ -11,17 +11,23 @@ sorted(glob(dir/--glob)) (default *.JPG, gen_real_data.py's rule).  The model, r
 align_images.py's.  --ref_frame picks the reference frame (-1: the middle one, N // 2); --feather is the blend's ramp in
 source pixels (0: a plain average of the overlapping frames).  --blend multiband blends across --bands frequency bands
 instead (cv2.detail_MultiBandBlender's rule, byte for byte): low frequencies over a wide region, high ones over a narrow
-one, which hides the seams a drifting chain or an exposure change leaves.
+one, which hides the seams a drifting chain leaves.  --compensate gain|channels compensates each frame's exposure before
+the blend (cv2.detail_GainCompensator / ChannelsCompensator's rule with --compensate_feeds feeds): one gain per frame, or
+one per channel, which also evens out white balance.  An exposure step between frames is otherwise left in the mosaic.
+cv2's rule pulls every gain towards 1, so one feed removes only part of a step; each further feed removes part of what
+is left (on a sweep with exposures 0.75 / 1 / 1.3, four gain-mode feeds recover the gain ratios to within 1 %).
 
 Writes in --out_dir:
   pairs.txt    `frame_k frame_k+1` and H's nine entries per consecutive pair, as align_images.py's homographies.txt;
   refine.txt   with refinement, `frame_k frame_k+1 rho status levels` per pair, as align_images.py writes it;
-  mosaic.txt   `canvas Hc Wc ref r` (` blend multiband B` appended with --blend multiband), then `name kept|dropped` and the nine entries of M_k (frame k -> canvas) per frame,
-               '%.9g' of their float32 values; the blend uses those float32 values, so the file reproduces mosaic.jpg;
+  mosaic.txt   `canvas Hc Wc ref r` (` blend multiband B` appended with --blend multiband, then ` compensate MODE F` with
+               --compensate), then `name kept|dropped` and the nine entries of M_k (frame k -> canvas) per frame,
+               '%.9g' of their float32 values; the blend uses those float32 values.  With --compensate each frame line
+               ends in its three gains, '%.17g' (exact); so the file reproduces mosaic.jpg;
   mosaic.jpg   the mosaic (BGR, JPEG quality 95, byte-identical to cv2.imencode of the same pixels).
 A frame whose grown corners map behind the reference camera is dropped.  The canvas must be one the JPEG encoder takes
 (about 110 MP in colour); a larger one stops with an error naming the frame that reaches farthest.  Prints the GPU time
-of each phase (CUDA events: prep, forward, refine, blend, encode; the blend named when it is multi-band).
+of each phase (CUDA events: prep, forward, refine, compensate, blend, encode; the blend named when it is multi-band).
 """
 from __future__ import absolute_import, division, print_function
 
@@ -46,6 +52,11 @@ def build_parser():
     p.add_argument('--blend', type=str, default='feather', choices=['feather', 'multiband'],
                    help='feather: feathered average; multiband: blend across frequency bands')
     p.add_argument('--bands', type=int, default=5, help='frequency bands of --blend multiband, 0..10')
+    p.add_argument('--compensate', type=str, default='none', choices=['none', 'gain', 'channels'],
+                   help='exposure compensation before the blend: none, one gain per frame, or one per channel')
+    p.add_argument('--compensate_feeds', type=int, default=1,
+                   help='feeds of the exposure compensator, 1..16; one feed removes only part of an exposure step (the '
+                        'rule pulls every gain towards 1), several (e.g. 4) remove nearly all of it')
     p.add_argument('--out_dir', type=str, default='mosaic')
     return p
 
@@ -74,15 +85,19 @@ def run(args, est, decode, encode):
         raise SystemExit("--feather must be in 0..1024 (got %d)" % args.feather)
     if not 0 <= args.bands <= 10:
         raise SystemExit("--bands must be in 0..10 (got %d)" % args.bands)
+    if not 1 <= args.compensate_feeds <= 16:
+        raise SystemExit("--compensate_feeds must be in 1..16 (got %d)" % args.compensate_feeds)
     names, paths = frame_list(args)
     os.makedirs(args.out_dir, exist_ok=True)
     refining = args.refine_levels != 0
     refine = dict(levels=None if args.refine_levels < 0 else args.refine_levels, iters=args.refine_iters, eps=args.refine_eps,
                   max_side=args.refine_max_side) if refining else None
+    compensating = args.compensate != "none"
+    comp = dict(compensate=args.compensate, compensate_feeds=args.compensate_feeds) if compensating else {}
     imgs = decode(paths)
     try:
         out = mosaic.build_mosaic(est, imgs, None if args.ref_frame < 0 else args.ref_frame, refine, args.feather,
-                                  float32_M=True, blend=args.blend, bands=args.bands)
+                                  float32_M=True, blend=args.blend, bands=args.bands, **comp)
     except ValueError as e:
         raise SystemExit(str(e))
     H = out["H_pairs"]
@@ -93,10 +108,12 @@ def run(args, est, decode, encode):
         with open(os.path.join(args.out_dir, "refine.txt"), "w") as f:
             f.write("".join("%s %s %.9g %d %d\n" % (names[k], names[k + 1], rho[k], status[k], level[k]) for k in range(len(H))))
     Hc, Wc = out["mask"].shape
-    lines = ["canvas %d %d ref %d" % (Hc, Wc, out["ref"]) + (" blend multiband %d" % args.bands if args.blend == "multiband" else "")]
+    lines = ["canvas %d %d ref %d" % (Hc, Wc, out["ref"]) + (" blend multiband %d" % args.bands if args.blend == "multiband" else "") +
+             (" compensate %s %d" % (args.compensate, args.compensate_feeds) if compensating else "")]
     for k, nm in enumerate(names):
         lines.append(" ".join([nm, "kept" if out["kept"][k] else "dropped"] +
-                              ["%.9g" % v for v in align.homography_as_written(out["M"][k])[0]]))
+                              ["%.9g" % v for v in align.homography_as_written(out["M"][k])[0]] +
+                              (["%.17g" % g for g in out["gains"][k]] if compensating else [])))
         if not out["kept"][k]:
             print("===> dropped %s: it maps behind the reference frame's camera" % nm)
     with open(os.path.join(args.out_dir, "mosaic.txt"), "w") as f:
@@ -111,10 +128,11 @@ def run(args, est, decode, encode):
     with open(os.path.join(args.out_dir, "mosaic.jpg"), "wb") as f:
         f.write(blob)
     cover = float((out["mask"] != 0).float().mean())
-    print("===> %d frames (%d kept) on a %dx%d canvas (ref %s, %.1f %% covered): GPU %.3f ms (prep %.3f, forward %.3f, %s"
+    print("===> %d frames (%d kept) on a %dx%d canvas (ref %s, %.1f %% covered): GPU %.3f ms (prep %.3f, forward %.3f, %s%s"
           "%sblend %.3f, encode %.3f)" % (len(names), int(np.sum(out["kept"])), Hc, Wc, names[out["ref"]], 100 * cover,
                                           sum(ms.values()), ms["prep"], ms["forward"],
                                           "refine %.3f, " % ms["refine"] if refining else "",
+                                          "compensate %.3f, " % ms["compensate"] if compensating else "",
                                           "multiband %d " % args.bands if args.blend == "multiband" else "", ms["blend"],
                                           ms["encode"]), flush=True)
     return out

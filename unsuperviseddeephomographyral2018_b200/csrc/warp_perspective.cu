@@ -128,16 +128,20 @@ __global__ void mosaic_invert_kernel(const double* __restrict__ M, MosaicFrame* 
   if (k < n) cv_invert3(M + (int64_t)k * 9, fr[k].mi);
 }
 
+// Exposure compensation's apply, cv2.multiply(uint8, double): saturate_u8(rint(v g)) in float64, ties to even.
+__device__ __forceinline__ int ex_apply(int v, double g) {
+  return min(max(__double2int_rn(__dmul_rn((double)v, g)), 0), 255);
+}
+
 // Gather form: one CTA per UDH_MOSAIC_TILE_H x UDH_MOSAIC_TILE_W canvas tile, each thread four consecutive pixels of one
 // row.  The thread walks the tile's candidate frames, adds wt * v and wt of every frame valid at its pixels into 64-bit
 // registers and stores the pixels once: no atomics, no accumulation buffer.  Integer sums: the result does not depend on
-// the frames' order.
-template <int C>
-__global__ void __launch_bounds__(256) mosaic_blend_u8_kernel(const MosaicFrame* __restrict__ fr, int n,
-                                                              const int32_t* __restrict__ tile_ptr,
-                                                              const int32_t* __restrict__ tile_frames, int dh, int dw, int bw,
-                                                              int feather32, uint8_t* __restrict__ dst,
-                                                              uint8_t* __restrict__ mask) {
+// the frames' order.  GAIN: each frame's value is first compensated, ex_apply(v, gains[f][c]) (channel 0's gain when C = 1).
+template <int C, bool GAIN>
+__device__ __forceinline__ void mosaic_blend_tile(const MosaicFrame* __restrict__ fr, int n, const int32_t* __restrict__ tile_ptr,
+                                                  const int32_t* __restrict__ tile_frames, int dh, int dw, int bw, int feather32,
+                                                  const double* __restrict__ gains, uint8_t* __restrict__ dst,
+                                                  uint8_t* __restrict__ mask) {
   const int y = blockIdx.y * UDH_MOSAIC_TILE_H + threadIdx.x / (UDH_MOSAIC_TILE_W / 4);
   const int x0 = blockIdx.x * UDH_MOSAIC_TILE_W + threadIdx.x % (UDH_MOSAIC_TILE_W / 4) * 4;
   if (y >= dh || x0 >= dw) return;
@@ -170,6 +174,10 @@ __global__ void __launch_bounds__(256) mosaic_blend_u8_kernel(const MosaicFrame*
         const int wt = 1 + min(min(min(X, xm - X), min(Y, ym - Y)), feather32);
         int v[C];
         wp_sample<C>(s, h, w, X, Y, v);
+        if (GAIN) {
+#pragma unroll
+          for (int c = 0; c < C; ++c) v[c] = ex_apply(v[c], __ldg(gains + 3 * f + c));
+        }
 #pragma unroll
         for (int c = 0; c < C; ++c) S[k][c] += (uint64_t)(wt * v[c]);
         D[k] += (uint64_t)wt;
@@ -202,6 +210,25 @@ __global__ void __launch_bounds__(256) mosaic_blend_u8_kernel(const MosaicFrame*
     for (int k = 0; k < 4; ++k)
       if (k < np) m[k] = mk[k];
   }
+}
+
+template <int C>
+__global__ void __launch_bounds__(256) mosaic_blend_u8_kernel(const MosaicFrame* __restrict__ fr, int n,
+                                                              const int32_t* __restrict__ tile_ptr,
+                                                              const int32_t* __restrict__ tile_frames, int dh, int dw, int bw,
+                                                              int feather32, uint8_t* __restrict__ dst,
+                                                              uint8_t* __restrict__ mask) {
+  mosaic_blend_tile<C, false>(fr, n, tile_ptr, tile_frames, dh, dw, bw, feather32, nullptr, dst, mask);
+}
+
+// The feathered blend of exposure-compensated frames: gains [n][3] float64.
+template <int C>
+__global__ void __launch_bounds__(256) exposure_blend_u8_kernel(const MosaicFrame* __restrict__ fr, int n,
+                                                                const int32_t* __restrict__ tile_ptr,
+                                                                const int32_t* __restrict__ tile_frames, int dh, int dw, int bw,
+                                                                int feather32, const double* __restrict__ gains,
+                                                                uint8_t* __restrict__ dst, uint8_t* __restrict__ mask) {
+  mosaic_blend_tile<C, true>(fr, n, tile_ptr, tile_frames, dh, dw, bw, feather32, gains, dst, mask);
 }
 
 // ---- multi-band blend: cv2.detail_MultiBandBlender with CV_16S weights (the rule: oracle/multiband.py) ----------------
@@ -242,9 +269,21 @@ __device__ __forceinline__ void mb_up_taps(int o, int n, int* t, int* wt) {
 
 __device__ __forceinline__ int mb_sat16(int v) { return min(max(v, -32768), 32767); }
 
+// Frame (s, h, w)'s ROI warp at ROI pixel (sx, sy) (tile width bw): its value, and whether the pixel is valid.
+__device__ __forceinline__ bool mb_roi_warp(const uint8_t* __restrict__ s, int h, int w, const double* mi, int sx, int sy, int bw,
+                                            int* v) {
+  int X, Y;
+  const double Wd = wp_coords(mi, sx, sy, bw, X, Y);
+  wp_sample<3>(s, h, w, X, Y, v);
+  return Wd != 0.0 && X >= 0 && X <= 32 * (w - 1) && Y >= 0 && Y <= 32 * (h - 1);
+}
+
 // Level 0 of every frame: the ROI warp bordered with BORDER_REFLECT, and the 0 / 256 weight with a constant 0 border.
+// gains (null: none) [n][3]: the ROI warp is exposure-compensated first, ex_apply(v, gains[k][c]), as cv2's stitcher
+// applies its compensator to the whole warped image before it feeds the blender.
 __global__ void __launch_bounds__(256) multiband_base_kernel(const MultibandFrame* __restrict__ fr, const double* __restrict__ M,
-                                                             uchar4* __restrict__ G, int16_t* __restrict__ Wt) {
+                                                             const double* __restrict__ gains, uchar4* __restrict__ G,
+                                                             int16_t* __restrict__ Wt) {
   __shared__ double mi[9];
   const int k = blockIdx.y;
   if (threadIdx.x == 0) cv_invert3(M + (int64_t)k * 9, mi);
@@ -255,15 +294,21 @@ __global__ void __launch_bounds__(256) multiband_base_kernel(const MultibandFram
   const int bw = __ldg(&F->bw), ox = __ldg(&F->x0) - rx, oy = __ldg(&F->y0) - ry, pw = __ldg(&F->pw);
   const int npx = pw * __ldg(&F->ph);                                 // < 2^31: padded sides < 32767 + 1024
   const int64_t off = __ldg(&F->off[0]);
-  const int xm = 32 * (w - 1), ym = 32 * (h - 1);
+  double g[3];
+  if (gains) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) g[c] = __ldg(gains + 3 * k + c);
+  }
   for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < npx; e += gridDim.x * blockDim.x) {
     const int y = e / pw, x = e - y * pw;
     const int ix = x + ox, iy = y + oy;
     const int sx = mb_reflect(ix, rw), sy = mb_reflect(iy, rh);
-    int X, Y, v[3];
-    const double Wd = wp_coords(mi, sx, sy, bw, X, Y);
-    wp_sample<3>(s, h, w, X, Y, v);
-    const bool valid = ix == sx && iy == sy && Wd != 0.0 && X >= 0 && X <= xm && Y >= 0 && Y <= ym;
+    int v[3];
+    const bool valid = mb_roi_warp(s, h, w, mi, sx, sy, bw, v) && ix == sx && iy == sy;
+    if (gains) {
+#pragma unroll
+      for (int c = 0; c < 3; ++c) v[c] = ex_apply(v[c], g[c]);
+    }
     G[off + e] = make_uchar4((unsigned char)v[0], (unsigned char)v[1], (unsigned char)v[2], 0);
     Wt[off + e] = valid ? 256 : 0;
   }
@@ -495,6 +540,152 @@ static unsigned mb_blocks(int64_t px) {
   return (unsigned)(b < 1 ? 1 : b > 4096 ? 4096 : b);
 }
 
+// ---- exposure compensation: per-pair statistics of the ROI warps (cv2.detail's gain compensators; oracle/exposure.py) ----
+// For every listed pair i <= j of frames whose ROIs intersect, over the canvas pixels where both ROI warps are valid:
+// the count, each frame's channel sums and, with norms, each frame's sum of sqrt(r^2 + g^2 + b^2) (cv2's norm(Vec3b)).
+// Such a norm is 0 or a multiple of 2^-52 below 2^9, so q = norm 2^52 is an integer below 2^61; it is summed exactly as
+// three 21-bit limbs (each limb's sum stays below 2^52 for up to 2^31 pixels), and the host rounds the total once.
+struct ExposureFrame {
+  double mi[9];                    // cv_invert3 of M'_k (frame -> its ROI)
+  const uint8_t* src;
+  int h, w;
+  int rx, ry, rw, rh, bw;          // the ROI on the canvas and the ROI warp's tile width
+};
+
+constexpr int EX_TILE_W = 32, EX_TILE_H = 64, EX_CHUNK = 8, EX_PAIRS = EX_CHUNK * EX_CHUNK;
+
+__global__ void exposure_invert_kernel(const double* __restrict__ M, ExposureFrame* fr, int n) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < n) cv_invert3(M + (int64_t)k * 9, fr[k].mi);
+}
+
+// Gather form: one CTA per EX_TILE_W x EX_TILE_H canvas tile, each warp one row of 32 pixels at a time.  The CTA lists
+// the frames whose ROI meets its tile in ascending frame order and takes them EX_CHUNK at a time, two chunks A <= B per
+// round.  Per row each lane stores the compensated ROI-warp value and validity of every frame of A and B at its pixel in
+// shared memory; then, for every listed pair of the round (looked up in the pair CSR), the warp sums its lanes' terms
+// with __reduce_add_sync and adds them to the CTA's 64-bit sums, which are added to the pair's global sums once per
+// round.  The ascending list puts the pair's lower frame i first in every slot (chunk A <= B, and a <= b within one
+// chunk), so frame i's sums always go to i's fields.  Every sum is an integer, so the result does not depend on the
+// frames' order, the tiling or the run.
+// hist [feeds][n][3]: frame k's value is ex_apply'd with hist[0][k][c], then hist[1][k][c], ... (feed `feeds` of cv2's loop).
+__global__ void __launch_bounds__(256) exposure_stats_kernel(const ExposureFrame* __restrict__ fr, int n,
+                                                             const int32_t* __restrict__ pair_ptr,
+                                                             const int32_t* __restrict__ pair_j, const double* __restrict__ hist,
+                                                             int feeds, int norms, unsigned long long* __restrict__ stats) {
+  __shared__ int cand[UDH_EXPOSURE_MAX_FRAMES];
+  __shared__ int wcount[8];
+  __shared__ uchar4 val[2 * EX_CHUNK][256];                             // .w: valid
+  __shared__ int pidx[EX_PAIRS];
+  __shared__ unsigned long long acc[EX_PAIRS][UDH_EXPOSURE_STATS];
+  const int tx0 = blockIdx.x * EX_TILE_W, ty0 = blockIdx.y * EX_TILE_H;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  // the candidates in ascending frame order: per 256 frames, each warp's ballot, ranked by the warps before it
+  int nc = 0;
+  for (int c0 = 0; c0 < n; c0 += blockDim.x) {
+    const int k = c0 + threadIdx.x;
+    bool hit = false;
+    if (k < n) {
+      const ExposureFrame* F = fr + k;
+      const int rx = __ldg(&F->rx), ry = __ldg(&F->ry);
+      hit = rx < tx0 + EX_TILE_W && rx + __ldg(&F->rw) > tx0 && ry < ty0 + EX_TILE_H && ry + __ldg(&F->rh) > ty0;
+    }
+    const unsigned bal = __ballot_sync(0xffffffffu, hit);
+    if (lane == 0) wcount[warp] = __popc(bal);
+    __syncthreads();
+    int base = nc, tot = 0;
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      base += q < warp ? wcount[q] : 0;
+      tot += wcount[q];
+    }
+    if (hit) cand[base + __popc(bal & ((1u << lane) - 1u))] = k;
+    nc += tot;
+    __syncthreads();                                                  // wcount is rewritten next round
+  }
+  const int nch = (nc + EX_CHUNK - 1) / EX_CHUNK;
+  for (int A = 0; A < nch; ++A) {
+    for (int B = A; B < nch; ++B) {
+      // the round's pairs: slot t = a EX_CHUNK + b pairs frame a of chunk A with frame b of chunk B (a <= b when A = B)
+      if (threadIdx.x < EX_PAIRS) {
+        const int a = threadIdx.x / EX_CHUNK, b = threadIdx.x % EX_CHUNK, ka = A * EX_CHUNK + a, kb = B * EX_CHUNK + b;
+        int p = -1;
+        if (ka < nc && kb < nc && (A != B || a <= b)) {
+          const int i = cand[ka], j = cand[kb];                       // i <= j: the list ascends
+          int lo = __ldg(pair_ptr + i), hi = __ldg(pair_ptr + i + 1);
+          while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (__ldg(pair_j + mid) < j) lo = mid + 1; else hi = mid;
+          }
+          if (lo < __ldg(pair_ptr + i + 1) && __ldg(pair_j + lo) == j) p = lo;
+        }
+        pidx[threadIdx.x] = p;
+      }
+      for (int e = threadIdx.x; e < EX_PAIRS * UDH_EXPOSURE_STATS; e += blockDim.x) (&acc[0][0])[e] = 0;
+      __syncthreads();
+      const int nA = min(EX_CHUNK, nc - A * EX_CHUNK), nB = A == B ? 0 : min(EX_CHUNK, nc - B * EX_CHUNK);
+      for (int r = warp; r < EX_TILE_H; r += 8) {
+        const int x = tx0 + lane, y = ty0 + r;
+        for (int q = 0; q < nA + nB; ++q) {
+          const int k = cand[q < nA ? A * EX_CHUNK + q : B * EX_CHUNK + q - nA];
+          const ExposureFrame* F = fr + k;
+          const int sx = x - __ldg(&F->rx), sy = y - __ldg(&F->ry);
+          int v[3] = {0, 0, 0};
+          bool ok = false;
+          if ((unsigned)sx < (unsigned)__ldg(&F->rw) && (unsigned)sy < (unsigned)__ldg(&F->rh)) {
+            double mi[9];
+#pragma unroll
+            for (int t = 0; t < 9; ++t) mi[t] = __ldg(F->mi + t);
+            const uint8_t* s = reinterpret_cast<const uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&F->src)));
+            ok = mb_roi_warp(s, __ldg(&F->h), __ldg(&F->w), mi, sx, sy, __ldg(&F->bw), v);
+            for (int f = 0; f < feeds; ++f) {
+#pragma unroll
+              for (int c = 0; c < 3; ++c) v[c] = ex_apply(v[c], __ldg(hist + ((int64_t)f * n + k) * 3 + c));
+            }
+          }
+          val[q < nA ? q : EX_CHUNK + q - nA][threadIdx.x] = make_uchar4(v[0], v[1], v[2], ok);
+        }
+        __syncwarp();
+        for (int t = 0; t < EX_PAIRS; ++t) {
+          const int p = pidx[t];
+          if (p < 0) continue;
+          const int a = t / EX_CHUNK, b = t % EX_CHUNK;
+          const uchar4 u = val[a][threadIdx.x], w = val[A == B ? b : EX_CHUNK + b][threadIdx.x];
+          const bool both = u.w && w.w;
+          if (!__any_sync(0xffffffffu, both)) continue;
+          const unsigned m = both ? 1u : 0u;
+          unsigned sum[UDH_EXPOSURE_STATS] = {};
+          sum[0] = m;
+          sum[1] = m * u.x; sum[2] = m * u.y; sum[3] = m * u.z;
+          sum[4] = m * w.x; sum[5] = m * w.y; sum[6] = m * w.z;
+          if (norms) {
+            const uint64_t qu = __double2ull_rn(__dmul_rn(__dsqrt_rn((double)(u.x * u.x + u.y * u.y + u.z * u.z)), 0x1p52)) * m;
+            const uint64_t qw = __double2ull_rn(__dmul_rn(__dsqrt_rn((double)(w.x * w.x + w.y * w.y + w.z * w.z)), 0x1p52)) * m;
+#pragma unroll
+            for (int l = 0; l < 3; ++l) {
+              sum[7 + l] = (unsigned)(qu >> (21 * l)) & 0x1fffffu;
+              sum[10 + l] = (unsigned)(qw >> (21 * l)) & 0x1fffffu;
+            }
+          }
+#pragma unroll
+          for (int q = 0; q < UDH_EXPOSURE_STATS; ++q) {
+            if (q >= 7 && !norms) break;
+            const unsigned tot = __reduce_add_sync(0xffffffffu, sum[q]);   // < 2^26: 32 lanes of < 2^21
+            if (lane == 0 && tot) atomicAdd(&acc[t][q], (unsigned long long)tot);
+          }
+        }
+        __syncwarp();
+      }
+      __syncthreads();
+      for (int e = threadIdx.x; e < EX_PAIRS * UDH_EXPOSURE_STATS; e += blockDim.x) {
+        const int t = e / UDH_EXPOSURE_STATS, q = e % UDH_EXPOSURE_STATS, p = pidx[t];
+        const unsigned long long v = acc[t][q];
+        if (p >= 0 && v) atomicAdd(stats + (int64_t)p * UDH_EXPOSURE_STATS + q, v);
+      }
+      __syncthreads();
+    }
+  }
+}
+
 }  // namespace udh
 
 using namespace udh;
@@ -521,9 +712,9 @@ extern "C" int udh_warp_perspective_u8(const uint8_t* src, const double* M, uint
 
 extern "C" size_t udh_mosaic_workspace_bytes(int n) { return n > 0 ? (size_t)n * sizeof(MosaicFrame) : 0; }
 
-extern "C" int udh_mosaic_blend_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, int n, int c,
-                                   const int32_t* tile_ptr, const int32_t* tile_frames, int dst_h, int dst_w, int feather,
-                                   uint8_t* dst, uint8_t* mask, void* ws, size_t ws_bytes, void* stream) {
+static int mosaic_blend(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains, int n, int c,
+                        const int32_t* tile_ptr, const int32_t* tile_frames, int dst_h, int dst_w, int feather, uint8_t* dst,
+                        uint8_t* mask, void* ws, size_t ws_bytes, void* stream) {
   UDH_REQUIRE(tile_ptr && tile_frames && dst && mask && (n == 0 || (frames && sizes && M && ws)), "udh_mosaic_blend_u8: null pointer");
   UDH_REQUIRE(c == 1 || c == 3, "udh_mosaic_blend_u8: channels must be 1 or 3 (got %d)", c);
   UDH_REQUIRE(n >= 0 && n <= 65535 && dst_h >= 1 && dst_w >= 1 && dst_h < 32767 && dst_w < 32767,
@@ -559,11 +750,28 @@ extern "C" int udh_mosaic_blend_u8(const uint8_t* const* frames, const int32_t* 
   const dim3 grid((unsigned)((dst_w + UDH_MOSAIC_TILE_W - 1) / UDH_MOSAIC_TILE_W),
                   (unsigned)((dst_h + UDH_MOSAIC_TILE_H - 1) / UDH_MOSAIC_TILE_H));
   const MosaicFrame* fr = static_cast<const MosaicFrame*>(ws);
-  if (c == 3)
+  if (gains && c == 3)
+    exposure_blend_u8_kernel<3><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, 32 * feather, gains, dst, mask);
+  else if (gains)
+    exposure_blend_u8_kernel<1><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, 32 * feather, gains, dst, mask);
+  else if (c == 3)
     mosaic_blend_u8_kernel<3><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, 32 * feather, dst, mask);
   else
     mosaic_blend_u8_kernel<1><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, 32 * feather, dst, mask);
   return check_launch("udh_mosaic_blend_u8");
+}
+
+extern "C" int udh_mosaic_blend_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, int n, int c,
+                                   const int32_t* tile_ptr, const int32_t* tile_frames, int dst_h, int dst_w, int feather,
+                                   uint8_t* dst, uint8_t* mask, void* ws, size_t ws_bytes, void* stream) {
+  return mosaic_blend(frames, sizes, M, nullptr, n, c, tile_ptr, tile_frames, dst_h, dst_w, feather, dst, mask, ws, ws_bytes, stream);
+}
+
+extern "C" int udh_mosaic_blend_gain_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains, int n,
+                                        int c, const int32_t* tile_ptr, const int32_t* tile_frames, int dst_h, int dst_w, int feather,
+                                        uint8_t* dst, uint8_t* mask, void* ws, size_t ws_bytes, void* stream) {
+  UDH_REQUIRE(gains || n == 0, "udh_mosaic_blend_gain_u8: null gains");
+  return mosaic_blend(frames, sizes, M, gains, n, c, tile_ptr, tile_frames, dst_h, dst_w, feather, dst, mask, ws, ws_bytes, stream);
 }
 
 extern "C" size_t udh_mosaic_multiband_workspace_bytes(const int32_t* rois, int n, int dst_h, int dst_w, int bands) {
@@ -584,9 +792,9 @@ extern "C" int udh_debug_multiband_layout(const int32_t* rois, int n, int dst_h,
   return UDH_OK;
 }
 
-extern "C" int udh_mosaic_multiband_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const int32_t* rois, int n,
-                                       int c, int dst_h, int dst_w, int bands, uint8_t* dst, uint8_t* mask, void* ws, size_t ws_bytes,
-                                       void* stream) {
+static int mosaic_multiband(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains,
+                            const int32_t* rois, int n, int c, int dst_h, int dst_w, int bands, uint8_t* dst, uint8_t* mask, void* ws,
+                            size_t ws_bytes, void* stream) {
   UDH_REQUIRE(frames && sizes && M && rois && dst && mask && ws, "udh_mosaic_multiband_u8: null pointer");
   UDH_REQUIRE(c == 3, "udh_mosaic_multiband_u8: channels must be 3 (got %d)", c);
   MultibandPlan p;
@@ -615,7 +823,7 @@ extern "C" int udh_mosaic_multiband_u8(const uint8_t* const* frames, const int32
   auto R = [&](int i) { return reinterpret_cast<short4*>(base + p.off_r[i]); };
   {
     ProfScope ps(PROF_MB_BASE, st);
-    multiband_base_kernel<<<dim3(mb_blocks(p.max_px[0]), (unsigned)n), 256, 0, st>>>(fr, M, G, Wt);
+    multiband_base_kernel<<<dim3(mb_blocks(p.max_px[0]), (unsigned)n), 256, 0, st>>>(fr, M, gains, G, Wt);
     if ((rc = check_launch("udh_mosaic_multiband_u8 (base)")) != UDH_OK) return rc;
   }
   {
@@ -644,4 +852,68 @@ extern "C" int udh_mosaic_multiband_u8(const uint8_t* const* frames, const int32
   multiband_collapse_kernel<true><<<mb_blocks((int64_t)dst_h * dst_w), 256, 0, st>>>(acc(0), p.B ? R(1) : nullptr, p.Wp, p.Hp, nullptr,
                                                                                      dst_h, dst_w, dst, mask);
   return check_launch("udh_mosaic_multiband_u8");
+}
+
+extern "C" int udh_mosaic_multiband_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const int32_t* rois, int n,
+                                       int c, int dst_h, int dst_w, int bands, uint8_t* dst, uint8_t* mask, void* ws, size_t ws_bytes,
+                                       void* stream) {
+  return mosaic_multiband(frames, sizes, M, nullptr, rois, n, c, dst_h, dst_w, bands, dst, mask, ws, ws_bytes, stream);
+}
+
+extern "C" int udh_mosaic_multiband_gain_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains,
+                                            const int32_t* rois, int n, int c, int dst_h, int dst_w, int bands, uint8_t* dst,
+                                            uint8_t* mask, void* ws, size_t ws_bytes, void* stream) {
+  UDH_REQUIRE(gains, "udh_mosaic_multiband_gain_u8: null gains");
+  return mosaic_multiband(frames, sizes, M, gains, rois, n, c, dst_h, dst_w, bands, dst, mask, ws, ws_bytes, stream);
+}
+
+extern "C" size_t udh_mosaic_exposure_workspace_bytes(int n) { return n > 0 ? (size_t)n * sizeof(ExposureFrame) : 0; }
+
+extern "C" int udh_mosaic_exposure_stats_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const int32_t* rois,
+                                            int n, const int32_t* pair_ptr, const int32_t* pair_j, int npairs, const double* history,
+                                            int feeds, int norms, int dst_h, int dst_w, uint64_t* stats, void* ws, size_t ws_bytes,
+                                            void* stream) {
+  UDH_REQUIRE(frames && sizes && M && rois && pair_ptr && pair_j && stats && ws && (feeds == 0 || history),
+              "udh_mosaic_exposure_stats_u8: null pointer");
+  UDH_REQUIRE(n >= 1 && n <= UDH_EXPOSURE_MAX_FRAMES && dst_h >= 1 && dst_w >= 1 && dst_h < 32767 && dst_w < 32767,
+              "udh_mosaic_exposure_stats_u8: bad dimensions (n %d of at most %d, canvas %dx%d)", n, UDH_EXPOSURE_MAX_FRAMES, dst_h,
+              dst_w);
+  UDH_REQUIRE(npairs >= n && npairs <= n * (n + 1) / 2 && feeds >= 0 && feeds <= UDH_EXPOSURE_MAX_FEEDS,
+              "udh_mosaic_exposure_stats_u8: %d pairs of %d frames, %d feeds (at most %d)", npairs, n, feeds, UDH_EXPOSURE_MAX_FEEDS);
+  if (ws_bytes < udh_mosaic_exposure_workspace_bytes(n)) {
+    set_error("udh_mosaic_exposure_stats_u8: workspace of %zu bytes, %zu needed", ws_bytes, udh_mosaic_exposure_workspace_bytes(n));
+    return UDH_EWS;
+  }
+  std::vector<ExposureFrame> host((size_t)n);
+  for (int k = 0; k < n; ++k) {
+    const int* r = rois + 4 * k;
+    UDH_REQUIRE(r[0] >= 0 && r[1] >= 0 && r[0] < r[2] && r[1] < r[3] && r[2] <= dst_w && r[3] <= dst_h,
+                "udh_mosaic_exposure_stats_u8: frame %d's ROI (%d, %d)..(%d, %d) is empty or leaves the %dx%d canvas", k, r[0], r[1],
+                r[2], r[3], dst_h, dst_w);
+    UDH_REQUIRE(frames[k], "udh_mosaic_exposure_stats_u8: frame %d is a null pointer", k);
+    ExposureFrame& F = host[k];
+    F.src = frames[k];
+    F.h = sizes[2 * k];
+    F.w = sizes[2 * k + 1];
+    UDH_REQUIRE(F.h >= 1 && F.w >= 1 && F.h < 32767 && F.w < 32767, "udh_mosaic_exposure_stats_u8: frame %d is %dx%d", k, F.h, F.w);
+    F.rx = r[0]; F.ry = r[1]; F.rw = r[2] - r[0]; F.rh = r[3] - r[1];
+    const int bh = F.rh < 16 ? F.rh : 16;
+    F.bw = 1024 / bh < F.rw ? 1024 / bh : F.rw;                      // the ROI warp's tile width, as mb_plan sets it
+  }
+  const cudaStream_t st = as_stream(stream);
+  // pageable source: the copy is staged before this call returns, so `host` may go
+  cudaError_t e = cudaMemcpyAsync(ws, host.data(), (size_t)n * sizeof(ExposureFrame), cudaMemcpyHostToDevice, st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(stats, 0, (size_t)npairs * UDH_EXPOSURE_STATS * sizeof(uint64_t), st);
+  if (e != cudaSuccess) {
+    set_error("udh_mosaic_exposure_stats_u8: %s", cudaGetErrorString(e));
+    return UDH_ECUDA;
+  }
+  ExposureFrame* fr = static_cast<ExposureFrame*>(ws);
+  exposure_invert_kernel<<<(n + 127) / 128, 128, 0, st>>>(M, fr, n);
+  int rc = check_launch("udh_mosaic_exposure_stats_u8 (inverses)");
+  if (rc != UDH_OK) return rc;
+  const dim3 grid((unsigned)((dst_w + EX_TILE_W - 1) / EX_TILE_W), (unsigned)((dst_h + EX_TILE_H - 1) / EX_TILE_H));
+  exposure_stats_kernel<<<grid, 256, 0, st>>>(fr, n, pair_ptr, pair_j, history, feeds, norms,
+                                              reinterpret_cast<unsigned long long*>(stats));
+  return check_launch("udh_mosaic_exposure_stats_u8");
 }

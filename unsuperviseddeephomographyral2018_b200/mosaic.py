@@ -1,8 +1,9 @@
 """Stitch an image sequence into one mosaic: chain the learned pairwise homographies to a reference frame, lay out a
 canvas, and blend every frame onto it on the GPU (udh_mosaic_blend_u8, or udh_mosaic_multiband_u8 across frequency bands).
 
-    out = build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None, blend="feather", bands=5)
-    out["mosaic"], out["mask"], out["M"], out["kept"], out["H_pairs"], out["last_ms"]
+    out = build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None, blend="feather", bands=5,
+                       compensate="none", compensate_feeds=1)
+    out["mosaic"], out["mask"], out["M"], out["kept"], out["H_pairs"], out["gains"], out["last_ms"]
 
 frames are CUDA uint8 RGB [h_k,w_k,3] tensors in sequence order (sizes may differ); est is an align.HomographyEstimator.
 
@@ -22,8 +23,14 @@ frame's edge in 1/32 px, 32 feather).
 
 Blend, blend="multiband".  oracle/multiband.py states the rule: cv2.detail_MultiBandBlender(0, bands, CV_16S) (Burt-Adelson:
 low frequencies blended over a wide region, high ones over a narrow one), fed each frame's warp on its ROI
-(multiband_rois) with the feathered blend's validity as its mask.  It hides the steps a drifting chain or an exposure
-change leaves where a feathered average would ghost or band.
+(multiband_rois) with the feathered blend's validity as its mask.  It hides the seams a drifting chain leaves where a
+feathered average would ghost.  An exposure step between frames it only spreads over its low-frequency region; exposure
+compensation removes it.
+
+Exposure compensation, compensate="gain" or "channels" (default "none").  Before either blend, ops.mosaic_exposure_gains
+computes what cv2.detail_GainCompensator(compensate_feeds) (one gain per frame) or ChannelsCompensator (one per channel)
+finds for the kept frames' ROI warps (oracle/exposure.py states the rule); the blend then takes each frame's warp value
+as saturate_u8(rint(v g)).  This is the stage cv2's stitcher runs between the warp and the blender.
 """
 import numpy as np
 
@@ -126,15 +133,21 @@ def farthest_frame(sizes, G, kept, ref):
     return far
 
 
-def build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None, float32_M=False, blend="feather", bands=5):
+COMPENSATE = ("none", "gain", "channels")
+
+
+def build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None, float32_M=False, blend="feather", bands=5,
+                 compensate="none", compensate_feeds=1):
     """est: align.HomographyEstimator; frames: CUDA uint8 RGB [h_k,w_k,3] tensors in sequence order.  blend: "feather"
     (udh_mosaic_blend_u8 with `feather`) or "multiband" (udh_mosaic_multiband_u8 with `bands`).  refine: None, or a
     dict of est.refine's keyword arguments (levels, iters, eps, max_side) to refine each pair's H.  max_pixels: the canvas
     limit (None: the JPEG encoder's, udh_jpeg_encode_capacity(Hc, Wc, 3) != 0).  float32_M: blend with each M_k rounded to
-    float32, the values a text file of '%.9g' float32 entries gives back.
+    float32, the values a text file of '%.9g' float32 entries gives back.  compensate: "none", "gain" or "channels"
+    (ops.mosaic_exposure_gains with compensate_feeds feeds, applied by the blend).
     -> dict(mosaic uint8 [Hc,Wc,3] RGB, mask uint8 [Hc,Wc], M [N,3,3] frame k -> canvas (float64, float32 values with
-    float32_M), kept bool [N], ref, H_pairs [N-1,3,3], refine (rho, status, level_reached) or None, last_ms {prep, forward,
-    refine, blend} of CUDA-event time)."""
+    float32_M), kept bool [N], ref, H_pairs [N-1,3,3], refine (rho, status, level_reached) or None, gains float64 [N,3]
+    (1 for a dropped frame, all 1 without compensation), last_ms {prep, forward, refine, compensate, blend} of CUDA-event
+    time; compensate only when compensating)."""
     frames = list(frames)
     if len(frames) < 2:
         raise ValueError("a mosaic needs at least two frames (got %d)" % len(frames))
@@ -154,8 +167,14 @@ def build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None
         check_encodable(Hc, Wc, sizes, G, kept, ref)
     if blend not in ("feather", "multiband"):
         raise ValueError("blend must be 'feather' or 'multiband' (got %r)" % (blend,))
-    mosaic, mask, ms["blend"] = blend_kept(frames, M, kept, Hc, Wc, feather, blend, bands)
-    return dict(mosaic=mosaic, mask=mask, M=M, kept=kept, ref=ref, H_pairs=H, refine=refined, last_ms=ms)
+    if compensate not in COMPENSATE:
+        raise ValueError("compensate must be 'none', 'gain' or 'channels' (got %r)" % (compensate,))
+    gains = np.ones((len(frames), 3))
+    if compensate != "none":
+        gains[kept], ms["compensate"] = compensate_kept(frames, M, kept, Hc, Wc, compensate, compensate_feeds)
+    mosaic, mask, ms["blend"] = blend_kept(frames, M, kept, Hc, Wc, feather, blend, bands,
+                                           None if compensate == "none" else gains)
+    return dict(mosaic=mosaic, mask=mask, M=M, kept=kept, ref=ref, H_pairs=H, refine=refined, gains=gains, last_ms=ms)
 
 
 def check_encodable(Hc, Wc, sizes, G, kept, ref):
@@ -166,18 +185,34 @@ def check_encodable(Hc, Wc, sizes, G, kept, ref):
                          "frame (drop it or pick another --ref_frame)" % (Hc, Wc, farthest_frame(sizes, G, kept, ref)))
 
 
-def blend_kept(frames, M, kept, Hc, Wc, feather, mode="feather", bands=5):
-    """The kept frames through ops.mosaic_blend_u8 (mode "feather") or ops.mosaic_multiband_u8 ("multiband") -> (mosaic,
-    mask, CUDA-event ms)."""
+def compensate_kept(frames, M, kept, Hc, Wc, mode, feeds=1):
+    """The kept frames' exposure gains (ops.mosaic_exposure_gains) -> (gains float64 [n_kept,3], CUDA-event ms)."""
     import torch
     from . import ops
     take = [k for k in range(len(frames)) if kept[k]]
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
+    g = ops.mosaic_exposure_gains([frames[k].contiguous() for k in take], np.asarray(M)[take], Hc, Wc, mode, feeds)
+    e1.record()
+    e1.synchronize()
+    return g, e0.elapsed_time(e1)
+
+
+def blend_kept(frames, M, kept, Hc, Wc, feather, mode="feather", bands=5, gains=None):
+    """The kept frames through ops.mosaic_blend_u8 (mode "feather") or ops.mosaic_multiband_u8 ("multiband") -> (mosaic,
+    mask, CUDA-event ms).  gains: None, or [N,3] per frame (exposure compensation)."""
+    import torch
+    from . import ops
+    take = [k for k in range(len(frames)) if kept[k]]
+    g = None if gains is None else np.asarray(gains, np.float64)[take]
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
     if mode == "multiband":
-        mosaic, mask = ops.mosaic_multiband_u8([frames[k].contiguous() for k in take], np.asarray(M)[take], Hc, Wc, bands)
+        mosaic, mask = ops.mosaic_multiband_u8([frames[k].contiguous() for k in take], np.asarray(M)[take], Hc, Wc, bands,
+                                               gains=g)
     else:
-        mosaic, mask = ops.mosaic_blend_u8([frames[k].contiguous() for k in take], np.asarray(M)[take], Hc, Wc, feather)
+        mosaic, mask = ops.mosaic_blend_u8([frames[k].contiguous() for k in take], np.asarray(M)[take], Hc, Wc, feather,
+                                           gains=g)
     e1.record()
     e1.synchronize()
     return mosaic, mask, e0.elapsed_time(e1)

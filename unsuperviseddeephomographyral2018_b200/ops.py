@@ -2,6 +2,7 @@
 autograd bookkeeping; all arithmetic happens in libudh's CUDA kernels.  Every function requires CUDA tensors."""
 import ctypes
 import functools
+import math
 
 import numpy as np
 import torch
@@ -636,11 +637,22 @@ def mosaic_tile_lists(M, sizes, dst_h, dst_w):
     return ptr.astype(np.int32), frames[order].astype(np.int32)
 
 
-def mosaic_blend_u8(frames, M, dst_h, dst_w, feather):
+def _gains(gains, n, dev, what):
+    """Exposure gains [n], [n,1] or [n,3] (numpy or tensor) -> float64 [n,3] on dev (one gain repeated over the channels)."""
+    g = (gains.detach().cpu().numpy() if isinstance(gains, torch.Tensor) else np.asarray(gains)).astype(np.float64)
+    g = g.reshape(len(g), -1) if g.ndim else g.reshape(1, 1)
+    if g.shape[0] != n or g.shape[1] not in (1, 3):
+        raise _lib.UdhError("%s: gains must be [n], [n,1] or [n,3] for %d frames (got %s)" % (what, n, g.shape))
+    return torch.from_numpy(np.broadcast_to(g, (n, 3)).copy()).to(dev)
+
+
+def mosaic_blend_u8(frames, M, dst_h, dst_w, feather, gains=None):
     """frames: n CUDA uint8 tensors [h_k,w_k,C] (C = 1 or 3, sizes may differ; or one [n,h,w,C] tensor), M float64 [n,3,3]
     (frame k -> canvas; numpy or tensor) -> (mosaic uint8 [dst_h,dst_w,C], mask uint8 [dst_h,dst_w]): udh_mosaic_blend_u8's
     feathered blend of cv2.warpPerspective(frame k, M_k, (dst_w, dst_h)), bit for bit with oracle/mosaic.py.  The tile
-    lists are built on the host (mosaic_tile_lists); the frames are read where they are."""
+    lists are built on the host (mosaic_tile_lists); the frames are read where they are.  gains ([n] or [n,3], e.g.
+    mosaic_exposure_gains'): each frame's warp value is exposure-compensated first, saturate_u8(rint(v g)) in float64
+    (udh_mosaic_blend_gain_u8)."""
     frames = list(frames.unbind(0)) if isinstance(frames, torch.Tensor) else list(frames)
     Mh = (M.detach().cpu().numpy() if isinstance(M, torch.Tensor) else np.asarray(M)).astype(np.float64).reshape(-1, 3, 3)
     n = len(frames)
@@ -664,18 +676,26 @@ def mosaic_blend_u8(frames, M, dst_h, dst_w, feather):
     ws = torch.empty(max(nb, 1), device=dev, dtype=torch.uint8)
     ptrs = (ctypes.c_void_p * n)(*[f.data_ptr() for f in frames])
     sz = np.ascontiguousarray(np.array(sizes, np.int32).reshape(n, 2))
-    check(lib.udh_mosaic_blend_u8(ptrs, sz.ctypes.data, _ptr(M_d), n, C, _ptr(ptr_d), _ptr(idx_d), int(dst_h), int(dst_w),
-                                  int(feather), _ptr(out), _ptr(mask), _ptr(ws), nb, _stream()), "udh_mosaic_blend_u8")
+    if gains is None:
+        check(lib.udh_mosaic_blend_u8(ptrs, sz.ctypes.data, _ptr(M_d), n, C, _ptr(ptr_d), _ptr(idx_d), int(dst_h), int(dst_w),
+                                      int(feather), _ptr(out), _ptr(mask), _ptr(ws), nb, _stream()), "udh_mosaic_blend_u8")
+    else:
+        g_d = _gains(gains, n, dev, "mosaic_blend_u8")
+        check(lib.udh_mosaic_blend_gain_u8(ptrs, sz.ctypes.data, _ptr(M_d), _ptr(g_d), n, C, _ptr(ptr_d), _ptr(idx_d), int(dst_h),
+                                           int(dst_w), int(feather), _ptr(out), _ptr(mask), _ptr(ws), nb, _stream()),
+              "udh_mosaic_blend_gain_u8")
     return out, mask
 
 
-def mosaic_multiband_u8(frames, M, dst_h, dst_w, bands, levels=False):
+def mosaic_multiband_u8(frames, M, dst_h, dst_w, bands, levels=False, gains=None):
     """frames: n CUDA uint8 RGB tensors [h_k,w_k,3] (sizes may differ), M float64 [n,3,3] (frame k -> canvas; numpy or
     tensor) -> (mosaic uint8 [dst_h,dst_w,3], mask uint8 [dst_h,dst_w]): udh_mosaic_multiband_u8, byte for byte
     cv2.detail_MultiBandBlender(0, bands, CV_16S) fed each frame's warp on its ROI (oracle/multiband.py).  The ROIs and the
     frame -> ROI maps are formed on the host (mosaic.multiband_rois, which raises ValueError for a frame whose corners do not
     map to finite points with a positive denominator); a frame whose ROI misses the canvas is left out.  levels=True also
-    returns the canvas pyramid as the feeds left it: [B' + 1] int16 CUDA tensors [Hp >> i, Wp >> i, 4] (acc, then wacc)."""
+    returns the canvas pyramid as the feeds left it: [B' + 1] int16 CUDA tensors [Hp >> i, Wp >> i, 4] (acc, then wacc).
+    gains ([n] or [n,3], e.g. mosaic_exposure_gains'): each ROI warp is exposure-compensated before it is fed,
+    saturate_u8(rint(v g)) in float64 (udh_mosaic_multiband_gain_u8), cv2's stitcher order."""
     from . import mosaic
     frames = list(frames.unbind(0)) if isinstance(frames, torch.Tensor) else list(frames)
     Mh = (M.detach().cpu().numpy() if isinstance(M, torch.Tensor) else np.asarray(M)).astype(np.float64).reshape(-1, 3, 3)
@@ -694,6 +714,7 @@ def mosaic_multiband_u8(frames, M, dst_h, dst_w, bands, levels=False):
     dev = frames[0].device
     out = torch.zeros(int(dst_h), int(dst_w), 3, device=dev, dtype=torch.uint8)
     mask = torch.zeros(int(dst_h), int(dst_w), device=dev, dtype=torch.uint8)
+    g_d = None if gains is None else _gains(gains, n, dev, "mosaic_multiband_u8")
     if not take:
         return (out, mask, []) if levels else (out, mask)
     m = len(take)
@@ -705,8 +726,14 @@ def mosaic_multiband_u8(frames, M, dst_h, dst_w, bands, levels=False):
     if nb == 0:
         raise _lib.UdhError("mosaic_multiband_u8: bad arguments (%d frames, canvas %dx%d, %d bands)" % (m, dst_h, dst_w, bands))
     ws = torch.empty(nb, device=dev, dtype=torch.uint8)
-    check(lib.udh_mosaic_multiband_u8(ptrs, sz.ctypes.data, _ptr(M_d), rr.ctypes.data, m, 3, int(dst_h), int(dst_w), int(bands),
-                                      _ptr(out), _ptr(mask), _ptr(ws), nb, _stream()), "udh_mosaic_multiband_u8")
+    if g_d is None:
+        check(lib.udh_mosaic_multiband_u8(ptrs, sz.ctypes.data, _ptr(M_d), rr.ctypes.data, m, 3, int(dst_h), int(dst_w), int(bands),
+                                          _ptr(out), _ptr(mask), _ptr(ws), nb, _stream()), "udh_mosaic_multiband_u8")
+    else:
+        g_d = g_d[take].contiguous()
+        check(lib.udh_mosaic_multiband_gain_u8(ptrs, sz.ctypes.data, _ptr(M_d), _ptr(g_d), rr.ctypes.data, m, 3, int(dst_h),
+                                               int(dst_w), int(bands), _ptr(out), _ptr(mask), _ptr(ws), nb, _stream()),
+              "udh_mosaic_multiband_gain_u8")
     if not levels:
         return out, mask
     off, dims = (ctypes.c_size_t * 11)(), (ctypes.c_int * 3)()
@@ -718,6 +745,176 @@ def mosaic_multiband_u8(frames, M, dst_h, dst_w, bands, levels=False):
         cnt = (Hp >> i) * (Wp >> i) * 4
         pyr.append(ws[off[i]:off[i] + 2 * cnt].view(torch.int16).reshape(Hp >> i, Wp >> i, 4))
     return out, mask, pyr
+
+
+# ------------------------------------------------------------------ exposure compensation
+EXPOSURE_ALPHA, EXPOSURE_BETA = 0.01, 100.0       # cv2.detail.GainCompensator's weights of the gain and intensity terms
+
+
+def exposure_pairs(rois):
+    """rois [m,4] (x_lo, y_lo, x_hi, y_hi) -> CSR (pair_ptr int32 [m+1], pair_j int32 [P]) of the pairs i <= j whose rectangles
+    intersect (cv2.detail.overlapRoi), the diagonal included, row-major."""
+    r = np.asarray(rois, np.int64).reshape(-1, 4)
+    x0, y0 = np.maximum(r[:, None, 0], r[None, :, 0]), np.maximum(r[:, None, 1], r[None, :, 1])
+    x1, y1 = np.minimum(r[:, None, 2], r[None, :, 2]), np.minimum(r[:, None, 3], r[None, :, 3])
+    hit = np.triu((x0 < x1) & (y0 < y1))
+    ptr = np.zeros(len(r) + 1, np.int64)
+    ptr[1:] = np.cumsum(hit.sum(1))
+    return ptr.astype(np.int32), np.nonzero(hit)[1].astype(np.int32)
+
+
+def exposure_norm_sum(l0, l1, l2):
+    """The three 21-bit limb sums of udh_mosaic_exposure_stats_u8's sum q (q = norm 2^52, an integer) -> sum norm: the exact
+    total, rounded to double once (ties to even)."""
+    return math.ldexp(float(int(l0) + (int(l1) << 21) + (int(l2) << 42)), -52)
+
+
+def _exposure_rois(frames, M, dst_h, dst_w, what):
+    from . import mosaic
+    frames = list(frames.unbind(0)) if isinstance(frames, torch.Tensor) else list(frames)
+    Mh = (M.detach().cpu().numpy() if isinstance(M, torch.Tensor) else np.asarray(M)).astype(np.float64).reshape(-1, 3, 3)
+    n = len(frames)
+    if Mh.shape[0] != n:
+        raise _lib.UdhError("%s: %d matrices for %d frames" % (what, Mh.shape[0], n))
+    if n == 0:
+        raise _lib.UdhError("%s: no frames" % what)
+    for k, f in enumerate(frames):
+        _req(f, torch.uint8, "frames[%d]" % k)
+        if f.dim() != 3 or f.shape[2] != 3:
+            raise _lib.UdhError("%s: frames must be [h,w,3] (frame %d is %s)" % (what, k, tuple(f.shape)))
+    sizes = [(int(f.shape[0]), int(f.shape[1])) for f in frames]
+    rois, Mr = mosaic.multiband_rois(Mh, sizes, int(dst_h), int(dst_w))
+    take = [k for k in range(n) if rois[k, 2] > rois[k, 0] and rois[k, 3] > rois[k, 1]]
+    if len(take) > _lib.EXPOSURE_MAX_FRAMES:
+        raise _lib.UdhError("%s: %d frames meet the canvas (at most %d)" % (what, len(take), _lib.EXPOSURE_MAX_FRAMES))
+    return frames, sizes, rois, Mr, take
+
+
+class _ExposureStats(object):
+    """udh_mosaic_exposure_stats_u8 on fixed frames: the device-side frame table, pairs and output, reused by every feed."""
+
+    def __init__(self, frames, M, dst_h, dst_w):
+        frames, sizes, rois, Mr, take = _exposure_rois(frames, M, dst_h, dst_w, "mosaic_exposure_stats")
+        self.n, self.take, self.dst = len(frames), take, (int(dst_h), int(dst_w))
+        m = self.m = len(take)
+        if not m:
+            self.i = self.j = np.zeros(0, np.int64)
+            return
+        dev = frames[0].device
+        self.frames = [frames[k] for k in take]
+        self.ptrs = (ctypes.c_void_p * m)(*[f.data_ptr() for f in self.frames])
+        self.sz = np.ascontiguousarray(np.array([sizes[k] for k in take], np.int32).reshape(m, 2))
+        self.rr = np.ascontiguousarray(rois[take].astype(np.int32))
+        self.M_d = torch.from_numpy(np.ascontiguousarray(Mr[take].reshape(m, 9))).to(dev)
+        ptr, pj = exposure_pairs(self.rr)
+        self.i = np.repeat(np.arange(m), np.diff(ptr)).astype(np.int64)
+        self.j = pj.astype(np.int64)
+        self.ptr_d, self.pj_d = torch.from_numpy(ptr).to(dev), torch.from_numpy(pj).to(dev)
+        self.out = torch.empty(len(pj), _lib.EXPOSURE_STATS, device=dev, dtype=torch.int64)
+        self.nb = lib.udh_mosaic_exposure_workspace_bytes(m)
+        self.ws = torch.empty(max(self.nb, 1), device=dev, dtype=torch.uint8)
+        self.dev = dev
+
+    def __call__(self, history=None, norms=True):
+        """history: None or float64 [t,m,3] (the fed frames' gains of feeds 0..t-1) -> uint64 [P,13] numpy."""
+        if not self.m:
+            return np.zeros((0, _lib.EXPOSURE_STATS), np.uint64)
+        t = 0 if history is None else int(np.asarray(history).shape[0])
+        h_d = None
+        if t:
+            h_d = torch.from_numpy(np.ascontiguousarray(np.asarray(history, np.float64).reshape(t, self.m, 3))).to(self.dev)
+        check(lib.udh_mosaic_exposure_stats_u8(self.ptrs, self.sz.ctypes.data, _ptr(self.M_d), self.rr.ctypes.data, self.m,
+                                               _ptr(self.ptr_d), _ptr(self.pj_d), len(self.j), _ptr(h_d) if t else None, t,
+                                               int(bool(norms)), self.dst[0], self.dst[1], _ptr(self.out), _ptr(self.ws), self.nb,
+                                               _stream()), "udh_mosaic_exposure_stats_u8")
+        return self.out.cpu().numpy().view(np.uint64)
+
+
+def mosaic_exposure_stats(frames, M, dst_h, dst_w, history=None, norms=True):
+    """The exposure compensators' pair statistics of the frames' ROI warps (udh_mosaic_exposure_stats_u8), for tests and
+    tools.  frames, M as mosaic_multiband_u8 takes them; history None or [t,m,3] over the fed frames.  -> dict(take (the fed
+    frames: those whose ROI meets the canvas), i, j [P] (pairs of fed-frame indices, i <= j, ROIs intersecting), count
+    int64 [P], sums int64 [P,2,3] (frame i's, frame j's channel sums), norms float64 [P,2] (sum of cv2's norm(Vec3b),
+    exact and rounded once; 0 without norms), raw uint64 [P,13])."""
+    st = _ExposureStats(frames, M, dst_h, dst_w)
+    raw = st(history, norms)
+    ns = np.array([[exposure_norm_sum(*r[7:10]), exposure_norm_sum(*r[10:13])] for r in raw]).reshape(-1, 2)
+    return dict(take=st.take, i=st.i, j=st.j, count=raw[:, 0].astype(np.int64), sums=raw[:, 1:7].astype(np.int64).reshape(-1, 2, 3),
+                norms=ns, raw=raw)
+
+
+def exposure_solve(m, i, j, count, Isum_i, Isum_j):
+    """One feed of cv2.detail.GainCompensator on m images from its pair statistics (pairs i <= j whose ROIs intersect,
+    their mask-intersection counts and the two sums) -> gains float64 [m].  N_ij = N_ji = max(1, count); where count > 0,
+    I_ij = Isum_i / N_ij and I_ji = Isum_j / N_ij, and an off-diagonal pair keeps both frames from being skipped.  Over the
+    unskipped frames in order: b_i += beta N_ij, A_ii += beta N_ij and, for j != i, A_ii += 2 alpha I_ij^2 N_ij,
+    A_ij -= 2 alpha I_ij I_ji N_ij; gains = cv2.solve(A, b) (LU) there, 1 for skipped frames.  The sums are formed in
+    cv2's order, so equal statistics give cv2's bits."""
+    import cv2
+    N = np.zeros((m, m), np.int64)
+    I = np.zeros((m, m), np.float64)
+    skip = np.ones(m, bool)
+    for a, b, c, s1, s2 in zip(i, j, count, Isum_i, Isum_j):
+        a, b = int(a), int(b)
+        N[a, b] = N[b, a] = max(1, int(c))
+        if c == 0:
+            continue
+        if a != b:
+            skip[a] = skip[b] = False
+        I[a, b] = float(s1) / N[a, b]
+        I[b, a] = float(s2) / N[a, b]
+    g = np.ones(m, np.float64)
+    idx = [k for k in range(m) if not skip[k]]
+    if not idx:
+        return g
+    A = np.zeros((len(idx), len(idx)), np.float64)
+    rhs = np.zeros((len(idx), 1), np.float64)
+    al, be = EXPOSURE_ALPHA, EXPOSURE_BETA
+    for ki, a in enumerate(idx):
+        for kj, b in enumerate(idx):
+            nab, iab, iba = int(N[a, b]), float(I[a, b]), float(I[b, a])
+            rhs[ki, 0] += be * nab
+            A[ki, ki] += be * nab
+            if b != a:
+                A[ki, ki] += 2 * al * iab * iab * nab
+                A[ki, kj] -= 2 * al * iab * iba * nab
+    _, x = cv2.solve(A, rhs)
+    g[idx] = x.reshape(-1)
+    return g
+
+
+def mosaic_exposure_gains(frames, M, dst_h, dst_w, mode="gain", feeds=1):
+    """frames: n CUDA uint8 RGB tensors [h_k,w_k,3], M float64 [n,3,3] (frame k -> canvas) -> gains float64 [n,3]: what
+    cv2.detail_GainCompensator(feeds) (mode "gain": one gain per frame, repeated over the channels) or
+    cv2.detail_ChannelsCompensator(feeds) ("channels": one per channel) computes when fed the multi-band blend's inputs
+    (each frame's ROI warp, its validity mask and the ROI's top-left; oracle/exposure.py).  A frame whose ROI misses the
+    canvas is not fed and gets 1.  Feed t sees the images compensated by feeds 0..t-1 in turn; the gains are the product
+    of the feeds'.  The pair statistics come from udh_mosaic_exposure_stats_u8 (exact integer sums; in "gain" mode the sums
+    of norms are exact and rounded once where cv2 adds in row order, so the gains agree to cv2's own summation error; in
+    "channels" mode they are cv2's bits); the small system is solved on the host."""
+    if mode not in ("gain", "channels"):
+        raise ValueError("mode must be 'gain' or 'channels' (got %r)" % (mode,))
+    if not 1 <= int(feeds) <= _lib.EXPOSURE_MAX_FEEDS:
+        raise ValueError("feeds must be in 1..%d (got %r)" % (_lib.EXPOSURE_MAX_FEEDS, feeds))
+    st = _ExposureStats(frames, M, dst_h, dst_w)
+    gains = np.ones((st.n, 3), np.float64)
+    if not st.m:
+        return gains
+    hist, acc = [], None
+    for _ in range(int(feeds)):
+        raw = st(np.stack(hist) if hist else None, norms=mode == "gain")
+        count = raw[:, 0].astype(np.int64)
+        if mode == "gain":
+            g = exposure_solve(st.m, st.i, st.j, count, [exposure_norm_sum(*r[7:10]) for r in raw],
+                               [exposure_norm_sum(*r[10:13]) for r in raw])
+            g3 = np.repeat(g[:, None], 3, 1)
+        else:
+            g3 = np.stack([exposure_solve(st.m, st.i, st.j, count, raw[:, 1 + c].astype(np.int64),
+                                          raw[:, 4 + c].astype(np.int64)) for c in range(3)], 1)
+        acc = g3.copy() if acc is None else acc * g3
+        hist.append(g3)
+    gains[st.take] = acc
+    return gains
 
 
 # ------------------------------------------------------------------ Adam
