@@ -655,6 +655,25 @@ size_t udh_debug_fc1_scratch_bytes(int B, int numeric_mode);
 int udh_debug_fc1(int numeric_mode, const float* x, const float* w, const float* dy, float* y, float* dW, float* dx, void* scratch,
                   int B, void* stream);
 
+/* ---- debug / test entry points of the fp32 CUDA-core path (UDH_NUMERIC_FP32), the calls the step makes ------------
+ * udh_debug_simt_conv: one 3x3 convolution, NHWC fp32, H % 8 == 0, W % 16 == 0.  dgrad == 0: out [B,H,W,cout] =
+ * relu?(conv(x, w) + bias) (bias nullable), with x2 != NULL the two single-channel planes x, x2 of conv1_1 (cin == 2).
+ * dgrad != 0: w is the layer's [3,3,cin,cout] kernel; it is rotated into wrot (9 cin cout floats) and out [B,H,W,cin] =
+ * conv(x = g [B,H,W,cout], wrot) with no bias, no ReLU and no second plane.  mask_src (nullable, shaped like out) zeroes
+ * every output element whose mask_src value is not > 0 (the fused ReLU backward of the layer below). */
+int udh_debug_simt_conv(const float* x, const float* x2, const float* w, const float* bias, const float* mask_src, float* out,
+                        float* wrot, int B, int H, int W, int cin, int cout, int relu, int dgrad, void* stream);
+/* weight gradient of one layer: dW [3,3,cin,cout] += sum x * g and db [cout] += sum g (fp32 atomics: not bit-reproducible),
+ * x [B,H,W,cin] (or the planes x, x2 with cin == 2), g [B,H,W,cout].  The partition (nullable outputs): CTA x (of ctas_x)
+ * walks pixel tiles [x tiles_per_cta, (x+1) tiles_per_cta) of the B (H/8) (W/16) 8x16 tiles in (n, tile row, tile column)
+ * order; its threads for rows s = 0 .. row_split-1 each sum rows s, s + row_split, ... of those tiles, in order of tile, row
+ * and column, with one fmaf per pixel, and add their partial to dW with one atomicAdd (db likewise with plain adds). */
+int udh_debug_simt_wgrad(const float* x, const float* x2, const float* g, float* dW, float* db, int B, int H, int W, int cin,
+                         int cout, int* ctas_x, int* tiles_per_cta, int* row_split, void* stream);
+/* 2x2 max-pool of in [B,H,W,C]: forward into out [B,H/2,W/2,C] when out != NULL; backward when din != NULL: din [B,H,W,C]
+ * receives dout [B,H/2,W/2,C] at the first maximum of each window in row-major order when that maximum is > 0, else 0. */
+int udh_debug_simt_pool(const float* in, float* out, const float* dout, float* din, int B, int H, int W, int C, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

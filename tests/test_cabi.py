@@ -112,6 +112,76 @@ def test_fc1_debug_entry_rejects_bad_arguments():
         assert b"unknown numeric_mode" in L.udh_last_error()
 
 
+def test_simt_debug_entries_reject_bad_arguments():
+    """udh_debug_simt_conv / _wgrad / _pool are exported and check their arguments before touching the device."""
+    from unsuperviseddeephomographyral2018_b200 import _lib
+    L = _lib.lib
+    raw = ctypes.CDLL(_lib.LIB_PATH)
+    assert all(hasattr(raw, s) for s in ("udh_debug_simt_conv", "udh_debug_simt_wgrad", "udh_debug_simt_pool"))
+    p = ctypes.c_void_p(256)                          # never dereferenced: every call below fails its argument checks
+    shape = (2, 16, 16, 64, 64)
+    for dgrad, nulls in ((0, (0, 2, 5)), (1, (0, 2, 5, 6))):   # x, w, out; wrot for the dgrad
+        for i in nulls:
+            a = [p, None, p, None, None, p, p]
+            a[i] = None
+            assert L.udh_debug_simt_conv(*a, *shape, 0, dgrad, None) == _lib.EINVAL, (dgrad, i)
+            assert b"udh_debug_simt_conv: null pointer" in L.udh_last_error()
+    conv = lambda x2, bias, B, H, W, cin, cout, relu, dgrad: L.udh_debug_simt_conv(p, x2, p, bias, None, p, p, B, H, W, cin, cout,
+                                                                                   relu, dgrad, None)
+    assert conv(p, None, 2, 16, 16, 2, 64, 0, 1) == _lib.EINVAL          # dgrad with a second plane
+    assert conv(None, p, 2, 16, 16, 64, 64, 0, 1) == _lib.EINVAL         # dgrad with a bias
+    assert conv(None, None, 2, 16, 16, 64, 64, 1, 1) == _lib.EINVAL      # dgrad with ReLU
+    assert b"the dgrad takes one input" in L.udh_last_error()
+    for B, H, W in ((0, 16, 16), (2, 12, 16), (2, 16, 24), (2, 0, 16)):
+        assert conv(None, None, B, H, W, 64, 64, 1, 0) == _lib.EINVAL, (B, H, W)
+        assert b"needs B >= 1" in L.udh_last_error()
+    for x2, cin, cout, dgrad in ((None, 64, 96, 0), (None, 12, 64, 0), (p, 3, 64, 0), (None, 64, 68, 1), (None, 96, 64, 1)):
+        assert conv(x2, None, 2, 16, 16, cin, cout, 0, dgrad) == _lib.EINVAL, (cin, cout, dgrad)
+        assert b"unsupported channels" in L.udh_last_error()
+    part = [ctypes.c_int(-1) for _ in range(3)]
+    refs = [ctypes.byref(v) for v in part]
+    for i in (0, 2, 3, 4):                            # x, g, dW, db
+        a = [p, None, p, p, p]
+        a[i] = None
+        assert L.udh_debug_simt_wgrad(*a, *shape, *refs, None) == _lib.EINVAL
+        assert b"udh_debug_simt_wgrad: null pointer" in L.udh_last_error()
+    assert L.udh_debug_simt_wgrad(p, None, p, p, p, 0, 16, 16, 64, 64, *refs, None) == _lib.EINVAL
+    assert L.udh_debug_simt_wgrad(p, None, p, p, p, 2, 16, 16, 8, 64, *refs, None) == _lib.EINVAL    # cin % 16
+    assert L.udh_debug_simt_wgrad(p, p, p, p, p, 2, 16, 16, 64, 64, *refs, None) == _lib.EINVAL      # two planes need cin == 2
+    assert b"unsupported channels" in L.udh_last_error()
+    assert [v.value for v in part] == [-1, -1, -1]    # nothing reported for a rejected call
+    for a in ((None, p, None, None), (p, None, None, None), (p, None, None, p), (p, None, p, None)):
+        assert L.udh_debug_simt_pool(*a, 2, 16, 16, 64, None) == _lib.EINVAL, a
+        assert b"udh_debug_simt_pool: null pointer" in L.udh_last_error()
+    for B, H, W, C in ((0, 16, 16, 64), (2, 15, 16, 64), (2, 16, 7, 64), (2, 16, 16, 6)):
+        assert L.udh_debug_simt_pool(p, p, p, p, B, H, W, C, None) == _lib.EINVAL
+        assert b"udh_debug_simt_pool: needs" in L.udh_last_error()
+
+
+def test_fp32_patch_size_is_limited_by_fc1_weight_gradient_grid():
+    """fc1's fp32 weight gradient launches (P/8)^2 * 128 / 64 CTA rows on grid.y (max 65535): P = 1408 is the largest patch
+    whose backward can launch, and every entry that takes a patch size rejects a larger one before touching the device."""
+    from unsuperviseddeephomographyral2018_b200 import _lib
+    L = _lib.lib
+    assert (1408 // 8) ** 2 * 128 // 64 <= 65535 < (1536 // 8) ** 2 * 128 // 64
+    assert L.udh_cnn_workspace_bytes(1, 1408, _lib.NUMERIC_FP32) > 0
+    assert L.udh_cnn_workspace_bytes(1, 256, _lib.NUMERIC_FP32) > 0
+    for P in (1536, 2048, 4096):
+        assert L.udh_cnn_workspace_bytes(1, P, _lib.NUMERIC_FP32) == 0, P
+        assert b"patch size %d is too large" % P in L.udh_last_error()
+        assert b"P <= 1408" in L.udh_last_error()
+        assert L.udh_cnn_workspace_init(None, 0, 1, P, _lib.NUMERIC_FP32, None) == _lib.EINVAL
+        assert b"udh_cnn_workspace_init: patch size %d is too large" % P in L.udh_last_error()
+        p = ctypes.c_void_p(256)
+        assert L.udh_cnn_fwd(p, p, p, p, p, 1 << 40, 1, P, 0, 0, _lib.NUMERIC_FP32, None) == _lib.EINVAL
+        assert L.udh_cnn_bwd(p, p, p, p, p, p, 1 << 40, 1, P, 1, _lib.NUMERIC_FP32, None) == _lib.EINVAL
+        assert b"too large" in L.udh_last_error()
+    assert L.udh_cnn_workspace_init(None, 0, 1, 1408, _lib.NUMERIC_FP32, None) == _lib.EINVAL
+    assert b"bad workspace" in L.udh_last_error()                        # 1408 passes the argument check
+    assert L.udh_cnn_workspace_bytes(1, 256, _lib.NUMERIC_BF16X3) == 0   # the tensor-core modes stay at 128
+    assert b"tiled for the reference's 128x128 patches" in L.udh_last_error()
+
+
 def test_schedule_matches_reference_constants():
     from unsuperviseddeephomographyral2018_b200 import engine
     assert engine.decay_steps(1e-4, 0.9e-4) == 58117 and engine.decay_steps(5e-4, 0.9e-4) == 3570

@@ -126,6 +126,11 @@ SIGNATURES = {
     "udh_debug_tc_wgrad": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "udh_debug_fc1_scratch_bytes": (c_size_t, [c_int, c_int]),
     "udh_debug_fc1": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
+    "udh_debug_simt_conv": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                    c_int, c_int, c_int, c_void_p]),
+    "udh_debug_simt_wgrad": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                     POINTER(c_int), POINTER(c_int), POINTER(c_int), c_void_p]),
+    "udh_debug_simt_pool": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "udh_step_forward_backward": (c_int, [POINTER(StepArgs), c_int, c_void_p]),
     "udh_prep_inputs_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                    c_void_p]),

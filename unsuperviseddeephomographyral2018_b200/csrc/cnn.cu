@@ -76,6 +76,10 @@ int check_cnn_args(const char* fn, int B, int P, int numeric_mode) {
               "%s: unknown numeric_mode %d", fn, numeric_mode);
   UDH_REQUIRE(numeric_mode == UDH_NUMERIC_FP32 || P == 128,
               "%s: the tensor-core modes are tiled for the reference's 128x128 patches (got %d); use UDH_NUMERIC_FP32", fn, P);
+  // fc1's weight gradient is an SGEMM with M = (P/8)^2 * 128 rows, one CTA row per 64 of them on grid.y (<= 65535)
+  UDH_REQUIRE((size_t)(P / 8) * (P / 8) * 128 / 64 <= 65535,
+              "%s: patch size %d is too large: fc1's weight gradient would need %zu CTA rows (max 65535), so P <= 1408", fn, P,
+              (size_t)(P / 8) * (P / 8) * 128 / 64);
   return UDH_OK;
 }
 
@@ -101,9 +105,7 @@ extern "C" int udh_param_offset(int P, int tensor, size_t* offset_floats, size_t
 }
 
 extern "C" size_t udh_cnn_workspace_bytes(int B, int P, int numeric_mode) {
-  if (B < 1 || P < 128 || P % 128) return 0;
-  if (numeric_mode != UDH_NUMERIC_FP32 && P != 128) return 0;
-  if (numeric_mode != UDH_NUMERIC_FP32 && numeric_mode != UDH_NUMERIC_BF16 && numeric_mode != UDH_NUMERIC_BF16X3) return 0;
+  if (check_cnn_args("udh_cnn_workspace_bytes", B, P, numeric_mode) != UDH_OK) return 0;
   return Workspace(B, P, numeric_mode).total;
 }
 
@@ -186,6 +188,46 @@ extern "C" int udh_debug_fc1(int numeric_mode, const float* x, const float* w, c
     TRY(fc1_fwd_simt(x, w, y, B, feat, st));
     if (dy) TRY(fc1_bwd_simt(x, w, dy, dW, dx, B, feat, st));
   }
+  return UDH_OK;
+}
+
+extern "C" int udh_debug_simt_conv(const float* x, const float* x2, const float* w, const float* bias, const float* mask_src,
+                                   float* out, float* wrot, int B, int H, int W, int cin, int cout, int relu, int dgrad,
+                                   void* stream) {
+  UDH_REQUIRE(x && w && out && (!dgrad || wrot), "udh_debug_simt_conv: null pointer");
+  UDH_REQUIRE(!dgrad || (!x2 && !bias && !relu), "udh_debug_simt_conv: the dgrad takes one input, no bias and no ReLU");
+  UDH_REQUIRE(B >= 1 && H > 0 && W > 0 && H % 8 == 0 && W % 16 == 0, "udh_debug_simt_conv: needs B >= 1, H % 8 == 0, W % 16 == 0");
+  const int kin = dgrad ? cout : cin, kout = dgrad ? cin : cout;
+  UDH_REQUIRE(kout > 0 && kout % 64 == 0 && (x2 ? kin == 2 : (kin > 0 && kin % 8 == 0)),
+              "udh_debug_simt_conv: unsupported channels (cin %d, cout %d, dgrad %d, two planes %d)", cin, cout, dgrad, x2 != nullptr);
+  cudaStream_t st = as_stream(stream);
+  // the calls of udh_cnn_fwd (forward) and udh_cnn_bwd_phase (dgrad: rotated weights, no bias, the layer below's ReLU mask)
+  if (!dgrad) return conv3x3_simt(x, x2, w, bias, mask_src, out, B, H, W, cin, cout, relu, st);
+  TRY(rotate_weights(w, wrot, cin, cout, st));
+  return conv3x3_simt(x, nullptr, wrot, nullptr, mask_src, out, B, H, W, cout, cin, 0, st);
+}
+
+extern "C" int udh_debug_simt_wgrad(const float* x, const float* x2, const float* g, float* dW, float* db, int B, int H, int W,
+                                    int cin, int cout, int* ctas_x, int* tiles_per_cta, int* row_split, void* stream) {
+  UDH_REQUIRE(x && g && dW && db, "udh_debug_simt_wgrad: null pointer");
+  UDH_REQUIRE(B >= 1 && H > 0 && W > 0 && H % 8 == 0 && W % 16 == 0, "udh_debug_simt_wgrad: needs B >= 1, H % 8 == 0, W % 16 == 0");
+  UDH_REQUIRE(cout > 0 && cout % 64 == 0 && (x2 ? cin == 2 : (cin > 0 && cin % 16 == 0)),
+              "udh_debug_simt_wgrad: unsupported channels (cin %d, cout %d, two planes %d)", cin, cout, x2 != nullptr);
+  const WgradPartition p = wgrad3x3_partition(B, H, W, cin, cout, x2 != nullptr);
+  if (ctas_x) *ctas_x = p.ctas_x;
+  if (tiles_per_cta) *tiles_per_cta = p.tiles_per_cta;
+  if (row_split) *row_split = p.row_split;
+  return wgrad3x3_simt(x, x2, g, dW, db, B, H, W, cin, cout, as_stream(stream));
+}
+
+extern "C" int udh_debug_simt_pool(const float* in, float* out, const float* dout, float* din, int B, int H, int W, int C,
+                                   void* stream) {
+  UDH_REQUIRE(in && (out || din) && (!din || dout), "udh_debug_simt_pool: null pointer");
+  UDH_REQUIRE(B >= 1 && H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0 && C > 0 && C % 4 == 0,
+              "udh_debug_simt_pool: needs B >= 1, even H and W and C % 4 == 0");
+  cudaStream_t st = as_stream(stream);
+  if (out) TRY(maxpool2x2_fwd(in, out, B, H, W, C, st));
+  if (din) TRY(maxpool2x2_bwd(in, dout, din, B, H, W, C, st));
   return UDH_OK;
 }
 

@@ -17,6 +17,10 @@ int conv3x3_simt(const float* in0, const float* in1, const float* w, const float
 // dW[ky,kx,ci,co] += sum_{n,y,x} x[n,y+ky-1,x+kx-1,ci] * g[n,y,x,co];  db[co] += sum g   (atomic accumulation)
 int wgrad3x3_simt(const float* x0, const float* x1, const float* g, float* dW, float* db, int B, int H, int W,
                   int Cin, int Cout, cudaStream_t st);
+// How wgrad3x3_simt splits the B (H/8) (W/16) pixel tiles: CTA x walks tiles [x tiles_per_cta, (x+1) tiles_per_cta) and
+// each of its threads sums the rows r = s, s + row_split, ... of every tile; every such partial is one atomicAdd.
+struct WgradPartition { int ctas_x, tiles_per_cta, row_split; };
+WgradPartition wgrad3x3_partition(int B, int H, int W, int Cin, int Cout, bool two_plane);
 
 // wrot[ky,kx,co,ci] = w[2-ky,2-kx,ci,co]  (weights of the dgrad convolution)
 int rotate_weights(const float* w, float* wrot, int Cin, int Cout, cudaStream_t st);

@@ -385,23 +385,36 @@ int conv3x3_simt(const float* in0, const float* in1, const float* w, const float
   return check_launch("conv3x3_simt");
 }
 
+WgradPartition wgrad3x3_partition(int B, int H, int W, int Cin, int Cout, bool two_plane) {
+  const int tiles = B * (H / TH) * (W / TW);
+  WgradPartition p;
+  int ctas;
+  if (two_plane) {
+    ctas = min(tiles, kSmCount * 4 / (Cout / 64));
+    p.row_split = 256 / (2 * 16);
+  } else {
+    const int groups = (Cin / 16) * (Cout / 64);
+    ctas = max(1, min(tiles, (kSmCount * 4 + groups - 1) / groups));
+    p.row_split = 256 / (16 * 16);
+  }
+  p.tiles_per_cta = (tiles + ctas - 1) / ctas;
+  p.ctas_x = (tiles + p.tiles_per_cta - 1) / p.tiles_per_cta;
+  return p;
+}
+
 int wgrad3x3_simt(const float* x0, const float* x1, const float* g, float* dW, float* db, int B, int H, int W, int Cin,
                   int Cout, cudaStream_t st) {
   UDH_REQUIRE(H % TH == 0 && W % TW == 0 && Cout % 64 == 0, "wgrad3x3: unsupported shape");
-  const int tiles = B * (H / TH) * (W / TW);
   if (x1) {
     UDH_REQUIRE(Cin == 2, "wgrad3x3: two-plane input needs Cin == 2");
-    const int ctas = min(tiles, kSmCount * 4 / (Cout / 64));
-    const int per = (tiles + ctas - 1) / ctas;
-    dim3 grid((tiles + per - 1) / per, 1, Cout / 64);
-    wgrad3x3_kernel<2, true><<<grid, 256, 0, st>>>(x0, x1, g, dW, db, B, H, W, Cin, Cout, per);
+    const WgradPartition p = wgrad3x3_partition(B, H, W, Cin, Cout, true);
+    dim3 grid(p.ctas_x, 1, Cout / 64);
+    wgrad3x3_kernel<2, true><<<grid, 256, 0, st>>>(x0, x1, g, dW, db, B, H, W, Cin, Cout, p.tiles_per_cta);
   } else {
     UDH_REQUIRE(Cin % 16 == 0, "wgrad3x3: Cin must be a multiple of 16 (got %d)", Cin);
-    const int groups = (Cin / 16) * (Cout / 64);
-    const int ctas = max(1, min(tiles, (kSmCount * 4 + groups - 1) / groups));
-    const int per = (tiles + ctas - 1) / ctas;
-    dim3 grid((tiles + per - 1) / per, Cin / 16, Cout / 64);
-    wgrad3x3_kernel<16, false><<<grid, 256, 0, st>>>(x0, nullptr, g, dW, db, B, H, W, Cin, Cout, per);
+    const WgradPartition p = wgrad3x3_partition(B, H, W, Cin, Cout, false);
+    dim3 grid(p.ctas_x, Cin / 16, Cout / 64);
+    wgrad3x3_kernel<16, false><<<grid, 256, 0, st>>>(x0, nullptr, g, dW, db, B, H, W, Cin, Cout, p.tiles_per_cta);
   }
   return check_launch("wgrad3x3_simt");
 }

@@ -99,7 +99,7 @@ class HomographyEngine(object):
             self.load_flat(P.init_flat(seed, patch_size))
         self.ws_bytes = lib.udh_cnn_workspace_bytes(self.B, self.Pz, self.numeric)
         if self.ws_bytes == 0:
-            raise _lib.UdhError("unsupported batch / patch size (%d, %d)" % (self.B, self.Pz))
+            raise _lib.UdhError("unsupported batch / patch size (%d, %d): %s" % (self.B, self.Pz, lib.udh_last_error().decode()))
         self.ws = self._alloc(self.ws_bytes, torch.uint8)
         check(lib.udh_cnn_workspace_init(self._p(self.ws), self.ws_bytes, self.B, self.Pz, self.numeric, ops._stream()),
               "udh_cnn_workspace_init")
