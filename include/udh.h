@@ -540,6 +540,40 @@ int udh_mosaic_exposure_stats_u8(const uint8_t* const* frames, const int32_t* si
                                  const int32_t* pair_ptr, const int32_t* pair_j, int npairs, const double* history, int feeds,
                                  int norms, int dst_h, int dst_w, uint64_t* stats, void* ws, size_t ws_bytes, void* stream);
 
+/* ---- seam finding (cv2.detail's Voronoi seam finder; oracle/seam.py restates the rule) -------------------------------
+ * udh_mosaic_seam_masks_u8: the seams between udh_mosaic_multiband_u8's frames (frames, sizes, M frame -> ROI (device),
+ *   rois (host), as that call takes them), byte for byte what cv2.detail.SeamFinder_createDefault(VORONOI_SEAM).find
+ *   leaves in their validity masks.  Each frame's mask starts as its ROI warp's validity (255 / 0).  Then, for every pair
+ *   in the CSR list pair_ptr [n + 1], pair_j (host int32; row i, ascending j > i; the pairs must have intersecting ROIs;
+ *   list every such pair for cv2's result), in that order, on the masks as the earlier pairs left them: over the ROIs'
+ *   intersection grown by 10 px (s_i: frame i's mask inside its ROI, 0 outside), d_i is the exact L1 distance to the
+ *   nearest pixel held by frame i alone (infinite if there is none), likewise d_j; over the intersection, frame j's mask
+ *   is cleared where d_i < d_j and frame i's elsewhere.  seam [sum of roi_h roi_w] uint8 (device) receives the masks,
+ *   frame k's rh x rw bytes at offset sum_{l<k} roi_h_l roi_w_l; blend (same layout) the blend masks cv2's stitcher feeds
+ *   its blender: the 3 x 3 dilation of the seam mask AND the validity.  Launches 2 + 2 (pairs).  n <= UDH_SEAM_MAX_FRAMES,
+ *   sides < 32767.  ws: udh_mosaic_seam_workspace_bytes(rois, n, pair_ptr, pair_j, dst_h, dst_w) bytes of device memory
+ *   (0: bad arguments).
+ * udh_mosaic_blend_masked_u8: udh_mosaic_blend_u8 (udh_mosaic_blend_gain_u8 when gains is not null) where frame k counts
+ *   only at the pixels its blend mask holds: masks [n] (host array of device pointers), frame k's uint8 mask on the
+ *   rectangle rois[k] (host int32 [n,4], x_lo, y_lo, x_hi, y_hi inside the canvas; an empty rectangle keeps the frame out,
+ *   its pointer may be null).  ws: udh_mosaic_blend_masked_workspace_bytes(n) bytes of device memory.
+ * udh_mosaic_multiband_masked_u8: udh_mosaic_multiband_u8 (with gains when not null) fed masks[k] (host array of device
+ *   pointers, frame k's roi_h x roi_w blend mask) in place of each frame's validity mask.  Same workspace. */
+#define UDH_SEAM_MAX_FRAMES 1024
+size_t udh_mosaic_seam_workspace_bytes(const int32_t* rois, int n, const int32_t* pair_ptr, const int32_t* pair_j, int dst_h,
+                                       int dst_w);
+int udh_mosaic_seam_masks_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const int32_t* rois, int n,
+                             const int32_t* pair_ptr, const int32_t* pair_j, int dst_h, int dst_w, uint8_t* seam, uint8_t* blend,
+                             void* ws, size_t ws_bytes, void* stream);
+size_t udh_mosaic_blend_masked_workspace_bytes(int n);
+int udh_mosaic_blend_masked_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains,
+                               const uint8_t* const* masks, const int32_t* rois, int n, int c, const int32_t* tile_ptr,
+                               const int32_t* tile_frames, int dst_h, int dst_w, int feather, uint8_t* dst, uint8_t* mask, void* ws,
+                               size_t ws_bytes, void* stream);
+int udh_mosaic_multiband_masked_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains,
+                                   const uint8_t* const* masks, const int32_t* rois, int n, int c, int dst_h, int dst_w, int bands,
+                                   uint8_t* dst, uint8_t* mask, void* ws, size_t ws_bytes, void* stream);
+
 /* ---- instrumentation read by bench.py -------------------------------------------------------------------------
  * udh_launch_count: kernels this library has launched in this process (monotonic).
  * udh_prof_*: when enabled, every tagged phase is bracketed by CUDA events recorded on the launching stream;

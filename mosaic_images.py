@@ -16,18 +16,22 @@ the blend (cv2.detail_GainCompensator / ChannelsCompensator's rule with --compen
 one per channel, which also evens out white balance.  An exposure step between frames is otherwise left in the mosaic.
 cv2's rule pulls every gain towards 1, so one feed removes only part of a step; each further feed removes part of what
 is left (on a sweep with exposures 0.75 / 1 / 1.3, four gain-mode feeds recover the gain ratios to within 1 %).
+--seam voronoi cuts seams between the frames before the blend (cv2.detail's Voronoi seam finder, byte for byte): each
+pixel of an overlap goes to one frame, so the blend no longer averages two drifted frames into a double image across
+the whole overlap; with --blend multiband only the low frequencies are spread across the seam.
 
 Writes in --out_dir:
   pairs.txt    `frame_k frame_k+1` and H's nine entries per consecutive pair, as align_images.py's homographies.txt;
   refine.txt   with refinement, `frame_k frame_k+1 rho status levels` per pair, as align_images.py writes it;
   mosaic.txt   `canvas Hc Wc ref r` (` blend multiband B` appended with --blend multiband, then ` compensate MODE F` with
-               --compensate), then `name kept|dropped` and the nine entries of M_k (frame k -> canvas) per frame,
+               --compensate, then ` seam voronoi` with --seam voronoi), then `name kept|dropped` and the nine entries of M_k (frame k -> canvas) per frame,
                '%.9g' of their float32 values; the blend uses those float32 values.  With --compensate each frame line
                ends in its three gains, '%.17g' (exact); so the file reproduces mosaic.jpg;
   mosaic.jpg   the mosaic (BGR, JPEG quality 95, byte-identical to cv2.imencode of the same pixels).
 A frame whose grown corners map behind the reference camera is dropped.  The canvas must be one the JPEG encoder takes
 (about 110 MP in colour); a larger one stops with an error naming the frame that reaches farthest.  Prints the GPU time
-of each phase (CUDA events: prep, forward, refine, compensate, blend, encode; the blend named when it is multi-band).
+of each phase (CUDA events: prep, forward, refine, compensate, seam, blend, encode; the blend named when it is
+multi-band).
 """
 from __future__ import absolute_import, division, print_function
 
@@ -57,6 +61,8 @@ def build_parser():
     p.add_argument('--compensate_feeds', type=int, default=1,
                    help='feeds of the exposure compensator, 1..16; one feed removes only part of an exposure step (the '
                         'rule pulls every gain towards 1), several (e.g. 4) remove nearly all of it')
+    p.add_argument('--seam', type=str, default='none', choices=['none', 'voronoi'],
+                   help='seams between the frames before the blend: none, or cv2.detail\'s Voronoi seam finder')
     p.add_argument('--out_dir', type=str, default='mosaic')
     return p
 
@@ -94,6 +100,9 @@ def run(args, est, decode, encode):
                   max_side=args.refine_max_side) if refining else None
     compensating = args.compensate != "none"
     comp = dict(compensate=args.compensate, compensate_feeds=args.compensate_feeds) if compensating else {}
+    seaming = args.seam != "none"
+    if seaming:
+        comp["seam"] = args.seam
     imgs = decode(paths)
     try:
         out = mosaic.build_mosaic(est, imgs, None if args.ref_frame < 0 else args.ref_frame, refine, args.feather,
@@ -109,7 +118,8 @@ def run(args, est, decode, encode):
             f.write("".join("%s %s %.9g %d %d\n" % (names[k], names[k + 1], rho[k], status[k], level[k]) for k in range(len(H))))
     Hc, Wc = out["mask"].shape
     lines = ["canvas %d %d ref %d" % (Hc, Wc, out["ref"]) + (" blend multiband %d" % args.bands if args.blend == "multiband" else "") +
-             (" compensate %s %d" % (args.compensate, args.compensate_feeds) if compensating else "")]
+             (" compensate %s %d" % (args.compensate, args.compensate_feeds) if compensating else "") +
+             (" seam %s" % args.seam if seaming else "")]
     for k, nm in enumerate(names):
         lines.append(" ".join([nm, "kept" if out["kept"][k] else "dropped"] +
                               ["%.9g" % v for v in align.homography_as_written(out["M"][k])[0]] +
@@ -129,12 +139,13 @@ def run(args, est, decode, encode):
         f.write(blob)
     cover = float((out["mask"] != 0).float().mean())
     print("===> %d frames (%d kept) on a %dx%d canvas (ref %s, %.1f %% covered): GPU %.3f ms (prep %.3f, forward %.3f, %s%s"
-          "%sblend %.3f, encode %.3f)" % (len(names), int(np.sum(out["kept"])), Hc, Wc, names[out["ref"]], 100 * cover,
-                                          sum(ms.values()), ms["prep"], ms["forward"],
-                                          "refine %.3f, " % ms["refine"] if refining else "",
-                                          "compensate %.3f, " % ms["compensate"] if compensating else "",
-                                          "multiband %d " % args.bands if args.blend == "multiband" else "", ms["blend"],
-                                          ms["encode"]), flush=True)
+          "%s%sblend %.3f, encode %.3f)" % (len(names), int(np.sum(out["kept"])), Hc, Wc, names[out["ref"]], 100 * cover,
+                                            sum(ms.values()), ms["prep"], ms["forward"],
+                                            "refine %.3f, " % ms["refine"] if refining else "",
+                                            "compensate %.3f, " % ms["compensate"] if compensating else "",
+                                            "seam %.3f, " % ms["seam"] if seaming else "",
+                                            "multiband %d " % args.bands if args.blend == "multiband" else "", ms["blend"],
+                                            ms["encode"]), flush=True)
     return out
 
 

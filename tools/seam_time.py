@@ -1,0 +1,131 @@
+"""Seam-finding timing, in one run on the GPU, on the synthetic camera sweeps of tools/mosaic_time.py (32 x 1080x1920 and
+16 x 3000x4000 RGB frames, about 60 % overlap between neighbours, placed with their true homographies):
+  * udh_mosaic_seam_masks_u8 (validity, every intersecting pair's column and row pass, blend masks), CUDA events over
+    repeated calls with the frame table and pair list built once; its launch count (udh_launch_count), the pairs, and
+    the seam stage alone with the validity and blend-mask launches subtracted (one call without pairs);
+  * the blends with and without blend masks: udh_mosaic_blend_u8 / udh_mosaic_blend_masked_u8 (feather 64) and
+    udh_mosaic_multiband_u8 / udh_mosaic_multiband_masked_u8 (5 bands), CUDA events over repeated launches;
+  * cv2.detail's Voronoi seam finder on the same validity masks (the oracle, CPU) with cv2.setNumThreads(1) and (16);
+    the masks are made once and not timed.
+Prints one JSON line with the card name, power limit and maximum SM clock read in the same run.
+
+    python tools/seam_time.py
+"""
+import ctypes
+import json
+import os
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
+
+from oracle import seam as SM  # noqa: E402
+from tools import jpeg_time, mosaic_time  # noqa: E402
+from tools.exposure_time import _p, _stream, events_ms  # noqa: E402
+from unsuperviseddeephomographyral2018_b200 import _lib, mosaic, ops  # noqa: E402
+
+
+def seam_time(dev, M, canvas, reps=5):
+    Hc, Wc = canvas
+    n = len(dev)
+    sizes = [tuple(int(v) for v in t.shape[:2]) for t in dev]
+    rois, Mr = mosaic.multiband_rois(M, sizes, Hc, Wc)
+    rr = np.ascontiguousarray(rois.astype(np.int32))
+    Mr_d = torch.from_numpy(np.ascontiguousarray(Mr.reshape(n, 9))).cuda()
+    sz = np.ascontiguousarray(np.array(sizes, np.int32))
+    ptrs = (ctypes.c_void_p * n)(*[t.data_ptr() for t in dev])
+    area = ((rr[:, 2] - rr[:, 0]) * (rr[:, 3] - rr[:, 1])).astype(np.int64)
+    seam = torch.empty(int(area.sum()), dtype=torch.uint8, device="cuda")
+    blend = torch.empty_like(seam)
+    res = {}
+    for label, (ptr, pj) in (("seam", ops.seam_pairs(rr)), ("no_pairs", (np.zeros(n + 1, np.int32), np.zeros(1, np.int32)))):
+        nb = _lib.lib.udh_mosaic_seam_workspace_bytes(rr.ctypes.data, n, ptr.ctypes.data, pj.ctypes.data, Hc, Wc)
+        ws = torch.empty(nb, dtype=torch.uint8, device="cuda")
+        call = lambda: _lib.check(_lib.lib.udh_mosaic_seam_masks_u8(
+            ptrs, sz.ctypes.data, _p(Mr_d), rr.ctypes.data, n, ptr.ctypes.data, pj.ctypes.data, Hc, Wc, _p(seam), _p(blend), _p(ws), nb,
+            _stream()), "udh_mosaic_seam_masks_u8")
+        l0 = _lib.lib.udh_launch_count()
+        call()
+        torch.cuda.synchronize()
+        res[label + "_launches"] = int(_lib.lib.udh_launch_count() - l0)
+        res[label + "_ms"] = events_ms(call, reps)
+        if label == "seam":
+            res["pairs"] = int(ptr[-1])
+            res["workspace_mb"] = nb / 2 ** 20
+    res["pair_loop_ms"] = res["seam_ms"] - res["no_pairs_ms"]
+    res["pair_loop_us_per_pair"] = 1e3 * res["pair_loop_ms"] / max(res["pairs"], 1)
+    return res, [blend[int(a):int(b)] for a, b in zip(np.concatenate([[0], np.cumsum(area)[:-1]]), np.cumsum(area))]
+
+
+def blend_time(dev, M, canvas, bmasks, reps=10):
+    Hc, Wc = canvas
+    n = len(dev)
+    sizes = [tuple(int(v) for v in t.shape[:2]) for t in dev]
+    out_img = torch.empty(Hc, Wc, 3, dtype=torch.uint8, device="cuda")
+    mask = torch.empty(Hc, Wc, dtype=torch.uint8, device="cuda")
+    ptrs = (ctypes.c_void_p * n)(*[t.data_ptr() for t in dev])
+    mptrs = (ctypes.c_void_p * n)(*[t.data_ptr() for t in bmasks])
+    sz = np.ascontiguousarray(np.array(sizes, np.int32))
+    rois, Mr = mosaic.multiband_rois(M, sizes, Hc, Wc)
+    rr = np.ascontiguousarray(rois.astype(np.int32))
+    res = {}
+    ptr, idx = ops.mosaic_tile_lists(M, sizes, Hc, Wc)
+    ptr_d, idx_d = torch.from_numpy(ptr).cuda(), torch.from_numpy(idx).cuda()
+    M_d = torch.from_numpy(np.ascontiguousarray(M.reshape(n, 9))).cuda()
+    nb = _lib.lib.udh_mosaic_blend_masked_workspace_bytes(n)
+    ws = torch.empty(nb, dtype=torch.uint8, device="cuda")
+    res["feather_ms"] = events_ms(lambda: _lib.check(_lib.lib.udh_mosaic_blend_u8(
+        ptrs, sz.ctypes.data, _p(M_d), n, 3, _p(ptr_d), _p(idx_d), Hc, Wc, 64, _p(out_img), _p(mask), _p(ws), nb, _stream())), reps)
+    res["feather_masked_ms"] = events_ms(lambda: _lib.check(_lib.lib.udh_mosaic_blend_masked_u8(
+        ptrs, sz.ctypes.data, _p(M_d), None, mptrs, rr.ctypes.data, n, 3, _p(ptr_d), _p(idx_d), Hc, Wc, 64, _p(out_img), _p(mask),
+        _p(ws), nb, _stream())), reps)
+    Mr_d = torch.from_numpy(np.ascontiguousarray(Mr.reshape(n, 9))).cuda()
+    nb = _lib.lib.udh_mosaic_multiband_workspace_bytes(rr.ctypes.data, n, Hc, Wc, 5)
+    ws = torch.empty(nb, dtype=torch.uint8, device="cuda")
+    res["multiband_ms"] = events_ms(lambda: _lib.check(_lib.lib.udh_mosaic_multiband_u8(
+        ptrs, sz.ctypes.data, _p(Mr_d), rr.ctypes.data, n, 3, Hc, Wc, 5, _p(out_img), _p(mask), _p(ws), nb, _stream())), reps)
+    res["multiband_masked_ms"] = events_ms(lambda: _lib.check(_lib.lib.udh_mosaic_multiband_masked_u8(
+        ptrs, sz.ctypes.data, _p(Mr_d), None, mptrs, rr.ctypes.data, n, 3, Hc, Wc, 5, _p(out_img), _p(mask), _p(ws), nb,
+        _stream())), reps)
+    return res
+
+
+def cv2_time(frames, M, canvas):
+    import cv2
+    _, _, masks, tls = SM.fed(frames, M, canvas[0], canvas[1])
+    out = {}
+    for t in (1, 16):
+        cv2.setNumThreads(t)
+        t0 = time.perf_counter()
+        SM.cv2_seams(masks, tls)
+        out["cv2_seam_ms_threads_%d" % t] = (time.perf_counter() - t0) * 1e3
+    cv2.setNumThreads(-1)
+    return out
+
+
+def main():
+    torch.cuda.set_device(0)
+    out = {"gpu": torch.cuda.get_device_name(0), "card": jpeg_time.card()}
+    for n, h, w in ((32, 1080, 1920), (16, 3000, 4000)):
+        frames, M, canvas = mosaic_time.placed_sweep(n, h, w)
+        dev = [torch.from_numpy(f).cuda() for f in frames]
+        r = {"canvas": list(canvas)}
+        s, bm = seam_time(dev, M, canvas)
+        r.update(s)
+        r.update(blend_time(dev, M, canvas, bm))
+        print(json.dumps(r), flush=True)
+        r.update(cv2_time(frames, M, canvas))
+        out["sweep_%dx%dx%d" % (n, h, w)] = r
+        print(json.dumps(r), flush=True)
+        del frames, dev, bm
+        torch.cuda.empty_cache()
+    print(json.dumps(out))
+
+
+if __name__ == "__main__":
+    main()

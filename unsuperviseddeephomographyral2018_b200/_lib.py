@@ -19,6 +19,7 @@ M_H_LOSS, M_BOUNDED_H_LOSS, M_NUM_FAIL, M_ACE = 0, 1, 2, 3
 ECC_OK, ECC_NAN, ECC_NOCONV = 0, 1, 2
 MOSAIC_TILE_H, MOSAIC_TILE_W = 16, 64            # UDH_MOSAIC_TILE_H / _W
 EXPOSURE_MAX_FRAMES, EXPOSURE_MAX_FEEDS, EXPOSURE_STATS = 1024, 16, 13   # UDH_EXPOSURE_MAX_FRAMES / _MAX_FEEDS / _STATS
+SEAM_MAX_FRAMES = 1024                            # UDH_SEAM_MAX_FRAMES
 
 class StepArgs(ctypes.Structure):
     """udh_step_args (include/udh.h)."""
@@ -189,6 +190,14 @@ SIGNATURES = {
     "udh_mosaic_exposure_workspace_bytes": (c_size_t, [c_int]),
     "udh_mosaic_exposure_stats_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int,
                                              c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "udh_mosaic_seam_workspace_bytes": (c_size_t, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int]),
+    "udh_mosaic_seam_masks_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p,
+                                         c_void_p, c_void_p, c_size_t, c_void_p]),
+    "udh_mosaic_blend_masked_workspace_bytes": (c_size_t, [c_int]),
+    "udh_mosaic_blend_masked_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
+                                           c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "udh_mosaic_multiband_masked_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                               c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "udh_draw_report_workspace_bytes": (c_size_t, [c_int]),
     "udh_draw_report_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_int, c_int, c_int,
                                    c_void_p]),

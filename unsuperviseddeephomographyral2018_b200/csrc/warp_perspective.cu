@@ -12,6 +12,8 @@
 // arithmetic, one IEEE division per pixel, is part of the rounding contract.
 // The sequence mosaic's blends (udh_mosaic_blend_u8 and udh_mosaic_multiband_u8, below) sample every frame with the same
 // coordinate and tap helpers.
+#include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdint>
 #include <vector>
@@ -128,6 +130,20 @@ __global__ void mosaic_invert_kernel(const double* __restrict__ M, MosaicFrame* 
   if (k < n) cv_invert3(M + (int64_t)k * 9, fr[k].mi);
 }
 
+// A frame's blend mask on the canvas (udh_mosaic_seam_masks_u8's output): 0 / 255 bytes on its ROI rectangle.  An empty
+// rectangle (rw = 0) masks the whole frame out.
+struct SeamMask {
+  const uint8_t* m;
+  int rx, ry, rw, rh;
+};
+
+__device__ __forceinline__ bool seam_mask_on(const SeamMask* __restrict__ sm, int x, int y) {
+  const int lx = x - __ldg(&sm->rx), ly = y - __ldg(&sm->ry), rw = __ldg(&sm->rw);
+  if ((unsigned)lx >= (unsigned)rw || (unsigned)ly >= (unsigned)__ldg(&sm->rh)) return false;
+  const uint8_t* m = reinterpret_cast<const uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&sm->m)));
+  return __ldg(m + (int64_t)ly * rw + lx) != 0;
+}
+
 // Exposure compensation's apply, cv2.multiply(uint8, double): saturate_u8(rint(v g)) in float64, ties to even.
 __device__ __forceinline__ int ex_apply(int v, double g) {
   return min(max(__double2int_rn(__dmul_rn((double)v, g)), 0), 255);
@@ -137,11 +153,12 @@ __device__ __forceinline__ int ex_apply(int v, double g) {
 // row.  The thread walks the tile's candidate frames, adds wt * v and wt of every frame valid at its pixels into 64-bit
 // registers and stores the pixels once: no atomics, no accumulation buffer.  Integer sums: the result does not depend on
 // the frames' order.  GAIN: each frame's value is first compensated, ex_apply(v, gains[f][c]) (channel 0's gain when C = 1).
-template <int C, bool GAIN>
+// MASK: a frame counts only where its blend mask smask[f] is set as well.
+template <int C, bool GAIN, bool MASK = false>
 __device__ __forceinline__ void mosaic_blend_tile(const MosaicFrame* __restrict__ fr, int n, const int32_t* __restrict__ tile_ptr,
                                                   const int32_t* __restrict__ tile_frames, int dh, int dw, int bw, int feather32,
                                                   const double* __restrict__ gains, uint8_t* __restrict__ dst,
-                                                  uint8_t* __restrict__ mask) {
+                                                  uint8_t* __restrict__ mask, const SeamMask* __restrict__ smask = nullptr) {
   const int y = blockIdx.y * UDH_MOSAIC_TILE_H + threadIdx.x / (UDH_MOSAIC_TILE_W / 4);
   const int x0 = blockIdx.x * UDH_MOSAIC_TILE_W + threadIdx.x % (UDH_MOSAIC_TILE_W / 4) * 4;
   if (y >= dh || x0 >= dw) return;
@@ -170,7 +187,7 @@ __device__ __forceinline__ void mosaic_blend_tile(const MosaicFrame* __restrict_
       if (k >= np) break;
       int X, Y;
       const double Wd = wp_coords(mi, x0 + k, y, bw, X, Y);
-      if (Wd != 0.0 && X >= 0 && X <= xm && Y >= 0 && Y <= ym) {
+      if (Wd != 0.0 && X >= 0 && X <= xm && Y >= 0 && Y <= ym && (!MASK || seam_mask_on(smask + f, x0 + k, y))) {
         const int wt = 1 + min(min(min(X, xm - X), min(Y, ym - Y)), feather32);
         int v[C];
         wp_sample<C>(s, h, w, X, Y, v);
@@ -231,6 +248,16 @@ __global__ void __launch_bounds__(256) exposure_blend_u8_kernel(const MosaicFram
   mosaic_blend_tile<C, true>(fr, n, tile_ptr, tile_frames, dh, dw, bw, feather32, gains, dst, mask);
 }
 
+// The feathered blend with each frame kept only where its blend mask is set (GAIN: of exposure-compensated frames).
+template <int C, bool GAIN>
+__global__ void __launch_bounds__(256) seam_blend_u8_kernel(const MosaicFrame* __restrict__ fr, int n, const int32_t* __restrict__ tile_ptr,
+                                                            const int32_t* __restrict__ tile_frames, int dh, int dw, int bw,
+                                                            int feather32, const double* __restrict__ gains,
+                                                            const SeamMask* __restrict__ smask, uint8_t* __restrict__ dst,
+                                                            uint8_t* __restrict__ mask) {
+  mosaic_blend_tile<C, GAIN, true>(fr, n, tile_ptr, tile_frames, dh, dw, bw, feather32, gains, dst, mask, smask);
+}
+
 // ---- multi-band blend: cv2.detail_MultiBandBlender with CV_16S weights (the rule: oracle/multiband.py) ----------------
 // Per frame k, its fed rectangle (ROI grown by the gap, aligned to 2^B) holds the image pyramid G_i (uchar4, RGB + pad)
 // and the weight pyramid W_i (int16) in two pools; the canvas pyramid keeps (acc, wacc) as short4 per pixel, and the
@@ -243,6 +270,7 @@ struct MultibandFrame {
   int rx, ry, rw, rh, bw;          // its ROI on the canvas, and the ROI warp's tile width
   int x0, y0, pw, ph;              // the fed rectangle at level 0 (canvas coordinates; multiples of 2^B)
   int64_t off[MB_MAX_BANDS + 1];   // element offset of level i in the G and W pools
+  const uint8_t* bmask;            // null, or the frame's blend mask on its ROI (rh x rw, 0 / 255): the weight's mask
 };
 
 // BORDER_REFLECT (fedcba|abcdef|fedcba) for any n >= 1, folding as often as needed.
@@ -280,7 +308,8 @@ __device__ __forceinline__ bool mb_roi_warp(const uint8_t* __restrict__ s, int h
 
 // Level 0 of every frame: the ROI warp bordered with BORDER_REFLECT, and the 0 / 256 weight with a constant 0 border.
 // gains (null: none) [n][3]: the ROI warp is exposure-compensated first, ex_apply(v, gains[k][c]), as cv2's stitcher
-// applies its compensator to the whole warped image before it feeds the blender.
+// applies its compensator to the whole warped image before it feeds the blender.  A frame with a blend mask (bmask) takes
+// its weight from that mask instead of the warp's validity.
 __global__ void __launch_bounds__(256) multiband_base_kernel(const MultibandFrame* __restrict__ fr, const double* __restrict__ M,
                                                              const double* __restrict__ gains, uchar4* __restrict__ G,
                                                              int16_t* __restrict__ Wt) {
@@ -294,6 +323,7 @@ __global__ void __launch_bounds__(256) multiband_base_kernel(const MultibandFram
   const int bw = __ldg(&F->bw), ox = __ldg(&F->x0) - rx, oy = __ldg(&F->y0) - ry, pw = __ldg(&F->pw);
   const int npx = pw * __ldg(&F->ph);                                 // < 2^31: padded sides < 32767 + 1024
   const int64_t off = __ldg(&F->off[0]);
+  const uint8_t* bm = reinterpret_cast<const uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&F->bmask)));
   double g[3];
   if (gains) {
 #pragma unroll
@@ -304,7 +334,8 @@ __global__ void __launch_bounds__(256) multiband_base_kernel(const MultibandFram
     const int ix = x + ox, iy = y + oy;
     const int sx = mb_reflect(ix, rw), sy = mb_reflect(iy, rh);
     int v[3];
-    const bool valid = mb_roi_warp(s, h, w, mi, sx, sy, bw, v) && ix == sx && iy == sy;
+    bool valid = mb_roi_warp(s, h, w, mi, sx, sy, bw, v) && ix == sx && iy == sy;
+    if (bm) valid = ix == sx && iy == sy && __ldg(bm + (int64_t)sy * rw + sx) != 0;
     if (gains) {
 #pragma unroll
       for (int c = 0; c < 3; ++c) v[c] = ex_apply(v[c], g[c]);
@@ -686,6 +717,219 @@ __global__ void __launch_bounds__(256) exposure_stats_kernel(const ExposureFrame
   }
 }
 
+// ---- seam finding: cv2.detail's Voronoi seam finder on the ROI validity masks (the rule: oracle/seam.py) ---------------
+// Every fed frame's mask lives on its ROI (rh x rw bytes at element offset off of a pool).  The pairs are visited on the host
+// in cv2's order; each pair runs two kernels over its window (the ROIs' intersection grown by SEAM_GAP): the column pass
+// gives each window pixel its distance along the column to the nearest unique pixel of either frame, and the row pass
+// turns that into the exact L1 distance (min over x' of g(x') + |x - x'|, a prefix and a suffix minimum) and clears one
+// frame's mask at every pixel of the intersection.  All in int32: SEAM_INF marks "no source" and survives the adds
+// (distances are below 2^17, the window's sides below 32767 + 2 SEAM_GAP).
+constexpr int SEAM_GAP = 10, SEAM_INF = 1 << 30, SEAM_SEGS = 16, SEAM_ROW_THREADS = 256;
+
+struct SeamFrame {
+  const uint8_t* src;
+  int h, w;
+  int rx, ry, rw, rh, bw;          // the ROI on the canvas and the ROI warp's tile width
+  int64_t off;                     // the ROI's element offset in the mask pools
+};
+
+struct SeamRect {                  // a frame's ROI and pool offset, passed by value to the pair kernels
+  int64_t off;
+  int rx, ry, rw, rh;
+};
+
+// Every frame's ROI validity (udh_mosaic_multiband_u8's mask, mb_roi_warp's rule), 0 / 255, into both pools.
+__global__ void __launch_bounds__(256) seam_valid_kernel(const SeamFrame* __restrict__ fr, const double* __restrict__ M,
+                                                         uint8_t* __restrict__ seam, uint8_t* __restrict__ blend) {
+  __shared__ double mi[9];
+  const int k = blockIdx.y;
+  if (threadIdx.x == 0) cv_invert3(M + (int64_t)k * 9, mi);
+  __syncthreads();
+  const SeamFrame* F = fr + k;
+  const uint8_t* s = reinterpret_cast<const uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&F->src)));
+  const int h = __ldg(&F->h), w = __ldg(&F->w), rw = __ldg(&F->rw), bw = __ldg(&F->bw), npx = rw * __ldg(&F->rh);
+  const int64_t off = __ldg(&F->off);
+  for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < npx; e += gridDim.x * blockDim.x) {
+    const int y = e / rw, x = e - y * rw;
+    int X, Y;
+    const double Wd = wp_coords(mi, x, y, bw, X, Y);
+    const uint8_t v = Wd != 0.0 && X >= 0 && X <= 32 * (w - 1) && Y >= 0 && Y <= 32 * (h - 1) ? 255 : 0;
+    seam[off + e] = v;
+    blend[off + e] = v;
+  }
+}
+
+__device__ __forceinline__ bool seam_at(const uint8_t* __restrict__ seam, const SeamRect& r, int cx, int cy) {
+  const int lx = cx - r.rx, ly = cy - r.ry;
+  return (unsigned)lx < (unsigned)r.rw && (unsigned)ly < (unsigned)r.rh && seam[r.off + (int64_t)ly * r.rw + lx] != 0;
+}
+
+// The pair's unique pixels at window pixel (x, y): bit 0 frame a's, bit 1 frame b's (a pixel both masks hold is neither's).
+__device__ __forceinline__ int seam_unique(const uint8_t* __restrict__ seam, const SeamRect& a, const SeamRect& b, int cx, int cy) {
+  const bool sa = seam_at(seam, a, cx, cy), sb = seam_at(seam, b, cx, cy);
+  return (sa && !sb ? 1 : 0) | (sb && !sa ? 2 : 0);
+}
+
+// Column pass: a CTA takes 32 window columns (one per lane, so every row's loads and stores are coalesced) and splits the
+// window's height into SEAM_SEGS segments, one per warp.  Each thread first finds the first and last unique row of its
+// segment for both frames; the CTA shares them, so every thread knows the nearest unique row above and below its segment;
+// then it scans its segment down (distance to the nearest source above) and up (below) and stores the minimum, g.
+__global__ void __launch_bounds__(32 * SEAM_SEGS) seam_column_kernel(const uint8_t* __restrict__ seam, SeamRect a, SeamRect b,
+                                                                     int wx0, int wy0, int ww, int wh, int* __restrict__ ga,
+                                                                     int* __restrict__ gb) {
+  __shared__ int first[2][SEAM_SEGS][32], last[2][SEAM_SEGS][32];
+  const int lane = threadIdx.x, seg = threadIdx.y, x = blockIdx.x * 32 + lane;
+  const int len = (wh + SEAM_SEGS - 1) / SEAM_SEGS, y0 = min(seg * len, wh), y1 = min(y0 + len, wh);
+  int fa = -1, la = -1, fb = -1, lb = -1;
+  if (x < ww) {
+    for (int y = y0; y < y1; ++y) {
+      const int u = seam_unique(seam, a, b, wx0 + x, wy0 + y);
+      if (u & 1) { if (fa < 0) fa = y; la = y; }
+      if (u & 2) { if (fb < 0) fb = y; lb = y; }
+    }
+  }
+  first[0][seg][lane] = fa; last[0][seg][lane] = la;
+  first[1][seg][lane] = fb; last[1][seg][lane] = lb;
+  __syncthreads();
+  if (x >= ww) return;
+  int up[2] = {-1, -1}, dn[2] = {-1, -1};                          // nearest unique row above / below the segment
+#pragma unroll
+  for (int f = 0; f < 2; ++f) {
+    for (int q = 0; q < seg; ++q)
+      if (last[f][q][lane] >= 0) up[f] = last[f][q][lane];
+    for (int q = SEAM_SEGS - 1; q > seg; --q)
+      if (first[f][q][lane] >= 0) dn[f] = first[f][q][lane];
+  }
+  int pa = up[0], pb = up[1];
+  for (int y = y0; y < y1; ++y) {
+    const int u = seam_unique(seam, a, b, wx0 + x, wy0 + y);
+    if (u & 1) pa = y;
+    if (u & 2) pb = y;
+    const int64_t e = (int64_t)y * ww + x;
+    ga[e] = pa >= 0 ? y - pa : SEAM_INF;
+    gb[e] = pb >= 0 ? y - pb : SEAM_INF;
+  }
+  int na = dn[0], nb = dn[1];
+  for (int y = y1 - 1; y >= y0; --y) {
+    const int u = seam_unique(seam, a, b, wx0 + x, wy0 + y);
+    if (u & 1) na = y;
+    if (u & 2) nb = y;
+    const int64_t e = (int64_t)y * ww + x;
+    if (na >= 0) ga[e] = min(ga[e], na - y);
+    if (nb >= 0) gb[e] = min(gb[e], nb - y);
+  }
+}
+
+__device__ __forceinline__ int2 seam_min2(int2 p, int2 q) { return make_int2(min(p.x, q.x), min(p.y, q.y)); }
+
+// The minimum of v over the CTA's threads before this one (INT_MAX for thread 0), and over all of them (tot).
+__device__ __forceinline__ int2 seam_scan_exclusive(int2 v, int2* wtot, int2& tot) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int2 u = make_int2(__shfl_up_sync(0xffffffffu, v.x, o), __shfl_up_sync(0xffffffffu, v.y, o));
+    if (lane >= o) v = seam_min2(v, u);
+  }
+  int2 ex = make_int2(__shfl_up_sync(0xffffffffu, v.x, 1), __shfl_up_sync(0xffffffffu, v.y, 1));
+  if (lane == 0) ex = make_int2(INT_MAX, INT_MAX);
+  if (lane == 31) wtot[warp] = v;
+  __syncthreads();
+  tot = make_int2(INT_MAX, INT_MAX);
+#pragma unroll
+  for (int q = 0; q < SEAM_ROW_THREADS / 32; ++q) {
+    if (q < warp) ex = seam_min2(ex, wtot[q]);
+    tot = seam_min2(tot, wtot[q]);
+  }
+  __syncthreads();                                                  // wtot is rewritten by the next scan
+  return ex;
+}
+
+// Row pass: one CTA per row of the intersection (window row SEAM_GAP + r).  d(x) = min(x + P(x), S(x) - x) with P the
+// prefix minimum of g(x') - x' and S the suffix minimum of g(x') + x', both frames at once, 4 elements per thread per
+// chunk; P goes to this row's scratch (pa, pb) on the forward sweep, S is formed on the backward sweep, which also clears,
+// at every intersection pixel, frame b's mask where d_a < d_b and frame a's elsewhere (ties and two infinite distances).
+__global__ void __launch_bounds__(SEAM_ROW_THREADS) seam_row_kernel(uint8_t* __restrict__ seam, SeamRect a, SeamRect b, int wx0,
+                                                                    int wy0, int ww, int iw, const int* __restrict__ ga,
+                                                                    const int* __restrict__ gb, int* __restrict__ pa,
+                                                                    int* __restrict__ pb) {
+  __shared__ int2 wtot[SEAM_ROW_THREADS / 32];
+  const int y = SEAM_GAP + blockIdx.x;
+  const int* ra = ga + (int64_t)y * ww;
+  const int* rb = gb + (int64_t)y * ww;
+  int* qa = pa + (int64_t)blockIdx.x * ww;
+  int* qb = pb + (int64_t)blockIdx.x * ww;
+  constexpr int CHUNK = 4 * SEAM_ROW_THREADS;
+  int2 carry = make_int2(INT_MAX, INT_MAX), tot;
+  for (int c0 = 0; c0 < ww; c0 += CHUNK) {
+    int2 run[4], m = make_int2(INT_MAX, INT_MAX);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int x = c0 + 4 * threadIdx.x + q;
+      if (x < ww) m = seam_min2(m, make_int2(ra[x] - x, rb[x] - x));
+      run[q] = m;
+    }
+    const int2 ex = seam_min2(seam_scan_exclusive(m, wtot, tot), carry);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int x = c0 + 4 * threadIdx.x + q;
+      if (x < ww) {
+        const int2 p = seam_min2(run[q], ex);
+        qa[x] = p.x;
+        qb[x] = p.y;
+      }
+    }
+    carry = seam_min2(carry, tot);
+  }
+  __syncthreads();                                                  // P of the whole row is in place
+  carry = make_int2(INT_MAX, INT_MAX);
+  for (int c0 = 0; c0 < ww; c0 += CHUNK) {                          // e = ww - 1 - x: the suffix is a prefix in e
+    int2 run[4], m = make_int2(INT_MAX, INT_MAX);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int x = ww - 1 - (c0 + 4 * threadIdx.x + q);
+      if (x >= 0) m = seam_min2(m, make_int2(ra[x] + x, rb[x] + x));
+      run[q] = m;
+    }
+    const int2 ex = seam_min2(seam_scan_exclusive(m, wtot, tot), carry);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int x = ww - 1 - (c0 + 4 * threadIdx.x + q);
+      if (x < SEAM_GAP || x >= SEAM_GAP + iw) continue;
+      const int2 S = seam_min2(run[q], ex);
+      int da = min(x + qa[x], S.x - x), db = min(x + qb[x], S.y - x);
+      da = da >= SEAM_INF / 2 ? SEAM_INF : da;
+      db = db >= SEAM_INF / 2 ? SEAM_INF : db;
+      const int cx = wx0 + x, cy = wy0 + y;
+      if (da < db)
+        seam[b.off + (int64_t)(cy - b.ry) * b.rw + (cx - b.rx)] = 0;
+      else
+        seam[a.off + (int64_t)(cy - a.ry) * a.rw + (cx - a.rx)] = 0;
+    }
+    carry = seam_min2(carry, tot);
+  }
+}
+
+// The blend masks, in place over the validity the pool holds: cv2.dilate(seam, 3 x 3 rectangle; pixels outside the ROI
+// never win) AND the validity.
+__global__ void __launch_bounds__(256) seam_blend_mask_kernel(const SeamFrame* __restrict__ fr, const uint8_t* __restrict__ seam,
+                                                              uint8_t* __restrict__ blend) {
+  const SeamFrame* F = fr + blockIdx.y;
+  const int rw = __ldg(&F->rw), rh = __ldg(&F->rh), npx = rw * rh;
+  const int64_t off = __ldg(&F->off);
+  for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < npx; e += gridDim.x * blockDim.x) {
+    if (!blend[off + e]) continue;
+    const int y = e / rw, x = e - y * rw;
+    bool on = false;
+    for (int dy = -1; dy <= 1 && !on; ++dy)
+      for (int dx = -1; dx <= 1; ++dx)
+        if ((unsigned)(x + dx) < (unsigned)rw && (unsigned)(y + dy) < (unsigned)rh && seam[off + (int64_t)(y + dy) * rw + x + dx]) {
+          on = true;
+          break;
+        }
+    if (!on) blend[off + e] = 0;
+  }
+}
+
 }  // namespace udh
 
 using namespace udh;
@@ -712,19 +956,45 @@ extern "C" int udh_warp_perspective_u8(const uint8_t* src, const double* M, uint
 
 extern "C" size_t udh_mosaic_workspace_bytes(int n) { return n > 0 ? (size_t)n * sizeof(MosaicFrame) : 0; }
 
+extern "C" size_t udh_mosaic_blend_masked_workspace_bytes(int n) {
+  return n > 0 ? mb_align((size_t)n * sizeof(MosaicFrame)) + (size_t)n * sizeof(SeamMask) : 0;
+}
+
+// masks (null: none) with mrois [n,4]: each frame's blend mask on its rectangle (x_lo, y_lo, x_hi, y_hi); an empty one
+// keeps the frame out of the blend.
 static int mosaic_blend(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains, int n, int c,
                         const int32_t* tile_ptr, const int32_t* tile_frames, int dst_h, int dst_w, int feather, uint8_t* dst,
-                        uint8_t* mask, void* ws, size_t ws_bytes, void* stream) {
+                        uint8_t* mask, void* ws, size_t ws_bytes, void* stream, const uint8_t* const* masks = nullptr,
+                        const int32_t* mrois = nullptr) {
   UDH_REQUIRE(tile_ptr && tile_frames && dst && mask && (n == 0 || (frames && sizes && M && ws)), "udh_mosaic_blend_u8: null pointer");
   UDH_REQUIRE(c == 1 || c == 3, "udh_mosaic_blend_u8: channels must be 1 or 3 (got %d)", c);
   UDH_REQUIRE(n >= 0 && n <= 65535 && dst_h >= 1 && dst_w >= 1 && dst_h < 32767 && dst_w < 32767,
               "udh_mosaic_blend_u8: bad dimensions (n %d, canvas %dx%d)", n, dst_h, dst_w);
   UDH_REQUIRE(feather >= 0 && feather <= 1024, "udh_mosaic_blend_u8: feather must be in [0, 1024] (got %d)", feather);
-  if (ws_bytes < udh_mosaic_workspace_bytes(n)) {
-    set_error("udh_mosaic_blend_u8: workspace of %zu bytes, %zu needed", ws_bytes, udh_mosaic_workspace_bytes(n));
+  const size_t need = masks ? udh_mosaic_blend_masked_workspace_bytes(n) : udh_mosaic_workspace_bytes(n);
+  if (ws_bytes < need) {
+    set_error("udh_mosaic_blend_u8: workspace of %zu bytes, %zu needed", ws_bytes, need);
     return UDH_EWS;
   }
   const cudaStream_t st = as_stream(stream);
+  if (masks && n > 0) {
+    std::vector<SeamMask> sm((size_t)n, SeamMask{nullptr, 0, 0, 0, 0});
+    for (int k = 0; k < n; ++k) {
+      const int* r = mrois + 4 * k;
+      if (r[2] <= r[0] || r[3] <= r[1]) continue;
+      UDH_REQUIRE(r[0] >= 0 && r[1] >= 0 && r[2] <= dst_w && r[3] <= dst_h,
+                  "udh_mosaic_blend_masked_u8: frame %d's mask rectangle (%d, %d)..(%d, %d) leaves the %dx%d canvas", k, r[0], r[1],
+                  r[2], r[3], dst_h, dst_w);
+      UDH_REQUIRE(masks[k], "udh_mosaic_blend_masked_u8: frame %d's mask is a null pointer", k);
+      sm[k] = SeamMask{masks[k], r[0], r[1], r[2] - r[0], r[3] - r[1]};
+    }
+    const cudaError_t e = cudaMemcpyAsync(static_cast<char*>(ws) + mb_align((size_t)n * sizeof(MosaicFrame)), sm.data(),
+                                          (size_t)n * sizeof(SeamMask), cudaMemcpyHostToDevice, st);
+    if (e != cudaSuccess) {
+      set_error("udh_mosaic_blend_masked_u8: mask table copy: %s", cudaGetErrorString(e));
+      return UDH_ECUDA;
+    }
+  }
   if (n > 0) {
     std::vector<MosaicFrame> host((size_t)n);
     for (int k = 0; k < n; ++k) {
@@ -750,6 +1020,19 @@ static int mosaic_blend(const uint8_t* const* frames, const int32_t* sizes, cons
   const dim3 grid((unsigned)((dst_w + UDH_MOSAIC_TILE_W - 1) / UDH_MOSAIC_TILE_W),
                   (unsigned)((dst_h + UDH_MOSAIC_TILE_H - 1) / UDH_MOSAIC_TILE_H));
   const MosaicFrame* fr = static_cast<const MosaicFrame*>(ws);
+  if (masks) {
+    const SeamMask* sm = reinterpret_cast<const SeamMask*>(static_cast<const char*>(ws) + mb_align((size_t)n * sizeof(MosaicFrame)));
+    const int f32 = 32 * feather;
+    if (gains && c == 3)
+      seam_blend_u8_kernel<3, true><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, f32, gains, sm, dst, mask);
+    else if (gains)
+      seam_blend_u8_kernel<1, true><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, f32, gains, sm, dst, mask);
+    else if (c == 3)
+      seam_blend_u8_kernel<3, false><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, f32, nullptr, sm, dst, mask);
+    else
+      seam_blend_u8_kernel<1, false><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, f32, nullptr, sm, dst, mask);
+    return check_launch("udh_mosaic_blend_masked_u8");
+  }
   if (gains && c == 3)
     exposure_blend_u8_kernel<3><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, 32 * feather, gains, dst, mask);
   else if (gains)
@@ -794,7 +1077,7 @@ extern "C" int udh_debug_multiband_layout(const int32_t* rois, int n, int dst_h,
 
 static int mosaic_multiband(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains,
                             const int32_t* rois, int n, int c, int dst_h, int dst_w, int bands, uint8_t* dst, uint8_t* mask, void* ws,
-                            size_t ws_bytes, void* stream) {
+                            size_t ws_bytes, void* stream, const uint8_t* const* masks = nullptr) {
   UDH_REQUIRE(frames && sizes && M && rois && dst && mask && ws, "udh_mosaic_multiband_u8: null pointer");
   UDH_REQUIRE(c == 3, "udh_mosaic_multiband_u8: channels must be 3 (got %d)", c);
   MultibandPlan p;
@@ -807,6 +1090,10 @@ static int mosaic_multiband(const uint8_t* const* frames, const int32_t* sizes, 
   for (int k = 0; k < n; ++k) {
     UDH_REQUIRE(frames[k], "udh_mosaic_multiband_u8: frame %d is a null pointer", k);
     p.fr[k].src = frames[k];
+    if (masks) {
+      UDH_REQUIRE(masks[k], "udh_mosaic_multiband_masked_u8: frame %d's mask is a null pointer", k);
+      p.fr[k].bmask = masks[k];
+    }
   }
   const cudaStream_t st = as_stream(stream);
   char* base = static_cast<char*>(ws);
@@ -916,4 +1203,128 @@ extern "C" int udh_mosaic_exposure_stats_u8(const uint8_t* const* frames, const 
   exposure_stats_kernel<<<grid, 256, 0, st>>>(fr, n, pair_ptr, pair_j, history, feeds, norms,
                                               reinterpret_cast<unsigned long long*>(stats));
   return check_launch("udh_mosaic_exposure_stats_u8");
+}
+
+extern "C" int udh_mosaic_blend_masked_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains,
+                                          const uint8_t* const* masks, const int32_t* rois, int n, int c, const int32_t* tile_ptr,
+                                          const int32_t* tile_frames, int dst_h, int dst_w, int feather, uint8_t* dst, uint8_t* mask,
+                                          void* ws, size_t ws_bytes, void* stream) {
+  UDH_REQUIRE(n == 0 || (masks && rois), "udh_mosaic_blend_masked_u8: null masks or rois");
+  static const uint8_t* const none[1] = {nullptr};
+  return mosaic_blend(frames, sizes, M, gains, n, c, tile_ptr, tile_frames, dst_h, dst_w, feather, dst, mask, ws, ws_bytes, stream,
+                      n ? masks : none, rois);
+}
+
+extern "C" int udh_mosaic_multiband_masked_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains,
+                                              const uint8_t* const* masks, const int32_t* rois, int n, int c, int dst_h, int dst_w,
+                                              int bands, uint8_t* dst, uint8_t* mask, void* ws, size_t ws_bytes, void* stream) {
+  UDH_REQUIRE(masks, "udh_mosaic_multiband_masked_u8: null masks");
+  return mosaic_multiband(frames, sizes, M, gains, rois, n, c, dst_h, dst_w, bands, dst, mask, ws, ws_bytes, stream, masks);
+}
+
+// The host's plan of one seam call: the frame table, the pairs in visiting order with their windows, and the workspace.
+struct SeamPlan {
+  std::vector<SeamFrame> fr;
+  std::vector<int> pi, pj;
+  int64_t max_px = 0, max_win = 0, max_inner = 0;
+  size_t off_g, off_p, total;
+};
+
+static int seam_plan(const int32_t* rois, const int32_t* sizes, int n, const int32_t* pair_ptr, const int32_t* pair_j, int dst_h,
+                     int dst_w, SeamPlan& p) {
+  UDH_REQUIRE(rois && pair_ptr && (pair_j || !pair_ptr[n]), "udh_mosaic_seam_masks_u8: null pointer");
+  UDH_REQUIRE(n >= 1 && n <= UDH_SEAM_MAX_FRAMES && dst_h >= 1 && dst_w >= 1 && dst_h < 32767 && dst_w < 32767,
+              "udh_mosaic_seam_masks_u8: bad dimensions (n %d of at most %d, canvas %dx%d)", n, UDH_SEAM_MAX_FRAMES, dst_h, dst_w);
+  p.fr.assign((size_t)n, SeamFrame{});
+  int64_t off = 0;
+  for (int k = 0; k < n; ++k) {
+    const int* r = rois + 4 * k;
+    UDH_REQUIRE(r[0] >= 0 && r[1] >= 0 && r[0] < r[2] && r[1] < r[3] && r[2] <= dst_w && r[3] <= dst_h,
+                "udh_mosaic_seam_masks_u8: frame %d's ROI (%d, %d)..(%d, %d) is empty or leaves the %dx%d canvas", k, r[0], r[1], r[2],
+                r[3], dst_h, dst_w);
+    SeamFrame& F = p.fr[k];
+    F.rx = r[0]; F.ry = r[1]; F.rw = r[2] - r[0]; F.rh = r[3] - r[1];
+    const int bh = F.rh < 16 ? F.rh : 16;
+    F.bw = 1024 / bh < F.rw ? 1024 / bh : F.rw;                      // the ROI warp's tile width, as mb_plan sets it
+    F.off = off;
+    off += (int64_t)F.rw * F.rh;
+    if ((int64_t)F.rw * F.rh > p.max_px) p.max_px = (int64_t)F.rw * F.rh;
+    if (sizes) {
+      F.h = sizes[2 * k];
+      F.w = sizes[2 * k + 1];
+      UDH_REQUIRE(F.h >= 1 && F.w >= 1 && F.h < 32767 && F.w < 32767, "udh_mosaic_seam_masks_u8: frame %d is %dx%d", k, F.h, F.w);
+    }
+  }
+  UDH_REQUIRE(pair_ptr[0] == 0, "udh_mosaic_seam_masks_u8: pair_ptr[0] is %d", pair_ptr[0]);
+  for (int i = 0; i < n; ++i) {
+    UDH_REQUIRE(pair_ptr[i + 1] >= pair_ptr[i], "udh_mosaic_seam_masks_u8: pair_ptr decreases at frame %d", i);
+    for (int e = pair_ptr[i]; e < pair_ptr[i + 1]; ++e) {
+      const int j = pair_j[e];
+      UDH_REQUIRE(j > i && j < n && (e == pair_ptr[i] || j > pair_j[e - 1]),
+                  "udh_mosaic_seam_masks_u8: pair (%d, %d) is out of order or range", i, j);
+      const SeamFrame &A = p.fr[i], &B = p.fr[j];
+      const int iw = std::min(A.rx + A.rw, B.rx + B.rw) - std::max(A.rx, B.rx), ih = std::min(A.ry + A.rh, B.ry + B.rh) - std::max(A.ry, B.ry);
+      UDH_REQUIRE(iw > 0 && ih > 0, "udh_mosaic_seam_masks_u8: the ROIs of pair (%d, %d) do not intersect", i, j);
+      const int64_t ww = iw + 2 * SEAM_GAP, wh = ih + 2 * SEAM_GAP;
+      p.max_win = std::max(p.max_win, ww * wh);
+      p.max_inner = std::max(p.max_inner, ww * ih);
+      p.pi.push_back(i);
+      p.pj.push_back(j);
+    }
+  }
+  p.off_g = mb_align((size_t)n * sizeof(SeamFrame));
+  p.off_p = mb_align(p.off_g + 2 * (size_t)p.max_win * sizeof(int));
+  p.total = mb_align(p.off_p + 2 * (size_t)p.max_inner * sizeof(int));
+  return UDH_OK;
+}
+
+extern "C" size_t udh_mosaic_seam_workspace_bytes(const int32_t* rois, int n, const int32_t* pair_ptr, const int32_t* pair_j,
+                                                  int dst_h, int dst_w) {
+  SeamPlan p;
+  return seam_plan(rois, nullptr, n, pair_ptr, pair_j, dst_h, dst_w, p) == UDH_OK ? p.total : 0;
+}
+
+extern "C" int udh_mosaic_seam_masks_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const int32_t* rois, int n,
+                                        const int32_t* pair_ptr, const int32_t* pair_j, int dst_h, int dst_w, uint8_t* seam,
+                                        uint8_t* blend, void* ws, size_t ws_bytes, void* stream) {
+  UDH_REQUIRE(frames && sizes && M && seam && blend && ws, "udh_mosaic_seam_masks_u8: null pointer");
+  SeamPlan p;
+  int rc = seam_plan(rois, sizes, n, pair_ptr, pair_j, dst_h, dst_w, p);
+  if (rc != UDH_OK) return rc;
+  if (ws_bytes < p.total) {
+    set_error("udh_mosaic_seam_masks_u8: workspace of %zu bytes, %zu needed", ws_bytes, p.total);
+    return UDH_EWS;
+  }
+  for (int k = 0; k < n; ++k) {
+    UDH_REQUIRE(frames[k], "udh_mosaic_seam_masks_u8: frame %d is a null pointer", k);
+    p.fr[k].src = frames[k];
+  }
+  const cudaStream_t st = as_stream(stream);
+  char* base = static_cast<char*>(ws);
+  // pageable source: the copy is staged before this call returns, so `p` may go
+  const cudaError_t e = cudaMemcpyAsync(base, p.fr.data(), (size_t)n * sizeof(SeamFrame), cudaMemcpyHostToDevice, st);
+  if (e != cudaSuccess) {
+    set_error("udh_mosaic_seam_masks_u8: frame table copy: %s", cudaGetErrorString(e));
+    return UDH_ECUDA;
+  }
+  const SeamFrame* fr = reinterpret_cast<const SeamFrame*>(base);
+  int* ga = reinterpret_cast<int*>(base + p.off_g);
+  int* gb = ga + p.max_win;
+  int* pa = reinterpret_cast<int*>(base + p.off_p);
+  int* pb = pa + p.max_inner;
+  seam_valid_kernel<<<dim3(mb_blocks(p.max_px), (unsigned)n), 256, 0, st>>>(fr, M, seam, blend);
+  if ((rc = check_launch("udh_mosaic_seam_masks_u8 (validity)")) != UDH_OK) return rc;
+  for (size_t q = 0; q < p.pi.size(); ++q) {
+    const SeamFrame &A = p.fr[p.pi[q]], &B = p.fr[p.pj[q]];
+    const SeamRect a{A.off, A.rx, A.ry, A.rw, A.rh}, b{B.off, B.rx, B.ry, B.rw, B.rh};
+    const int x0 = std::max(A.rx, B.rx), y0 = std::max(A.ry, B.ry);
+    const int iw = std::min(A.rx + A.rw, B.rx + B.rw) - x0, ih = std::min(A.ry + A.rh, B.ry + B.rh) - y0;
+    const int ww = iw + 2 * SEAM_GAP, wh = ih + 2 * SEAM_GAP, wx0 = x0 - SEAM_GAP, wy0 = y0 - SEAM_GAP;
+    seam_column_kernel<<<(unsigned)((ww + 31) / 32), dim3(32, SEAM_SEGS), 0, st>>>(seam, a, b, wx0, wy0, ww, wh, ga, gb);
+    if ((rc = check_launch("udh_mosaic_seam_masks_u8 (columns)")) != UDH_OK) return rc;
+    seam_row_kernel<<<(unsigned)ih, SEAM_ROW_THREADS, 0, st>>>(seam, a, b, wx0, wy0, ww, iw, ga, gb, pa, pb);
+    if ((rc = check_launch("udh_mosaic_seam_masks_u8 (rows)")) != UDH_OK) return rc;
+  }
+  seam_blend_mask_kernel<<<dim3(mb_blocks(p.max_px), (unsigned)n), 256, 0, st>>>(fr, seam, blend);
+  return check_launch("udh_mosaic_seam_masks_u8 (blend masks)");
 }

@@ -2,7 +2,7 @@
 canvas, and blend every frame onto it on the GPU (udh_mosaic_blend_u8, or udh_mosaic_multiband_u8 across frequency bands).
 
     out = build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None, blend="feather", bands=5,
-                       compensate="none", compensate_feeds=1)
+                       compensate="none", compensate_feeds=1, seam="none")
     out["mosaic"], out["mask"], out["M"], out["kept"], out["H_pairs"], out["gains"], out["last_ms"]
 
 frames are CUDA uint8 RGB [h_k,w_k,3] tensors in sequence order (sizes may differ); est is an align.HomographyEstimator.
@@ -31,6 +31,15 @@ Exposure compensation, compensate="gain" or "channels" (default "none").  Before
 computes what cv2.detail_GainCompensator(compensate_feeds) (one gain per frame) or ChannelsCompensator (one per channel)
 finds for the kept frames' ROI warps (oracle/exposure.py states the rule); the blend then takes each frame's warp value
 as saturate_u8(rint(v g)).  This is the stage cv2's stitcher runs between the warp and the blender.
+
+Seams, seam="voronoi" (default "none").  ops.mosaic_seam_masks cuts the kept frames' validity masks apart as
+cv2.detail's Voronoi seam finder does (oracle/seam.py states the rule): pair by pair in cv2's order, each pixel of an
+overlap goes to the frame whose own pixels lie nearer in L1 distance.  Each frame then blends only where the 3 x 3
+dilation of its seam mask meets its validity (cv2's stitcher's blend mask): the multi-band blend switches the high
+frequencies at the seam and spreads only the low ones, instead of averaging the frames across the whole overlap, which
+leaves a semi-transparent double image where the chain drifts; the feathered blend keeps its weights inside each
+frame's region.  The compensator still sees the un-seamed masks, as in cv2's stitcher.  A frame lying inside another
+one's region gets nothing (cv2's result).
 """
 import numpy as np
 
@@ -134,20 +143,22 @@ def farthest_frame(sizes, G, kept, ref):
 
 
 COMPENSATE = ("none", "gain", "channels")
+SEAM = ("none", "voronoi")
 
 
 def build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None, float32_M=False, blend="feather", bands=5,
-                 compensate="none", compensate_feeds=1):
+                 compensate="none", compensate_feeds=1, seam="none"):
     """est: align.HomographyEstimator; frames: CUDA uint8 RGB [h_k,w_k,3] tensors in sequence order.  blend: "feather"
     (udh_mosaic_blend_u8 with `feather`) or "multiband" (udh_mosaic_multiband_u8 with `bands`).  refine: None, or a
     dict of est.refine's keyword arguments (levels, iters, eps, max_side) to refine each pair's H.  max_pixels: the canvas
     limit (None: the JPEG encoder's, udh_jpeg_encode_capacity(Hc, Wc, 3) != 0).  float32_M: blend with each M_k rounded to
     float32, the values a text file of '%.9g' float32 entries gives back.  compensate: "none", "gain" or "channels"
-    (ops.mosaic_exposure_gains with compensate_feeds feeds, applied by the blend).
+    (ops.mosaic_exposure_gains with compensate_feeds feeds, applied by the blend).  seam: "none" or "voronoi"
+    (ops.mosaic_seam_masks; each frame blends only inside its blend mask).
     -> dict(mosaic uint8 [Hc,Wc,3] RGB, mask uint8 [Hc,Wc], M [N,3,3] frame k -> canvas (float64, float32 values with
     float32_M), kept bool [N], ref, H_pairs [N-1,3,3], refine (rho, status, level_reached) or None, gains float64 [N,3]
-    (1 for a dropped frame, all 1 without compensation), last_ms {prep, forward, refine, compensate, blend} of CUDA-event
-    time; compensate only when compensating)."""
+    (1 for a dropped frame, all 1 without compensation), last_ms {prep, forward, refine, compensate, seam, blend} of
+    CUDA-event time; compensate only when compensating, seam only with seams)."""
     frames = list(frames)
     if len(frames) < 2:
         raise ValueError("a mosaic needs at least two frames (got %d)" % len(frames))
@@ -169,11 +180,16 @@ def build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None
         raise ValueError("blend must be 'feather' or 'multiband' (got %r)" % (blend,))
     if compensate not in COMPENSATE:
         raise ValueError("compensate must be 'none', 'gain' or 'channels' (got %r)" % (compensate,))
+    if seam not in SEAM:
+        raise ValueError("seam must be 'none' or 'voronoi' (got %r)" % (seam,))
     gains = np.ones((len(frames), 3))
     if compensate != "none":
         gains[kept], ms["compensate"] = compensate_kept(frames, M, kept, Hc, Wc, compensate, compensate_feeds)
+    masks = None
+    if seam != "none":
+        masks, ms["seam"] = seam_kept(frames, M, kept, Hc, Wc)
     mosaic, mask, ms["blend"] = blend_kept(frames, M, kept, Hc, Wc, feather, blend, bands,
-                                           None if compensate == "none" else gains)
+                                           None if compensate == "none" else gains, masks)
     return dict(mosaic=mosaic, mask=mask, M=M, kept=kept, ref=ref, H_pairs=H, refine=refined, gains=gains, last_ms=ms)
 
 
@@ -198,9 +214,27 @@ def compensate_kept(frames, M, kept, Hc, Wc, mode, feeds=1):
     return g, e0.elapsed_time(e1)
 
 
-def blend_kept(frames, M, kept, Hc, Wc, feather, mode="feather", bands=5, gains=None):
+def seam_kept(frames, M, kept, Hc, Wc):
+    """The kept frames' blend masks (ops.mosaic_seam_masks) -> (masks [n_kept]: CUDA uint8 [roi_h,roi_w], None for a frame
+    whose ROI misses the canvas; CUDA-event ms)."""
+    import torch
+    from . import ops
+    take = [k for k in range(len(frames)) if kept[k]]
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    s = ops.mosaic_seam_masks([frames[k].contiguous() for k in take], np.asarray(M)[take], Hc, Wc)
+    e1.record()
+    e1.synchronize()
+    masks = [None] * len(take)
+    for q, b in zip(s["take"], s["blend"]):
+        masks[q] = b
+    return masks, e0.elapsed_time(e1)
+
+
+def blend_kept(frames, M, kept, Hc, Wc, feather, mode="feather", bands=5, gains=None, masks=None):
     """The kept frames through ops.mosaic_blend_u8 (mode "feather") or ops.mosaic_multiband_u8 ("multiband") -> (mosaic,
-    mask, CUDA-event ms).  gains: None, or [N,3] per frame (exposure compensation)."""
+    mask, CUDA-event ms).  gains: None, or [N,3] per frame (exposure compensation).  masks: None, or seam_kept's blend
+    masks of the kept frames."""
     import torch
     from . import ops
     take = [k for k in range(len(frames)) if kept[k]]
@@ -209,10 +243,10 @@ def blend_kept(frames, M, kept, Hc, Wc, feather, mode="feather", bands=5, gains=
     e0.record()
     if mode == "multiband":
         mosaic, mask = ops.mosaic_multiband_u8([frames[k].contiguous() for k in take], np.asarray(M)[take], Hc, Wc, bands,
-                                               gains=g)
+                                               gains=g, masks=masks)
     else:
         mosaic, mask = ops.mosaic_blend_u8([frames[k].contiguous() for k in take], np.asarray(M)[take], Hc, Wc, feather,
-                                           gains=g)
+                                           gains=g, masks=masks)
     e1.record()
     e1.synchronize()
     return mosaic, mask, e0.elapsed_time(e1)

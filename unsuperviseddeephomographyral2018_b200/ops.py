@@ -646,13 +646,38 @@ def _gains(gains, n, dev, what):
     return torch.from_numpy(np.broadcast_to(g, (n, 3)).copy()).to(dev)
 
 
-def mosaic_blend_u8(frames, M, dst_h, dst_w, feather, gains=None):
+def _mask_table(masks, rois, n, what):
+    """Blend masks [n] (frame k's CUDA uint8 [roi_h,roi_w] on its multi-band ROI; ignored, may be None, where the ROI is
+    empty) -> (host array of device pointers, rois int32 [n,4] with empty rows for the frames left out)."""
+    masks = list(masks)
+    if len(masks) != n:
+        raise _lib.UdhError("%s: %d masks for %d frames" % (what, len(masks), n))
+    rr = np.ascontiguousarray(np.asarray(rois, np.int64).astype(np.int32).reshape(n, 4))
+    ptrs = (ctypes.c_void_p * max(n, 1))()
+    for k, m in enumerate(masks):
+        x0, y0, x1, y1 = (int(v) for v in rr[k])
+        if x1 <= x0 or y1 <= y0:
+            rr[k] = 0
+            continue
+        if m is None:
+            raise _lib.UdhError("%s: frame %d meets the canvas but has no mask" % (what, k))
+        _req(m, torch.uint8, "masks[%d]" % k)
+        if tuple(m.shape) != (y1 - y0, x1 - x0):
+            raise _lib.UdhError("%s: masks[%d] must be [%d,%d] (its ROI; got %s)" % (what, k, y1 - y0, x1 - x0, tuple(m.shape)))
+        ptrs[k] = m.data_ptr()
+    return ptrs, rr
+
+
+def mosaic_blend_u8(frames, M, dst_h, dst_w, feather, gains=None, masks=None):
     """frames: n CUDA uint8 tensors [h_k,w_k,C] (C = 1 or 3, sizes may differ; or one [n,h,w,C] tensor), M float64 [n,3,3]
     (frame k -> canvas; numpy or tensor) -> (mosaic uint8 [dst_h,dst_w,C], mask uint8 [dst_h,dst_w]): udh_mosaic_blend_u8's
     feathered blend of cv2.warpPerspective(frame k, M_k, (dst_w, dst_h)), bit for bit with oracle/mosaic.py.  The tile
     lists are built on the host (mosaic_tile_lists); the frames are read where they are.  gains ([n] or [n,3], e.g.
     mosaic_exposure_gains'): each frame's warp value is exposure-compensated first, saturate_u8(rint(v g)) in float64
-    (udh_mosaic_blend_gain_u8)."""
+    (udh_mosaic_blend_gain_u8).  masks ([n], e.g. mosaic_seam_masks' blend masks): frame k counts only where its mask,
+    a CUDA uint8 [roi_h,roi_w] on its ROI (mosaic.multiband_rois), is set; a frame whose ROI misses the canvas takes None
+    and counts nowhere (udh_mosaic_blend_masked_u8)."""
+    from . import mosaic
     frames = list(frames.unbind(0)) if isinstance(frames, torch.Tensor) else list(frames)
     Mh = (M.detach().cpu().numpy() if isinstance(M, torch.Tensor) else np.asarray(M)).astype(np.float64).reshape(-1, 3, 3)
     n = len(frames)
@@ -676,7 +701,15 @@ def mosaic_blend_u8(frames, M, dst_h, dst_w, feather, gains=None):
     ws = torch.empty(max(nb, 1), device=dev, dtype=torch.uint8)
     ptrs = (ctypes.c_void_p * n)(*[f.data_ptr() for f in frames])
     sz = np.ascontiguousarray(np.array(sizes, np.int32).reshape(n, 2))
-    if gains is None:
+    if masks is not None:
+        mp, rr = _mask_table(masks, mosaic.multiband_rois(Mh, sizes, int(dst_h), int(dst_w))[0], n, "mosaic_blend_u8")
+        g_d = None if gains is None else _gains(gains, n, dev, "mosaic_blend_u8")
+        nb = lib.udh_mosaic_blend_masked_workspace_bytes(n)
+        ws = torch.empty(max(nb, 1), device=dev, dtype=torch.uint8)
+        check(lib.udh_mosaic_blend_masked_u8(ptrs, sz.ctypes.data, _ptr(M_d), None if g_d is None else _ptr(g_d), mp, rr.ctypes.data, n,
+                                             C, _ptr(ptr_d), _ptr(idx_d), int(dst_h), int(dst_w), int(feather), _ptr(out), _ptr(mask),
+                                             _ptr(ws), nb, _stream()), "udh_mosaic_blend_masked_u8")
+    elif gains is None:
         check(lib.udh_mosaic_blend_u8(ptrs, sz.ctypes.data, _ptr(M_d), n, C, _ptr(ptr_d), _ptr(idx_d), int(dst_h), int(dst_w),
                                       int(feather), _ptr(out), _ptr(mask), _ptr(ws), nb, _stream()), "udh_mosaic_blend_u8")
     else:
@@ -687,7 +720,7 @@ def mosaic_blend_u8(frames, M, dst_h, dst_w, feather, gains=None):
     return out, mask
 
 
-def mosaic_multiband_u8(frames, M, dst_h, dst_w, bands, levels=False, gains=None):
+def mosaic_multiband_u8(frames, M, dst_h, dst_w, bands, levels=False, gains=None, masks=None):
     """frames: n CUDA uint8 RGB tensors [h_k,w_k,3] (sizes may differ), M float64 [n,3,3] (frame k -> canvas; numpy or
     tensor) -> (mosaic uint8 [dst_h,dst_w,3], mask uint8 [dst_h,dst_w]): udh_mosaic_multiband_u8, byte for byte
     cv2.detail_MultiBandBlender(0, bands, CV_16S) fed each frame's warp on its ROI (oracle/multiband.py).  The ROIs and the
@@ -695,7 +728,9 @@ def mosaic_multiband_u8(frames, M, dst_h, dst_w, bands, levels=False, gains=None
     map to finite points with a positive denominator); a frame whose ROI misses the canvas is left out.  levels=True also
     returns the canvas pyramid as the feeds left it: [B' + 1] int16 CUDA tensors [Hp >> i, Wp >> i, 4] (acc, then wacc).
     gains ([n] or [n,3], e.g. mosaic_exposure_gains'): each ROI warp is exposure-compensated before it is fed,
-    saturate_u8(rint(v g)) in float64 (udh_mosaic_multiband_gain_u8), cv2's stitcher order."""
+    saturate_u8(rint(v g)) in float64 (udh_mosaic_multiband_gain_u8), cv2's stitcher order.  masks ([n], e.g.
+    mosaic_seam_masks' blend masks; None for a frame whose ROI misses the canvas): frame k is fed its mask, a CUDA uint8
+    [roi_h,roi_w], in place of its validity mask (udh_mosaic_multiband_masked_u8)."""
     from . import mosaic
     frames = list(frames.unbind(0)) if isinstance(frames, torch.Tensor) else list(frames)
     Mh = (M.detach().cpu().numpy() if isinstance(M, torch.Tensor) else np.asarray(M)).astype(np.float64).reshape(-1, 3, 3)
@@ -726,7 +761,16 @@ def mosaic_multiband_u8(frames, M, dst_h, dst_w, bands, levels=False, gains=None
     if nb == 0:
         raise _lib.UdhError("mosaic_multiband_u8: bad arguments (%d frames, canvas %dx%d, %d bands)" % (m, dst_h, dst_w, bands))
     ws = torch.empty(nb, device=dev, dtype=torch.uint8)
-    if g_d is None:
+    if masks is not None:
+        masks = list(masks)
+        if len(masks) != n:
+            raise _lib.UdhError("mosaic_multiband_u8: %d masks for %d frames" % (len(masks), n))
+        mp, _ = _mask_table([masks[k] for k in take], rr, m, "mosaic_multiband_u8")
+        g_d = None if g_d is None else g_d[take].contiguous()
+        check(lib.udh_mosaic_multiband_masked_u8(ptrs, sz.ctypes.data, _ptr(M_d), None if g_d is None else _ptr(g_d), mp, rr.ctypes.data,
+                                                 m, 3, int(dst_h), int(dst_w), int(bands), _ptr(out), _ptr(mask), _ptr(ws), nb,
+                                                 _stream()), "udh_mosaic_multiband_masked_u8")
+    elif g_d is None:
         check(lib.udh_mosaic_multiband_u8(ptrs, sz.ctypes.data, _ptr(M_d), rr.ctypes.data, m, 3, int(dst_h), int(dst_w), int(bands),
                                           _ptr(out), _ptr(mask), _ptr(ws), nb, _stream()), "udh_mosaic_multiband_u8")
     else:
@@ -915,6 +959,54 @@ def mosaic_exposure_gains(frames, M, dst_h, dst_w, mode="gain", feeds=1):
         hist.append(g3)
     gains[st.take] = acc
     return gains
+
+
+# ------------------------------------------------------------------ seam finding
+def seam_pairs(rois):
+    """rois [m,4] (x_lo, y_lo, x_hi, y_hi) -> CSR (pair_ptr int32 [m+1], pair_j int32 [P]) of the pairs i < j whose rectangles
+    intersect, row-major: cv2.detail.PairwiseSeamFinder's visiting order."""
+    r = np.asarray(rois, np.int64).reshape(-1, 4)
+    x0, y0 = np.maximum(r[:, None, 0], r[None, :, 0]), np.maximum(r[:, None, 1], r[None, :, 1])
+    x1, y1 = np.minimum(r[:, None, 2], r[None, :, 2]), np.minimum(r[:, None, 3], r[None, :, 3])
+    hit = np.triu((x0 < x1) & (y0 < y1), 1)
+    ptr = np.zeros(len(r) + 1, np.int64)
+    ptr[1:] = np.cumsum(hit.sum(1))
+    return ptr.astype(np.int32), np.nonzero(hit)[1].astype(np.int32)
+
+
+def mosaic_seam_masks(frames, M, dst_h, dst_w):
+    """frames: n CUDA uint8 RGB tensors [h_k,w_k,3], M float64 [n,3,3] (frame k -> canvas) -> dict(take (the fed frames:
+    those whose ROI meets the canvas), rois int64 [n,4] (mosaic.multiband_rois), seam [m], blend [m]): per fed frame its
+    seam mask and blend mask, CUDA uint8 [roi_h,roi_w] (0 / 255), byte for byte what cv2.detail's Voronoi seam finder
+    leaves in the multi-band blend's validity masks, and cv2.dilate of that AND the validity, the mask cv2's stitcher feeds
+    its blender (udh_mosaic_seam_masks_u8; oracle/seam.py states the rule).  A frame lying inside another one's seam region
+    vanishes (an all-zero mask), as in cv2."""
+    frames, sizes, rois, Mr, take = _exposure_rois(frames, M, dst_h, dst_w, "mosaic_seam_masks")
+    out = dict(take=take, rois=rois, seam=[], blend=[])
+    if not take:
+        return out
+    m, dev = len(take), frames[0].device
+    rr = np.ascontiguousarray(rois[take].astype(np.int32))
+    M_d = torch.from_numpy(np.ascontiguousarray(Mr[take].reshape(m, 9))).to(dev)
+    sz = np.ascontiguousarray(np.array([sizes[k] for k in take], np.int32).reshape(m, 2))
+    ptrs = (ctypes.c_void_p * m)(*[frames[k].data_ptr() for k in take])
+    ptr, pj = seam_pairs(rr)
+    pj = pj if len(pj) else np.zeros(1, np.int32)
+    hw = np.stack([rr[:, 3] - rr[:, 1], rr[:, 2] - rr[:, 0]], 1).astype(np.int64)
+    off = np.concatenate([[0], np.cumsum(hw[:, 0] * hw[:, 1])])
+    seam = torch.empty(int(off[-1]), device=dev, dtype=torch.uint8)
+    blend = torch.empty(int(off[-1]), device=dev, dtype=torch.uint8)
+    nb = lib.udh_mosaic_seam_workspace_bytes(rr.ctypes.data, m, ptr.ctypes.data, pj.ctypes.data, int(dst_h), int(dst_w))
+    if nb == 0:
+        raise _lib.UdhError("mosaic_seam_masks: bad arguments (%d frames, canvas %dx%d)" % (m, dst_h, dst_w))
+    ws = torch.empty(nb, device=dev, dtype=torch.uint8)
+    check(lib.udh_mosaic_seam_masks_u8(ptrs, sz.ctypes.data, _ptr(M_d), rr.ctypes.data, m, ptr.ctypes.data, pj.ctypes.data, int(dst_h),
+                                       int(dst_w), _ptr(seam), _ptr(blend), _ptr(ws), nb, _stream()), "udh_mosaic_seam_masks_u8")
+    for k in range(m):
+        h, w = (int(v) for v in hw[k])
+        out["seam"].append(seam[off[k]:off[k + 1]].view(h, w))
+        out["blend"].append(blend[off[k]:off[k + 1]].view(h, w))
+    return out
 
 
 # ------------------------------------------------------------------ Adam
