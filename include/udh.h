@@ -540,6 +540,68 @@ int udh_mosaic_exposure_stats_u8(const uint8_t* const* frames, const int32_t* si
                                  const int32_t* pair_ptr, const int32_t* pair_j, int npairs, const double* history, int feeds,
                                  int norms, int dst_h, int dst_w, uint64_t* stats, void* ws, size_t ws_bytes, void* stream);
 
+/* ---- block exposure compensation (cv2.detail_BlocksGainCompensator / BlocksChannelsCompensator; oracle/exposure_blocks.py)
+ * Each fed frame's ROI (roi_w x roi_h) is cut into bpx x bpy blocks of bw x bh pixels (bpx = ceil(roi_w / block),
+ * bw = ceil(roi_w / bpx), likewise in y); blocks are numbered frame-major, then row-major, frame k's from boff[k].
+ * udh_mosaic_exposure_block_stats_u8: udh_mosaic_exposure_stats_u8's statistics per block pair.  For each listed frame pair
+ *   p = (i, j), i <= j, over the ROIs' intersection the block columns of both frames merge: a pixel in block column bx_i of
+ *   frame i and bx_j of frame j lies in cell column (bx_i - bx_i0) + (bx_j - bx_j0) (bx_i0, bx_j0: the columns at the
+ *   intersection's left edge), likewise in y, and cell (cx, cy) is slot cell_off[p] + cy cell_nx[p] + cx of stats
+ *   (uint64 [slots][UDH_EXPOSURE_STATS], device, zeroed here): the same 13 sums over the pixels of that block pair where
+ *   both ROI warps are valid.  A frame's pair with itself gives each block's own count at cell (2 bx, 2 by).  blocks
+ *   (host int32 [n][4]): bw, bh, bpx, bpy per frame; boff (host int64 [n]).  history [feeds][nblocks][3] float64 (device): a
+ *   pixel of block b is compensated by history[0][b][c], then history[1][b][c], ... (cv2's feeds over the blocks).
+ *   cell_off int64 [npairs], cell_nx int32 [npairs] (device).  Limits as udh_mosaic_exposure_stats_u8, nblocks <=
+ *   UDH_EXPOSURE_MAX_BLOCKS.  ws: udh_mosaic_exposure_block_workspace_bytes(n).
+ * udh_exposure_block_solve: x = A^-1 b for a symmetric positive definite A in CSR (row_ptr [n + 1] int32, col int32, val
+ *   float64, device) by Jacobi-preconditioned conjugate gradients in float64, from x = 1, in one CTA whose reductions
+ *   have a fixed order (the result does not depend on the run).  Stops when |r| <= tol |b| or after max_iter iterations;
+ *   info (device int64 [2]) receives the iterations and the final |r| / |b| as a double's bits.  ws:
+ *   udh_exposure_block_solve_workspace_bytes(n).
+ * udh_exposure_gain_maps: per frame k its bpy x bpx map float32(gains[b][c]) (c < channels; gains [nblocks][3] float64,
+ *   device), filtered twice by cv2.sepFilter2D([1/4, 1/2, 1/4] both ways, BORDER_REFLECT_101, float32: each output
+ *   (a + c) 1/4 + b 1/2, the row pass then the column pass) into maps (float32 [nblocks][channels], device, frame k's at
+ *   boff[k] channels).  blocks, boff as above (host).  ws: udh_exposure_gain_maps_workspace_bytes(nblocks, channels).
+ * udh_mosaic_blend_gainmap_u8 / udh_mosaic_multiband_gainmap_u8: the blends (masks null: unmasked; else as the _masked_
+ *   calls) with each frame's value v at ROI pixel (lx, ly) compensated by its map: v' = saturate_u8(rint(float32(v) g))
+ *   in float32, g = the map's bilinear resize to the ROI at (lx, ly) (udh_gain_map: the taps of every ROI column and row,
+ *   the row pass then the column pass, each product and sum rounded to float32; channel c's gain, or the one gain when
+ *   channels = 1).  maps [n] (host).  The feathered blend evaluates frame k at canvas pixel (x, y) at (x - x_lo, y - y_lo)
+ *   of its rectangle rois[k] (host int32 [n,4]), clamped to it.  ws: udh_mosaic_blend_gainmap_workspace_bytes(n) /
+ *   udh_mosaic_multiband_gainmap_workspace_bytes(rois, n, dst_h, dst_w, bands). */
+#define UDH_EXPOSURE_MAX_BLOCKS (1 << 24)
+typedef struct udh_map_tap {
+  int32_t s0, s1; /* the two source columns (rows) of the map */
+  float a0, a1;   /* their weights */
+} udh_map_tap;
+typedef struct udh_gain_map {
+  const float* map;        /* device: bpy x bpx x channels float32 */
+  const udh_map_tap* cols; /* device: one per ROI column */
+  const udh_map_tap* rows; /* device: one per ROI row */
+  int32_t bpx, bpy, channels, pad;
+} udh_gain_map;
+size_t udh_mosaic_exposure_block_workspace_bytes(int n);
+int udh_mosaic_exposure_block_stats_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const int32_t* rois, int n,
+                                       const int32_t* blocks, const int64_t* boff, int64_t nblocks, const int32_t* pair_ptr,
+                                       const int32_t* pair_j, int npairs, const int64_t* cell_off, const int32_t* cell_nx,
+                                       int64_t nslots, const double* history, int feeds, int norms, int dst_h, int dst_w,
+                                       uint64_t* stats, void* ws, size_t ws_bytes, void* stream);
+size_t udh_exposure_block_solve_workspace_bytes(int n);
+int udh_exposure_block_solve(int n, const int32_t* row_ptr, const int32_t* col, const double* val, const double* b, double tol,
+                             int max_iter, double* x, int64_t* info, void* ws, size_t ws_bytes, void* stream);
+size_t udh_exposure_gain_maps_workspace_bytes(int64_t nblocks, int channels);
+int udh_exposure_gain_maps(const double* gains, int n, const int32_t* blocks, const int64_t* boff, int64_t nblocks, int channels,
+                           float* maps, void* ws, size_t ws_bytes, void* stream);
+size_t udh_mosaic_blend_gainmap_workspace_bytes(int n);
+int udh_mosaic_blend_gainmap_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const udh_gain_map* maps,
+                                const uint8_t* const* masks, const int32_t* rois, int n, int c, const int32_t* tile_ptr,
+                                const int32_t* tile_frames, int dst_h, int dst_w, int feather, uint8_t* dst, uint8_t* mask, void* ws,
+                                size_t ws_bytes, void* stream);
+size_t udh_mosaic_multiband_gainmap_workspace_bytes(const int32_t* rois, int n, int dst_h, int dst_w, int bands);
+int udh_mosaic_multiband_gainmap_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const udh_gain_map* maps,
+                                    const uint8_t* const* masks, const int32_t* rois, int n, int c, int dst_h, int dst_w, int bands,
+                                    uint8_t* dst, uint8_t* mask, void* ws, size_t ws_bytes, void* stream);
+
 /* ---- seam finding (cv2.detail's Voronoi seam finder; oracle/seam.py restates the rule) -------------------------------
  * udh_mosaic_seam_masks_u8: the seams between udh_mosaic_multiband_u8's frames (frames, sizes, M frame -> ROI (device),
  *   rois (host), as that call takes them), byte for byte what cv2.detail.SeamFinder_createDefault(VORONOI_SEAM).find

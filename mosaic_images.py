@@ -13,7 +13,10 @@ source pixels (0: a plain average of the overlapping frames).  --blend multiband
 instead (cv2.detail_MultiBandBlender's rule, byte for byte): low frequencies over a wide region, high ones over a narrow
 one, which hides the seams a drifting chain leaves.  --compensate gain|channels compensates each frame's exposure before
 the blend (cv2.detail_GainCompensator / ChannelsCompensator's rule with --compensate_feeds feeds): one gain per frame, or
-one per channel, which also evens out white balance.  An exposure step between frames is otherwise left in the mosaic.
+one per channel, which also evens out white balance.  --compensate gain_blocks|channels_blocks (cv2's stitcher's default,
+cv2.detail_BlocksGainCompensator / BlocksChannelsCompensator) solves for a gain per block of about --compensate_block px
+of each frame and applies the smoothed map of them, which also removes brightness that varies across a frame, such as
+vignetting.  An exposure step between frames is otherwise left in the mosaic.
 cv2's rule pulls every gain towards 1, so one feed removes only part of a step; each further feed removes part of what
 is left (on a sweep with exposures 0.75 / 1 / 1.3, four gain-mode feeds recover the gain ratios to within 1 %).
 --seam voronoi cuts seams between the frames before the blend (cv2.detail's Voronoi seam finder, byte for byte): each
@@ -26,7 +29,10 @@ Writes in --out_dir:
   mosaic.txt   `canvas Hc Wc ref r` (` blend multiband B` appended with --blend multiband, then ` compensate MODE F` with
                --compensate, then ` seam voronoi` with --seam voronoi), then `name kept|dropped` and the nine entries of M_k (frame k -> canvas) per frame,
                '%.9g' of their float32 values; the blend uses those float32 values.  With --compensate each frame line
-               ends in its three gains, '%.17g' (exact); so the file reproduces mosaic.jpg;
+               ends in its three gains, '%.17g' (exact); so the file reproduces mosaic.jpg.  With a block mode the
+               compensate field is ` compensate MODE F B` (B: --compensate_block) and the frame lines carry no gains;
+  gain_maps.npz with --compensate gain_blocks|channels_blocks, each fed frame's gain map (float32 [bpy,bpx] or
+               [bpy,bpx,3], keyed by frame name), as cv2's compensator's getMatGains() returns it;
   mosaic.jpg   the mosaic (BGR, JPEG quality 95, byte-identical to cv2.imencode of the same pixels).
 A frame whose grown corners map behind the reference camera is dropped.  The canvas must be one the JPEG encoder takes
 (about 110 MP in colour); a larger one stops with an error naming the frame that reaches farthest.  Prints the GPU time
@@ -56,8 +62,11 @@ def build_parser():
     p.add_argument('--blend', type=str, default='feather', choices=['feather', 'multiband'],
                    help='feather: feathered average; multiband: blend across frequency bands')
     p.add_argument('--bands', type=int, default=5, help='frequency bands of --blend multiband, 0..10')
-    p.add_argument('--compensate', type=str, default='none', choices=['none', 'gain', 'channels'],
-                   help='exposure compensation before the blend: none, one gain per frame, or one per channel')
+    p.add_argument('--compensate', type=str, default='none', choices=['none', 'gain', 'channels', 'gain_blocks', 'channels_blocks'],
+                   help='exposure compensation before the blend: none, one gain per frame, one per channel, or a smooth '
+                        'map of gains per block of each frame (gain_blocks: one gain, channels_blocks: one per channel)')
+    p.add_argument('--compensate_block', type=int, default=32,
+                   help='block side in pixels of --compensate gain_blocks|channels_blocks, 1..1024')
     p.add_argument('--compensate_feeds', type=int, default=1,
                    help='feeds of the exposure compensator, 1..16; one feed removes only part of an exposure step (the '
                         'rule pulls every gain towards 1), several (e.g. 4) remove nearly all of it')
@@ -93,13 +102,18 @@ def run(args, est, decode, encode):
         raise SystemExit("--bands must be in 0..10 (got %d)" % args.bands)
     if not 1 <= args.compensate_feeds <= 16:
         raise SystemExit("--compensate_feeds must be in 1..16 (got %d)" % args.compensate_feeds)
+    if not 1 <= args.compensate_block <= 1024:
+        raise SystemExit("--compensate_block must be in 1..1024 (got %d)" % args.compensate_block)
     names, paths = frame_list(args)
     os.makedirs(args.out_dir, exist_ok=True)
     refining = args.refine_levels != 0
     refine = dict(levels=None if args.refine_levels < 0 else args.refine_levels, iters=args.refine_iters, eps=args.refine_eps,
                   max_side=args.refine_max_side) if refining else None
     compensating = args.compensate != "none"
+    blocks = args.compensate.endswith("_blocks")
     comp = dict(compensate=args.compensate, compensate_feeds=args.compensate_feeds) if compensating else {}
+    if blocks:
+        comp["compensate_block"] = args.compensate_block
     seaming = args.seam != "none"
     if seaming:
         comp["seam"] = args.seam
@@ -119,15 +133,19 @@ def run(args, est, decode, encode):
     Hc, Wc = out["mask"].shape
     lines = ["canvas %d %d ref %d" % (Hc, Wc, out["ref"]) + (" blend multiband %d" % args.bands if args.blend == "multiband" else "") +
              (" compensate %s %d" % (args.compensate, args.compensate_feeds) if compensating else "") +
+             (" %d" % args.compensate_block if blocks else "") +
              (" seam %s" % args.seam if seaming else "")]
     for k, nm in enumerate(names):
         lines.append(" ".join([nm, "kept" if out["kept"][k] else "dropped"] +
                               ["%.9g" % v for v in align.homography_as_written(out["M"][k])[0]] +
-                              (["%.17g" % g for g in out["gains"][k]] if compensating else [])))
+                              (["%.17g" % g for g in out["gains"][k]] if compensating and not blocks else [])))
         if not out["kept"][k]:
             print("===> dropped %s: it maps behind the reference frame's camera" % nm)
     with open(os.path.join(args.out_dir, "mosaic.txt"), "w") as f:
         f.write("\n".join(lines) + "\n")
+    if blocks:
+        np.savez(os.path.join(args.out_dir, "gain_maps.npz"),
+                 **{nm: m.cpu().numpy() for nm, m in zip(names, out["gain_maps"]) if m is not None})
     ms = out["last_ms"]
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()

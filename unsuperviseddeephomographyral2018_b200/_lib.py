@@ -20,6 +20,7 @@ ECC_OK, ECC_NAN, ECC_NOCONV = 0, 1, 2
 MOSAIC_TILE_H, MOSAIC_TILE_W = 16, 64            # UDH_MOSAIC_TILE_H / _W
 EXPOSURE_MAX_FRAMES, EXPOSURE_MAX_FEEDS, EXPOSURE_STATS = 1024, 16, 13   # UDH_EXPOSURE_MAX_FRAMES / _MAX_FEEDS / _STATS
 SEAM_MAX_FRAMES = 1024                            # UDH_SEAM_MAX_FRAMES
+EXPOSURE_MAX_BLOCKS = 1 << 24                     # UDH_EXPOSURE_MAX_BLOCKS
 
 class StepArgs(ctypes.Structure):
     """udh_step_args (include/udh.h)."""
@@ -34,6 +35,13 @@ class StepArgs(ctypes.Structure):
 
 
 FWD_FC1_MIRROR_CURRENT = 1
+
+
+class GainMap(ctypes.Structure):
+    """udh_gain_map (include/udh.h): a frame's block gain map and its ROI's resize taps (udh_map_tap: int32 s0, s1,
+    float32 a0, a1 per column / row), all device pointers."""
+    _fields_ = [("map", c_void_p), ("cols", c_void_p), ("rows", c_void_p), ("bpx", c_int), ("bpy", c_int), ("channels", c_int),
+                ("pad", c_int)]
 
 
 class JpegInfo(ctypes.Structure):
@@ -198,6 +206,21 @@ SIGNATURES = {
                                            c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "udh_mosaic_multiband_masked_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                                c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "udh_mosaic_exposure_block_workspace_bytes": (c_size_t, [c_int]),
+    "udh_mosaic_exposure_block_stats_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int64, c_void_p,
+                                                   c_void_p, c_int, c_void_p, c_void_p, c_int64, c_void_p, c_int, c_int, c_int, c_int,
+                                                   c_void_p, c_void_p, c_size_t, c_void_p]),
+    "udh_exposure_block_solve_workspace_bytes": (c_size_t, [c_int]),
+    "udh_exposure_block_solve": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_double, c_int, c_void_p, c_void_p, c_void_p,
+                                         c_size_t, c_void_p]),
+    "udh_exposure_gain_maps_workspace_bytes": (c_size_t, [c_int64, c_int]),
+    "udh_exposure_gain_maps": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "udh_mosaic_blend_gainmap_workspace_bytes": (c_size_t, [c_int]),
+    "udh_mosaic_blend_gainmap_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
+                                            c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "udh_mosaic_multiband_gainmap_workspace_bytes": (c_size_t, [c_void_p, c_int, c_int, c_int, c_int]),
+    "udh_mosaic_multiband_gainmap_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                                c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "udh_draw_report_workspace_bytes": (c_size_t, [c_int]),
     "udh_draw_report_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_int, c_int, c_int,
                                    c_void_p]),

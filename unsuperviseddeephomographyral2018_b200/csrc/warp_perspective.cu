@@ -149,16 +149,51 @@ __device__ __forceinline__ int ex_apply(int v, double g) {
   return min(max(__double2int_rn(__dmul_rn((double)v, g)), 0), 255);
 }
 
+// Block exposure compensation's apply, cv2.multiply(uint8, float32 map, CV_8U): saturate_u8(rint(float32(v) g)) in float32.
+__device__ __forceinline__ int ex_apply_f(int v, float g) {
+  return min(max(__float2int_rn(__fmul_rn((float)v, g)), 0), 255);
+}
+
+// A frame's gain map with its ROI rectangle (rx, ry, rw, rh) on the canvas.
+struct GainMapDev {
+  udh_gain_map m;
+  int rx, ry, rw, rh;
+};
+
+// The gain map's bilinear resize at ROI pixel (lx, ly): g[c] for c < 3 (the one gain repeated when the map has 1 channel).
+// The row pass, then the column pass, every product and sum rounded to float32 (oracle/exposure_blocks.resize_map).
+__device__ __forceinline__ void gm_gains(const GainMapDev* __restrict__ G, int lx, int ly, float* g) {
+  const float* mp = reinterpret_cast<const float*>(__ldg(reinterpret_cast<const unsigned long long*>(&G->m.map)));
+  const udh_map_tap* ct = reinterpret_cast<const udh_map_tap*>(__ldg(reinterpret_cast<const unsigned long long*>(&G->m.cols)));
+  const udh_map_tap* rt = reinterpret_cast<const udh_map_tap*>(__ldg(reinterpret_cast<const unsigned long long*>(&G->m.rows)));
+  const int bpx = __ldg(&G->m.bpx), ch = __ldg(&G->m.channels);
+  const int cs0 = __ldg(&ct[lx].s0), cs1 = __ldg(&ct[lx].s1), rs0 = __ldg(&rt[ly].s0), rs1 = __ldg(&rt[ly].s1);
+  const float ca0 = __ldg(&ct[lx].a0), ca1 = __ldg(&ct[lx].a1), ra0 = __ldg(&rt[ly].a0), ra1 = __ldg(&rt[ly].a1);
+  for (int c = 0; c < 3; ++c) {
+    if (c >= ch) {
+      g[c] = g[0];
+      continue;
+    }
+    const float* r0 = mp + ((int64_t)rs0 * bpx) * ch + c;
+    const float* r1 = mp + ((int64_t)rs1 * bpx) * ch + c;
+    const float h0 = __fadd_rn(__fmul_rn(__ldg(r0 + cs0 * ch), ca0), __fmul_rn(__ldg(r0 + cs1 * ch), ca1));
+    const float h1 = __fadd_rn(__fmul_rn(__ldg(r1 + cs0 * ch), ca0), __fmul_rn(__ldg(r1 + cs1 * ch), ca1));
+    g[c] = __fadd_rn(__fmul_rn(h0, ra0), __fmul_rn(h1, ra1));
+  }
+}
+
 // Gather form: one CTA per UDH_MOSAIC_TILE_H x UDH_MOSAIC_TILE_W canvas tile, each thread four consecutive pixels of one
 // row.  The thread walks the tile's candidate frames, adds wt * v and wt of every frame valid at its pixels into 64-bit
 // registers and stores the pixels once: no atomics, no accumulation buffer.  Integer sums: the result does not depend on
 // the frames' order.  GAIN: each frame's value is first compensated, ex_apply(v, gains[f][c]) (channel 0's gain when C = 1).
-// MASK: a frame counts only where its blend mask smask[f] is set as well.
-template <int C, bool GAIN, bool MASK = false>
+// MASK: a frame counts only where its blend mask smask[f] is set as well.  MAP: each frame's value is compensated by its
+// gain map at the pixel's ROI coordinates (gm_gains).
+template <int C, bool GAIN, bool MASK = false, bool MAP = false>
 __device__ __forceinline__ void mosaic_blend_tile(const MosaicFrame* __restrict__ fr, int n, const int32_t* __restrict__ tile_ptr,
                                                   const int32_t* __restrict__ tile_frames, int dh, int dw, int bw, int feather32,
                                                   const double* __restrict__ gains, uint8_t* __restrict__ dst,
-                                                  uint8_t* __restrict__ mask, const SeamMask* __restrict__ smask = nullptr) {
+                                                  uint8_t* __restrict__ mask, const SeamMask* __restrict__ smask = nullptr,
+                                                  const GainMapDev* __restrict__ gmap = nullptr) {
   const int y = blockIdx.y * UDH_MOSAIC_TILE_H + threadIdx.x / (UDH_MOSAIC_TILE_W / 4);
   const int x0 = blockIdx.x * UDH_MOSAIC_TILE_W + threadIdx.x % (UDH_MOSAIC_TILE_W / 4) * 4;
   if (y >= dh || x0 >= dw) return;
@@ -194,6 +229,13 @@ __device__ __forceinline__ void mosaic_blend_tile(const MosaicFrame* __restrict_
         if (GAIN) {
 #pragma unroll
           for (int c = 0; c < C; ++c) v[c] = ex_apply(v[c], __ldg(gains + 3 * f + c));
+        }
+        if (MAP) {
+          const GainMapDev* G = gmap + f;
+          float g[3];
+          gm_gains(G, min(max(x0 + k - __ldg(&G->rx), 0), __ldg(&G->rw) - 1), min(max(y - __ldg(&G->ry), 0), __ldg(&G->rh) - 1), g);
+#pragma unroll
+          for (int c = 0; c < C; ++c) v[c] = ex_apply_f(v[c], g[c]);
         }
 #pragma unroll
         for (int c = 0; c < C; ++c) S[k][c] += (uint64_t)(wt * v[c]);
@@ -258,6 +300,16 @@ __global__ void __launch_bounds__(256) seam_blend_u8_kernel(const MosaicFrame* _
   mosaic_blend_tile<C, GAIN, true>(fr, n, tile_ptr, tile_frames, dh, dw, bw, feather32, gains, dst, mask, smask);
 }
 
+// The feathered blend of frames compensated by their gain maps (MASK: kept only where their blend masks are set).
+template <int C, bool MASK>
+__global__ void __launch_bounds__(256) gainmap_blend_u8_kernel(const MosaicFrame* __restrict__ fr, int n, const int32_t* __restrict__ tile_ptr,
+                                                               const int32_t* __restrict__ tile_frames, int dh, int dw, int bw,
+                                                               int feather32, const SeamMask* __restrict__ smask,
+                                                               const GainMapDev* __restrict__ gmap, uint8_t* __restrict__ dst,
+                                                               uint8_t* __restrict__ mask) {
+  mosaic_blend_tile<C, false, MASK, true>(fr, n, tile_ptr, tile_frames, dh, dw, bw, feather32, nullptr, dst, mask, smask, gmap);
+}
+
 // ---- multi-band blend: cv2.detail_MultiBandBlender with CV_16S weights (the rule: oracle/multiband.py) ----------------
 // Per frame k, its fed rectangle (ROI grown by the gap, aligned to 2^B) holds the image pyramid G_i (uchar4, RGB + pad)
 // and the weight pyramid W_i (int16) in two pools; the canvas pyramid keeps (acc, wacc) as short4 per pixel, and the
@@ -310,9 +362,11 @@ __device__ __forceinline__ bool mb_roi_warp(const uint8_t* __restrict__ s, int h
 // gains (null: none) [n][3]: the ROI warp is exposure-compensated first, ex_apply(v, gains[k][c]), as cv2's stitcher
 // applies its compensator to the whole warped image before it feeds the blender.  A frame with a blend mask (bmask) takes
 // its weight from that mask instead of the warp's validity.
-__global__ void __launch_bounds__(256) multiband_base_kernel(const MultibandFrame* __restrict__ fr, const double* __restrict__ M,
-                                                             const double* __restrict__ gains, uchar4* __restrict__ G,
-                                                             int16_t* __restrict__ Wt) {
+// MAP: the ROI warp is compensated by the frame's gain map at each ROI pixel instead (gm_gains, ex_apply_f).
+template <bool MAP>
+__device__ __forceinline__ void mb_base(const MultibandFrame* __restrict__ fr, const double* __restrict__ M,
+                                        const double* __restrict__ gains, const GainMapDev* __restrict__ gmap,
+                                        uchar4* __restrict__ G, int16_t* __restrict__ Wt) {
   __shared__ double mi[9];
   const int k = blockIdx.y;
   if (threadIdx.x == 0) cv_invert3(M + (int64_t)k * 9, mi);
@@ -325,7 +379,7 @@ __global__ void __launch_bounds__(256) multiband_base_kernel(const MultibandFram
   const int64_t off = __ldg(&F->off[0]);
   const uint8_t* bm = reinterpret_cast<const uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&F->bmask)));
   double g[3];
-  if (gains) {
+  if (!MAP && gains) {
 #pragma unroll
     for (int c = 0; c < 3; ++c) g[c] = __ldg(gains + 3 * k + c);
   }
@@ -336,13 +390,31 @@ __global__ void __launch_bounds__(256) multiband_base_kernel(const MultibandFram
     int v[3];
     bool valid = mb_roi_warp(s, h, w, mi, sx, sy, bw, v) && ix == sx && iy == sy;
     if (bm) valid = ix == sx && iy == sy && __ldg(bm + (int64_t)sy * rw + sx) != 0;
-    if (gains) {
+    if (MAP) {
+      float gf[3];
+      gm_gains(gmap + k, sx, sy, gf);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) v[c] = ex_apply_f(v[c], gf[c]);
+    } else if (gains) {
 #pragma unroll
       for (int c = 0; c < 3; ++c) v[c] = ex_apply(v[c], g[c]);
     }
     G[off + e] = make_uchar4((unsigned char)v[0], (unsigned char)v[1], (unsigned char)v[2], 0);
     Wt[off + e] = valid ? 256 : 0;
   }
+}
+
+__global__ void __launch_bounds__(256) multiband_base_kernel(const MultibandFrame* __restrict__ fr, const double* __restrict__ M,
+                                                             const double* __restrict__ gains, uchar4* __restrict__ G,
+                                                             int16_t* __restrict__ Wt) {
+  mb_base<false>(fr, M, gains, nullptr, G, Wt);
+}
+
+// Level 0 with every frame's ROI warp compensated by its gain map.
+__global__ void __launch_bounds__(256) gainmap_mb_base_kernel(const MultibandFrame* __restrict__ fr, const double* __restrict__ M,
+                                                                     const GainMapDev* __restrict__ gmap, uchar4* __restrict__ G,
+                                                                     int16_t* __restrict__ Wt) {
+  mb_base<true>(fr, M, nullptr, gmap, G, Wt);
 }
 
 // Level lvl -> lvl + 1 of every frame's G and W: cv2.pyrDown (taps 1 4 6 4 1, BORDER_REFLECT_101, (sum + 128) >> 8).
@@ -717,6 +789,285 @@ __global__ void __launch_bounds__(256) exposure_stats_kernel(const ExposureFrame
   }
 }
 
+// ---- block exposure compensation (cv2.detail's block compensators; oracle/exposure_blocks.py) ----------------------------
+// The statistics of every block pair, in one pass over the canvas laid out as exposure_stats_kernel: the CTA's frames in
+// ascending order, two chunks per round, each frame's compensated value, validity and block (bx, by) per row in shared
+// memory.  A listed frame pair's block pair at a pixel names one cell of the pair's merged block grid (udh.h), so each
+// warp groups its lanes by cell (__match_any_sync), sums each group's terms with __reduce_add_sync and its leader adds
+// them to the cell's global sums.  Every sum is an integer: the result does not depend on the order or the run.
+struct ExposureBlockFrame {
+  double mi[9];                    // cv_invert3 of M'_k (frame -> its ROI)
+  const uint8_t* src;
+  int h, w;
+  int rx, ry, rw, rh, bw;          // the ROI on the canvas and the ROI warp's tile width
+  int bkw, bkh, bpx;               // the blocks' width and height, blocks per row
+  int64_t boff;                    // the frame's first block
+};
+
+__global__ void gainblock_invert_kernel(const double* __restrict__ M, ExposureBlockFrame* fr, int n) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < n) cv_invert3(M + (int64_t)k * 9, fr[k].mi);
+}
+
+__global__ void __launch_bounds__(256) gainblock_stats_kernel(const ExposureBlockFrame* __restrict__ fr, int n,
+                                                                   const int32_t* __restrict__ pair_ptr,
+                                                                   const int32_t* __restrict__ pair_j,
+                                                                   const int64_t* __restrict__ cell_off,
+                                                                   const int32_t* __restrict__ cell_nx, const double* __restrict__ hist,
+                                                                   int64_t nblocks, int feeds, int norms,
+                                                                   unsigned long long* __restrict__ stats) {
+  __shared__ int cand[UDH_EXPOSURE_MAX_FRAMES];
+  __shared__ int wcount[8], nchunks;
+  __shared__ uchar4 val[2 * EX_CHUNK][256];                             // .w: valid
+  __shared__ short2 blk[2 * EX_CHUNK][256];
+  __shared__ long long soff[EX_PAIRS];                                  // the slot's cell offset, -1: no listed pair
+  __shared__ int snx[EX_PAIRS], sb0[EX_PAIRS][4];                       // cells per row; bx_i0, by_i0, bx_j0, by_j0
+  const int tx0 = blockIdx.x * EX_TILE_W, ty0 = blockIdx.y * EX_TILE_H;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int nc = 0;
+  for (int c0 = 0; c0 < n; c0 += blockDim.x) {
+    const int k = c0 + threadIdx.x;
+    bool hit = false;
+    if (k < n) {
+      const ExposureBlockFrame* F = fr + k;
+      const int rx = __ldg(&F->rx), ry = __ldg(&F->ry);
+      hit = rx < tx0 + EX_TILE_W && rx + __ldg(&F->rw) > tx0 && ry < ty0 + EX_TILE_H && ry + __ldg(&F->rh) > ty0;
+    }
+    const unsigned bal = __ballot_sync(0xffffffffu, hit);
+    if (lane == 0) wcount[warp] = __popc(bal);
+    __syncthreads();
+    int base = nc, tot = 0;
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      base += q < warp ? wcount[q] : 0;
+      tot += wcount[q];
+    }
+    if (hit) cand[base + __popc(bal & ((1u << lane) - 1u))] = k;
+    nc += tot;
+    __syncthreads();
+  }
+  // the chunk count is re-read from shared memory: kept in a register it lives across the warp's double-division call
+  // and ptxas spills it
+  if (threadIdx.x == 0) nchunks = (nc + EX_CHUNK - 1) / EX_CHUNK;
+  __syncthreads();
+  for (int A = 0; A < *(volatile int*)&nchunks; ++A) {
+    for (int B = A; B < *(volatile int*)&nchunks; ++B) {
+      if (threadIdx.x < EX_PAIRS) {
+        const int a = threadIdx.x / EX_CHUNK, b = threadIdx.x % EX_CHUNK, ka = A * EX_CHUNK + a, kb = B * EX_CHUNK + b;
+        long long o = -1;
+        if (ka < nc && kb < nc && (A != B || a <= b)) {
+          const int i = cand[ka], j = cand[kb];
+          int lo = __ldg(pair_ptr + i), hi = __ldg(pair_ptr + i + 1);
+          while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (__ldg(pair_j + mid) < j) lo = mid + 1; else hi = mid;
+          }
+          if (lo < __ldg(pair_ptr + i + 1) && __ldg(pair_j + lo) == j) {
+            const ExposureBlockFrame *Fi = fr + i, *Fj = fr + j;
+            const int x0 = max(__ldg(&Fi->rx), __ldg(&Fj->rx)), y0 = max(__ldg(&Fi->ry), __ldg(&Fj->ry));
+            o = __ldg(cell_off + lo);
+            snx[threadIdx.x] = __ldg(cell_nx + lo);
+            sb0[threadIdx.x][0] = (x0 - __ldg(&Fi->rx)) / __ldg(&Fi->bkw);
+            sb0[threadIdx.x][1] = (y0 - __ldg(&Fi->ry)) / __ldg(&Fi->bkh);
+            sb0[threadIdx.x][2] = (x0 - __ldg(&Fj->rx)) / __ldg(&Fj->bkw);
+            sb0[threadIdx.x][3] = (y0 - __ldg(&Fj->ry)) / __ldg(&Fj->bkh);
+          }
+        }
+        soff[threadIdx.x] = o;
+      }
+      __syncthreads();
+      const int nA = min(EX_CHUNK, nc - A * EX_CHUNK), nB = A == B ? 0 : min(EX_CHUNK, nc - B * EX_CHUNK);
+      for (int r = warp; r < EX_TILE_H; r += 8) {
+        const int x = tx0 + lane, y = ty0 + r;
+        for (int q = 0; q < nA + nB; ++q) {
+          const int k = cand[q < nA ? A * EX_CHUNK + q : B * EX_CHUNK + q - nA];
+          const ExposureBlockFrame* F = fr + k;
+          const int sx = x - __ldg(&F->rx), sy = y - __ldg(&F->ry);
+          int v[3] = {0, 0, 0};
+          bool ok = false;
+          int bx = 0, by = 0;
+          if ((unsigned)sx < (unsigned)__ldg(&F->rw) && (unsigned)sy < (unsigned)__ldg(&F->rh)) {
+            double mi[9];
+#pragma unroll
+            for (int t = 0; t < 9; ++t) mi[t] = __ldg(F->mi + t);
+            const uint8_t* s = reinterpret_cast<const uint8_t*>(__ldg(reinterpret_cast<const unsigned long long*>(&F->src)));
+            ok = mb_roi_warp(s, __ldg(&F->h), __ldg(&F->w), mi, sx, sy, __ldg(&F->bw), v);
+            bx = sx / __ldg(&F->bkw);
+            by = sy / __ldg(&F->bkh);
+            const int64_t b = __ldg(&F->boff) + (int64_t)by * __ldg(&F->bpx) + bx;
+            for (int f = 0; f < feeds; ++f) {
+#pragma unroll
+              for (int c = 0; c < 3; ++c) v[c] = ex_apply(v[c], __ldg(hist + ((int64_t)f * nblocks + b) * 3 + c));
+            }
+          }
+          const int slot = q < nA ? q : EX_CHUNK + q - nA;
+          val[slot][threadIdx.x] = make_uchar4(v[0], v[1], v[2], ok);
+          blk[slot][threadIdx.x] = make_short2((short)bx, (short)by);
+        }
+        __syncwarp();
+        for (int t = 0; t < EX_PAIRS; ++t) {
+          const long long o = soff[t];
+          if (o < 0) continue;
+          const int a = t / EX_CHUNK, b = A == B ? t % EX_CHUNK : EX_CHUNK + t % EX_CHUNK;
+          const uchar4 u = val[a][threadIdx.x], w = val[b][threadIdx.x];
+          const bool both = u.w && w.w;
+          if (!__any_sync(0xffffffffu, both)) continue;
+          const short2 bu = blk[a][threadIdx.x], bv = blk[b][threadIdx.x];
+          const int cell = (int)o + (bu.y - sb0[t][1] + bv.y - sb0[t][3]) * snx[t] + (bu.x - sb0[t][0] + bv.x - sb0[t][2]);
+          const unsigned grp = __match_any_sync(0xffffffffu, both ? cell : -1);
+          const bool leader = both && lane == __ffs(grp) - 1;         // lanes without the pair form one group that adds nothing
+          unsigned long long* dst = stats + (int64_t)cell * UDH_EXPOSURE_STATS;
+          auto add = [&](int q, unsigned v) {
+            const unsigned tot = __reduce_add_sync(grp, v);                // < 2^26: 32 lanes of < 2^21
+            if (leader && tot) atomicAdd(dst + q, (unsigned long long)tot);
+          };
+          add(0, 1u);
+          add(1, u.x); add(2, u.y); add(3, u.z);
+          add(4, w.x); add(5, w.y); add(6, w.z);
+          if (norms) {
+            const uint64_t qu = __double2ull_rn(__dmul_rn(__dsqrt_rn((double)(u.x * u.x + u.y * u.y + u.z * u.z)), 0x1p52));
+#pragma unroll
+            for (int l = 0; l < 3; ++l) add(7 + l, (unsigned)(qu >> (21 * l)) & 0x1fffffu);
+            const uint64_t qw = __double2ull_rn(__dmul_rn(__dsqrt_rn((double)(w.x * w.x + w.y * w.y + w.z * w.z)), 0x1p52));
+#pragma unroll
+            for (int l = 0; l < 3; ++l) add(10 + l, (unsigned)(qw >> (21 * l)) & 0x1fffffu);
+          }
+        }
+        __syncwarp();
+      }
+      __syncthreads();
+    }
+  }
+}
+
+// Jacobi-preconditioned conjugate gradients in one CTA.  Each thread owns rows tid, tid + blockDim.x, ..; every reduction
+// is a fixed butterfly per warp and then over the warps, so all threads see the same bits and the run repeats exactly.
+constexpr int SOLVE_THREADS = 1024;
+
+__device__ __forceinline__ double2 solve_sum2(double2 v, double2* red) {
+#pragma unroll
+  for (int o = 16; o >= 1; o >>= 1) {
+    v.x += __shfl_xor_sync(0xffffffffu, v.x, o);
+    v.y += __shfl_xor_sync(0xffffffffu, v.y, o);
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) red[warp] = v;
+  __syncthreads();
+  if (warp == 0) {
+    v = lane < (int)(blockDim.x >> 5) ? red[lane] : make_double2(0.0, 0.0);
+#pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) {
+      v.x += __shfl_xor_sync(0xffffffffu, v.x, o);
+      v.y += __shfl_xor_sync(0xffffffffu, v.y, o);
+    }
+    if (lane == 0) red[32] = v;
+  }
+  __syncthreads();
+  v = red[32];
+  __syncthreads();
+  return v;
+}
+
+__device__ __forceinline__ double csr_row(const int32_t* __restrict__ row_ptr, const int32_t* __restrict__ col,
+                                          const double* __restrict__ val, const double* v, int i) {
+  double s = 0.0;
+  for (int e = __ldg(row_ptr + i); e < __ldg(row_ptr + i + 1); ++e) s += __ldg(val + e) * v[__ldg(col + e)];
+  return s;
+}
+
+__global__ void __launch_bounds__(SOLVE_THREADS) gainblock_solve_kernel(int n, const int32_t* __restrict__ row_ptr,
+                                                                             const int32_t* __restrict__ col,
+                                                                             const double* __restrict__ val,
+                                                                             const double* __restrict__ b, double tol, int max_iter,
+                                                                             double* __restrict__ x, int64_t* __restrict__ info,
+                                                                             double* __restrict__ r, double* __restrict__ p,
+                                                                             double* __restrict__ q, double* __restrict__ dinv) {
+  __shared__ double2 red[33];
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    x[i] = 1.0;
+    double d = 0.0;
+    for (int e = __ldg(row_ptr + i); e < __ldg(row_ptr + i + 1); ++e)
+      if (__ldg(col + e) == i) d = __ldg(val + e);
+    dinv[i] = 1.0 / d;
+  }
+  __syncthreads();
+  double2 acc = make_double2(0.0, 0.0);
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    const double ri = __ldg(b + i) - csr_row(row_ptr, col, val, x, i);
+    r[i] = ri;
+    p[i] = dinv[i] * ri;
+    acc.x += ri * p[i];
+    acc.y += __ldg(b + i) * __ldg(b + i);
+  }
+  const double2 s0 = solve_sum2(acc, red);
+  double rz = s0.x;
+  const double bn = sqrt(s0.y);
+  acc = make_double2(0.0, 0.0);
+  for (int i = threadIdx.x; i < n; i += blockDim.x) acc.x += r[i] * r[i];
+  double rel = sqrt(solve_sum2(acc, red).x) / bn;
+  int it = 0;
+  while (it < max_iter && rel > tol) {
+    acc = make_double2(0.0, 0.0);
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+      const double qi = csr_row(row_ptr, col, val, p, i);
+      q[i] = qi;
+      acc.x += p[i] * qi;
+    }
+    const double alpha = rz / solve_sum2(acc, red).x;
+    acc = make_double2(0.0, 0.0);
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+      x[i] += alpha * p[i];
+      const double ri = r[i] - alpha * q[i];
+      r[i] = ri;
+      acc.x += ri * ri;
+      acc.y += ri * (dinv[i] * ri);
+    }
+    const double2 s = solve_sum2(acc, red);
+    rel = sqrt(s.x) / bn;
+    const double beta = s.y / rz;
+    rz = s.y;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) p[i] = dinv[i] * r[i] + beta * p[i];
+    __syncthreads();
+    ++it;
+  }
+  if (threadIdx.x == 0) {
+    info[0] = it;
+    info[1] = __double_as_longlong(rel);
+  }
+}
+
+// The gain maps: one CTA per frame, float32(gains) filtered twice in place (tmp holds each row pass).
+__device__ __forceinline__ int gm_reflect(int i, int n) { return n == 1 ? 0 : i < 0 ? -i : i >= n ? 2 * n - 2 - i : i; }
+
+__global__ void __launch_bounds__(256) gainblock_maps_kernel(const double* __restrict__ gains, const int4* __restrict__ fb, int ch,
+                                                                 float* __restrict__ maps, float* __restrict__ tmp) {
+  const int4 f = fb[blockIdx.x];                                      // bpx, bpy, boff (low, high)
+  const int bpx = f.x, bpy = f.y;
+  const int64_t boff = (int64_t)(unsigned)f.z | ((int64_t)f.w << 32);
+  const int ne = bpx * bpy * ch;
+  float* a = maps + boff * ch;
+  float* t = tmp + boff * ch;
+  for (int e = threadIdx.x; e < ne; e += blockDim.x) a[e] = (float)__ldg(gains + (boff + e / ch) * 3 + e % ch);
+  __syncthreads();
+  for (int pass = 0; pass < 2; ++pass) {
+    for (int e = threadIdx.x; e < ne; e += blockDim.x) {
+      const int c = e % ch, bx = e / ch % bpx, by = e / ch / bpx;
+      const float* row = a + (int64_t)by * bpx * ch + c;
+      t[e] = __fadd_rn(__fmul_rn(__fadd_rn(row[gm_reflect(bx - 1, bpx) * ch], row[gm_reflect(bx + 1, bpx) * ch]), 0.25f),
+                       __fmul_rn(row[bx * ch], 0.5f));
+    }
+    __syncthreads();
+    for (int e = threadIdx.x; e < ne; e += blockDim.x) {
+      const int c = e % ch, bx = e / ch % bpx, by = e / ch / bpx;
+      const float* cl = t + (int64_t)bx * ch + c;
+      const int64_t st = (int64_t)bpx * ch;
+      a[e] = __fadd_rn(__fmul_rn(__fadd_rn(cl[gm_reflect(by - 1, bpy) * st], cl[gm_reflect(by + 1, bpy) * st]), 0.25f),
+                       __fmul_rn(cl[by * st], 0.5f));
+    }
+    __syncthreads();
+  }
+}
+
 // ---- seam finding: cv2.detail's Voronoi seam finder on the ROI validity masks (the rule: oracle/seam.py) ---------------
 // Every fed frame's mask lives on its ROI (rh x rw bytes at element offset off of a pool).  The pairs are visited on the host
 // in cv2's order; each pair runs two kernels over its window (the ROIs' intersection grown by SEAM_GAP): the column pass
@@ -960,23 +1311,60 @@ extern "C" size_t udh_mosaic_blend_masked_workspace_bytes(int n) {
   return n > 0 ? mb_align((size_t)n * sizeof(MosaicFrame)) + (size_t)n * sizeof(SeamMask) : 0;
 }
 
+extern "C" size_t udh_mosaic_blend_gainmap_workspace_bytes(int n) {
+  return n > 0 ? mb_align((size_t)n * sizeof(MosaicFrame)) + mb_align((size_t)n * sizeof(SeamMask)) + (size_t)n * sizeof(GainMapDev) : 0;
+}
+
+// The device table of n gain maps on the rectangles rois [n,4] (an empty rectangle: the frame has no map and counts nowhere).
+static int gm_table(const udh_gain_map* maps, const int32_t* rois, int n, int dst_h, int dst_w, std::vector<GainMapDev>& out,
+                    const char* what) {
+  UDH_REQUIRE(maps && rois, "%s: null maps or rois", what);
+  for (int k = 0; k < n; ++k) {
+    const int* r = rois + 4 * k;
+    GainMapDev& G = out[(size_t)k];
+    G = GainMapDev{};
+    if (r[2] <= r[0] || r[3] <= r[1]) continue;
+    UDH_REQUIRE(r[0] >= 0 && r[1] >= 0 && r[2] <= dst_w && r[3] <= dst_h, "%s: frame %d's rectangle (%d, %d)..(%d, %d) leaves the %dx%d canvas",
+                what, k, r[0], r[1], r[2], r[3], dst_h, dst_w);
+    const udh_gain_map& m = maps[k];
+    UDH_REQUIRE(m.map && m.cols && m.rows && m.bpx >= 1 && m.bpy >= 1 && (m.channels == 1 || m.channels == 3),
+                "%s: frame %d's gain map is malformed (%dx%d blocks, %d channels)", what, k, m.bpy, m.bpx, m.channels);
+    G.m = m;
+    G.rx = r[0]; G.ry = r[1]; G.rw = r[2] - r[0]; G.rh = r[3] - r[1];
+  }
+  return UDH_OK;
+}
+
 // masks (null: none) with mrois [n,4]: each frame's blend mask on its rectangle (x_lo, y_lo, x_hi, y_hi); an empty one
 // keeps the frame out of the blend.
 static int mosaic_blend(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains, int n, int c,
                         const int32_t* tile_ptr, const int32_t* tile_frames, int dst_h, int dst_w, int feather, uint8_t* dst,
                         uint8_t* mask, void* ws, size_t ws_bytes, void* stream, const uint8_t* const* masks = nullptr,
-                        const int32_t* mrois = nullptr) {
+                        const int32_t* mrois = nullptr, const udh_gain_map* gmaps = nullptr) {
   UDH_REQUIRE(tile_ptr && tile_frames && dst && mask && (n == 0 || (frames && sizes && M && ws)), "udh_mosaic_blend_u8: null pointer");
   UDH_REQUIRE(c == 1 || c == 3, "udh_mosaic_blend_u8: channels must be 1 or 3 (got %d)", c);
   UDH_REQUIRE(n >= 0 && n <= 65535 && dst_h >= 1 && dst_w >= 1 && dst_h < 32767 && dst_w < 32767,
               "udh_mosaic_blend_u8: bad dimensions (n %d, canvas %dx%d)", n, dst_h, dst_w);
   UDH_REQUIRE(feather >= 0 && feather <= 1024, "udh_mosaic_blend_u8: feather must be in [0, 1024] (got %d)", feather);
-  const size_t need = masks ? udh_mosaic_blend_masked_workspace_bytes(n) : udh_mosaic_workspace_bytes(n);
+  const size_t need = gmaps ? udh_mosaic_blend_gainmap_workspace_bytes(n)
+                     : masks ? udh_mosaic_blend_masked_workspace_bytes(n) : udh_mosaic_workspace_bytes(n);
   if (ws_bytes < need) {
     set_error("udh_mosaic_blend_u8: workspace of %zu bytes, %zu needed", ws_bytes, need);
     return UDH_EWS;
   }
   const cudaStream_t st = as_stream(stream);
+  const size_t off_gm = mb_align((size_t)n * sizeof(MosaicFrame)) + mb_align((size_t)n * sizeof(SeamMask));
+  if (gmaps && n > 0) {
+    std::vector<GainMapDev> gm((size_t)n);
+    int rc = gm_table(gmaps, mrois, n, dst_h, dst_w, gm, "udh_mosaic_blend_gainmap_u8");
+    if (rc != UDH_OK) return rc;
+    const cudaError_t e = cudaMemcpyAsync(static_cast<char*>(ws) + off_gm, gm.data(), (size_t)n * sizeof(GainMapDev),
+                                          cudaMemcpyHostToDevice, st);
+    if (e != cudaSuccess) {
+      set_error("udh_mosaic_blend_gainmap_u8: map table copy: %s", cudaGetErrorString(e));
+      return UDH_ECUDA;
+    }
+  }
   if (masks && n > 0) {
     std::vector<SeamMask> sm((size_t)n, SeamMask{nullptr, 0, 0, 0, 0});
     for (int k = 0; k < n; ++k) {
@@ -1020,6 +1408,21 @@ static int mosaic_blend(const uint8_t* const* frames, const int32_t* sizes, cons
   const dim3 grid((unsigned)((dst_w + UDH_MOSAIC_TILE_W - 1) / UDH_MOSAIC_TILE_W),
                   (unsigned)((dst_h + UDH_MOSAIC_TILE_H - 1) / UDH_MOSAIC_TILE_H));
   const MosaicFrame* fr = static_cast<const MosaicFrame*>(ws);
+  if (gmaps) {
+    const SeamMask* sm = masks ? reinterpret_cast<const SeamMask*>(static_cast<const char*>(ws) + mb_align((size_t)n * sizeof(MosaicFrame)))
+                               : nullptr;
+    const GainMapDev* gm = reinterpret_cast<const GainMapDev*>(static_cast<const char*>(ws) + off_gm);
+    const int f32 = 32 * feather;
+    if (masks && c == 3)
+      gainmap_blend_u8_kernel<3, true><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, f32, sm, gm, dst, mask);
+    else if (masks)
+      gainmap_blend_u8_kernel<1, true><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, f32, sm, gm, dst, mask);
+    else if (c == 3)
+      gainmap_blend_u8_kernel<3, false><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, f32, sm, gm, dst, mask);
+    else
+      gainmap_blend_u8_kernel<1, false><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, f32, sm, gm, dst, mask);
+    return check_launch("udh_mosaic_blend_gainmap_u8");
+  }
   if (masks) {
     const SeamMask* sm = reinterpret_cast<const SeamMask*>(static_cast<const char*>(ws) + mb_align((size_t)n * sizeof(MosaicFrame)));
     const int f32 = 32 * feather;
@@ -1077,14 +1480,16 @@ extern "C" int udh_debug_multiband_layout(const int32_t* rois, int n, int dst_h,
 
 static int mosaic_multiband(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains,
                             const int32_t* rois, int n, int c, int dst_h, int dst_w, int bands, uint8_t* dst, uint8_t* mask, void* ws,
-                            size_t ws_bytes, void* stream, const uint8_t* const* masks = nullptr) {
+                            size_t ws_bytes, void* stream, const uint8_t* const* masks = nullptr,
+                            const udh_gain_map* gmaps = nullptr) {
   UDH_REQUIRE(frames && sizes && M && rois && dst && mask && ws, "udh_mosaic_multiband_u8: null pointer");
   UDH_REQUIRE(c == 3, "udh_mosaic_multiband_u8: channels must be 3 (got %d)", c);
   MultibandPlan p;
   int rc = mb_plan(rois, sizes, n, dst_h, dst_w, bands, p);
   if (rc != UDH_OK) return rc;
-  if (ws_bytes < p.total) {
-    set_error("udh_mosaic_multiband_u8: workspace of %zu bytes, %zu needed", ws_bytes, p.total);
+  const size_t need = p.total + (gmaps ? (size_t)n * sizeof(GainMapDev) : 0);
+  if (ws_bytes < need) {
+    set_error("udh_mosaic_multiband_u8: workspace of %zu bytes, %zu needed", ws_bytes, need);
     return UDH_EWS;
   }
   for (int k = 0; k < n; ++k) {
@@ -1103,6 +1508,16 @@ static int mosaic_multiband(const uint8_t* const* frames, const int32_t* sizes, 
     set_error("udh_mosaic_multiband_u8: frame table copy: %s", cudaGetErrorString(e));
     return UDH_ECUDA;
   }
+  GainMapDev* gm = reinterpret_cast<GainMapDev*>(base + p.total);
+  if (gmaps) {
+    std::vector<GainMapDev> host((size_t)n);
+    if ((rc = gm_table(gmaps, rois, n, dst_h, dst_w, host, "udh_mosaic_multiband_gainmap_u8")) != UDH_OK) return rc;
+    const cudaError_t e2 = cudaMemcpyAsync(gm, host.data(), (size_t)n * sizeof(GainMapDev), cudaMemcpyHostToDevice, st);
+    if (e2 != cudaSuccess) {
+      set_error("udh_mosaic_multiband_gainmap_u8: map table copy: %s", cudaGetErrorString(e2));
+      return UDH_ECUDA;
+    }
+  }
   const MultibandFrame* fr = reinterpret_cast<const MultibandFrame*>(base);
   uchar4* G = reinterpret_cast<uchar4*>(base + p.off_g);
   int16_t* Wt = reinterpret_cast<int16_t*>(base + p.off_w);
@@ -1110,7 +1525,10 @@ static int mosaic_multiband(const uint8_t* const* frames, const int32_t* sizes, 
   auto R = [&](int i) { return reinterpret_cast<short4*>(base + p.off_r[i]); };
   {
     ProfScope ps(PROF_MB_BASE, st);
-    multiband_base_kernel<<<dim3(mb_blocks(p.max_px[0]), (unsigned)n), 256, 0, st>>>(fr, M, gains, G, Wt);
+    if (gmaps)
+      gainmap_mb_base_kernel<<<dim3(mb_blocks(p.max_px[0]), (unsigned)n), 256, 0, st>>>(fr, M, gm, G, Wt);
+    else
+      multiband_base_kernel<<<dim3(mb_blocks(p.max_px[0]), (unsigned)n), 256, 0, st>>>(fr, M, gains, G, Wt);
     if ((rc = check_launch("udh_mosaic_multiband_u8 (base)")) != UDH_OK) return rc;
   }
   {
@@ -1327,4 +1745,141 @@ extern "C" int udh_mosaic_seam_masks_u8(const uint8_t* const* frames, const int3
   }
   seam_blend_mask_kernel<<<dim3(mb_blocks(p.max_px), (unsigned)n), 256, 0, st>>>(fr, seam, blend);
   return check_launch("udh_mosaic_seam_masks_u8 (blend masks)");
+}
+
+extern "C" int udh_mosaic_blend_gainmap_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const udh_gain_map* maps,
+                                           const uint8_t* const* masks, const int32_t* rois, int n, int c, const int32_t* tile_ptr,
+                                           const int32_t* tile_frames, int dst_h, int dst_w, int feather, uint8_t* dst, uint8_t* mask,
+                                           void* ws, size_t ws_bytes, void* stream) {
+  UDH_REQUIRE(n >= 1 && maps && rois, "udh_mosaic_blend_gainmap_u8: no frames, or null maps or rois");
+  return mosaic_blend(frames, sizes, M, nullptr, n, c, tile_ptr, tile_frames, dst_h, dst_w, feather, dst, mask, ws, ws_bytes, stream,
+                      masks, rois, maps);
+}
+
+extern "C" size_t udh_mosaic_multiband_gainmap_workspace_bytes(const int32_t* rois, int n, int dst_h, int dst_w, int bands) {
+  MultibandPlan p;
+  return mb_plan(rois, nullptr, n, dst_h, dst_w, bands, p) == UDH_OK ? p.total + (size_t)n * sizeof(GainMapDev) : 0;
+}
+
+extern "C" int udh_mosaic_multiband_gainmap_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M,
+                                               const udh_gain_map* maps, const uint8_t* const* masks, const int32_t* rois, int n, int c,
+                                               int dst_h, int dst_w, int bands, uint8_t* dst, uint8_t* mask, void* ws, size_t ws_bytes,
+                                               void* stream) {
+  UDH_REQUIRE(maps, "udh_mosaic_multiband_gainmap_u8: null maps");
+  return mosaic_multiband(frames, sizes, M, nullptr, rois, n, c, dst_h, dst_w, bands, dst, mask, ws, ws_bytes, stream, masks, maps);
+}
+
+extern "C" size_t udh_mosaic_exposure_block_workspace_bytes(int n) { return n > 0 ? (size_t)n * sizeof(ExposureBlockFrame) : 0; }
+
+extern "C" int udh_mosaic_exposure_block_stats_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const int32_t* rois,
+                                                  int n, const int32_t* blocks, const int64_t* boff, int64_t nblocks,
+                                                  const int32_t* pair_ptr, const int32_t* pair_j, int npairs, const int64_t* cell_off,
+                                                  const int32_t* cell_nx, int64_t nslots, const double* history, int feeds, int norms,
+                                                  int dst_h, int dst_w, uint64_t* stats, void* ws, size_t ws_bytes, void* stream) {
+  const char* what = "udh_mosaic_exposure_block_stats_u8";
+  UDH_REQUIRE(frames && sizes && M && rois && blocks && boff && pair_ptr && pair_j && cell_off && cell_nx && stats && ws &&
+                  (feeds == 0 || history),
+              "%s: null pointer", what);
+  UDH_REQUIRE(n >= 1 && n <= UDH_EXPOSURE_MAX_FRAMES && dst_h >= 1 && dst_w >= 1 && dst_h < 32767 && dst_w < 32767,
+              "%s: bad dimensions (n %d of at most %d, canvas %dx%d)", what, n, UDH_EXPOSURE_MAX_FRAMES, dst_h, dst_w);
+  UDH_REQUIRE(npairs >= n && npairs <= n * (n + 1) / 2 && feeds >= 0 && feeds <= UDH_EXPOSURE_MAX_FEEDS,
+              "%s: %d pairs of %d frames, %d feeds (at most %d)", what, npairs, n, feeds, UDH_EXPOSURE_MAX_FEEDS);
+  UDH_REQUIRE(nblocks >= n && nblocks <= UDH_EXPOSURE_MAX_BLOCKS && nslots >= 1,
+              "%s: %lld blocks (at most %d), %lld cells", what, (long long)nblocks, UDH_EXPOSURE_MAX_BLOCKS, (long long)nslots);
+  if (ws_bytes < udh_mosaic_exposure_block_workspace_bytes(n)) {
+    set_error("%s: workspace of %zu bytes, %zu needed", what, ws_bytes, udh_mosaic_exposure_block_workspace_bytes(n));
+    return UDH_EWS;
+  }
+  std::vector<ExposureBlockFrame> host((size_t)n);
+  for (int k = 0; k < n; ++k) {
+    const int* r = rois + 4 * k;
+    UDH_REQUIRE(r[0] >= 0 && r[1] >= 0 && r[0] < r[2] && r[1] < r[3] && r[2] <= dst_w && r[3] <= dst_h,
+                "%s: frame %d's ROI (%d, %d)..(%d, %d) is empty or leaves the %dx%d canvas", what, k, r[0], r[1], r[2], r[3], dst_h,
+                dst_w);
+    UDH_REQUIRE(frames[k], "%s: frame %d is a null pointer", what, k);
+    ExposureBlockFrame& F = host[k];
+    F.src = frames[k];
+    F.h = sizes[2 * k];
+    F.w = sizes[2 * k + 1];
+    UDH_REQUIRE(F.h >= 1 && F.w >= 1 && F.h < 32767 && F.w < 32767, "%s: frame %d is %dx%d", what, k, F.h, F.w);
+    F.rx = r[0]; F.ry = r[1]; F.rw = r[2] - r[0]; F.rh = r[3] - r[1];
+    const int bh = F.rh < 16 ? F.rh : 16;
+    F.bw = 1024 / bh < F.rw ? 1024 / bh : F.rw;                      // the ROI warp's tile width, as mb_plan sets it
+    F.bkw = blocks[4 * k];
+    F.bkh = blocks[4 * k + 1];
+    F.bpx = blocks[4 * k + 2];
+    F.boff = boff[k];
+    UDH_REQUIRE(F.bkw >= 1 && F.bkh >= 1 && F.bpx == (F.rw + F.bkw - 1) / F.bkw &&
+                    blocks[4 * k + 3] == (F.rh + F.bkh - 1) / F.bkh && F.boff >= 0 && F.boff + (int64_t)F.bpx * blocks[4 * k + 3] <= nblocks,
+                "%s: frame %d's blocks (%dx%d, %d per row, from %lld) do not tile its %dx%d ROI within %lld blocks", what, k, F.bkw,
+                F.bkh, F.bpx, (long long)F.boff, F.rw, F.rh, (long long)nblocks);
+  }
+  const cudaStream_t st = as_stream(stream);
+  cudaError_t e = cudaMemcpyAsync(ws, host.data(), (size_t)n * sizeof(ExposureBlockFrame), cudaMemcpyHostToDevice, st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(stats, 0, (size_t)nslots * UDH_EXPOSURE_STATS * sizeof(uint64_t), st);
+  if (e != cudaSuccess) {
+    set_error("%s: %s", what, cudaGetErrorString(e));
+    return UDH_ECUDA;
+  }
+  ExposureBlockFrame* fr = static_cast<ExposureBlockFrame*>(ws);
+  gainblock_invert_kernel<<<(n + 127) / 128, 128, 0, st>>>(M, fr, n);
+  int rc = check_launch("udh_mosaic_exposure_block_stats_u8 (inverses)");
+  if (rc != UDH_OK) return rc;
+  const dim3 grid((unsigned)((dst_w + EX_TILE_W - 1) / EX_TILE_W), (unsigned)((dst_h + EX_TILE_H - 1) / EX_TILE_H));
+  gainblock_stats_kernel<<<grid, 256, 0, st>>>(fr, n, pair_ptr, pair_j, cell_off, cell_nx, history, nblocks, feeds, norms,
+                                                    reinterpret_cast<unsigned long long*>(stats));
+  return check_launch(what);
+}
+
+extern "C" size_t udh_exposure_block_solve_workspace_bytes(int n) { return n > 0 ? (size_t)4 * n * sizeof(double) : 0; }
+
+extern "C" int udh_exposure_block_solve(int n, const int32_t* row_ptr, const int32_t* col, const double* val, const double* b,
+                                        double tol, int max_iter, double* x, int64_t* info, void* ws, size_t ws_bytes, void* stream) {
+  UDH_REQUIRE(row_ptr && col && val && b && x && info && ws, "udh_exposure_block_solve: null pointer");
+  UDH_REQUIRE(n >= 1 && n <= UDH_EXPOSURE_MAX_BLOCKS && max_iter >= 0 && tol >= 0.0,
+              "udh_exposure_block_solve: n %d (at most %d), max_iter %d, tol %g", n, UDH_EXPOSURE_MAX_BLOCKS, max_iter, tol);
+  if (ws_bytes < udh_exposure_block_solve_workspace_bytes(n)) {
+    set_error("udh_exposure_block_solve: workspace of %zu bytes, %zu needed", ws_bytes, udh_exposure_block_solve_workspace_bytes(n));
+    return UDH_EWS;
+  }
+  double* w = static_cast<double*>(ws);
+  gainblock_solve_kernel<<<1, SOLVE_THREADS, 0, as_stream(stream)>>>(n, row_ptr, col, val, b, tol, max_iter, x, info, w, w + n,
+                                                                          w + 2 * (size_t)n, w + 3 * (size_t)n);
+  return check_launch("udh_exposure_block_solve");
+}
+
+extern "C" size_t udh_exposure_gain_maps_workspace_bytes(int64_t nblocks, int channels) {
+  return nblocks > 0 && (channels == 1 || channels == 3)
+             ? mb_align((size_t)nblocks * channels * sizeof(float)) + (size_t)UDH_EXPOSURE_MAX_FRAMES * sizeof(int4)
+             : 0;
+}
+
+extern "C" int udh_exposure_gain_maps(const double* gains, int n, const int32_t* blocks, const int64_t* boff, int64_t nblocks,
+                                      int channels, float* maps, void* ws, size_t ws_bytes, void* stream) {
+  UDH_REQUIRE(gains && blocks && boff && maps && ws, "udh_exposure_gain_maps: null pointer");
+  UDH_REQUIRE(n >= 1 && n <= UDH_EXPOSURE_MAX_FRAMES && nblocks >= n && nblocks <= UDH_EXPOSURE_MAX_BLOCKS &&
+                  (channels == 1 || channels == 3),
+              "udh_exposure_gain_maps: %d frames, %lld blocks, %d channels", n, (long long)nblocks, channels);
+  if (ws_bytes < udh_exposure_gain_maps_workspace_bytes(nblocks, channels)) {
+    set_error("udh_exposure_gain_maps: workspace of %zu bytes, %zu needed", ws_bytes,
+              udh_exposure_gain_maps_workspace_bytes(nblocks, channels));
+    return UDH_EWS;
+  }
+  std::vector<int4> fb((size_t)n);
+  for (int k = 0; k < n; ++k) {
+    const int bpx = blocks[4 * k + 2], bpy = blocks[4 * k + 3];
+    UDH_REQUIRE(bpx >= 1 && bpy >= 1 && boff[k] >= 0 && boff[k] + (int64_t)bpx * bpy <= nblocks,
+                "udh_exposure_gain_maps: frame %d's %dx%d blocks from %lld exceed %lld", k, bpy, bpx, (long long)boff[k],
+                (long long)nblocks);
+    fb[(size_t)k] = make_int4(bpx, bpy, (int)(uint32_t)boff[k], (int)(boff[k] >> 32));
+  }
+  const cudaStream_t st = as_stream(stream);
+  int4* fb_d = reinterpret_cast<int4*>(static_cast<char*>(ws) + mb_align((size_t)nblocks * channels * sizeof(float)));
+  const cudaError_t e = cudaMemcpyAsync(fb_d, fb.data(), (size_t)n * sizeof(int4), cudaMemcpyHostToDevice, st);
+  if (e != cudaSuccess) {
+    set_error("udh_exposure_gain_maps: %s", cudaGetErrorString(e));
+    return UDH_ECUDA;
+  }
+  gainblock_maps_kernel<<<(unsigned)n, 256, 0, st>>>(gains, fb_d, channels, maps, static_cast<float*>(ws));
+  return check_launch("udh_exposure_gain_maps");
 }

@@ -30,7 +30,10 @@ compensation removes it.
 Exposure compensation, compensate="gain" or "channels" (default "none").  Before either blend, ops.mosaic_exposure_gains
 computes what cv2.detail_GainCompensator(compensate_feeds) (one gain per frame) or ChannelsCompensator (one per channel)
 finds for the kept frames' ROI warps (oracle/exposure.py states the rule); the blend then takes each frame's warp value
-as saturate_u8(rint(v g)).  This is the stage cv2's stitcher runs between the warp and the blender.
+as saturate_u8(rint(v g)).  This is the stage cv2's stitcher runs between the warp and the blender.  compensate=
+"gain_blocks" or "channels_blocks" runs cv2's default, the block compensators (oracle/exposure_blocks.py): a gain per
+block of about compensate_block px of each ROI warp, whose filtered map ops.mosaic_exposure_gain_maps returns and the
+blend applies per pixel, so brightness that varies across a frame (vignetting) is compensated too.
 
 Seams, seam="voronoi" (default "none").  ops.mosaic_seam_masks cuts the kept frames' validity masks apart as
 cv2.detail's Voronoi seam finder does (oracle/seam.py states the rule): pair by pair in cv2's order, each pixel of an
@@ -142,22 +145,25 @@ def farthest_frame(sizes, G, kept, ref):
     return far
 
 
-COMPENSATE = ("none", "gain", "channels")
+COMPENSATE = ("none", "gain", "channels", "gain_blocks", "channels_blocks")
 SEAM = ("none", "voronoi")
 
 
 def build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None, float32_M=False, blend="feather", bands=5,
-                 compensate="none", compensate_feeds=1, seam="none"):
+                 compensate="none", compensate_feeds=1, seam="none", compensate_block=32):
     """est: align.HomographyEstimator; frames: CUDA uint8 RGB [h_k,w_k,3] tensors in sequence order.  blend: "feather"
     (udh_mosaic_blend_u8 with `feather`) or "multiband" (udh_mosaic_multiband_u8 with `bands`).  refine: None, or a
     dict of est.refine's keyword arguments (levels, iters, eps, max_side) to refine each pair's H.  max_pixels: the canvas
     limit (None: the JPEG encoder's, udh_jpeg_encode_capacity(Hc, Wc, 3) != 0).  float32_M: blend with each M_k rounded to
     float32, the values a text file of '%.9g' float32 entries gives back.  compensate: "none", "gain" or "channels"
-    (ops.mosaic_exposure_gains with compensate_feeds feeds, applied by the blend).  seam: "none" or "voronoi"
+    (ops.mosaic_exposure_gains with compensate_feeds feeds, applied by the blend), or "gain_blocks" / "channels_blocks"
+    (ops.mosaic_exposure_gain_maps with blocks of about compensate_block px: a gain map per frame, cv2's
+    BlocksGainCompensator / BlocksChannelsCompensator; gains stay 1).  seam: "none" or "voronoi"
     (ops.mosaic_seam_masks; each frame blends only inside its blend mask).
     -> dict(mosaic uint8 [Hc,Wc,3] RGB, mask uint8 [Hc,Wc], M [N,3,3] frame k -> canvas (float64, float32 values with
     float32_M), kept bool [N], ref, H_pairs [N-1,3,3], refine (rho, status, level_reached) or None, gains float64 [N,3]
-    (1 for a dropped frame, all 1 without compensation), last_ms {prep, forward, refine, compensate, seam, blend} of
+    (1 for a dropped frame, all 1 without per-frame compensation), gain_maps [N] (the block modes only: CUDA float32
+    maps, None for a dropped frame or one whose ROI misses the canvas), last_ms {prep, forward, refine, compensate, seam, blend} of
     CUDA-event time; compensate only when compensating, seam only with seams)."""
     frames = list(frames)
     if len(frames) < 2:
@@ -179,18 +185,26 @@ def build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None
     if blend not in ("feather", "multiband"):
         raise ValueError("blend must be 'feather' or 'multiband' (got %r)" % (blend,))
     if compensate not in COMPENSATE:
-        raise ValueError("compensate must be 'none', 'gain' or 'channels' (got %r)" % (compensate,))
+        raise ValueError("compensate must be one of %s (got %r)" % (", ".join(COMPENSATE), compensate))
     if seam not in SEAM:
         raise ValueError("seam must be 'none' or 'voronoi' (got %r)" % (seam,))
     gains = np.ones((len(frames), 3))
-    if compensate != "none":
+    gain_maps = None
+    if compensate in ("gain", "channels"):
         gains[kept], ms["compensate"] = compensate_kept(frames, M, kept, Hc, Wc, compensate, compensate_feeds)
+    elif compensate != "none":
+        gain_maps, ms["compensate"] = compensate_blocks_kept(frames, M, kept, Hc, Wc, compensate[:-len("_blocks")], compensate_feeds,
+                                                             compensate_block)
     masks = None
     if seam != "none":
         masks, ms["seam"] = seam_kept(frames, M, kept, Hc, Wc)
     mosaic, mask, ms["blend"] = blend_kept(frames, M, kept, Hc, Wc, feather, blend, bands,
-                                           None if compensate == "none" else gains, masks)
-    return dict(mosaic=mosaic, mask=mask, M=M, kept=kept, ref=ref, H_pairs=H, refine=refined, gains=gains, last_ms=ms)
+                                           gains if compensate in ("gain", "channels") else None, masks,
+                                           None if gain_maps is None else [gain_maps[k] for k in range(len(frames)) if kept[k]])
+    out = dict(mosaic=mosaic, mask=mask, M=M, kept=kept, ref=ref, H_pairs=H, refine=refined, gains=gains, last_ms=ms)
+    if gain_maps is not None:
+        out["gain_maps"] = gain_maps
+    return out
 
 
 def check_encodable(Hc, Wc, sizes, G, kept, ref):
@@ -214,6 +228,23 @@ def compensate_kept(frames, M, kept, Hc, Wc, mode, feeds=1):
     return g, e0.elapsed_time(e1)
 
 
+def compensate_blocks_kept(frames, M, kept, Hc, Wc, mode, feeds=1, block=32):
+    """The kept frames' block gain maps (ops.mosaic_exposure_gain_maps) -> (maps [N], None for a dropped frame or one whose
+    ROI misses the canvas; CUDA-event ms)."""
+    import torch
+    from . import ops
+    take = [k for k in range(len(frames)) if kept[k]]
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    g = ops.mosaic_exposure_gain_maps([frames[k].contiguous() for k in take], np.asarray(M)[take], Hc, Wc, mode, feeds, block)
+    e1.record()
+    e1.synchronize()
+    maps = [None] * len(frames)
+    for q, k in enumerate(take):
+        maps[k] = g[q]
+    return maps, e0.elapsed_time(e1)
+
+
 def seam_kept(frames, M, kept, Hc, Wc):
     """The kept frames' blend masks (ops.mosaic_seam_masks) -> (masks [n_kept]: CUDA uint8 [roi_h,roi_w], None for a frame
     whose ROI misses the canvas; CUDA-event ms)."""
@@ -231,10 +262,10 @@ def seam_kept(frames, M, kept, Hc, Wc):
     return masks, e0.elapsed_time(e1)
 
 
-def blend_kept(frames, M, kept, Hc, Wc, feather, mode="feather", bands=5, gains=None, masks=None):
+def blend_kept(frames, M, kept, Hc, Wc, feather, mode="feather", bands=5, gains=None, masks=None, gain_maps=None):
     """The kept frames through ops.mosaic_blend_u8 (mode "feather") or ops.mosaic_multiband_u8 ("multiband") -> (mosaic,
     mask, CUDA-event ms).  gains: None, or [N,3] per frame (exposure compensation).  masks: None, or seam_kept's blend
-    masks of the kept frames."""
+    masks of the kept frames.  gain_maps: None, or the kept frames' block gain maps."""
     import torch
     from . import ops
     take = [k for k in range(len(frames)) if kept[k]]
@@ -243,10 +274,10 @@ def blend_kept(frames, M, kept, Hc, Wc, feather, mode="feather", bands=5, gains=
     e0.record()
     if mode == "multiband":
         mosaic, mask = ops.mosaic_multiband_u8([frames[k].contiguous() for k in take], np.asarray(M)[take], Hc, Wc, bands,
-                                               gains=g, masks=masks)
+                                               gains=g, masks=masks, gain_maps=gain_maps)
     else:
         mosaic, mask = ops.mosaic_blend_u8([frames[k].contiguous() for k in take], np.asarray(M)[take], Hc, Wc, feather,
-                                           gains=g, masks=masks)
+                                           gains=g, masks=masks, gain_maps=gain_maps)
     e1.record()
     e1.synchronize()
     return mosaic, mask, e0.elapsed_time(e1)

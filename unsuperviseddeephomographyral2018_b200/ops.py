@@ -668,7 +668,7 @@ def _mask_table(masks, rois, n, what):
     return ptrs, rr
 
 
-def mosaic_blend_u8(frames, M, dst_h, dst_w, feather, gains=None, masks=None):
+def mosaic_blend_u8(frames, M, dst_h, dst_w, feather, gains=None, masks=None, gain_maps=None):
     """frames: n CUDA uint8 tensors [h_k,w_k,C] (C = 1 or 3, sizes may differ; or one [n,h,w,C] tensor), M float64 [n,3,3]
     (frame k -> canvas; numpy or tensor) -> (mosaic uint8 [dst_h,dst_w,C], mask uint8 [dst_h,dst_w]): udh_mosaic_blend_u8's
     feathered blend of cv2.warpPerspective(frame k, M_k, (dst_w, dst_h)), bit for bit with oracle/mosaic.py.  The tile
@@ -676,7 +676,9 @@ def mosaic_blend_u8(frames, M, dst_h, dst_w, feather, gains=None, masks=None):
     mosaic_exposure_gains'): each frame's warp value is exposure-compensated first, saturate_u8(rint(v g)) in float64
     (udh_mosaic_blend_gain_u8).  masks ([n], e.g. mosaic_seam_masks' blend masks): frame k counts only where its mask,
     a CUDA uint8 [roi_h,roi_w] on its ROI (mosaic.multiband_rois), is set; a frame whose ROI misses the canvas takes None
-    and counts nowhere (udh_mosaic_blend_masked_u8)."""
+    and counts nowhere (udh_mosaic_blend_masked_u8).  gain_maps ([n], e.g. mosaic_exposure_gain_maps'; not with gains):
+    each frame's warp value is compensated by its block gain map resized to its ROI, at the pixel's ROI coordinates,
+    saturate_u8(rint(float32(v) g)) (udh_mosaic_blend_gainmap_u8)."""
     from . import mosaic
     frames = list(frames.unbind(0)) if isinstance(frames, torch.Tensor) else list(frames)
     Mh = (M.detach().cpu().numpy() if isinstance(M, torch.Tensor) else np.asarray(M)).astype(np.float64).reshape(-1, 3, 3)
@@ -701,7 +703,20 @@ def mosaic_blend_u8(frames, M, dst_h, dst_w, feather, gains=None, masks=None):
     ws = torch.empty(max(nb, 1), device=dev, dtype=torch.uint8)
     ptrs = (ctypes.c_void_p * n)(*[f.data_ptr() for f in frames])
     sz = np.ascontiguousarray(np.array(sizes, np.int32).reshape(n, 2))
-    if masks is not None:
+    if gain_maps is not None:
+        if gains is not None:
+            raise _lib.UdhError("mosaic_blend_u8: gains and gain_maps exclude each other")
+        rr = np.ascontiguousarray(mosaic.multiband_rois(Mh, sizes, int(dst_h), int(dst_w))[0].astype(np.int32))
+        gm, _keep = _gain_map_table(gain_maps, rr, n, dev, "mosaic_blend_u8")
+        mp = None
+        if masks is not None:
+            mp, rr = _mask_table(masks, rr, n, "mosaic_blend_u8")
+        nb = lib.udh_mosaic_blend_gainmap_workspace_bytes(n)
+        ws = torch.empty(max(nb, 1), device=dev, dtype=torch.uint8)
+        check(lib.udh_mosaic_blend_gainmap_u8(ptrs, sz.ctypes.data, _ptr(M_d), gm, mp, rr.ctypes.data, n, C, _ptr(ptr_d), _ptr(idx_d),
+                                              int(dst_h), int(dst_w), int(feather), _ptr(out), _ptr(mask), _ptr(ws), nb, _stream()),
+              "udh_mosaic_blend_gainmap_u8")
+    elif masks is not None:
         mp, rr = _mask_table(masks, mosaic.multiband_rois(Mh, sizes, int(dst_h), int(dst_w))[0], n, "mosaic_blend_u8")
         g_d = None if gains is None else _gains(gains, n, dev, "mosaic_blend_u8")
         nb = lib.udh_mosaic_blend_masked_workspace_bytes(n)
@@ -720,7 +735,7 @@ def mosaic_blend_u8(frames, M, dst_h, dst_w, feather, gains=None, masks=None):
     return out, mask
 
 
-def mosaic_multiband_u8(frames, M, dst_h, dst_w, bands, levels=False, gains=None, masks=None):
+def mosaic_multiband_u8(frames, M, dst_h, dst_w, bands, levels=False, gains=None, masks=None, gain_maps=None):
     """frames: n CUDA uint8 RGB tensors [h_k,w_k,3] (sizes may differ), M float64 [n,3,3] (frame k -> canvas; numpy or
     tensor) -> (mosaic uint8 [dst_h,dst_w,3], mask uint8 [dst_h,dst_w]): udh_mosaic_multiband_u8, byte for byte
     cv2.detail_MultiBandBlender(0, bands, CV_16S) fed each frame's warp on its ROI (oracle/multiband.py).  The ROIs and the
@@ -730,7 +745,9 @@ def mosaic_multiband_u8(frames, M, dst_h, dst_w, bands, levels=False, gains=None
     gains ([n] or [n,3], e.g. mosaic_exposure_gains'): each ROI warp is exposure-compensated before it is fed,
     saturate_u8(rint(v g)) in float64 (udh_mosaic_multiband_gain_u8), cv2's stitcher order.  masks ([n], e.g.
     mosaic_seam_masks' blend masks; None for a frame whose ROI misses the canvas): frame k is fed its mask, a CUDA uint8
-    [roi_h,roi_w], in place of its validity mask (udh_mosaic_multiband_masked_u8)."""
+    [roi_h,roi_w], in place of its validity mask (udh_mosaic_multiband_masked_u8).  gain_maps ([n], e.g.
+    mosaic_exposure_gain_maps'; not with gains): each ROI warp is compensated by its block gain map resized to the ROI,
+    saturate_u8(rint(float32(v) g)), before it is fed (udh_mosaic_multiband_gainmap_u8)."""
     from . import mosaic
     frames = list(frames.unbind(0)) if isinstance(frames, torch.Tensor) else list(frames)
     Mh = (M.detach().cpu().numpy() if isinstance(M, torch.Tensor) else np.asarray(M)).astype(np.float64).reshape(-1, 3, 3)
@@ -761,7 +778,25 @@ def mosaic_multiband_u8(frames, M, dst_h, dst_w, bands, levels=False, gains=None
     if nb == 0:
         raise _lib.UdhError("mosaic_multiband_u8: bad arguments (%d frames, canvas %dx%d, %d bands)" % (m, dst_h, dst_w, bands))
     ws = torch.empty(nb, device=dev, dtype=torch.uint8)
-    if masks is not None:
+    if gain_maps is not None:
+        if gains is not None:
+            raise _lib.UdhError("mosaic_multiband_u8: gains and gain_maps exclude each other")
+        gain_maps = list(gain_maps)
+        if len(gain_maps) != n:
+            raise _lib.UdhError("mosaic_multiband_u8: %d gain maps for %d frames" % (len(gain_maps), n))
+        gm, _keep = _gain_map_table([gain_maps[k] for k in take], rr, m, dev, "mosaic_multiband_u8")
+        mp = None
+        if masks is not None:
+            masks = list(masks)
+            if len(masks) != n:
+                raise _lib.UdhError("mosaic_multiband_u8: %d masks for %d frames" % (len(masks), n))
+            mp, _ = _mask_table([masks[k] for k in take], rr, m, "mosaic_multiband_u8")
+        nb = lib.udh_mosaic_multiband_gainmap_workspace_bytes(rr.ctypes.data, m, int(dst_h), int(dst_w), int(bands))
+        ws = torch.empty(nb, device=dev, dtype=torch.uint8)
+        check(lib.udh_mosaic_multiband_gainmap_u8(ptrs, sz.ctypes.data, _ptr(M_d), gm, mp, rr.ctypes.data, m, 3, int(dst_h),
+                                                  int(dst_w), int(bands), _ptr(out), _ptr(mask), _ptr(ws), nb, _stream()),
+              "udh_mosaic_multiband_gainmap_u8")
+    elif masks is not None:
         masks = list(masks)
         if len(masks) != n:
             raise _lib.UdhError("mosaic_multiband_u8: %d masks for %d frames" % (len(masks), n))
@@ -959,6 +994,304 @@ def mosaic_exposure_gains(frames, M, dst_h, dst_w, mode="gain", feeds=1):
         hist.append(g3)
     gains[st.take] = acc
     return gains
+
+
+# ------------------------------------------------------------------ block exposure compensation
+EXPOSURE_BLOCK_TOL, EXPOSURE_BLOCK_MAX_ITER = 1e-15, 2000  # udh_exposure_block_solve's stop: |r| <= tol |b|
+
+
+def exposure_block_grid(rois, block):
+    """rois [m,4] (x_lo, y_lo, x_hi, y_hi), block side -> (blocks int32 [m,4]: bw, bh, bpx, bpy; boff int64 [m+1]): cv2's
+    BlocksCompensator blocks of each ROI (bpx = ceil(roi_w / block), bw = ceil(roi_w / bpx), likewise in y), numbered
+    frame-major, then row-major, frame k's from boff[k]."""
+    r = np.asarray(rois, np.int64).reshape(-1, 4)
+    w, h = r[:, 2] - r[:, 0], r[:, 3] - r[:, 1]
+    bpx, bpy = -(-w // int(block)), -(-h // int(block))
+    bw, bh = -(-w // bpx), -(-h // bpy)
+    if ((bpx - 1) * bw >= w).any() or ((bpy - 1) * bh >= h).any():
+        raise _lib.UdhError("exposure_block_grid: a %d-px block leaves an empty block in a ROI" % block)
+    boff = np.zeros(len(r) + 1, np.int64)
+    boff[1:] = np.cumsum(bpx * bpy)
+    if boff[-1] > _lib.EXPOSURE_MAX_BLOCKS:
+        raise _lib.UdhError("exposure_block_grid: %d blocks (at most %d)" % (boff[-1], _lib.EXPOSURE_MAX_BLOCKS))
+    return np.stack([bw, bh, bpx, bpy], 1).astype(np.int32), boff
+
+
+def _block_axis(ra, ea, bwa, rb, eb, bwb, lo, hi):
+    """One axis of a frame pair: block intervals [r + i bw, min(r + (i + 1) bw, e)) of both frames over [lo, hi) -> (i_a, i_b,
+    cell) of every intersecting pair of intervals, the number of cells, and the first blocks i_a0, i_b0."""
+    a0, a1 = (lo - ra) // bwa, (hi - 1 - ra) // bwa
+    b0, b1 = (lo - rb) // bwb, (hi - 1 - rb) // bwb
+    ia, ib = np.arange(a0, a1 + 1), np.arange(b0, b1 + 1)
+    x0 = np.maximum(ra + ia[:, None] * bwa, rb + ib[None, :] * bwb)
+    x1 = np.minimum(np.minimum(ra + (ia[:, None] + 1) * bwa, ea), np.minimum(rb + (ib[None, :] + 1) * bwb, eb))
+    hit = np.nonzero(x0 < x1)
+    return ia[hit[0]], ib[hit[1]], hit[0] + hit[1], (a1 - a0) + (b1 - b0) + 1
+
+
+def exposure_block_cells(rois, blocks, boff):
+    """The block pairs of cv2's block compensator and where udh_mosaic_exposure_block_stats_u8 sums them.  -> dict(pair_ptr,
+    pair_j (the frame pairs i <= j whose ROIs intersect, exposure_pairs), cell_off int64 [P], cell_nx int32 [P], nslots,
+    a, b int64 [Q] (every pair of blocks a <= b whose rectangles intersect, a block with itself included), slot int64 [Q])."""
+    r = np.asarray(rois, np.int64).reshape(-1, 4)
+    ptr, pj = exposure_pairs(r)
+    P = len(pj)
+    cell_off, cell_nx = np.zeros(P, np.int64), np.zeros(P, np.int32)
+    A, B, S = [], [], []
+    o, p = 0, 0
+    for i in range(len(r)):
+        for j in pj[ptr[i]:ptr[i + 1]]:
+            bw_i, bh_i, bpx_i, _ = (int(v) for v in blocks[i])
+            bw_j, bh_j, bpx_j, _ = (int(v) for v in blocks[j])
+            x0, y0 = max(r[i, 0], r[j, 0]), max(r[i, 1], r[j, 1])
+            x1, y1 = min(r[i, 2], r[j, 2]), min(r[i, 3], r[j, 3])
+            xa, xb, cx, nx = _block_axis(r[i, 0], r[i, 2], bw_i, r[j, 0], r[j, 2], bw_j, x0, x1)
+            ya, yb, cy, ny = _block_axis(r[i, 1], r[i, 3], bh_i, r[j, 1], r[j, 3], bh_j, y0, y1)
+            cell_off[p], cell_nx[p] = o, nx
+            A.append((boff[i] + ya[:, None] * bpx_i + xa[None, :]).ravel())
+            B.append((boff[j] + yb[:, None] * bpx_j + xb[None, :]).ravel())
+            S.append((o + cy[:, None] * nx + cx[None, :]).ravel())
+            o += nx * ny
+            p += 1
+    return dict(pair_ptr=ptr, pair_j=pj, cell_off=cell_off, cell_nx=cell_nx, nslots=o, a=np.concatenate(A).astype(np.int64),
+                b=np.concatenate(B).astype(np.int64), slot=np.concatenate(S).astype(np.int64))
+
+
+def exposure_block_system(nblocks, a, b, count, sum_a, sum_b):
+    """One feed of cv2.detail.GainCompensator over the blocks as a sparse system: block pairs a <= b whose rectangles
+    intersect (each block with itself included), their counts and sums -> (keep int64 [n] (the unskipped blocks, in order),
+    CSR row_ptr int32 [n+1], col int32, val float64, rhs float64 [n]).  The rule is exposure_solve's: N = max(1, count),
+    I_ab = sum_a / N and I_ba = sum_b / N where count > 0, a block is skipped unless it has a positive-count pair with
+    another block, and over the unskipped blocks, for row i and j ascending: b_i += beta N_ij, A_ii += beta N_ij and, for
+    j != i, A_ii += 2 alpha I_ij^2 N_ij, A_ij -= 2 alpha I_ij I_ji N_ij, in that order, so A and b equal cv2's dense ones bit
+    for bit (pairs whose rectangles do not intersect add nothing)."""
+    a, b, count = (np.asarray(v, np.int64) for v in (a, b, count))
+    N = np.maximum(count, 1).astype(np.float64)
+    pos, off = count > 0, a != b
+    Iab = np.where(pos, np.asarray(sum_a, np.float64) / N, 0.0)
+    Iba = np.where(pos, np.asarray(sum_b, np.float64) / N, 0.0)
+    skip = np.ones(int(nblocks), bool)
+    skip[a[pos & off]] = False
+    skip[b[pos & off]] = False
+    keep = np.flatnonzero(~skip)
+    idx = np.full(int(nblocks), -1, np.int64)
+    idx[keep] = np.arange(len(keep))
+    use = ~skip[a] & ~skip[b]
+    u2 = use & off
+    row = np.concatenate([idx[a[use]], idx[b[u2]]])
+    col = np.concatenate([idx[b[use]], idx[a[u2]]])
+    n_e = np.concatenate([N[use], N[u2]])
+    i_rc = np.concatenate([Iab[use], Iba[u2]])
+    i_cr = np.concatenate([Iba[use], Iab[u2]])
+    order = np.lexsort((col, row))
+    row, col, n_e, i_rc, i_cr = row[order], col[order], n_e[order], i_rc[order], i_cr[order]
+    n = len(keep)
+    ptr = np.zeros(n + 1, np.int64)
+    ptr[1:] = np.cumsum(np.bincount(row, minlength=n))
+    k_in_row = np.arange(len(row)) - ptr[row]
+    al, be = EXPOSURE_ALPHA, EXPOSURE_BETA
+    diag, rhs = np.zeros(n), np.zeros(n)
+    nd = col != row
+    val = np.where(nd, 0.0 - 2 * al * i_rc * i_cr * n_e, 0.0)
+    by_k = np.argsort(k_in_row, kind="stable")
+    bounds = np.searchsorted(k_in_row[by_k], np.arange(int(k_in_row.max(initial=-1)) + 2))
+    for k in range(len(bounds) - 1):
+        e = by_k[bounds[k]:bounds[k + 1]]                   # one entry per row: the k-th of each row
+        rr = row[e]
+        rhs[rr] += be * n_e[e]
+        diag[rr] += be * n_e[e]
+        e2 = e[nd[e]]
+        diag[row[e2]] += 2 * al * i_rc[e2] * i_rc[e2] * n_e[e2]
+    val[~nd] = diag[row[~nd]]
+    return keep, ptr.astype(np.int32), col.astype(np.int32), val, rhs
+
+
+def exposure_block_solve(row_ptr, col, val, rhs, dev, tol=EXPOSURE_BLOCK_TOL, max_iter=EXPOSURE_BLOCK_MAX_ITER):
+    """udh_exposure_block_solve on the device dev -> (x float64 [n] numpy, iterations, final |r| / |b|)."""
+    n = len(rhs)
+    t = [torch.from_numpy(np.ascontiguousarray(v)).to(dev) for v in (row_ptr, col, val, rhs)]
+    x = torch.empty(n, device=dev, dtype=torch.float64)
+    info = torch.zeros(2, device=dev, dtype=torch.int64)
+    nb = lib.udh_exposure_block_solve_workspace_bytes(n)
+    ws = torch.empty(max(nb, 1), device=dev, dtype=torch.uint8)
+    check(lib.udh_exposure_block_solve(n, _ptr(t[0]), _ptr(t[1]), _ptr(t[2]), _ptr(t[3]), float(tol), int(max_iter), _ptr(x), _ptr(info),
+                                       _ptr(ws), nb, _stream()), "udh_exposure_block_solve")
+    inf = info.cpu().numpy()
+    return x.cpu().numpy(), int(inf[0]), float(inf[1:2].view(np.float64)[0])
+
+
+def _norm_sums(l0, l1, l2):
+    """exposure_norm_sum over arrays of limb sums (exact in Python integers, rounded once)."""
+    tot = np.asarray(l0, np.uint64).astype(object) + (np.asarray(l1, np.uint64).astype(object) << 21) + \
+        (np.asarray(l2, np.uint64).astype(object) << 42)
+    return np.array([math.ldexp(float(v), -52) for v in tot], np.float64)
+
+
+class _ExposureBlockStats(object):
+    """udh_mosaic_exposure_block_stats_u8 on fixed frames and blocks: tables, cells and output, reused by every feed."""
+
+    def __init__(self, frames, M, dst_h, dst_w, block):
+        if int(block) < 1:
+            raise ValueError("block must be >= 1 (got %r)" % (block,))
+        frames, sizes, rois, Mr, take = _exposure_rois(frames, M, dst_h, dst_w, "mosaic_exposure_gain_maps")
+        self.n, self.take, self.dst = len(frames), take, (int(dst_h), int(dst_w))
+        m = self.m = len(take)
+        if not m:
+            return
+        dev = self.dev = frames[0].device
+        self.frames = [frames[k] for k in take]
+        self.ptrs = (ctypes.c_void_p * m)(*[f.data_ptr() for f in self.frames])
+        self.sz = np.ascontiguousarray(np.array([sizes[k] for k in take], np.int32).reshape(m, 2))
+        self.rr = np.ascontiguousarray(rois[take].astype(np.int32))
+        self.M_d = torch.from_numpy(np.ascontiguousarray(Mr[take].reshape(m, 9))).to(dev)
+        self.blocks, boff = exposure_block_grid(self.rr, block)
+        self.blocks = np.ascontiguousarray(self.blocks)
+        self.boff, self.nblocks = np.ascontiguousarray(boff[:-1]), int(boff[-1])
+        c = self.cells = exposure_block_cells(self.rr, self.blocks, boff)
+        self.ptr_d, self.pj_d = torch.from_numpy(c["pair_ptr"]).to(dev), torch.from_numpy(c["pair_j"]).to(dev)
+        self.off_d, self.nx_d = torch.from_numpy(c["cell_off"]).to(dev), torch.from_numpy(c["cell_nx"]).to(dev)
+        self.slot_d = torch.from_numpy(c["slot"]).to(dev)
+        self.out = torch.empty(c["nslots"], _lib.EXPOSURE_STATS, device=dev, dtype=torch.int64)
+        self.nb = lib.udh_mosaic_exposure_block_workspace_bytes(m)
+        self.ws = torch.empty(max(self.nb, 1), device=dev, dtype=torch.uint8)
+
+    def __call__(self, history=None, norms=True):
+        """history: None or a CUDA float64 [t,nblocks,3] -> uint64 [Q,13] numpy, the statistics of cells['a'], cells['b']."""
+        t = 0 if history is None else int(history.shape[0])
+        c = self.cells
+        check(lib.udh_mosaic_exposure_block_stats_u8(self.ptrs, self.sz.ctypes.data, _ptr(self.M_d), self.rr.ctypes.data, self.m,
+                                                     self.blocks.ctypes.data, self.boff.ctypes.data, self.nblocks, _ptr(self.ptr_d),
+                                                     _ptr(self.pj_d), len(c["pair_j"]), _ptr(self.off_d), _ptr(self.nx_d), c["nslots"],
+                                                     _ptr(history) if t else None, t, int(bool(norms)), self.dst[0], self.dst[1],
+                                                     _ptr(self.out), _ptr(self.ws), self.nb, _stream()),
+              "udh_mosaic_exposure_block_stats_u8")
+        return self.out.index_select(0, self.slot_d).cpu().numpy().view(np.uint64)
+
+
+def mosaic_exposure_block_stats(frames, M, dst_h, dst_w, block=32, history=None, norms=True):
+    """The block compensators' block-pair statistics of the frames' ROI warps (udh_mosaic_exposure_block_stats_u8), for
+    tests and tools.  history None or float64 [t,nblocks,3].  -> dict(take, blocks, boff, a, b [Q] (block pairs a <= b whose
+    rectangles intersect), count int64 [Q], sums int64 [Q,2,3], norms float64 [Q,2] (0 without norms))."""
+    st = _ExposureBlockStats(frames, M, dst_h, dst_w, block)
+    if not st.m:
+        return dict(take=[], a=np.zeros(0, np.int64), b=np.zeros(0, np.int64))
+    h = None if history is None else torch.from_numpy(np.ascontiguousarray(history, np.float64)).to(st.dev)
+    raw = st(h, norms)
+    return dict(take=st.take, blocks=st.blocks, boff=st.boff, a=st.cells["a"], b=st.cells["b"], count=raw[:, 0].astype(np.int64),
+                sums=raw[:, 1:7].astype(np.int64).reshape(-1, 2, 3),
+                norms=np.stack([_norm_sums(*raw[:, 7:10].T), _norm_sums(*raw[:, 10:13].T)], 1), raw=raw)
+
+
+def mosaic_exposure_block_gains(frames, M, dst_h, dst_w, mode="gain", feeds=1, block=32):
+    """mosaic_exposure_gain_maps with its working: -> dict(take, maps [n] (None where not fed), gains float64 [nblocks,3]
+    (the blocks' unfiltered gains, the product of the feeds'), blocks, boff, unknowns [per feed and system], iters,
+    residual)."""
+    if mode not in ("gain", "channels"):
+        raise ValueError("mode must be 'gain' or 'channels' (got %r)" % (mode,))
+    if not 1 <= int(feeds) <= _lib.EXPOSURE_MAX_FEEDS:
+        raise ValueError("feeds must be in 1..%d (got %r)" % (_lib.EXPOSURE_MAX_FEEDS, feeds))
+    st = _ExposureBlockStats(frames, M, dst_h, dst_w, block)
+    out = dict(take=st.take, maps=[None] * st.n, unknowns=[], iters=[], residual=[])
+    if not st.m:
+        return out
+    nbk, c = st.nblocks, st.cells
+    hist = torch.empty(int(feeds), nbk, 3, device=st.dev, dtype=torch.float64)
+    acc = None
+    for t in range(int(feeds)):
+        raw = st(hist[:t] if t else None, norms=mode == "gain")
+        count = raw[:, 0].astype(np.int64)
+        if mode == "gain":
+            pos = (count > 0) & (c["a"] != c["b"])              # a block's own mean never enters the system
+            sa, sb = np.zeros(len(count)), np.zeros(len(count))
+            sa[pos], sb[pos] = _norm_sums(*raw[pos, 7:10].T), _norm_sums(*raw[pos, 10:13].T)
+            sums = [(sa, sb)]
+        else:
+            sums = [(raw[:, 1 + ch].astype(np.int64), raw[:, 4 + ch].astype(np.int64)) for ch in range(3)]
+        g3 = np.ones((nbk, 3), np.float64)
+        for ch, (sa, sb) in enumerate(sums):
+            keep, ptr, col, val, rhs = exposure_block_system(nbk, c["a"], c["b"], count, sa, sb)
+            out["unknowns"].append(len(keep))
+            if not len(keep):
+                continue
+            x, it, res = exposure_block_solve(ptr, col, val, rhs, st.dev)
+            out["iters"].append(it)
+            out["residual"].append(res)
+            if mode == "gain":
+                g3[keep] = x[:, None]
+            else:
+                g3[keep, ch] = x
+        acc = g3.copy() if acc is None else acc * g3
+        hist[t] = torch.from_numpy(g3).to(st.dev)
+    ch = 1 if mode == "gain" else 3
+    g_d = torch.from_numpy(acc).to(st.dev)
+    maps = torch.empty(nbk * ch, device=st.dev, dtype=torch.float32)
+    nb = lib.udh_exposure_gain_maps_workspace_bytes(nbk, ch)
+    ws = torch.empty(nb, device=st.dev, dtype=torch.uint8)
+    check(lib.udh_exposure_gain_maps(_ptr(g_d), st.m, st.blocks.ctypes.data, st.boff.ctypes.data, nbk, ch, _ptr(maps), _ptr(ws), nb,
+                                     _stream()), "udh_exposure_gain_maps")
+    for q, k in enumerate(st.take):
+        bpx, bpy = int(st.blocks[q, 2]), int(st.blocks[q, 3])
+        o = int(st.boff[q]) * ch
+        mp = maps[o:o + bpx * bpy * ch]
+        out["maps"][k] = mp.view(bpy, bpx) if ch == 1 else mp.view(bpy, bpx, 3)
+    out.update(gains=acc, blocks=st.blocks, boff=st.boff)
+    return out
+
+
+def mosaic_exposure_gain_maps(frames, M, dst_h, dst_w, mode="gain", feeds=1, block=32):
+    """frames: n CUDA uint8 RGB tensors [h_k,w_k,3], M float64 [n,3,3] (frame k -> canvas) -> per frame its gain map, a CUDA
+    float32 [bpy,bpx] ("gain") or [bpy,bpx,3] ("channels") tensor (None for a frame whose ROI misses the canvas): what
+    cv2.detail_BlocksGainCompensator(block, block, feeds) / BlocksChannelsCompensator's getMatGains() gives when fed the
+    multi-band blend's inputs (oracle/exposure_blocks.py).  Each ROI warp is cut into blocks of about block x block px;
+    udh_mosaic_exposure_block_stats_u8 sums every block pair's statistics exactly, the sparse system is assembled on the
+    host in cv2's order (exposure_block_system) and solved on the GPU by conjugate gradients (udh_exposure_block_solve, to
+    |r| <= 1e-15 |b|), and udh_exposure_gain_maps filters the float32 maps as cv2 does.  The blends apply them with
+    gain_maps=."""
+    return mosaic_exposure_block_gains(frames, M, dst_h, dst_w, mode, feeds, block)["maps"]
+
+
+def map_taps(n, N):
+    """The resize taps of a map axis of n -> an ROI axis of N (udh_map_tap [N] as int32 [N,4]: s0, s1, and the float32
+    weights' bits): generic INTER_LINEAR in float32 (oracle/exposure_blocks.resize_map)."""
+    if n == N:
+        s = np.arange(N)
+        f = np.zeros(N, np.float32)
+    else:
+        f = ((np.arange(N) + 0.5) * (1.0 / (float(N) / float(n))) - 0.5).astype(np.float32)
+        s = np.floor(f).astype(np.int64)
+        f = (f - s.astype(np.float32)).astype(np.float32)
+        f[(s < 0) | (s >= n - 1)] = 0
+        s = np.clip(s, 0, n - 1)
+    t = np.zeros((N, 4), np.int32)
+    t[:, 0], t[:, 1] = s, np.minimum(s + 1, n - 1)
+    t[:, 2] = (np.float32(1) - f).astype(np.float32).view(np.int32)
+    t[:, 3] = f.view(np.int32)
+    return t
+
+
+def _gain_map_table(gain_maps, rois, n, dev, what):
+    """Per-frame gain maps (CUDA float32 [bpy,bpx(,3)], None where the ROI is empty) on rois [n,4] -> (udh_gain_map [n],
+    the tensors it points to)."""
+    gain_maps = list(gain_maps)
+    if len(gain_maps) != n:
+        raise _lib.UdhError("%s: %d gain maps for %d frames" % (what, len(gain_maps), n))
+    table = (_lib.GainMap * n)()
+    keep = []
+    for k, mp in enumerate(gain_maps):
+        x0, y0, x1, y1 = (int(v) for v in rois[k])
+        if x1 <= x0 or y1 <= y0:
+            continue
+        if mp is None:
+            raise _lib.UdhError("%s: frame %d meets the canvas but has no gain map" % (what, k))
+        _req(mp, torch.float32, "gain_maps[%d]" % k)
+        if mp.dim() not in (2, 3) or (mp.dim() == 3 and mp.shape[2] != 3) or not mp.is_contiguous():
+            raise _lib.UdhError("%s: gain_maps[%d] must be a contiguous [bpy,bpx] or [bpy,bpx,3] (got %s)" % (what, k, tuple(mp.shape)))
+        cols = torch.from_numpy(map_taps(mp.shape[1], x1 - x0)).to(dev)
+        rows = torch.from_numpy(map_taps(mp.shape[0], y1 - y0)).to(dev)
+        keep += [mp, cols, rows]
+        table[k] = _lib.GainMap(mp.data_ptr(), cols.data_ptr(), rows.data_ptr(), int(mp.shape[1]), int(mp.shape[0]),
+                                1 if mp.dim() == 2 else 3, 0)
+    return table, keep
 
 
 # ------------------------------------------------------------------ seam finding
