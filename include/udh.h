@@ -736,10 +736,24 @@ int udh_debug_x3_wgrad(const float* x, const float* g, float* dW, float* db, voi
                        void* stream);
 int udh_debug_x3_conv1(const float* I1, const float* I2, const float* w, const float* bias, float* out, const float* g, float* dW,
                        float* db, void* scratch, int B, int H, int W, void* stream);
+/* udh_debug_x3_conv1 with conv1_1's fused ReLU-mask epilogue of the train step: mask_out (nullable; needs out) receives
+ * out > 0 as the uint32 words of udh_debug_x3_conv_ex over the padded positions (2 words per position); the words of border
+ * positions are not written. */
+int udh_debug_x3_conv1_ex(const float* I1, const float* I2, const float* w, const float* bias, uint32_t* mask_out, float* out,
+                          const float* g, float* dW, float* db, void* scratch, int B, int H, int W, void* stream);
 /* fused conv (64 -> 64 channels, W == 128) + bias + ReLU + 2x2 max-pool (conv1_2 + pool1): x [B,H,128,64] ->
  * pooled [B,H/2,64,64] fp32 and routing codes [B,H/2,64,8] uint32 (3 bits per channel, 4 = no gradient). */
 int udh_debug_tc_conv_pool(const float* x, const float* w, const float* bias, float* pooled, uint32_t* codes, void* scratch,
                            int B, int H, int W, void* stream);
+/* the 2x2 max-pool kernels the step runs in numeric_mode UDH_NUMERIC_BF16X3 (pool_fwd_x3 / pool_bwd_x3) or UDH_NUMERIC_BF16
+ * (pool_fwd_bf16 / pool_bwd_bf16), on fp32 NHWC tensors through the step's padded streams (two-limb split, or bf16 rounding).
+ * Forward when in != NULL: in [B,H,W,C] -> out [B,H/2,W/2,C] (the stored pooled value, read back as fp32) and codes
+ * [B,H/2,W/2,C/8] uint32 (3 bits per channel at (c % 8) * 3 of word c / 8: window index 0-3 of the first maximum in row-major
+ * order, 4 where the maximum is not positive).  Backward when din != NULL: codes + dout [B,H/2,W/2,C] -> din [B,H,W,C] (the
+ * stored gradient at the routed element, 0 elsewhere); a call with both runs the forward first.  H, W even, C % 8 == 0.  The
+ * streams are allocated on `stream` and freed behind the kernels. */
+int udh_debug_tc_pool(int numeric_mode, const float* in, float* out, uint32_t* codes, const float* dout, float* din, int B, int H,
+                      int W, int C, void* stream);
 /* fc1 (32768 -> 1024, the 128x128-patch regressor) through exactly the calls the step makes in `numeric_mode`:
  * y[B,1024] = x[B,32768] . w[32768,1024] (no bias, no ReLU); with dy[B,1024] != NULL also dW[32768,1024] = x^T . dy and
  * dx[B,32768] = dy . w^T, computed from the operand copies the forward made.  dW is STORED in the tensor-core modes and

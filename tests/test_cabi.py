@@ -81,6 +81,41 @@ def test_x3_mask_and_row_tile_debug_entries_reject_bad_arguments():
     assert b"udh_debug_x3_conv_rows" in L.udh_last_error()
 
 
+def test_tc_pool_debug_entry_rejects_bad_arguments():
+    """udh_debug_tc_pool is exported and checks its arguments before touching the device."""
+    from unsuperviseddeephomographyral2018_b200 import _lib
+    L = _lib.lib
+    assert hasattr(ctypes.CDLL(_lib.LIB_PATH), "udh_debug_tc_pool")
+    p = ctypes.c_void_p(256)                          # never dereferenced: every call below fails its argument checks
+    for mode in (_lib.NUMERIC_FP32, -1, 3):
+        assert L.udh_debug_tc_pool(mode, p, p, p, p, p, 2, 16, 16, 64, None) == _lib.EINVAL
+        assert b"unknown numeric_mode" in L.udh_last_error()
+    for mode in (_lib.NUMERIC_BF16, _lib.NUMERIC_BF16X3):
+        # (in, out, codes, dout, din): no direction, forward without out, no codes, backward without dout
+        for a in ((None, p, p, p, None), (p, None, p, None, None), (p, p, None, None, None), (None, None, p, None, p)):
+            assert L.udh_debug_tc_pool(mode, *a, 2, 16, 16, 64, None) == _lib.EINVAL, (mode, a)
+            assert b"udh_debug_tc_pool: null pointer" in L.udh_last_error()
+        for B, H, W, C in ((0, 16, 16, 64), (2, 15, 16, 64), (2, 16, 7, 64), (2, 16, 16, 4), (2, 0, 16, 64)):
+            assert L.udh_debug_tc_pool(mode, p, p, p, p, p, B, H, W, C, None) == _lib.EINVAL, (B, H, W, C)
+            assert b"udh_debug_tc_pool: needs" in L.udh_last_error()
+
+
+def test_x3_conv1_mask_debug_entry_rejects_bad_arguments():
+    """udh_debug_x3_conv1_ex is exported and checks its arguments before touching the device."""
+    from unsuperviseddeephomographyral2018_b200 import _lib
+    L = _lib.lib
+    p = ctypes.c_void_p(256)                          # never dereferenced: every call below fails its argument checks
+    # (I1, I2, w, bias, mask_out, out, g, dW, db, scratch)
+    for a, msg in (((None, p, p, p, p, p, None, None, None, p), b"null pointer"),
+                   ((p, p, p, p, p, p, None, None, None, None), b"null pointer"),
+                   ((p, p, p, p, None, None, None, None, None, p), b"null pointer"),
+                   ((p, p, None, p, None, p, None, None, None, p), b"forward needs weights and bias"),
+                   ((p, p, None, None, p, None, p, p, p, p), b"mask_out needs the forward"),
+                   ((p, p, None, None, None, None, p, None, p, p), b"wgrad needs dW and db")):
+        assert L.udh_debug_x3_conv1_ex(*a, 2, 16, 128, None) == _lib.EINVAL, a
+        assert b"udh_debug_x3_conv1_ex: " + msg in L.udh_last_error()
+
+
 def test_fc1_debug_entry_rejects_bad_arguments():
     """udh_debug_fc1 / udh_debug_fc1_scratch_bytes are exported and check their arguments before touching the device."""
     from unsuperviseddeephomographyral2018_b200 import _lib

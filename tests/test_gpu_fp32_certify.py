@@ -31,6 +31,7 @@ pytestmark = pytest.mark.gpu
 
 from oracle import oracle as O                                               # noqa: E402
 from oracle import simt_fp32 as S                                            # noqa: E402
+from _pool_ties import tie_windows                                           # noqa: E402
 
 
 @pytest.fixture(scope="module")
@@ -298,24 +299,6 @@ def test_wgrad_exact_partials_and_fp64(udh, BP, name, div, cin, cout):
 
 
 # ------------------------------------------------------------------------------------------------ 4. pools
-def _tie_windows(gen, B, H, W, C):
-    """Post-ReLU-like values with many exact ties: each 2x2 window holds 2, 3 or 4 equal positive maxima, or is all zero
-    (with -0 mixed in), or is random; values are multiples of 0.25 so equal ones are common anyway."""
-    x = torch.randint(0, 8, (B, H, W, C), device="cuda", generator=gen).float() * 0.25
-    win = x.reshape(B, H // 2, 2, W // 2, 2, C).permute(0, 1, 3, 5, 2, 4).reshape(B, H // 2, W // 2, C, 4)
-    kind = torch.randint(0, 5, win.shape[:4], device="cuda", generator=gen)
-    top = win.max(dim=4).values + 0.25
-    for k in (2, 3, 4):                                    # k equal maxima at random positions of the window
-        sel = kind == k - 2
-        order = torch.rand(win.shape, device="cuda", generator=gen).argsort(dim=4)
-        hit = order < k
-        win = torch.where(sel[..., None] & hit, top[..., None], win)
-    zero = kind == 3
-    signs = torch.where(torch.rand(win.shape, device="cuda", generator=gen) < 0.5, -0.0, 0.0)
-    win = torch.where(zero[..., None], signs, win)
-    return win.reshape(B, H // 2, W // 2, C, 2, 2).permute(0, 1, 4, 2, 5, 3).reshape(B, H, W, C).contiguous()
-
-
 def check_pool(udh, x, dout, what):
     out, din = simt_pool(udh, x, dout)
     check_exact(out, S.pool_fwd(x).double(), what + " forward")          # values; the sign of a zero maximum is not pinned
@@ -335,7 +318,7 @@ def test_pool_routing_rule_on_ties(udh, BP, name, div, C):
     B, Pz = BP
     H = Pz // div
     gen = torch.Generator(device="cuda").manual_seed(B * 31 + H + C)
-    x = _tie_windows(gen, B, H, H, C)
+    x = tie_windows(gen, B, H, H, C)
     dout = torch.randn(B, H // 2, H // 2, C, device="cuda", generator=gen)
     dout[..., 0] = -0.0                                    # a negative-zero gradient is routed as itself
     ties, zeros = check_pool(udh, x, dout, "fp32 %s B=%d P=%d" % (name, B, Pz))

@@ -191,6 +191,30 @@ extern "C" int udh_debug_fc1(int numeric_mode, const float* x, const float* w, c
   return UDH_OK;
 }
 
+extern "C" int udh_debug_tc_pool(int numeric_mode, const float* in, float* out, uint32_t* codes, const float* dout, float* din, int B,
+                                 int H, int W, int C, void* stream) {
+  UDH_REQUIRE(numeric_mode == UDH_NUMERIC_BF16 || numeric_mode == UDH_NUMERIC_BF16X3, "udh_debug_tc_pool: unknown numeric_mode %d",
+              numeric_mode);
+  UDH_REQUIRE((in || din) && codes && (!in || out) && (!din || dout), "udh_debug_tc_pool: null pointer");
+  UDH_REQUIRE(B >= 1 && H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0 && C > 0 && C % 8 == 0,
+              "udh_debug_tc_pool: needs B >= 1, even H and W and C %% 8 == 0");
+  cudaStream_t st = as_stream(stream);
+  // the two padded streams of the step (in-shaped and out-shaped), in this mode's format: 2 bytes per limb
+  const size_t limbs = numeric_mode == UDH_NUMERIC_BF16X3 ? 2 : 1;
+  const size_t in_bytes = (size_t)B * (H + 2) * (W + 2) * C * 2 * limbs, out_bytes = (size_t)B * (H / 2 + 2) * (W / 2 + 2) * C * 2 * limbs;
+  void* s = nullptr;
+  UDH_CUDA(cudaMallocAsync(&s, in_bytes + out_bytes, st));
+  uint16_t* s_in = static_cast<uint16_t*>(s);
+  uint16_t* s_out = s_in + in_bytes / 2;
+  const cudaError_t e = cudaMemsetAsync(s, 0, in_bytes + out_bytes, st);
+  int rc = UDH_ECUDA;
+  if (e != cudaSuccess) set_error("udh_debug_tc_pool: cudaMemsetAsync failed: %s", cudaGetErrorString(e));
+  else if (numeric_mode == UDH_NUMERIC_BF16X3) rc = x3_debug_pool(in, out, codes, dout, din, s_in, s_out, B, H, W, C, st);
+  else rc = tc_debug_pool(in, out, codes, dout, din, s_in, s_out, B, H, W, C, st);
+  UDH_CUDA(cudaFreeAsync(s, st));                 // stream-ordered: after the kernels above
+  return rc;
+}
+
 extern "C" int udh_debug_simt_conv(const float* x, const float* x2, const float* w, const float* bias, const float* mask_src,
                                    float* out, float* wrot, int B, int H, int W, int cin, int cout, int relu, int dgrad,
                                    void* stream) {

@@ -676,6 +676,25 @@ int tc_debug_wgrad(const float* x, const float* gsrc, float* dW, float* db, void
   return tc_wgrad(xp, gp, dW, db, B, H, W, cin, cout, st);
 }
 
+// Debug / test entry: the step's pool kernels of this mode on fp32 tensors (see x3_debug_pool); s_in / s_out: zeroed bf16
+// streams shaped like in and like out.
+int tc_debug_pool(const float* in, float* out, uint32_t* codes, const float* dout, float* din, uint16_t* s_in16, uint16_t* s_out16, int B,
+                  int H, int W, int C, cudaStream_t st) {
+  __nv_bfloat16* s_in = reinterpret_cast<__nv_bfloat16*>(s_in16);
+  __nv_bfloat16* s_out = reinterpret_cast<__nv_bfloat16*>(s_out16);
+  if (in) {
+    TRY(pad_cast(in, s_in, B, H, W, C, st));
+    TRY(pool_fwd_bf16(s_in, s_out, codes, B, H, W, C, st));
+    TRY(unpad_cast(s_out, out, B, H / 2, W / 2, C, st));
+  }
+  if (din) {
+    TRY(pad_cast(dout, s_out, B, H / 2, W / 2, C, st));
+    TRY(pool_bwd_bf16(codes, s_out, s_in, B, H, W, C, st));
+    TRY(unpad_cast(s_in, din, B, H, W, C, st));
+  }
+  return UDH_OK;
+}
+
 }  // namespace udh
 
 extern "C" int udh_debug_tc_wgrad(const float* x, const float* g, float* dW, float* db, void* scratch, int B, int H, int W, int cin,

@@ -38,4 +38,11 @@ void* x3_fc1_mirror(void* ws, size_t tc_off, int B, int P);
 int x3_materialize_acts(void* ws, const size_t* act_off, size_t tc_off, int B, int P, cudaStream_t st);
 int x3_fc1_bwd(const float* dy, float* dW, float* dx, void* ws, size_t tc_off, int B, int P, cudaStream_t st);
 
+// udh_debug_tc_pool: the step's 2x2 max-pool kernels of each tensor-core mode on fp32 tensors, through zeroed streams
+// s_in (shaped like in) and s_out (shaped like out) of that mode's format
+int tc_debug_pool(const float* in, float* out, uint32_t* codes, const float* dout, float* din, uint16_t* s_in, uint16_t* s_out, int B,
+                  int H, int W, int C, cudaStream_t st);
+int x3_debug_pool(const float* in, float* out, uint32_t* codes, const float* dout, float* din, uint16_t* s_in, uint16_t* s_out, int B,
+                  int H, int W, int C, cudaStream_t st);
+
 }  // namespace udh

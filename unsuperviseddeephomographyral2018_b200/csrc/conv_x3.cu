@@ -718,15 +718,34 @@ int x3_debug_wgrad(const float* x, const float* gsrc, float* dW, float* db, void
   return tc_wgrad_x3(xp, gp, dW, db, B, H, W, cin, cout, st);
 }
 
-int x3_debug_conv1(const float* I1, const float* I2, const float* w, const float* bias, float* out, const float* g, float* dW, float* db,
-                   void* scratch, int B, int H, int W, cudaStream_t st) {
-  // forward (out != nullptr): out [B,H,W,64] = relu(conv1_1(I1, I2)); wgrad (g != nullptr): dW [3,3,2,64], db [64] accumulated
+// the step's pool kernels of this mode on fp32 tensors: in -> limb stream (the step's split) -> pool_fwd_x3 -> out (hi + lo)
+// and codes; dout -> gradient limb stream -> pool_bwd_x3 from codes -> din (hi + lo).  s_in / s_out: zeroed limb streams
+// shaped like in and like out.
+int x3_debug_pool(const float* in, float* out, uint32_t* codes, const float* dout, float* din, uint16_t* s_in, uint16_t* s_out, int B,
+                  int H, int W, int C, cudaStream_t st) {
+  if (in) {
+    TRY(pad_cast_x3(in, s_in, B, H, W, C, false, st));
+    TRY(pool_fwd_x3(s_in, s_out, codes, B, H, W, C, st));
+    TRY(unpad_cast_x3(s_out, out, B, H / 2, W / 2, C, false, st));
+  }
+  if (din) {
+    TRY(pad_cast_x3(dout, s_out, B, H / 2, W / 2, C, true, st));
+    TRY(pool_bwd_x3(codes, s_out, s_in, B, H, W, C, st));
+    TRY(unpad_cast_x3(s_in, din, B, H, W, C, true, st));
+  }
+  return UDH_OK;
+}
+
+int x3_debug_conv1(const float* I1, const float* I2, const float* w, const float* bias, uint32_t* mask_out, float* out, const float* g,
+                   float* dW, float* db, void* scratch, int B, int H, int W, cudaStream_t st) {
+  // forward (out != nullptr): out [B,H,W,64] = relu(conv1_1(I1, I2)) (+ its mask words when mask_out != nullptr);
+  // wgrad (g != nullptr): dW [3,3,2,64], db [64] accumulated
   char* s = reinterpret_cast<char*>(scratch);
   uint16_t* op = reinterpret_cast<uint16_t*>(s);
   const size_t sbytes = al256((size_t)B * (H + 2) * (W + 2) * 64 * 4);
   UDH_CUDA(cudaMemsetAsync(scratch, 0, sbytes, st));
   if (out) {
-    TRY(conv1_x3_fwd(I1, I2, w, bias, op, nullptr, B, H, W, st));
+    TRY(conv1_x3_fwd(I1, I2, w, bias, op, mask_out, B, H, W, st));
     TRY(unpad_cast_x3(op, out, B, H, W, 64, false, st));
   }
   if (g) {
@@ -778,5 +797,14 @@ extern "C" int udh_debug_x3_conv1(const float* I1, const float* I2, const float*
   UDH_REQUIRE(I1 && I2 && scratch && (out || g), "udh_debug_x3_conv1: null pointer");
   UDH_REQUIRE(!out || (w && bias), "udh_debug_x3_conv1: forward needs weights and bias");
   UDH_REQUIRE(!g || (dW && db), "udh_debug_x3_conv1: wgrad needs dW and db");
-  return udh::x3_debug_conv1(I1, I2, w, bias, out, g, dW, db, scratch, B, H, W, udh::as_stream(stream));
+  return udh::x3_debug_conv1(I1, I2, w, bias, nullptr, out, g, dW, db, scratch, B, H, W, udh::as_stream(stream));
+}
+
+extern "C" int udh_debug_x3_conv1_ex(const float* I1, const float* I2, const float* w, const float* bias, uint32_t* mask_out, float* out,
+                                     const float* g, float* dW, float* db, void* scratch, int B, int H, int W, void* stream) {
+  UDH_REQUIRE(I1 && I2 && scratch && (out || g), "udh_debug_x3_conv1_ex: null pointer");
+  UDH_REQUIRE(!out || (w && bias), "udh_debug_x3_conv1_ex: forward needs weights and bias");
+  UDH_REQUIRE(!mask_out || out, "udh_debug_x3_conv1_ex: mask_out needs the forward");
+  UDH_REQUIRE(!g || (dW && db), "udh_debug_x3_conv1_ex: wgrad needs dW and db");
+  return udh::x3_debug_conv1(I1, I2, w, bias, mask_out, out, g, dW, db, scratch, B, H, W, udh::as_stream(stream));
 }
