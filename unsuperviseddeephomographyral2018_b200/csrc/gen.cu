@@ -15,30 +15,43 @@ namespace udh {
 __constant__ float kGenMean[3] = {118.93f, 113.97f, 102.60f};
 __constant__ float kGenStd[3] = {69.85f, 68.81f, 72.45f};
 
-__device__ __forceinline__ uint32_t hash_u32(uint64_t x) {               // splitmix64 finaliser
+__device__ __forceinline__ uint64_t mix64(uint64_t x) {                 // splitmix64: the golden-ratio step and the finaliser
   x += 0x9E3779B97F4A7C15ull;
   x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
   x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
-  x ^= x >> 31;
-  return (uint32_t)(x >> 32);
+  return x ^ (x >> 31);
 }
+__device__ __forceinline__ uint32_t hash_u32(uint64_t x) { return (uint32_t)(mix64(x) >> 32); }
 __device__ __forceinline__ float hash_unit(uint64_t key) { return (float)(hash_u32(key) >> 8) * (1.0f / 16777216.0f) - 0.5f; }   // [-0.5, 0.5)
 
-// lattice value of octave o at integer (gx, gy) for (image b, channel c)
-__device__ __forceinline__ float lattice(uint64_t seed, int b, int c, int o, int gx, int gy) {
-  return hash_unit(seed ^ ((uint64_t)(uint32_t)gx | ((uint64_t)(uint32_t)gy << 16) | ((uint64_t)o << 32) | ((uint64_t)c << 36) | ((uint64_t)b << 40)));
+// Key of one random stream of sample b: the seed, then b, then the stream's tag each pass through the finaliser before the
+// next is mixed in, so that seeds, samples and streams that differ in a few low bits (the dataloader's seed + step,
+// consecutive samples, consecutive draws) give unrelated keys.  Keying on seed ^ index or seed + index would not: a
+// seed one apart then shifts or permutes the other seed's draws.  Tags: 3 * 6 texture lattices (c * 6 + o), then the
+// corner draws.
+__device__ __forceinline__ uint64_t stream_key(uint64_t seed, int b, int tag) {
+  return mix64(mix64(mix64(seed) ^ (uint64_t)(uint32_t)b) ^ (uint64_t)(uint32_t)tag);
+}
+constexpr int kTagCorners = 18;
+
+// lattice value at integer (gx, gy) of the lattice whose stream key is k (one per sample, channel and octave)
+__device__ __forceinline__ float lattice(uint64_t k, int gx, int gy) {
+  return hash_unit(k ^ ((uint64_t)(uint32_t)gx | ((uint64_t)(uint32_t)gy << 32)));
 }
 
 // Multi-octave value noise: lattices at 1, 1/2, ... 1/32 resolution, smoothstep-interpolated, amplitude 2^(0.9 o)
 // (roughly the 1/f spectrum of natural images: structure at the scale of the rho = 45 px displacements and fine detail).
 __global__ void __launch_bounds__(256) texture_u8_kernel(uint8_t* __restrict__ out, int Hh, int W, uint64_t seed) {
   const int b = blockIdx.y;
+  __shared__ uint64_t key[3][6];
+  if (threadIdx.x < 18) key[threadIdx.x / 6][threadIdx.x % 6] = stream_key(seed, b, threadIdx.x);
+  __syncthreads();
   for (int o = blockIdx.x * blockDim.x + threadIdx.x; o < Hh * W; o += gridDim.x * blockDim.x) {
     const int y = o / W, x = o - y * W;
     uint8_t* dst = out + ((size_t)b * Hh * W + o) * 3;
-#pragma unroll
+#pragma unroll 1
     for (int c = 0; c < 3; ++c) {
-      float v = lattice(seed, b, c, 0, x, y);
+      float v = lattice(key[c][0], x, y);
       float amp = 1.0f;
 #pragma unroll
       for (int oc = 1; oc < 6; ++oc) {
@@ -47,8 +60,8 @@ __global__ void __launch_bounds__(256) texture_u8_kernel(uint8_t* __restrict__ o
         const int gx = (int)fx, gy = (int)fy;
         float tx = fx - (float)gx, ty = fy - (float)gy;
         tx = tx * tx * (3.0f - 2.0f * tx); ty = ty * ty * (3.0f - 2.0f * ty);
-        const float a = lattice(seed, b, c, oc, gx, gy), bb = lattice(seed, b, c, oc, gx + 1, gy);
-        const float cc = lattice(seed, b, c, oc, gx, gy + 1), d = lattice(seed, b, c, oc, gx + 1, gy + 1);
+        const float a = lattice(key[c][oc], gx, gy), bb = lattice(key[c][oc], gx + 1, gy);
+        const float cc = lattice(key[c][oc], gx, gy + 1), d = lattice(key[c][oc], gx + 1, gy + 1);
         v = fmaf(amp, (a + (bb - a) * tx) + ((cc + (d - cc) * tx) - (a + (bb - a) * tx)) * ty, v);
       }
       dst[c] = (uint8_t)fminf(fmaxf(127.5f + v * 9.8f, 0.0f), 255.0f);
@@ -60,20 +73,20 @@ __global__ void __launch_bounds__(256) texture_u8_kernel(uint8_t* __restrict__ o
 __global__ void corners_kernel(float* __restrict__ pts1, float* __restrict__ gt, int B, int Hh, int W, int P, int rho, uint64_t seed) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
-  const uint64_t k = seed ^ 0xC0FFEE1234ull ^ ((uint64_t)b << 20);
-  const int x0 = rho + (int)(hash_u32(k) % (uint32_t)(W - 2 * rho - P + 1));
-  const int y0 = rho + (int)(hash_u32(k + 1) % (uint32_t)(Hh - 2 * rho - P + 1));
+  // draw i of sample b: hash_u32 of its own stream key (0: x0, 1: y0, 2..9: gt)
+  const int x0 = rho + (int)(hash_u32(stream_key(seed, b, kTagCorners)) % (uint32_t)(W - 2 * rho - P + 1));
+  const int y0 = rho + (int)(hash_u32(stream_key(seed, b, kTagCorners + 1)) % (uint32_t)(Hh - 2 * rho - P + 1));
   const float xs[4] = {(float)x0, (float)(x0 + P), (float)(x0 + P), (float)x0};
   const float ys[4] = {(float)y0, (float)y0, (float)(y0 + P), (float)(y0 + P)};
 #pragma unroll
   for (int i = 0; i < 4; ++i) { pts1[b * 8 + 2 * i] = xs[i]; pts1[b * 8 + 2 * i + 1] = ys[i]; }
 #pragma unroll
-  for (int i = 0; i < 8; ++i) gt[b * 8 + i] = (float)((int)(hash_u32(k + 2 + i) % (uint32_t)(2 * rho + 1)) - rho);
+  for (int i = 0; i < 8; ++i) gt[b * 8 + i] = (float)((int)(hash_u32(stream_key(seed, b, kTagCorners + 2 + i)) % (uint32_t)(2 * rho + 1)) - rho);
 }
 
 // ---- fused augment + normalise + gray + patch gather ---------------------------------------------------------------
 // aug: [B][11] = {on, gamma_I, bright_I, colR_I, colG_I, colB_I, gamma_Ip, bright_Ip, colR_Ip, colG_Ip, colB_Ip} (nullable)
-__global__ void __launch_bounds__(256) prep_u8_ex_kernel(const uint8_t* __restrict__ I, const uint8_t* __restrict__ Ip,
+__global__ void __launch_bounds__(256, 8) prep_u8_ex_kernel(const uint8_t* __restrict__ I, const uint8_t* __restrict__ Ip,
                                                          const float* __restrict__ pts1, const float* __restrict__ aug,
                                                          float* __restrict__ I_gray, float* __restrict__ I_aug3,
                                                          float* __restrict__ I1, float* __restrict__ I2, float* __restrict__ I1_aug,
@@ -82,17 +95,23 @@ __global__ void __launch_bounds__(256) prep_u8_ex_kernel(const uint8_t* __restri
   __shared__ float lut[2][3][256];
   const int b = blockIdx.y;
   const bool on = aug && aug[b * 11] != 0.0f;
-  for (int i = threadIdx.x; i < 2 * 3 * 256; i += blockDim.x) {
-    const int im = i / 768, c = (i / 256) % 3, x = i & 255;
-    float v = (float)x;
-    if (on) {
-      const float* a = aug + b * 11 + 1 + im * 5;
-      v = powf(v, a[0]);                                                   // img ** gamma on the raw 0..255 value
-      v = v * a[1];                                                        // brightness
-      v = v * a[2 + c];                                                    // colour
-      v = fminf(fmaxf(v, 0.0f), 255.0f);                                   // clip_by_value(0, 255)
+  // img ** gamma on the raw 0..255 value: pow in fp64 rounded once to fp32, as denorm_u8 (common.cuh) and the ECC and
+  // report tables define it, so that one augmentation row gives the same pixels on every path.  Gamma is per image, so
+  // each (image, value) takes one pow for its three channels.
+  for (int i = threadIdx.x; i < 2 * 256; i += blockDim.x) {
+    const int im = i >> 8, x = i & 255;
+    const float* a = on ? aug + b * 11 + 1 + im * 5 : nullptr;
+    const float p = on ? (float)pow((double)x, (double)a[0]) : 0.0f;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      float v = (float)x;
+      if (on) {
+        v = __fmul_rn(p, a[1]);                                            // brightness
+        v = __fmul_rn(v, a[2 + c]);                                        // colour
+        v = fminf(fmaxf(v, 0.0f), 255.0f);                                 // clip_by_value(0, 255)
+      }
+      lut[im][c][x] = __fdiv_rn(v - kGenMean[c], kGenStd[c]);              // both images use I's statistics (dataloader.py:173-177)
     }
-    lut[im][c][x] = __fdiv_rn(v - kGenMean[c], kGenStd[c]);                // both images use I's statistics (dataloader.py:173-177)
   }
   __syncthreads();
   const int x0 = (int)pts1[b * 8], y0 = (int)pts1[b * 8 + 1];
