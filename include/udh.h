@@ -478,13 +478,33 @@ int udh_warp_perspective_u8(const uint8_t* src, const double* M, uint8_t* dst, i
  *   tile_ptr [ntiles + 1] and tile_frames [tile_ptr[ntiles]] int32 (device, CSR): the frames whose footprint can reach each
  *   UDH_MOSAIC_TILE_H x UDH_MOSAIC_TILE_W canvas tile, tiles row-major, ceil(dst_w / UDH_MOSAIC_TILE_W) per row.  The lists
  *   must be conservative (a frame valid at a pixel is listed for its tile); a frame listed twice counts twice.
- *   ws: udh_mosaic_workspace_bytes(n) bytes of device memory.  n <= 65535, all sides < 32767, 0 <= feather <= 1024. */
+ *   Optional inputs (each may be null; gains and maps exclude each other):
+ *   gains [n][3] float64 (device): v_k is compensated before it is weighted (exposure compensation's apply, below, with
+ *     g = gains[k][c], channel 0's gain when c = 1).
+ *   maps [n] (host): v_k is compensated by frame k's gain map (block exposure compensation's apply, below) at
+ *     (x - x_lo, y - y_lo) of its rectangle rois[k], clamped to it.
+ *   masks [n] (host array of device pointers): frame k counts only where its uint8 blend mask on the rectangle rois[k] is set.
+ *   rois [n,4] int32 (host) x_lo, y_lo, x_hi, y_hi (exclusive), required with masks or maps: an empty rectangle keeps the
+ *     frame out (its mask and map may then be null); a non-empty one lies inside the canvas and needs a non-null mask (with
+ *     masks) and a well-formed map (with maps).
+ *   ws: udh_mosaic_workspace_bytes(n) bytes of device memory (whichever inputs are given).  n <= 65535, all sides < 32767,
+ *   0 <= feather <= 1024. */
 #define UDH_MOSAIC_TILE_H 16
 #define UDH_MOSAIC_TILE_W 64
+typedef struct udh_map_tap {
+  int32_t s0, s1; /* the two source columns (rows) of the map */
+  float a0, a1;   /* their weights */
+} udh_map_tap;
+typedef struct udh_gain_map {
+  const float* map;        /* device: bpy x bpx x channels float32 */
+  const udh_map_tap* cols; /* device: one per ROI column */
+  const udh_map_tap* rows; /* device: one per ROI row */
+  int32_t bpx, bpy, channels, pad;
+} udh_gain_map;
 size_t udh_mosaic_workspace_bytes(int n);
-int udh_mosaic_blend_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, int n, int c, const int32_t* tile_ptr,
-                        const int32_t* tile_frames, int dst_h, int dst_w, int feather, uint8_t* dst, uint8_t* mask, void* ws,
-                        size_t ws_bytes, void* stream);
+int udh_mosaic_blend_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains, const udh_gain_map* maps,
+                        const uint8_t* const* masks, const int32_t* rois, int n, int c, const int32_t* tile_ptr, const int32_t* tile_frames,
+                        int dst_h, int dst_w, int feather, uint8_t* dst, uint8_t* mask, void* ws, size_t ws_bytes, void* stream);
 /* udh_mosaic_multiband_u8: n frames blended onto one dst_h x dst_w canvas across frequency bands, byte for byte
  *   cv2.detail_MultiBandBlender(0, bands, CV_16S) on the CPU (oracle/multiband.py restates the rule).  Frame k is fed as
  *   udh_warp_perspective_u8(frame k, M_k, roi_h, roi_w) at the ROI's top-left (x_lo, y_lo), with mask 255 where that warp is
@@ -500,10 +520,17 @@ int udh_mosaic_blend_u8(const uint8_t* const* frames, const int32_t* sizes, cons
  *   (exclusive), non-empty and inside the canvas; dst [dst_h,dst_w,3] and mask [dst_h,dst_w] uint8 (device).  The sums are
  *   gathered per canvas pixel in int32 and stored once, so the bytes do not depend on the frames' order.  Only c = 3 (the
  *   blender takes 3 channels).  n <= 65535, sides < 32767, 0 <= bands <= 10.
+ *   Optional inputs (each may be null; gains and maps exclude each other), applied to every pixel of the ROI warp, valid or
+ *   not, before it is fed, as cv2's stitcher applies its compensator before the blender:
+ *   gains [n][3] float64 (device): exposure compensation's apply with g = gains[k][c].
+ *   maps [n] (host): block exposure compensation's apply with frame k's gain map at the ROI pixel; well-formed.
+ *   masks [n] (host array of device pointers, each non-null): frame k's roi_h x roi_w blend mask, fed in place of its
+ *     validity mask.
  *   ws: udh_mosaic_multiband_workspace_bytes(rois, n, dst_h, dst_w, bands) bytes of device memory (0: bad arguments). */
 size_t udh_mosaic_multiband_workspace_bytes(const int32_t* rois, int n, int dst_h, int dst_w, int bands);
-int udh_mosaic_multiband_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const int32_t* rois, int n, int c,
-                            int dst_h, int dst_w, int bands, uint8_t* dst, uint8_t* mask, void* ws, size_t ws_bytes, void* stream);
+int udh_mosaic_multiband_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains,
+                            const udh_gain_map* maps, const uint8_t* const* masks, const int32_t* rois, int n, int c, int dst_h, int dst_w,
+                            int bands, uint8_t* dst, uint8_t* mask, void* ws, size_t ws_bytes, void* stream);
 /* udh_debug_multiband_layout: where udh_mosaic_multiband_u8's workspace keeps the canvas pyramid, for tests that read it.
  *   off[i] (i <= B'): byte offset of level i, int16 [Hp >> i][Wp >> i][4] (acc's three channels, then wacc), as the feeds
  *   left it (the blend does not overwrite it); dims = {B', Hp, Wp}, the padded canvas. */
@@ -511,10 +538,6 @@ int udh_debug_multiband_layout(const int32_t* rois, int n, int dst_h, int dst_w,
 
 /* ---- exposure compensation (cv2.detail_GainCompensator / ChannelsCompensator; oracle/exposure.py restates the rule) ----
  * apply: v' = saturate_u8(rint(v g)) in float64, ties to even, per channel (cv2.multiply(uint8, double)).
- * udh_mosaic_blend_gain_u8: udh_mosaic_blend_u8 with each frame's warp value compensated before it is weighted, v' with
- *   g = gains[k][c] (gains [n][3] float64, device; channel 0's gain when c = 1).  Same arguments and limits otherwise.
- * udh_mosaic_multiband_gain_u8: udh_mosaic_multiband_u8 fed each frame's compensated ROI warp (v' with gains[k][c] on every
- *   pixel of the ROI warp, valid or not), as cv2's stitcher applies the compensator before the blender.
  * udh_mosaic_exposure_stats_u8: the compensators' per-pair statistics of the frames' ROI warps (udh_mosaic_multiband_u8's
  *   frames, M (frame -> ROI, device) and rois (host)), in one pass over the canvas.  For each listed pair p = (i, j), i <= j,
  *   over the canvas pixels where both ROI warps are valid, stats[p] (uint64, device) holds UDH_EXPOSURE_STATS sums: [0] the
@@ -529,12 +552,6 @@ int udh_debug_multiband_layout(const int32_t* rois, int n, int dst_h, int dst_w,
 #define UDH_EXPOSURE_MAX_FRAMES 1024
 #define UDH_EXPOSURE_MAX_FEEDS 16
 #define UDH_EXPOSURE_STATS 13
-int udh_mosaic_blend_gain_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains, int n, int c,
-                             const int32_t* tile_ptr, const int32_t* tile_frames, int dst_h, int dst_w, int feather, uint8_t* dst,
-                             uint8_t* mask, void* ws, size_t ws_bytes, void* stream);
-int udh_mosaic_multiband_gain_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains,
-                                 const int32_t* rois, int n, int c, int dst_h, int dst_w, int bands, uint8_t* dst, uint8_t* mask,
-                                 void* ws, size_t ws_bytes, void* stream);
 size_t udh_mosaic_exposure_workspace_bytes(int n);
 int udh_mosaic_exposure_stats_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const int32_t* rois, int n,
                                  const int32_t* pair_ptr, const int32_t* pair_j, int npairs, const double* history, int feeds,
@@ -562,24 +579,10 @@ int udh_mosaic_exposure_stats_u8(const uint8_t* const* frames, const int32_t* si
  *   device), filtered twice by cv2.sepFilter2D([1/4, 1/2, 1/4] both ways, BORDER_REFLECT_101, float32: each output
  *   (a + c) 1/4 + b 1/2, the row pass then the column pass) into maps (float32 [nblocks][channels], device, frame k's at
  *   boff[k] channels).  blocks, boff as above (host).  ws: udh_exposure_gain_maps_workspace_bytes(nblocks, channels).
- * udh_mosaic_blend_gainmap_u8 / udh_mosaic_multiband_gainmap_u8: the blends (masks null: unmasked; else as the _masked_
- *   calls) with each frame's value v at ROI pixel (lx, ly) compensated by its map: v' = saturate_u8(rint(float32(v) g))
- *   in float32, g = the map's bilinear resize to the ROI at (lx, ly) (udh_gain_map: the taps of every ROI column and row,
- *   the row pass then the column pass, each product and sum rounded to float32; channel c's gain, or the one gain when
- *   channels = 1).  maps [n] (host).  The feathered blend evaluates frame k at canvas pixel (x, y) at (x - x_lo, y - y_lo)
- *   of its rectangle rois[k] (host int32 [n,4]), clamped to it.  ws: udh_mosaic_blend_gainmap_workspace_bytes(n) /
- *   udh_mosaic_multiband_gainmap_workspace_bytes(rois, n, dst_h, dst_w, bands). */
+ * apply (the blends' maps): v at ROI pixel (lx, ly) becomes v' = saturate_u8(rint(float32(v) g)) in float32, g = the map's
+ *   bilinear resize to the ROI at (lx, ly) (udh_gain_map: the taps of every ROI column and row, the row pass then the column
+ *   pass, each product and sum rounded to float32; channel c's gain, or the one gain when channels = 1). */
 #define UDH_EXPOSURE_MAX_BLOCKS (1 << 24)
-typedef struct udh_map_tap {
-  int32_t s0, s1; /* the two source columns (rows) of the map */
-  float a0, a1;   /* their weights */
-} udh_map_tap;
-typedef struct udh_gain_map {
-  const float* map;        /* device: bpy x bpx x channels float32 */
-  const udh_map_tap* cols; /* device: one per ROI column */
-  const udh_map_tap* rows; /* device: one per ROI row */
-  int32_t bpx, bpy, channels, pad;
-} udh_gain_map;
 size_t udh_mosaic_exposure_block_workspace_bytes(int n);
 int udh_mosaic_exposure_block_stats_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const int32_t* rois, int n,
                                        const int32_t* blocks, const int64_t* boff, int64_t nblocks, const int32_t* pair_ptr,
@@ -592,15 +595,6 @@ int udh_exposure_block_solve(int n, const int32_t* row_ptr, const int32_t* col, 
 size_t udh_exposure_gain_maps_workspace_bytes(int64_t nblocks, int channels);
 int udh_exposure_gain_maps(const double* gains, int n, const int32_t* blocks, const int64_t* boff, int64_t nblocks, int channels,
                            float* maps, void* ws, size_t ws_bytes, void* stream);
-size_t udh_mosaic_blend_gainmap_workspace_bytes(int n);
-int udh_mosaic_blend_gainmap_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const udh_gain_map* maps,
-                                const uint8_t* const* masks, const int32_t* rois, int n, int c, const int32_t* tile_ptr,
-                                const int32_t* tile_frames, int dst_h, int dst_w, int feather, uint8_t* dst, uint8_t* mask, void* ws,
-                                size_t ws_bytes, void* stream);
-size_t udh_mosaic_multiband_gainmap_workspace_bytes(const int32_t* rois, int n, int dst_h, int dst_w, int bands);
-int udh_mosaic_multiband_gainmap_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const udh_gain_map* maps,
-                                    const uint8_t* const* masks, const int32_t* rois, int n, int c, int dst_h, int dst_w, int bands,
-                                    uint8_t* dst, uint8_t* mask, void* ws, size_t ws_bytes, void* stream);
 
 /* ---- seam finding (cv2.detail's Voronoi seam finder; oracle/seam.py restates the rule) -------------------------------
  * udh_mosaic_seam_masks_u8: the seams between udh_mosaic_multiband_u8's frames (frames, sizes, M frame -> ROI (device),
@@ -614,27 +608,13 @@ int udh_mosaic_multiband_gainmap_u8(const uint8_t* const* frames, const int32_t*
  *   frame k's rh x rw bytes at offset sum_{l<k} roi_h_l roi_w_l; blend (same layout) the blend masks cv2's stitcher feeds
  *   its blender: the 3 x 3 dilation of the seam mask AND the validity.  Launches 2 + 2 (pairs).  n <= UDH_SEAM_MAX_FRAMES,
  *   sides < 32767.  ws: udh_mosaic_seam_workspace_bytes(rois, n, pair_ptr, pair_j, dst_h, dst_w) bytes of device memory
- *   (0: bad arguments).
- * udh_mosaic_blend_masked_u8: udh_mosaic_blend_u8 (udh_mosaic_blend_gain_u8 when gains is not null) where frame k counts
- *   only at the pixels its blend mask holds: masks [n] (host array of device pointers), frame k's uint8 mask on the
- *   rectangle rois[k] (host int32 [n,4], x_lo, y_lo, x_hi, y_hi inside the canvas; an empty rectangle keeps the frame out,
- *   its pointer may be null).  ws: udh_mosaic_blend_masked_workspace_bytes(n) bytes of device memory.
- * udh_mosaic_multiband_masked_u8: udh_mosaic_multiband_u8 (with gains when not null) fed masks[k] (host array of device
- *   pointers, frame k's roi_h x roi_w blend mask) in place of each frame's validity mask.  Same workspace. */
+ *   (0: bad arguments). */
 #define UDH_SEAM_MAX_FRAMES 1024
 size_t udh_mosaic_seam_workspace_bytes(const int32_t* rois, int n, const int32_t* pair_ptr, const int32_t* pair_j, int dst_h,
                                        int dst_w);
 int udh_mosaic_seam_masks_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const int32_t* rois, int n,
                              const int32_t* pair_ptr, const int32_t* pair_j, int dst_h, int dst_w, uint8_t* seam, uint8_t* blend,
                              void* ws, size_t ws_bytes, void* stream);
-size_t udh_mosaic_blend_masked_workspace_bytes(int n);
-int udh_mosaic_blend_masked_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains,
-                               const uint8_t* const* masks, const int32_t* rois, int n, int c, const int32_t* tile_ptr,
-                               const int32_t* tile_frames, int dst_h, int dst_w, int feather, uint8_t* dst, uint8_t* mask, void* ws,
-                               size_t ws_bytes, void* stream);
-int udh_mosaic_multiband_masked_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains,
-                                   const uint8_t* const* masks, const int32_t* rois, int n, int c, int dst_h, int dst_w, int bands,
-                                   uint8_t* dst, uint8_t* mask, void* ws, size_t ws_bytes, void* stream);
 
 /* ---- instrumentation read by bench.py -------------------------------------------------------------------------
  * udh_launch_count: kernels this library has launched in this process (monotonic).

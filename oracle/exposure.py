@@ -1,5 +1,5 @@
-"""The mosaic's exposure compensation (udh_mosaic_exposure_stats_u8 and ops.mosaic_exposure_gains; the compensated blends
-udh_mosaic_blend_gain_u8 and udh_mosaic_multiband_gain_u8): cv2.detail_GainCompensator and cv2.detail_ChannelsCompensator
+"""The mosaic's exposure compensation (udh_mosaic_exposure_stats_u8 and ops.mosaic_exposure_gains; the compensated blends,
+udh_mosaic_blend_u8 and udh_mosaic_multiband_u8 with gains): cv2.detail_GainCompensator and cv2.detail_ChannelsCompensator
 fed the multi-band blend's inputs (test infrastructure only).
 
 Inputs: exactly what oracle/multiband.fed gives the blender, for each kept frame k whose ROI meets the canvas: corner_k =

@@ -1,5 +1,5 @@
 """The mosaic's block exposure compensation (udh_mosaic_exposure_block_stats_u8, udh_exposure_block_solve and
-ops.mosaic_exposure_gain_maps; the compensated blends udh_mosaic_blend_gainmap_u8 and udh_mosaic_multiband_gainmap_u8):
+ops.mosaic_exposure_gain_maps; the compensated blends, udh_mosaic_blend_u8 and udh_mosaic_multiband_u8 with maps):
 cv2.detail_BlocksGainCompensator and cv2.detail_BlocksChannelsCompensator fed the multi-band blend's inputs, as
 oracle/exposure.fed gives them (test infrastructure only).
 

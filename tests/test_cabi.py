@@ -81,6 +81,40 @@ def test_x3_mask_and_row_tile_debug_entries_reject_bad_arguments():
     assert b"udh_debug_x3_conv_rows" in L.udh_last_error()
 
 
+def test_mosaic_blends_reject_bad_optional_inputs_before_touching_the_device():
+    """udh_mosaic_blend_u8 / udh_mosaic_multiband_u8 check gains, maps, masks, rois and the workspace before their first
+    CUDA call: every rejection below names its problem and returns before any device pointer is used."""
+    from unsuperviseddeephomographyral2018_b200 import _lib
+    L = _lib.lib
+    p = ctypes.c_void_p(256)                          # never dereferenced: every call below fails its argument checks
+    n, H, W = 2, 8, 8
+    frames = (ctypes.c_void_p * n)(256, 512)
+    sizes = (ctypes.c_int32 * (2 * n))(4, 4, 4, 4)
+    rois = (ctypes.c_int32 * (4 * n))(0, 0, 4, 4, 2, 2, 6, 6)
+    masks = (ctypes.c_void_p * n)(256, 512)
+    null_mask = (ctypes.c_void_p * n)(256, None)
+    maps = (_lib.GainMap * n)(*[_lib.GainMap(256, 256, 256, 2, 2, 1, 0)] * n)
+    bad_maps = (_lib.GainMap * n)(_lib.GainMap(256, 256, 256, 2, 2, 1, 0), _lib.GainMap(256, 256, 256, 0, 2, 1, 0))
+    cases = [(p, maps, None, rois, "gains and maps exclude each other"), (None, None, masks, None, "masks and maps need rois"),
+             (None, maps, None, None, "masks and maps need rois"), (None, None, null_mask, rois, "frame 1's mask is a null pointer"),
+             (None, bad_maps, None, rois, "frame 1's gain map is malformed")]
+    nb = L.udh_mosaic_workspace_bytes(n)
+    for gains, mp, mk, rr, msg in cases:
+        assert L.udh_mosaic_blend_u8(frames, sizes, p, gains, mp, mk, rr, n, 3, p, p, H, W, 4, p, p, p, nb, None) == _lib.EINVAL, msg
+        assert ("udh_mosaic_blend_u8: " + msg).encode() in L.udh_last_error()
+    assert L.udh_mosaic_blend_u8(frames, sizes, p, None, maps, masks, rois, n, 3, p, p, H, W, 4, p, p, p, nb - 1, None) == _lib.EWS
+    assert b"udh_mosaic_blend_u8: workspace of" in L.udh_last_error()
+    nb = L.udh_mosaic_multiband_workspace_bytes(rois, n, H, W, 2)
+    assert nb > 0
+    for gains, mp, mk, rr, msg in cases:
+        if rr is None:
+            msg = "null pointer"                      # the multi-band blend always takes rois
+        assert L.udh_mosaic_multiband_u8(frames, sizes, p, gains, mp, mk, rr, n, 3, H, W, 2, p, p, p, nb, None) == _lib.EINVAL, msg
+        assert ("udh_mosaic_multiband_u8: " + msg).encode() in L.udh_last_error()
+    assert L.udh_mosaic_multiband_u8(frames, sizes, p, None, maps, masks, rois, n, 3, H, W, 2, p, p, p, nb - 1, None) == _lib.EWS
+    assert b"udh_mosaic_multiband_u8: workspace of" in L.udh_last_error()
+
+
 def test_tc_pool_debug_entry_rejects_bad_arguments():
     """udh_debug_tc_pool is exported and checks its arguments before touching the device."""
     from unsuperviseddeephomographyral2018_b200 import _lib

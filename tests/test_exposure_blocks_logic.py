@@ -203,7 +203,7 @@ def test_build_mosaic_rejects_other_modes():
     assert "gain_blocks" in mosaic.COMPENSATE and "channels_blocks" in mosaic.COMPENSATE
 
 
-def test_block_kernels_do_not_spill(tmp_path):
+def test_block_and_gain_map_kernels_do_not_spill(tmp_path):
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     if not os.path.exists(nvcc) and not shutil.which("nvcc"):
         pytest.skip("nvcc not available")
@@ -216,7 +216,8 @@ def test_block_kernels_do_not_spill(tmp_path):
     seen = 0
     for b in blocks:
         name = b.split("'")[0]
-        if "gainblock" in name or "gainmap" in name:
+        if "gainblock" in name or "ExposureBlockFrame" in name or re.search(r"mosaic_blend_u8_kernelILi\dELb0ELb[01]ELb1E|"
+                                                                             r"multiband_base_kernelILb1E", name):
             seen += 1
             assert "0 bytes spill stores, 0 bytes spill loads" in b, (name, b)
     assert seen >= 8

@@ -285,7 +285,7 @@ def warp_object(tmp_path_factory):
 
 
 @NEEDS_TOOLKIT
-def test_mosaic_kernels_do_not_spill(warp_object):
+def test_feathered_blend_instantiations_do_not_spill(warp_object):
     seen, current = {}, None
     for line in warp_object[1].splitlines():
         m = re.search(r"Compiling entry function '([^']+)'", line)
@@ -295,7 +295,7 @@ def test_mosaic_kernels_do_not_spill(warp_object):
         m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", line)
         if m and current and "mosaic_" in current:
             seen[current] = tuple(int(v) for v in m.groups())
-    assert len(seen) == 3, seen                                   # invert, blend C = 1 and C = 3
+    assert len(seen) == 12, seen                                  # the blend: C = 1 and 3, plain, gains, masks, maps and combinations
     assert all(v == (0, 0, 0) for v in seen.values()), seen
 
 

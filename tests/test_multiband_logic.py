@@ -219,9 +219,9 @@ NEEDS_TOOLKIT = pytest.mark.skipif(_tool("nvcc") is None or _tool("cuobjdump") i
 SASS_SHA256 = {"V12.9.86": {
     "_ZN3udh26warp_perspective_u8_kernelILi1EEEvPKhPKdiiPhiii": "4cf086833dca9fb1541e6ce6be759ab5dd46f95819f7b0a32bd20acbfd61752e",
     "_ZN3udh26warp_perspective_u8_kernelILi3EEEvPKhPKdiiPhiii": "6b66c89805d0a06eb07c220cac82937d435e41fde36bd4b1366552b15add20bf",
-    "_ZN3udh22mosaic_blend_u8_kernelILi1EEEvPKNS_11MosaicFrameEiPKiS5_iiiiPhS6_":
+    "_ZN3udh22mosaic_blend_u8_kernelILi1ELb0ELb0ELb0EEEvPKNS_11MosaicFrameEiPKiS5_iiiiPhS6_PKdPKNS_8SeamMaskEPKNS_10GainMapDevE":
         "21efaa682281ae1163e2b5ece1ae58cdbca4af2f9fc5977050081a14a84a8136",
-    "_ZN3udh22mosaic_blend_u8_kernelILi3EEEvPKNS_11MosaicFrameEiPKiS5_iiiiPhS6_":
+    "_ZN3udh22mosaic_blend_u8_kernelILi3ELb0ELb0ELb0EEEvPKNS_11MosaicFrameEiPKiS5_iiiiPhS6_PKdPKNS_8SeamMaskEPKNS_10GainMapDevE":
         "78dc2a9572571dea4c17fbebed4415bbafd4a50d6313609f0b6852dcfde96f59"}}
 
 
@@ -237,7 +237,7 @@ def warp_object(tmp_path_factory):
 
 
 @NEEDS_TOOLKIT
-def test_multiband_kernels_do_not_spill(warp_object):
+def test_warp_perspective_kernels_do_not_spill(warp_object):
     seen, current = {}, None
     for line in warp_object[1].splitlines():
         m = re.search(r"Compiling entry function '([^']+)'", line)
@@ -245,14 +245,16 @@ def test_multiband_kernels_do_not_spill(warp_object):
             current = m.group(1)
             continue
         m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", line)
-        if m and current and "multiband_" in current:
+        if m and current:
             seen[current] = tuple(int(v) for v in m.groups())
-    assert len(seen) == 5, seen                                   # base, pyrDown, accumulate, collapse (level > 0 and 0)
+    mb = [k for k in seen if "multiband_" in k]
+    assert len(mb) == 6, mb                                       # base (plain, gain map), pyrDown, accumulate, collapse (level > 0, 0)
+    assert len(seen) == 31, sorted(seen)                          # every entry function in warp_perspective.cu
     assert all(v == (0, 0, 0) for v in seen.values()), seen
 
 
 @NEEDS_TOOLKIT
-def test_warp_and_feathered_blend_sass_is_unchanged(warp_object):
+def test_warp_and_plain_blend_sass_is_unchanged(warp_object):
     ver = re.search(r"V\d+\.\d+\.\d+", subprocess.run([_tool("nvcc"), "--version"], stdout=subprocess.PIPE, text=True).stdout)
     if not ver or ver.group(0) not in SASS_SHA256:
         pytest.skip("the reference digest was taken with another nvcc (%s)" % (ver.group(0) if ver else "unknown"))

@@ -195,14 +195,14 @@ def test_multiband_reference_equals_cv2_fed_cv2_seams(name):
     assert not np.array_equal(out, unseamed)
 
 
-def test_seam_pairs_are_cv2s_visiting_order():
+def test_roi_pairs_without_the_diagonal_are_cv2s_visiting_order():
     from unsuperviseddeephomographyral2018_b200 import ops
     rng = np.random.default_rng(5)
     for _ in range(20):
         m = int(rng.integers(1, 30))
         x0, y0 = rng.integers(0, 200, m), rng.integers(0, 200, m)
         rois = np.stack([x0, y0, x0 + rng.integers(1, 60, m), y0 + rng.integers(1, 60, m)], 1)
-        ptr, pj = ops.seam_pairs(rois)
+        ptr, pj = ops.roi_pairs(rois, False)
         got = [(i, int(j)) for i in range(m) for j in pj[ptr[i]:ptr[i + 1]]]
         assert got == [(i, j) for i, j, _ in SM.pairs([(int(a), int(b)) for a, b in rois[:, :2]],
                                                       [(int(r[3] - r[1]), int(r[2] - r[0])) for r in rois])]
@@ -289,7 +289,7 @@ def _tool(name):
 
 
 @pytest.mark.skipif(_tool("nvcc") is None, reason="the CUDA toolkit is not installed")
-def test_seam_kernels_do_not_spill(tmp_path):
+def test_seam_and_masked_blend_kernels_do_not_spill(tmp_path):
     from unsuperviseddeephomographyral2018_b200 import build_ext
     cmd = [_tool("nvcc")] + build_ext.NVCC_FLAGS + ["-Xptxas", "-v", "-c", os.path.join(build_ext.CSRC, "warp_perspective.cu"),
                                                     "-o", str(tmp_path / "wp.o")]
@@ -302,7 +302,7 @@ def test_seam_kernels_do_not_spill(tmp_path):
             current = m.group(1)
             continue
         m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", line)
-        if m and current and ("seam_" in current or "multiband_base" in current):
+        if m and current and re.search(r"seam_|mosaic_blend_u8_kernelILi\dELb[01]ELb1ELb0E|multiband_base_kernelILb0E", current):
             seen[current] = tuple(int(v) for v in m.groups())
     # validity, columns, rows, blend masks, the masked feathered blend (C = 1 and 3, with and without gains), the
     # multi-band base (which takes the masks)

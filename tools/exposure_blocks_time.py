@@ -6,15 +6,14 @@
   * the host's sparse assembly (wall time), udh_exposure_block_solve (CUDA events, with its iteration count) and
     udh_exposure_gain_maps (CUDA events);
   * the whole ops.mosaic_exposure_gain_maps in both modes with 1 feed, wall time per call after a warm-up;
-  * the blends with and without gain maps: udh_mosaic_blend_u8 / udh_mosaic_blend_gainmap_u8 (feather 64) and
-    udh_mosaic_multiband_u8 / udh_mosaic_multiband_gainmap_u8 (5 bands), CUDA events over repeated launches.
+  * the blends with and without gain maps: udh_mosaic_blend_u8 (feather 64) and udh_mosaic_multiband_u8 (5 bands),
+    CUDA events over repeated launches (mosaic_time.blend_time).
 cv2.detail_BlocksGainCompensator's dense solve cannot run at these sizes, so it is timed (feed, 1 and 16 threads) on a
 small sweep, 8 x 270x480, next to ops.mosaic_exposure_gain_maps on the same frames.  Prints one JSON line per sweep and
 one with everything, with the card name, power limit and maximum SM clock read in the same run.
 
     python tools/exposure_blocks_time.py
 """
-import ctypes
 import json
 import os
 import sys
@@ -30,8 +29,8 @@ import torch  # noqa: E402
 from oracle import exposure as EX  # noqa: E402
 from oracle import exposure_blocks as XB  # noqa: E402
 from tools import jpeg_time, mosaic_time  # noqa: E402
-from tools.exposure_time import _p, _stream, events_ms  # noqa: E402
-from unsuperviseddeephomographyral2018_b200 import _lib, mosaic, ops  # noqa: E402
+from tools.mosaic_time import _p, _stream, events_ms  # noqa: E402
+from unsuperviseddeephomographyral2018_b200 import _lib, ops  # noqa: E402
 
 BLOCK = 32
 
@@ -50,7 +49,7 @@ def stats_time(dev, M, canvas, reps=10):
     count = raw[:, 0].astype(np.int64)
     pos = count > 0
     sa, sb = np.zeros(len(count)), np.zeros(len(count))
-    sa[pos], sb[pos] = ops._norm_sums(*raw[pos, 7:10].T), ops._norm_sums(*raw[pos, 10:13].T)
+    sa[pos], sb[pos] = ops.exposure_norm_sum(*raw[pos, 7:10].T), ops.exposure_norm_sum(*raw[pos, 10:13].T)
     t0 = time.perf_counter()
     keep, ptr, col, val, rhs = ops.exposure_block_system(st.nblocks, c["a"], c["b"], count, sa, sb)
     out["assembly_ms_host"] = (time.perf_counter() - t0) * 1e3
@@ -88,39 +87,6 @@ def maps_time(dev, M, canvas, reps=3):
     return out
 
 
-def blend_time(dev, M, canvas, reps=10):
-    Hc, Wc = canvas
-    n = len(dev)
-    h, w = dev[0].shape[:2]
-    out_img = torch.empty(Hc, Wc, 3, dtype=torch.uint8, device="cuda")
-    mask = torch.empty(Hc, Wc, dtype=torch.uint8, device="cuda")
-    ptrs = (ctypes.c_void_p * n)(*[t.data_ptr() for t in dev])
-    sz = np.array([(h, w)] * n, np.int32)
-    rois, Mr = mosaic.multiband_rois(M, [(h, w)] * n, Hc, Wc)
-    rr = np.ascontiguousarray(rois.astype(np.int32))
-    gmaps = ops.mosaic_exposure_gain_maps(dev, M, Hc, Wc, "channels", 1, BLOCK)
-    gm, keep = ops._gain_map_table(gmaps, rr, n, torch.device("cuda"), "exposure_blocks_time")
-    res = {}
-    ptr, idx = ops.mosaic_tile_lists(M, [(h, w)] * n, Hc, Wc)
-    ptr_d, idx_d = torch.from_numpy(ptr).cuda(), torch.from_numpy(idx).cuda()
-    M_d = torch.from_numpy(np.ascontiguousarray(M.reshape(n, 9))).cuda()
-    nb = _lib.lib.udh_mosaic_blend_gainmap_workspace_bytes(n)
-    ws = torch.empty(nb, dtype=torch.uint8, device="cuda")
-    res["feather_ms"] = events_ms(lambda: _lib.check(_lib.lib.udh_mosaic_blend_u8(
-        ptrs, sz.ctypes.data, _p(M_d), n, 3, _p(ptr_d), _p(idx_d), Hc, Wc, 64, _p(out_img), _p(mask), _p(ws), nb, _stream())), reps)
-    res["feather_gainmap_ms"] = events_ms(lambda: _lib.check(_lib.lib.udh_mosaic_blend_gainmap_u8(
-        ptrs, sz.ctypes.data, _p(M_d), gm, None, rr.ctypes.data, n, 3, _p(ptr_d), _p(idx_d), Hc, Wc, 64, _p(out_img), _p(mask),
-        _p(ws), nb, _stream())), reps)
-    Mr_d = torch.from_numpy(np.ascontiguousarray(Mr.reshape(n, 9))).cuda()
-    nb = _lib.lib.udh_mosaic_multiband_gainmap_workspace_bytes(rr.ctypes.data, n, Hc, Wc, 5)
-    ws = torch.empty(nb, dtype=torch.uint8, device="cuda")
-    res["multiband_ms"] = events_ms(lambda: _lib.check(_lib.lib.udh_mosaic_multiband_u8(
-        ptrs, sz.ctypes.data, _p(Mr_d), rr.ctypes.data, n, 3, Hc, Wc, 5, _p(out_img), _p(mask), _p(ws), nb, _stream())), reps)
-    res["multiband_gainmap_ms"] = events_ms(lambda: _lib.check(_lib.lib.udh_mosaic_multiband_gainmap_u8(
-        ptrs, sz.ctypes.data, _p(Mr_d), gm, None, rr.ctypes.data, n, 3, Hc, Wc, 5, _p(out_img), _p(mask), _p(ws), nb, _stream())), reps)
-    return res
-
-
 def cv2_small():
     """cv2's block compensators on 8 x 270x480 frames (about 1000 blocks: its dense LU still runs) and ours on the same."""
     import cv2
@@ -150,7 +116,8 @@ def main():
         r = {"canvas": list(canvas)}
         r.update(stats_time(dev, M, canvas))
         r.update(maps_time(dev, M, canvas))
-        r.update(blend_time(dev, M, canvas))
+        r.update(mosaic_time.blend_time(dev, M, canvas, gain_maps=ops.mosaic_exposure_gain_maps(dev, M, canvas[0], canvas[1], "channels", 1,
+                                                                                                  BLOCK)))
         out["sweep_%dx%dx%d" % (n, h, w)] = r
         print(json.dumps(r), flush=True)
         del frames, dev

@@ -6,13 +6,12 @@
     system and cv2.solve), wall time per call after a warm-up;
   * cv2.detail_GainCompensator / ChannelsCompensator's feed on the same ROI warps and masks (the oracle, CPU) with
     cv2.setNumThreads(1) and (16); the ROI warps are made once and not timed;
-  * the blends with and without gains: udh_mosaic_blend_u8 / udh_mosaic_blend_gain_u8 (feather 64) and
-    udh_mosaic_multiband_u8 / udh_mosaic_multiband_gain_u8 (5 bands), CUDA events over repeated launches.
+  * the blends with and without gains: udh_mosaic_blend_u8 (feather 64) and udh_mosaic_multiband_u8 (5 bands),
+    CUDA events over repeated launches (mosaic_time.blend_time).
 Prints one JSON line with the card name, power limit and maximum SM clock read in the same run.
 
     python tools/exposure_time.py
 """
-import ctypes
 import json
 import os
 import sys
@@ -27,27 +26,8 @@ import torch  # noqa: E402
 
 from oracle import exposure as EX  # noqa: E402
 from tools import jpeg_time, mosaic_time  # noqa: E402
-from unsuperviseddeephomographyral2018_b200 import _lib, mosaic, ops  # noqa: E402
-
-
-def _p(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def events_ms(call, reps):
-    call()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        call()
-    e1.record()
-    e1.synchronize()
-    return e0.elapsed_time(e1) / reps
+from tools.mosaic_time import _p, _stream, events_ms  # noqa: E402
+from unsuperviseddeephomographyral2018_b200 import _lib, ops  # noqa: E402
 
 
 def stats_time(dev, M, canvas, reps=10):
@@ -87,40 +67,6 @@ def cv2_time(frames, M, canvas):
     return out
 
 
-def blend_time(dev, M, canvas, reps=10):
-    Hc, Wc = canvas
-    n = len(dev)
-    h, w = dev[0].shape[:2]
-    g = torch.from_numpy(np.random.default_rng(0).uniform(0.8, 1.25, (n, 3))).cuda()
-    out_img = torch.empty(Hc, Wc, 3, dtype=torch.uint8, device="cuda")
-    mask = torch.empty(Hc, Wc, dtype=torch.uint8, device="cuda")
-    ptrs = (ctypes.c_void_p * n)(*[t.data_ptr() for t in dev])
-    sz = np.array([(h, w)] * n, np.int32)
-    res = {}
-    # feathered
-    ptr, idx = ops.mosaic_tile_lists(M, [(h, w)] * n, Hc, Wc)
-    ptr_d, idx_d = torch.from_numpy(ptr).cuda(), torch.from_numpy(idx).cuda()
-    M_d = torch.from_numpy(np.ascontiguousarray(M.reshape(n, 9))).cuda()
-    nb = _lib.lib.udh_mosaic_workspace_bytes(n)
-    ws = torch.empty(nb, dtype=torch.uint8, device="cuda")
-    res["feather_ms"] = events_ms(lambda: _lib.check(_lib.lib.udh_mosaic_blend_u8(
-        ptrs, sz.ctypes.data, _p(M_d), n, 3, _p(ptr_d), _p(idx_d), Hc, Wc, 64, _p(out_img), _p(mask), _p(ws), nb, _stream())), reps)
-    res["feather_gain_ms"] = events_ms(lambda: _lib.check(_lib.lib.udh_mosaic_blend_gain_u8(
-        ptrs, sz.ctypes.data, _p(M_d), _p(g), n, 3, _p(ptr_d), _p(idx_d), Hc, Wc, 64, _p(out_img), _p(mask), _p(ws), nb,
-        _stream())), reps)
-    # multi-band
-    rois, Mr = mosaic.multiband_rois(M, [(h, w)] * n, Hc, Wc)
-    rr = np.ascontiguousarray(rois.astype(np.int32))
-    Mr_d = torch.from_numpy(np.ascontiguousarray(Mr.reshape(n, 9))).cuda()
-    nb = _lib.lib.udh_mosaic_multiband_workspace_bytes(rr.ctypes.data, n, Hc, Wc, 5)
-    ws = torch.empty(nb, dtype=torch.uint8, device="cuda")
-    res["multiband_ms"] = events_ms(lambda: _lib.check(_lib.lib.udh_mosaic_multiband_u8(
-        ptrs, sz.ctypes.data, _p(Mr_d), rr.ctypes.data, n, 3, Hc, Wc, 5, _p(out_img), _p(mask), _p(ws), nb, _stream())), reps)
-    res["multiband_gain_ms"] = events_ms(lambda: _lib.check(_lib.lib.udh_mosaic_multiband_gain_u8(
-        ptrs, sz.ctypes.data, _p(Mr_d), _p(g), rr.ctypes.data, n, 3, Hc, Wc, 5, _p(out_img), _p(mask), _p(ws), nb, _stream())), reps)
-    return res
-
-
 def main():
     torch.cuda.set_device(0)
     out = {"gpu": torch.cuda.get_device_name(0), "card": jpeg_time.card()}
@@ -130,7 +76,8 @@ def main():
         r = {"canvas": list(canvas)}
         r.update(stats_time(dev, M, canvas))
         r.update(gains_time(dev, M, canvas))
-        r.update(blend_time(dev, M, canvas))
+        g = torch.from_numpy(np.random.default_rng(0).uniform(0.8, 1.25, (len(dev), 3))).cuda()
+        r.update(mosaic_time.blend_time(dev, M, canvas, gains=g))
         print(json.dumps(r), flush=True)
         r.update(cv2_time(frames, M, canvas))
         out["sweep_%dx%dx%d" % (n, h, w)] = r

@@ -17,6 +17,7 @@ Prints one JSON line with the card name and power limit read in the same run.
     python tools/mosaic_time.py [--legs feather,multiband]
 """
 import argparse
+import ctypes
 import json
 import os
 import shutil
@@ -54,8 +55,71 @@ def mapped_area(M, h, w):
     return 0.5 * abs(np.dot(x, np.roll(y, -1)) - np.dot(y, np.roll(x, -1)))
 
 
+def _p(t):
+    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
+
+
+def _stream():
+    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def events_ms(call, reps):
+    call()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(reps):
+        call()
+    e1.record()
+    e1.synchronize()
+    return e0.elapsed_time(e1) / reps
+
+
+VARIANTS = {"gains": "gain", "masks": "masked", "gain_maps": "gainmap"}
+
+
+def blend_time(dev, M, canvas, reps=10, **variant):
+    """Both blends alone, plain and with one optional input: CUDA events over repeated calls of udh_mosaic_blend_u8 (feather
+    64) and udh_mosaic_multiband_u8 (5 bands) on the RGB frames dev (CUDA) placed by M (frame -> canvas), every frame's ROI
+    meeting the canvas.  variant: gains= (CUDA float64 [n,3]), masks= ([n] CUDA uint8 blend masks on the ROIs) or
+    gain_maps= ([n], as ops.mosaic_exposure_gain_maps gives them).  -> feather_ms, feather_<v>_ms, multiband_ms and
+    multiband_<v>_ms, <v> the variant's name in VARIANTS."""
+    (kind, value), = variant.items()
+    Hc, Wc = canvas
+    n = len(dev)
+    sizes = [tuple(int(v) for v in t.shape[:2]) for t in dev]
+    out_img = torch.empty(Hc, Wc, 3, dtype=torch.uint8, device="cuda")
+    mask = torch.empty(Hc, Wc, dtype=torch.uint8, device="cuda")
+    ptrs = (ctypes.c_void_p * n)(*[t.data_ptr() for t in dev])
+    sz = np.ascontiguousarray(np.array(sizes, np.int32))
+    rois, Mr = mosaic.multiband_rois(M, sizes, Hc, Wc)
+    rr = np.ascontiguousarray(rois.astype(np.int32))
+    g = value if kind == "gains" else None
+    gm, _keep = ops._gain_map_table(value, rr, n, torch.device("cuda"), "blend_time") if kind == "gain_maps" else (None, None)
+    mp = (ctypes.c_void_p * n)(*[t.data_ptr() for t in value]) if kind == "masks" else None
+    rois_arg = None if kind == "gains" else rr.ctypes.data
+    ptr, idx = ops.mosaic_tile_lists(M, sizes, Hc, Wc)
+    ptr_d, idx_d = torch.from_numpy(ptr).cuda(), torch.from_numpy(idx).cuda()
+    M_d = torch.from_numpy(np.ascontiguousarray(M.reshape(n, 9))).cuda()
+    nb = _lib.lib.udh_mosaic_workspace_bytes(n)
+    ws = torch.empty(nb, dtype=torch.uint8, device="cuda")
+    feather = lambda g, gm, mp, r: lambda: _lib.check(_lib.lib.udh_mosaic_blend_u8(
+        ptrs, sz.ctypes.data, _p(M_d), _p(g), gm, mp, r, n, 3, _p(ptr_d), _p(idx_d), Hc, Wc, 64, _p(out_img), _p(mask), _p(ws), nb,
+        _stream()), "udh_mosaic_blend_u8")
+    res = {"feather_ms": events_ms(feather(None, None, None, None), reps)}
+    res["feather_%s_ms" % VARIANTS[kind]] = events_ms(feather(g, gm, mp, rois_arg), reps)
+    Mr_d = torch.from_numpy(np.ascontiguousarray(Mr.reshape(n, 9))).cuda()
+    nb_mb = _lib.lib.udh_mosaic_multiband_workspace_bytes(rr.ctypes.data, n, Hc, Wc, 5)
+    ws_mb = torch.empty(nb_mb, dtype=torch.uint8, device="cuda")
+    multiband = lambda g, gm, mp: lambda: _lib.check(_lib.lib.udh_mosaic_multiband_u8(
+        ptrs, sz.ctypes.data, _p(Mr_d), _p(g), gm, mp, rr.ctypes.data, n, 3, Hc, Wc, 5, _p(out_img), _p(mask), _p(ws_mb), nb_mb,
+        _stream()), "udh_mosaic_multiband_u8")
+    res["multiband_ms"] = events_ms(multiband(None, None, None), reps)
+    res["multiband_%s_ms" % VARIANTS[kind]] = events_ms(multiband(g, gm, mp), reps)
+    return res
+
+
 def kernel_time(frames, M, canvas, feather=64, reps=10):
-    import ctypes
     Hc, Wc = canvas
     n, (h, w, C) = len(frames), frames[0].shape
     dev = [torch.from_numpy(f).cuda() for f in frames]
@@ -70,8 +134,8 @@ def kernel_time(frames, M, canvas, feather=64, reps=10):
     sz = np.array([(h, w)] * n, np.int32)
     p = lambda t: ctypes.c_void_p(t.data_ptr())
     st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    call = lambda: _lib.check(_lib.lib.udh_mosaic_blend_u8(ptrs, sz.ctypes.data, p(M_d), n, C, p(ptr_d), p(idx_d), Hc, Wc, feather,
-                                                           p(out), p(mask), p(ws), nb, st), "udh_mosaic_blend_u8")
+    call = lambda: _lib.check(_lib.lib.udh_mosaic_blend_u8(ptrs, sz.ctypes.data, p(M_d), None, None, None, None, n, C, p(ptr_d), p(idx_d),
+                                                           Hc, Wc, feather, p(out), p(mask), p(ws), nb, st), "udh_mosaic_blend_u8")
     call()
     torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)

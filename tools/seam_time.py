@@ -3,8 +3,8 @@
   * udh_mosaic_seam_masks_u8 (validity, every intersecting pair's column and row pass, blend masks), CUDA events over
     repeated calls with the frame table and pair list built once; its launch count (udh_launch_count), the pairs, and
     the seam stage alone with the validity and blend-mask launches subtracted (one call without pairs);
-  * the blends with and without blend masks: udh_mosaic_blend_u8 / udh_mosaic_blend_masked_u8 (feather 64) and
-    udh_mosaic_multiband_u8 / udh_mosaic_multiband_masked_u8 (5 bands), CUDA events over repeated launches;
+  * the blends with and without blend masks: udh_mosaic_blend_u8 (feather 64) and udh_mosaic_multiband_u8 (5 bands),
+    CUDA events over repeated launches (mosaic_time.blend_time);
   * cv2.detail's Voronoi seam finder on the same validity masks (the oracle, CPU) with cv2.setNumThreads(1) and (16);
     the masks are made once and not timed.
 Prints one JSON line with the card name, power limit and maximum SM clock read in the same run.
@@ -26,7 +26,7 @@ import torch  # noqa: E402
 
 from oracle import seam as SM  # noqa: E402
 from tools import jpeg_time, mosaic_time  # noqa: E402
-from tools.exposure_time import _p, _stream, events_ms  # noqa: E402
+from tools.mosaic_time import _p, _stream, events_ms  # noqa: E402
 from unsuperviseddeephomographyral2018_b200 import _lib, mosaic, ops  # noqa: E402
 
 
@@ -43,7 +43,7 @@ def seam_time(dev, M, canvas, reps=5):
     seam = torch.empty(int(area.sum()), dtype=torch.uint8, device="cuda")
     blend = torch.empty_like(seam)
     res = {}
-    for label, (ptr, pj) in (("seam", ops.seam_pairs(rr)), ("no_pairs", (np.zeros(n + 1, np.int32), np.zeros(1, np.int32)))):
+    for label, (ptr, pj) in (("seam", ops.roi_pairs(rr, False)), ("no_pairs", (np.zeros(n + 1, np.int32), np.zeros(1, np.int32)))):
         nb = _lib.lib.udh_mosaic_seam_workspace_bytes(rr.ctypes.data, n, ptr.ctypes.data, pj.ctypes.data, Hc, Wc)
         ws = torch.empty(nb, dtype=torch.uint8, device="cuda")
         call = lambda: _lib.check(_lib.lib.udh_mosaic_seam_masks_u8(
@@ -60,39 +60,6 @@ def seam_time(dev, M, canvas, reps=5):
     res["pair_loop_ms"] = res["seam_ms"] - res["no_pairs_ms"]
     res["pair_loop_us_per_pair"] = 1e3 * res["pair_loop_ms"] / max(res["pairs"], 1)
     return res, [blend[int(a):int(b)] for a, b in zip(np.concatenate([[0], np.cumsum(area)[:-1]]), np.cumsum(area))]
-
-
-def blend_time(dev, M, canvas, bmasks, reps=10):
-    Hc, Wc = canvas
-    n = len(dev)
-    sizes = [tuple(int(v) for v in t.shape[:2]) for t in dev]
-    out_img = torch.empty(Hc, Wc, 3, dtype=torch.uint8, device="cuda")
-    mask = torch.empty(Hc, Wc, dtype=torch.uint8, device="cuda")
-    ptrs = (ctypes.c_void_p * n)(*[t.data_ptr() for t in dev])
-    mptrs = (ctypes.c_void_p * n)(*[t.data_ptr() for t in bmasks])
-    sz = np.ascontiguousarray(np.array(sizes, np.int32))
-    rois, Mr = mosaic.multiband_rois(M, sizes, Hc, Wc)
-    rr = np.ascontiguousarray(rois.astype(np.int32))
-    res = {}
-    ptr, idx = ops.mosaic_tile_lists(M, sizes, Hc, Wc)
-    ptr_d, idx_d = torch.from_numpy(ptr).cuda(), torch.from_numpy(idx).cuda()
-    M_d = torch.from_numpy(np.ascontiguousarray(M.reshape(n, 9))).cuda()
-    nb = _lib.lib.udh_mosaic_blend_masked_workspace_bytes(n)
-    ws = torch.empty(nb, dtype=torch.uint8, device="cuda")
-    res["feather_ms"] = events_ms(lambda: _lib.check(_lib.lib.udh_mosaic_blend_u8(
-        ptrs, sz.ctypes.data, _p(M_d), n, 3, _p(ptr_d), _p(idx_d), Hc, Wc, 64, _p(out_img), _p(mask), _p(ws), nb, _stream())), reps)
-    res["feather_masked_ms"] = events_ms(lambda: _lib.check(_lib.lib.udh_mosaic_blend_masked_u8(
-        ptrs, sz.ctypes.data, _p(M_d), None, mptrs, rr.ctypes.data, n, 3, _p(ptr_d), _p(idx_d), Hc, Wc, 64, _p(out_img), _p(mask),
-        _p(ws), nb, _stream())), reps)
-    Mr_d = torch.from_numpy(np.ascontiguousarray(Mr.reshape(n, 9))).cuda()
-    nb = _lib.lib.udh_mosaic_multiband_workspace_bytes(rr.ctypes.data, n, Hc, Wc, 5)
-    ws = torch.empty(nb, dtype=torch.uint8, device="cuda")
-    res["multiband_ms"] = events_ms(lambda: _lib.check(_lib.lib.udh_mosaic_multiband_u8(
-        ptrs, sz.ctypes.data, _p(Mr_d), rr.ctypes.data, n, 3, Hc, Wc, 5, _p(out_img), _p(mask), _p(ws), nb, _stream())), reps)
-    res["multiband_masked_ms"] = events_ms(lambda: _lib.check(_lib.lib.udh_mosaic_multiband_masked_u8(
-        ptrs, sz.ctypes.data, _p(Mr_d), None, mptrs, rr.ctypes.data, n, 3, Hc, Wc, 5, _p(out_img), _p(mask), _p(ws), nb,
-        _stream())), reps)
-    return res
 
 
 def cv2_time(frames, M, canvas):
@@ -117,7 +84,7 @@ def main():
         r = {"canvas": list(canvas)}
         s, bm = seam_time(dev, M, canvas)
         r.update(s)
-        r.update(blend_time(dev, M, canvas, bm))
+        r.update(mosaic_time.blend_time(dev, M, canvas, masks=bm))
         print(json.dumps(r), flush=True)
         r.update(cv2_time(frames, M, canvas))
         out["sweep_%dx%dx%d" % (n, h, w)] = r

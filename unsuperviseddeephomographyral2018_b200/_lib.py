@@ -188,27 +188,18 @@ SIGNATURES = {
     "udh_gray_u8": (c_int, [c_void_p, c_int64, c_void_p, c_void_p]),
     "udh_warp_perspective_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "udh_mosaic_workspace_bytes": (c_size_t, [c_int]),
-    "udh_mosaic_blend_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p,
-                                    c_void_p, c_void_p, c_size_t, c_void_p]),
+    "udh_mosaic_blend_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
+                                    c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "udh_mosaic_multiband_workspace_bytes": (c_size_t, [c_void_p, c_int, c_int, c_int, c_int]),
-    "udh_mosaic_multiband_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
-                                        c_void_p, c_size_t, c_void_p]),
+    "udh_mosaic_multiband_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                        c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "udh_debug_multiband_layout": (c_int, [c_void_p, c_int, c_int, c_int, c_int, POINTER(c_size_t), POINTER(c_int)]),
-    "udh_mosaic_blend_gain_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
-                                         c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
-    "udh_mosaic_multiband_gain_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
-                                             c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "udh_mosaic_exposure_workspace_bytes": (c_size_t, [c_int]),
     "udh_mosaic_exposure_stats_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int,
                                              c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     "udh_mosaic_seam_workspace_bytes": (c_size_t, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int]),
     "udh_mosaic_seam_masks_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p,
                                          c_void_p, c_void_p, c_size_t, c_void_p]),
-    "udh_mosaic_blend_masked_workspace_bytes": (c_size_t, [c_int]),
-    "udh_mosaic_blend_masked_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
-                                           c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
-    "udh_mosaic_multiband_masked_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
-                                               c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "udh_mosaic_exposure_block_workspace_bytes": (c_size_t, [c_int]),
     "udh_mosaic_exposure_block_stats_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int64, c_void_p,
                                                    c_void_p, c_int, c_void_p, c_void_p, c_int64, c_void_p, c_int, c_int, c_int, c_int,
@@ -218,12 +209,6 @@ SIGNATURES = {
                                          c_size_t, c_void_p]),
     "udh_exposure_gain_maps_workspace_bytes": (c_size_t, [c_int64, c_int]),
     "udh_exposure_gain_maps": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
-    "udh_mosaic_blend_gainmap_workspace_bytes": (c_size_t, [c_int]),
-    "udh_mosaic_blend_gainmap_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
-                                            c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
-    "udh_mosaic_multiband_gainmap_workspace_bytes": (c_size_t, [c_void_p, c_int, c_int, c_int, c_int]),
-    "udh_mosaic_multiband_gainmap_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
-                                                c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "udh_draw_report_workspace_bytes": (c_size_t, [c_int]),
     "udh_draw_report_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_int, c_int, c_int,
                                    c_void_p]),

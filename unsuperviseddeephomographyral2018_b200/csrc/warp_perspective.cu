@@ -120,12 +120,22 @@ __global__ void __launch_bounds__(256) warp_perspective_u8_kernel(const uint8_t*
 
 // ---- sequence mosaic: every frame warped onto one canvas and blended (the blend rule: oracle/mosaic.py) ---------------
 struct MosaicFrame {
-  double mi[9];                   // cv_invert3 of the frame's M (frame -> canvas), filled by mosaic_invert_kernel
+  double mi[9];                   // cv_invert3 of the frame's M (frame -> canvas), filled by invert_kernel
   const uint8_t* src;
   int h, w;
 };
 
-__global__ void mosaic_invert_kernel(const double* __restrict__ M, MosaicFrame* fr, int n) {
+// A frame warped onto its ROI rectangle of the canvas (the multi-band blend's feed, the exposure statistics, the seams):
+// the frame, the ROI (rx, ry, rw, rh) and the ROI warp's tile width.  roi_frame fills it on the host.
+struct RoiFrame {
+  const uint8_t* src;
+  int h, w;
+  int rx, ry, rw, rh, bw;
+};
+
+// Every frame's inverse into its table entry: fr[k].mi = cv_invert3(M_k).
+template <class Frame>
+__global__ void invert_kernel(const double* __restrict__ M, Frame* fr, int n) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k < n) cv_invert3(M + (int64_t)k * 9, fr[k].mi);
 }
@@ -187,13 +197,14 @@ __device__ __forceinline__ void gm_gains(const GainMapDev* __restrict__ G, int l
 // registers and stores the pixels once: no atomics, no accumulation buffer.  Integer sums: the result does not depend on
 // the frames' order.  GAIN: each frame's value is first compensated, ex_apply(v, gains[f][c]) (channel 0's gain when C = 1).
 // MASK: a frame counts only where its blend mask smask[f] is set as well.  MAP: each frame's value is compensated by its
-// gain map at the pixel's ROI coordinates (gm_gains).
-template <int C, bool GAIN, bool MASK = false, bool MAP = false>
-__device__ __forceinline__ void mosaic_blend_tile(const MosaicFrame* __restrict__ fr, int n, const int32_t* __restrict__ tile_ptr,
-                                                  const int32_t* __restrict__ tile_frames, int dh, int dw, int bw, int feather32,
-                                                  const double* __restrict__ gains, uint8_t* __restrict__ dst,
-                                                  uint8_t* __restrict__ mask, const SeamMask* __restrict__ smask = nullptr,
-                                                  const GainMapDev* __restrict__ gmap = nullptr) {
+// gain map at the pixel's ROI coordinates (gm_gains).  The optional tables come last, so the plain blend's parameters keep
+// their offsets and its code is the feathered blend's own.
+template <int C, bool GAIN, bool MASK, bool MAP>
+__global__ void __launch_bounds__(256) mosaic_blend_u8_kernel(const MosaicFrame* __restrict__ fr, int n, const int32_t* __restrict__ tile_ptr,
+                                                              const int32_t* __restrict__ tile_frames, int dh, int dw, int bw,
+                                                              int feather32, uint8_t* __restrict__ dst, uint8_t* __restrict__ mask,
+                                                              const double* __restrict__ gains, const SeamMask* __restrict__ smask,
+                                                              const GainMapDev* __restrict__ gmap) {
   const int y = blockIdx.y * UDH_MOSAIC_TILE_H + threadIdx.x / (UDH_MOSAIC_TILE_W / 4);
   const int x0 = blockIdx.x * UDH_MOSAIC_TILE_W + threadIdx.x % (UDH_MOSAIC_TILE_W / 4) * 4;
   if (y >= dh || x0 >= dw) return;
@@ -271,55 +282,13 @@ __device__ __forceinline__ void mosaic_blend_tile(const MosaicFrame* __restrict_
   }
 }
 
-template <int C>
-__global__ void __launch_bounds__(256) mosaic_blend_u8_kernel(const MosaicFrame* __restrict__ fr, int n,
-                                                              const int32_t* __restrict__ tile_ptr,
-                                                              const int32_t* __restrict__ tile_frames, int dh, int dw, int bw,
-                                                              int feather32, uint8_t* __restrict__ dst,
-                                                              uint8_t* __restrict__ mask) {
-  mosaic_blend_tile<C, false>(fr, n, tile_ptr, tile_frames, dh, dw, bw, feather32, nullptr, dst, mask);
-}
-
-// The feathered blend of exposure-compensated frames: gains [n][3] float64.
-template <int C>
-__global__ void __launch_bounds__(256) exposure_blend_u8_kernel(const MosaicFrame* __restrict__ fr, int n,
-                                                                const int32_t* __restrict__ tile_ptr,
-                                                                const int32_t* __restrict__ tile_frames, int dh, int dw, int bw,
-                                                                int feather32, const double* __restrict__ gains,
-                                                                uint8_t* __restrict__ dst, uint8_t* __restrict__ mask) {
-  mosaic_blend_tile<C, true>(fr, n, tile_ptr, tile_frames, dh, dw, bw, feather32, gains, dst, mask);
-}
-
-// The feathered blend with each frame kept only where its blend mask is set (GAIN: of exposure-compensated frames).
-template <int C, bool GAIN>
-__global__ void __launch_bounds__(256) seam_blend_u8_kernel(const MosaicFrame* __restrict__ fr, int n, const int32_t* __restrict__ tile_ptr,
-                                                            const int32_t* __restrict__ tile_frames, int dh, int dw, int bw,
-                                                            int feather32, const double* __restrict__ gains,
-                                                            const SeamMask* __restrict__ smask, uint8_t* __restrict__ dst,
-                                                            uint8_t* __restrict__ mask) {
-  mosaic_blend_tile<C, GAIN, true>(fr, n, tile_ptr, tile_frames, dh, dw, bw, feather32, gains, dst, mask, smask);
-}
-
-// The feathered blend of frames compensated by their gain maps (MASK: kept only where their blend masks are set).
-template <int C, bool MASK>
-__global__ void __launch_bounds__(256) gainmap_blend_u8_kernel(const MosaicFrame* __restrict__ fr, int n, const int32_t* __restrict__ tile_ptr,
-                                                               const int32_t* __restrict__ tile_frames, int dh, int dw, int bw,
-                                                               int feather32, const SeamMask* __restrict__ smask,
-                                                               const GainMapDev* __restrict__ gmap, uint8_t* __restrict__ dst,
-                                                               uint8_t* __restrict__ mask) {
-  mosaic_blend_tile<C, false, MASK, true>(fr, n, tile_ptr, tile_frames, dh, dw, bw, feather32, nullptr, dst, mask, smask, gmap);
-}
-
 // ---- multi-band blend: cv2.detail_MultiBandBlender with CV_16S weights (the rule: oracle/multiband.py) ----------------
 // Per frame k, its fed rectangle (ROI grown by the gap, aligned to 2^B) holds the image pyramid G_i (uchar4, RGB + pad)
 // and the weight pyramid W_i (int16) in two pools; the canvas pyramid keeps (acc, wacc) as short4 per pixel, and the
 // collapsed levels R_i (i >= 1) as short4 in a second pyramid, so acc and wacc survive the blend.
 constexpr int MB_MAX_BANDS = 10;
 
-struct MultibandFrame {
-  const uint8_t* src;
-  int h, w;                        // the frame
-  int rx, ry, rw, rh, bw;          // its ROI on the canvas, and the ROI warp's tile width
+struct MultibandFrame : RoiFrame {
   int x0, y0, pw, ph;              // the fed rectangle at level 0 (canvas coordinates; multiples of 2^B)
   int64_t off[MB_MAX_BANDS + 1];   // element offset of level i in the G and W pools
   const uint8_t* bmask;            // null, or the frame's blend mask on its ROI (rh x rw, 0 / 255): the weight's mask
@@ -364,9 +333,9 @@ __device__ __forceinline__ bool mb_roi_warp(const uint8_t* __restrict__ s, int h
 // its weight from that mask instead of the warp's validity.
 // MAP: the ROI warp is compensated by the frame's gain map at each ROI pixel instead (gm_gains, ex_apply_f).
 template <bool MAP>
-__device__ __forceinline__ void mb_base(const MultibandFrame* __restrict__ fr, const double* __restrict__ M,
-                                        const double* __restrict__ gains, const GainMapDev* __restrict__ gmap,
-                                        uchar4* __restrict__ G, int16_t* __restrict__ Wt) {
+__global__ void __launch_bounds__(256) multiband_base_kernel(const MultibandFrame* __restrict__ fr, const double* __restrict__ M,
+                                                             const double* __restrict__ gains, const GainMapDev* __restrict__ gmap,
+                                                             uchar4* __restrict__ G, int16_t* __restrict__ Wt) {
   __shared__ double mi[9];
   const int k = blockIdx.y;
   if (threadIdx.x == 0) cv_invert3(M + (int64_t)k * 9, mi);
@@ -402,19 +371,6 @@ __device__ __forceinline__ void mb_base(const MultibandFrame* __restrict__ fr, c
     G[off + e] = make_uchar4((unsigned char)v[0], (unsigned char)v[1], (unsigned char)v[2], 0);
     Wt[off + e] = valid ? 256 : 0;
   }
-}
-
-__global__ void __launch_bounds__(256) multiband_base_kernel(const MultibandFrame* __restrict__ fr, const double* __restrict__ M,
-                                                             const double* __restrict__ gains, uchar4* __restrict__ G,
-                                                             int16_t* __restrict__ Wt) {
-  mb_base<false>(fr, M, gains, nullptr, G, Wt);
-}
-
-// Level 0 with every frame's ROI warp compensated by its gain map.
-__global__ void __launch_bounds__(256) gainmap_mb_base_kernel(const MultibandFrame* __restrict__ fr, const double* __restrict__ M,
-                                                                     const GainMapDev* __restrict__ gmap, uchar4* __restrict__ G,
-                                                                     int16_t* __restrict__ Wt) {
-  mb_base<true>(fr, M, nullptr, gmap, G, Wt);
 }
 
 // Level lvl -> lvl + 1 of every frame's G and W: cv2.pyrDown (taps 1 4 6 4 1, BORDER_REFLECT_101, (sum + 128) >> 8).
@@ -574,8 +530,48 @@ struct MultibandPlan {
 
 static size_t mb_align(size_t v) { return (v + 255) & ~(size_t)255; }
 
-// rois [n,4] (x_lo, y_lo, x_hi, y_hi) -> plan (sizes may be null: the frame fields are left unset).  0 or an error.
-static int mb_plan(const int32_t* rois, const int32_t* sizes, int n, int Hc, int Wc, int bands, MultibandPlan& p) {
+// The warp's tile width for an h x w output: tiles of up to 16 rows and 1024 pixels.
+static int warp_tile_w(int h, int w) {
+  const int bh = h < 16 ? h : 16;
+  return 1024 / bh < w ? 1024 / bh : w;
+}
+
+// Frame k's ROI rois[k] (x_lo, y_lo, x_hi, y_hi: non-empty, inside the dst_h x dst_w canvas) -> F, with the frame's
+// pointer and size unless frames and sizes are null (the workspace-size calls leave them unset).  0 or an error.
+static int roi_frame(const uint8_t* const* frames, const int32_t* sizes, const int32_t* rois, int k, int dst_h, int dst_w, RoiFrame& F,
+                     const char* what) {
+  const int* r = rois + 4 * k;
+  UDH_REQUIRE(r[0] >= 0 && r[1] >= 0 && r[0] < r[2] && r[1] < r[3] && r[2] <= dst_w && r[3] <= dst_h,
+              "%s: frame %d's ROI (%d, %d)..(%d, %d) is empty or leaves the %dx%d canvas", what, k, r[0], r[1], r[2], r[3], dst_h,
+              dst_w);
+  F.rx = r[0]; F.ry = r[1]; F.rw = r[2] - r[0]; F.rh = r[3] - r[1];
+  F.bw = warp_tile_w(F.rh, F.rw);
+  if (frames) {
+    UDH_REQUIRE(frames[k], "%s: frame %d is a null pointer", what, k);
+    F.src = frames[k];
+  }
+  if (sizes) {
+    F.h = sizes[2 * k];
+    F.w = sizes[2 * k + 1];
+    UDH_REQUIRE(F.h >= 1 && F.w >= 1 && F.h < 32767 && F.w < 32767, "%s: frame %d is %dx%d", what, k, F.h, F.w);
+  }
+  return UDH_OK;
+}
+
+// Copies a host table to dst on the device (pageable source: the copy is staged before this returns, so the table may go).
+template <class T>
+static int upload(void* dst, const std::vector<T>& table, cudaStream_t st, const char* what) {
+  const cudaError_t e = cudaMemcpyAsync(dst, table.data(), table.size() * sizeof(T), cudaMemcpyHostToDevice, st);
+  if (e != cudaSuccess) {
+    set_error("%s: table copy: %s", what, cudaGetErrorString(e));
+    return UDH_ECUDA;
+  }
+  return UDH_OK;
+}
+
+// rois [n,4] (x_lo, y_lo, x_hi, y_hi) -> plan (frames and sizes may be null: the frame fields are left unset).  0 or an error.
+static int mb_plan(const uint8_t* const* frames, const int32_t* rois, const int32_t* sizes, int n, int Hc, int Wc, int bands,
+                   MultibandPlan& p) {
   UDH_REQUIRE(n >= 1 && n <= 65535 && Hc >= 1 && Wc >= 1 && Hc < 32767 && Wc < 32767,
               "udh_mosaic_multiband_u8: bad dimensions (n %d, canvas %dx%d)", n, Hc, Wc);
   UDH_REQUIRE(bands >= 0 && bands <= MB_MAX_BANDS, "udh_mosaic_multiband_u8: bands must be in [0, %d] (got %d)", MB_MAX_BANDS, bands);
@@ -590,17 +586,12 @@ static int mb_plan(const int32_t* rois, const int32_t* sizes, int n, int Hc, int
   for (int i = 0; i <= MB_MAX_BANDS; ++i) p.max_px[i] = 0;
   int64_t E = 0;
   for (int k = 0; k < n; ++k) {
-    const int* r = rois + 4 * k;
-    UDH_REQUIRE(r[0] >= 0 && r[1] >= 0 && r[0] < r[2] && r[1] < r[3] && r[2] <= Wc && r[3] <= Hc,
-                "udh_mosaic_multiband_u8: frame %d's ROI (%d, %d)..(%d, %d) is empty or leaves the %dx%d canvas", k, r[0], r[1],
-                r[2], r[3], Hc, Wc);
     MultibandFrame& F = p.fr[k];
-    F.rx = r[0]; F.ry = r[1]; F.rw = r[2] - r[0]; F.rh = r[3] - r[1];
-    const int bh = F.rh < 16 ? F.rh : 16;
-    F.bw = 1024 / bh < F.rw ? 1024 / bh : F.rw;
+    const int rc = roi_frame(frames, sizes, rois, k, Hc, Wc, F, "udh_mosaic_multiband_u8");
+    if (rc != UDH_OK) return rc;
     // cv2's tl_new / br_new: grow by the gap, clip, align to 2^B, shift back inside the padded canvas
     int x0 = F.rx - gap > 0 ? F.rx - gap : 0, y0 = F.ry - gap > 0 ? F.ry - gap : 0;
-    int x1 = r[2] + gap < p.Wp ? r[2] + gap : p.Wp, y1 = r[3] + gap < p.Hp ? r[3] + gap : p.Hp;
+    int x1 = F.rx + F.rw + gap < p.Wp ? F.rx + F.rw + gap : p.Wp, y1 = F.ry + F.rh + gap < p.Hp ? F.ry + F.rh + gap : p.Hp;
     x0 = (x0 >> p.B) << p.B;
     y0 = (y0 >> p.B) << p.B;
     x1 = x0 + (x1 - x0) + (a - (x1 - x0) % a) % a;
@@ -612,11 +603,6 @@ static int mb_plan(const int32_t* rois, const int32_t* sizes, int n, int Hc, int
       F.off[i] = E;
       E += px;
       if (px > p.max_px[i]) p.max_px[i] = px;
-    }
-    if (sizes) {
-      F.h = sizes[2 * k];
-      F.w = sizes[2 * k + 1];
-      UDH_REQUIRE(F.h >= 1 && F.w >= 1 && F.h < 32767 && F.w < 32767, "udh_mosaic_multiband_u8: frame %d is %dx%d", k, F.h, F.w);
     }
   }
   p.E = E;
@@ -648,18 +634,50 @@ static unsigned mb_blocks(int64_t px) {
 // the count, each frame's channel sums and, with norms, each frame's sum of sqrt(r^2 + g^2 + b^2) (cv2's norm(Vec3b)).
 // Such a norm is 0 or a multiple of 2^-52 below 2^9, so q = norm 2^52 is an integer below 2^61; it is summed exactly as
 // three 21-bit limbs (each limb's sum stays below 2^52 for up to 2^31 pixels), and the host rounds the total once.
-struct ExposureFrame {
+struct ExposureFrame : RoiFrame {
   double mi[9];                    // cv_invert3 of M'_k (frame -> its ROI)
-  const uint8_t* src;
-  int h, w;
-  int rx, ry, rw, rh, bw;          // the ROI on the canvas and the ROI warp's tile width
 };
 
 constexpr int EX_TILE_W = 32, EX_TILE_H = 64, EX_CHUNK = 8, EX_PAIRS = EX_CHUNK * EX_CHUNK;
 
-__global__ void exposure_invert_kernel(const double* __restrict__ M, ExposureFrame* fr, int n) {
-  const int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k < n) cv_invert3(M + (int64_t)k * 9, fr[k].mi);
+// The frames whose ROI meets the CTA's EX_TILE_W x EX_TILE_H tile at (tx0, ty0), in ascending frame order, into cand: per
+// 256 frames, each warp's ballot, ranked by the warps before it.  Returns their count.
+template <class Frame>
+__device__ __forceinline__ int ex_candidates(const Frame* __restrict__ fr, int n, int tx0, int ty0, int* cand, int* wcount) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int nc = 0;
+  for (int c0 = 0; c0 < n; c0 += blockDim.x) {
+    const int k = c0 + threadIdx.x;
+    bool hit = false;
+    if (k < n) {
+      const Frame* F = fr + k;
+      const int rx = __ldg(&F->rx), ry = __ldg(&F->ry);
+      hit = rx < tx0 + EX_TILE_W && rx + __ldg(&F->rw) > tx0 && ry < ty0 + EX_TILE_H && ry + __ldg(&F->rh) > ty0;
+    }
+    const unsigned bal = __ballot_sync(0xffffffffu, hit);
+    if (lane == 0) wcount[warp] = __popc(bal);
+    __syncthreads();
+    int base = nc, tot = 0;
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      base += q < warp ? wcount[q] : 0;
+      tot += wcount[q];
+    }
+    if (hit) cand[base + __popc(bal & ((1u << lane) - 1u))] = k;
+    nc += tot;
+    __syncthreads();                                                  // wcount is rewritten next round
+  }
+  return nc;
+}
+
+// The index of pair (i, j) in the CSR pair list (row i, ascending j), or -1 when the pair is not listed.
+__device__ __forceinline__ int ex_pair(const int32_t* __restrict__ pair_ptr, const int32_t* __restrict__ pair_j, int i, int j) {
+  int lo = __ldg(pair_ptr + i), hi = __ldg(pair_ptr + i + 1);
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (__ldg(pair_j + mid) < j) lo = mid + 1; else hi = mid;
+  }
+  return lo < __ldg(pair_ptr + i + 1) && __ldg(pair_j + lo) == j ? lo : -1;
 }
 
 // Gather form: one CTA per EX_TILE_W x EX_TILE_H canvas tile, each warp one row of 32 pixels at a time.  The CTA lists
@@ -682,29 +700,7 @@ __global__ void __launch_bounds__(256) exposure_stats_kernel(const ExposureFrame
   __shared__ unsigned long long acc[EX_PAIRS][UDH_EXPOSURE_STATS];
   const int tx0 = blockIdx.x * EX_TILE_W, ty0 = blockIdx.y * EX_TILE_H;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  // the candidates in ascending frame order: per 256 frames, each warp's ballot, ranked by the warps before it
-  int nc = 0;
-  for (int c0 = 0; c0 < n; c0 += blockDim.x) {
-    const int k = c0 + threadIdx.x;
-    bool hit = false;
-    if (k < n) {
-      const ExposureFrame* F = fr + k;
-      const int rx = __ldg(&F->rx), ry = __ldg(&F->ry);
-      hit = rx < tx0 + EX_TILE_W && rx + __ldg(&F->rw) > tx0 && ry < ty0 + EX_TILE_H && ry + __ldg(&F->rh) > ty0;
-    }
-    const unsigned bal = __ballot_sync(0xffffffffu, hit);
-    if (lane == 0) wcount[warp] = __popc(bal);
-    __syncthreads();
-    int base = nc, tot = 0;
-#pragma unroll
-    for (int q = 0; q < 8; ++q) {
-      base += q < warp ? wcount[q] : 0;
-      tot += wcount[q];
-    }
-    if (hit) cand[base + __popc(bal & ((1u << lane) - 1u))] = k;
-    nc += tot;
-    __syncthreads();                                                  // wcount is rewritten next round
-  }
+  const int nc = ex_candidates(fr, n, tx0, ty0, cand, wcount);
   const int nch = (nc + EX_CHUNK - 1) / EX_CHUNK;
   for (int A = 0; A < nch; ++A) {
     for (int B = A; B < nch; ++B) {
@@ -712,15 +708,7 @@ __global__ void __launch_bounds__(256) exposure_stats_kernel(const ExposureFrame
       if (threadIdx.x < EX_PAIRS) {
         const int a = threadIdx.x / EX_CHUNK, b = threadIdx.x % EX_CHUNK, ka = A * EX_CHUNK + a, kb = B * EX_CHUNK + b;
         int p = -1;
-        if (ka < nc && kb < nc && (A != B || a <= b)) {
-          const int i = cand[ka], j = cand[kb];                       // i <= j: the list ascends
-          int lo = __ldg(pair_ptr + i), hi = __ldg(pair_ptr + i + 1);
-          while (lo < hi) {
-            const int mid = (lo + hi) >> 1;
-            if (__ldg(pair_j + mid) < j) lo = mid + 1; else hi = mid;
-          }
-          if (lo < __ldg(pair_ptr + i + 1) && __ldg(pair_j + lo) == j) p = lo;
-        }
+        if (ka < nc && kb < nc && (A != B || a <= b)) p = ex_pair(pair_ptr, pair_j, cand[ka], cand[kb]);   // i <= j: the list ascends
         pidx[threadIdx.x] = p;
       }
       for (int e = threadIdx.x; e < EX_PAIRS * UDH_EXPOSURE_STATS; e += blockDim.x) (&acc[0][0])[e] = 0;
@@ -795,19 +783,11 @@ __global__ void __launch_bounds__(256) exposure_stats_kernel(const ExposureFrame
 // memory.  A listed frame pair's block pair at a pixel names one cell of the pair's merged block grid (udh.h), so each
 // warp groups its lanes by cell (__match_any_sync), sums each group's terms with __reduce_add_sync and its leader adds
 // them to the cell's global sums.  Every sum is an integer: the result does not depend on the order or the run.
-struct ExposureBlockFrame {
+struct ExposureBlockFrame : RoiFrame {
   double mi[9];                    // cv_invert3 of M'_k (frame -> its ROI)
-  const uint8_t* src;
-  int h, w;
-  int rx, ry, rw, rh, bw;          // the ROI on the canvas and the ROI warp's tile width
   int bkw, bkh, bpx;               // the blocks' width and height, blocks per row
   int64_t boff;                    // the frame's first block
 };
-
-__global__ void gainblock_invert_kernel(const double* __restrict__ M, ExposureBlockFrame* fr, int n) {
-  const int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k < n) cv_invert3(M + (int64_t)k * 9, fr[k].mi);
-}
 
 __global__ void __launch_bounds__(256) gainblock_stats_kernel(const ExposureBlockFrame* __restrict__ fr, int n,
                                                                    const int32_t* __restrict__ pair_ptr,
@@ -824,28 +804,7 @@ __global__ void __launch_bounds__(256) gainblock_stats_kernel(const ExposureBloc
   __shared__ int snx[EX_PAIRS], sb0[EX_PAIRS][4];                       // cells per row; bx_i0, by_i0, bx_j0, by_j0
   const int tx0 = blockIdx.x * EX_TILE_W, ty0 = blockIdx.y * EX_TILE_H;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  int nc = 0;
-  for (int c0 = 0; c0 < n; c0 += blockDim.x) {
-    const int k = c0 + threadIdx.x;
-    bool hit = false;
-    if (k < n) {
-      const ExposureBlockFrame* F = fr + k;
-      const int rx = __ldg(&F->rx), ry = __ldg(&F->ry);
-      hit = rx < tx0 + EX_TILE_W && rx + __ldg(&F->rw) > tx0 && ry < ty0 + EX_TILE_H && ry + __ldg(&F->rh) > ty0;
-    }
-    const unsigned bal = __ballot_sync(0xffffffffu, hit);
-    if (lane == 0) wcount[warp] = __popc(bal);
-    __syncthreads();
-    int base = nc, tot = 0;
-#pragma unroll
-    for (int q = 0; q < 8; ++q) {
-      base += q < warp ? wcount[q] : 0;
-      tot += wcount[q];
-    }
-    if (hit) cand[base + __popc(bal & ((1u << lane) - 1u))] = k;
-    nc += tot;
-    __syncthreads();
-  }
+  const int nc = ex_candidates(fr, n, tx0, ty0, cand, wcount);
   // the chunk count is re-read from shared memory: kept in a register it lives across the warp's double-division call
   // and ptxas spills it
   if (threadIdx.x == 0) nchunks = (nc + EX_CHUNK - 1) / EX_CHUNK;
@@ -856,13 +815,8 @@ __global__ void __launch_bounds__(256) gainblock_stats_kernel(const ExposureBloc
         const int a = threadIdx.x / EX_CHUNK, b = threadIdx.x % EX_CHUNK, ka = A * EX_CHUNK + a, kb = B * EX_CHUNK + b;
         long long o = -1;
         if (ka < nc && kb < nc && (A != B || a <= b)) {
-          const int i = cand[ka], j = cand[kb];
-          int lo = __ldg(pair_ptr + i), hi = __ldg(pair_ptr + i + 1);
-          while (lo < hi) {
-            const int mid = (lo + hi) >> 1;
-            if (__ldg(pair_j + mid) < j) lo = mid + 1; else hi = mid;
-          }
-          if (lo < __ldg(pair_ptr + i + 1) && __ldg(pair_j + lo) == j) {
+          const int i = cand[ka], j = cand[kb], lo = ex_pair(pair_ptr, pair_j, i, j);
+          if (lo >= 0) {
             const ExposureBlockFrame *Fi = fr + i, *Fj = fr + j;
             const int x0 = max(__ldg(&Fi->rx), __ldg(&Fj->rx)), y0 = max(__ldg(&Fi->ry), __ldg(&Fj->ry));
             o = __ldg(cell_off + lo);
@@ -1077,11 +1031,8 @@ __global__ void __launch_bounds__(256) gainblock_maps_kernel(const double* __res
 // (distances are below 2^17, the window's sides below 32767 + 2 SEAM_GAP).
 constexpr int SEAM_GAP = 10, SEAM_INF = 1 << 30, SEAM_SEGS = 16, SEAM_ROW_THREADS = 256;
 
-struct SeamFrame {
-  const uint8_t* src;
-  int h, w;
-  int rx, ry, rw, rh, bw;          // the ROI on the canvas and the ROI warp's tile width
-  int64_t off;                     // the ROI's element offset in the mask pools
+struct SeamFrame : RoiFrame {
+  int64_t off;                  // the ROI's element offset in the mask pools
 };
 
 struct SeamRect {                  // a frame's ROI and pool offset, passed by value to the pair kernels
@@ -1294,8 +1245,7 @@ extern "C" int udh_warp_perspective_u8(const uint8_t* src, const double* M, uint
                   dst_w < 32767,
               "udh_warp_perspective_u8: bad dimensions (n %d, %dx%d -> %dx%d)", n, h, w, dst_h, dst_w);
   if (n == 0) return UDH_OK;
-  const int bh = dst_h < 16 ? dst_h : 16;
-  const int bw = 1024 / bh < dst_w ? 1024 / bh : dst_w;
+  const int bw = warp_tile_w(dst_h, dst_w);
   const int groups = (dst_h * dst_w + 3) / 4;
   const dim3 grid((unsigned)((groups + 255) / 256), (unsigned)n);
   if (c == 3)
@@ -1305,171 +1255,107 @@ extern "C" int udh_warp_perspective_u8(const uint8_t* src, const double* M, uint
   return check_launch("udh_warp_perspective_u8");
 }
 
-extern "C" size_t udh_mosaic_workspace_bytes(int n) { return n > 0 ? (size_t)n * sizeof(MosaicFrame) : 0; }
-
-extern "C" size_t udh_mosaic_blend_masked_workspace_bytes(int n) {
-  return n > 0 ? mb_align((size_t)n * sizeof(MosaicFrame)) + (size_t)n * sizeof(SeamMask) : 0;
-}
-
-extern "C" size_t udh_mosaic_blend_gainmap_workspace_bytes(int n) {
+// The feathered blend's workspace: the frame table, then the mask table, then the map table.
+extern "C" size_t udh_mosaic_workspace_bytes(int n) {
   return n > 0 ? mb_align((size_t)n * sizeof(MosaicFrame)) + mb_align((size_t)n * sizeof(SeamMask)) + (size_t)n * sizeof(GainMapDev) : 0;
 }
 
-// The device table of n gain maps on the rectangles rois [n,4] (an empty rectangle: the frame has no map and counts nowhere).
+// The table of n gain maps on the rectangles rois [n,4] (an empty rectangle: the frame has no map and counts nowhere).
 static int gm_table(const udh_gain_map* maps, const int32_t* rois, int n, int dst_h, int dst_w, std::vector<GainMapDev>& out,
                     const char* what) {
-  UDH_REQUIRE(maps && rois, "%s: null maps or rois", what);
+  out.assign((size_t)n, GainMapDev{});
   for (int k = 0; k < n; ++k) {
     const int* r = rois + 4 * k;
-    GainMapDev& G = out[(size_t)k];
-    G = GainMapDev{};
     if (r[2] <= r[0] || r[3] <= r[1]) continue;
     UDH_REQUIRE(r[0] >= 0 && r[1] >= 0 && r[2] <= dst_w && r[3] <= dst_h, "%s: frame %d's rectangle (%d, %d)..(%d, %d) leaves the %dx%d canvas",
                 what, k, r[0], r[1], r[2], r[3], dst_h, dst_w);
     const udh_gain_map& m = maps[k];
     UDH_REQUIRE(m.map && m.cols && m.rows && m.bpx >= 1 && m.bpy >= 1 && (m.channels == 1 || m.channels == 3),
                 "%s: frame %d's gain map is malformed (%dx%d blocks, %d channels)", what, k, m.bpy, m.bpx, m.channels);
-    G.m = m;
-    G.rx = r[0]; G.ry = r[1]; G.rw = r[2] - r[0]; G.rh = r[3] - r[1];
+    out[(size_t)k] = GainMapDev{m, r[0], r[1], r[2] - r[0], r[3] - r[1]};
   }
   return UDH_OK;
 }
 
-// masks (null: none) with mrois [n,4]: each frame's blend mask on its rectangle (x_lo, y_lo, x_hi, y_hi); an empty one
-// keeps the frame out of the blend.
-static int mosaic_blend(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains, int n, int c,
-                        const int32_t* tile_ptr, const int32_t* tile_frames, int dst_h, int dst_w, int feather, uint8_t* dst,
-                        uint8_t* mask, void* ws, size_t ws_bytes, void* stream, const uint8_t* const* masks = nullptr,
-                        const int32_t* mrois = nullptr, const udh_gain_map* gmaps = nullptr) {
-  UDH_REQUIRE(tile_ptr && tile_frames && dst && mask && (n == 0 || (frames && sizes && M && ws)), "udh_mosaic_blend_u8: null pointer");
-  UDH_REQUIRE(c == 1 || c == 3, "udh_mosaic_blend_u8: channels must be 1 or 3 (got %d)", c);
+using BlendKernel = void (*)(const MosaicFrame*, int, const int32_t*, const int32_t*, int, int, int, int, uint8_t*, uint8_t*, const double*,
+                             const SeamMask*, const GainMapDev*);
+
+// The feathered blend's instantiation for C channels and the optional inputs given (gains and maps exclude each other).
+template <int C>
+static BlendKernel blend_kernel(bool gain, bool masked, bool map) {
+  if (map) return masked ? mosaic_blend_u8_kernel<C, false, true, true> : mosaic_blend_u8_kernel<C, false, false, true>;
+  if (gain) return masked ? mosaic_blend_u8_kernel<C, true, true, false> : mosaic_blend_u8_kernel<C, true, false, false>;
+  return masked ? mosaic_blend_u8_kernel<C, false, true, false> : mosaic_blend_u8_kernel<C, false, false, false>;
+}
+
+extern "C" int udh_mosaic_blend_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains,
+                                   const udh_gain_map* maps, const uint8_t* const* masks, const int32_t* rois, int n, int c,
+                                   const int32_t* tile_ptr, const int32_t* tile_frames, int dst_h, int dst_w, int feather, uint8_t* dst,
+                                   uint8_t* mask, void* ws, size_t ws_bytes, void* stream) {
+  const char* what = "udh_mosaic_blend_u8";
+  UDH_REQUIRE(tile_ptr && tile_frames && dst && mask && (n == 0 || (frames && sizes && M && ws)), "%s: null pointer", what);
+  UDH_REQUIRE(c == 1 || c == 3, "%s: channels must be 1 or 3 (got %d)", what, c);
   UDH_REQUIRE(n >= 0 && n <= 65535 && dst_h >= 1 && dst_w >= 1 && dst_h < 32767 && dst_w < 32767,
-              "udh_mosaic_blend_u8: bad dimensions (n %d, canvas %dx%d)", n, dst_h, dst_w);
-  UDH_REQUIRE(feather >= 0 && feather <= 1024, "udh_mosaic_blend_u8: feather must be in [0, 1024] (got %d)", feather);
-  const size_t need = gmaps ? udh_mosaic_blend_gainmap_workspace_bytes(n)
-                     : masks ? udh_mosaic_blend_masked_workspace_bytes(n) : udh_mosaic_workspace_bytes(n);
+              "%s: bad dimensions (n %d, canvas %dx%d)", what, n, dst_h, dst_w);
+  UDH_REQUIRE(feather >= 0 && feather <= 1024, "%s: feather must be in [0, 1024] (got %d)", what, feather);
+  UDH_REQUIRE(!(gains && maps), "%s: gains and maps exclude each other", what);
+  UDH_REQUIRE(n == 0 || rois || !(masks || maps), "%s: masks and maps need rois", what);
+  const size_t need = udh_mosaic_workspace_bytes(n);
   if (ws_bytes < need) {
-    set_error("udh_mosaic_blend_u8: workspace of %zu bytes, %zu needed", ws_bytes, need);
+    set_error("%s: workspace of %zu bytes, %zu needed", what, ws_bytes, need);
     return UDH_EWS;
   }
+  std::vector<MosaicFrame> fr((size_t)n);
+  for (int k = 0; k < n; ++k) {
+    const int h = sizes[2 * k], w = sizes[2 * k + 1];
+    UDH_REQUIRE(frames[k], "%s: frame %d is a null pointer", what, k);
+    UDH_REQUIRE(h >= 1 && w >= 1 && h < 32767 && w < 32767, "%s: frame %d is %dx%d", what, k, h, w);
+    fr[(size_t)k].src = frames[k];
+    fr[(size_t)k].h = h;
+    fr[(size_t)k].w = w;
+  }
+  std::vector<SeamMask> sm(masks ? (size_t)n : 0, SeamMask{nullptr, 0, 0, 0, 0});
+  for (int k = 0; k < (int)sm.size(); ++k) {
+    const int* r = rois + 4 * k;
+    if (r[2] <= r[0] || r[3] <= r[1]) continue;
+    UDH_REQUIRE(r[0] >= 0 && r[1] >= 0 && r[2] <= dst_w && r[3] <= dst_h,
+                "%s: frame %d's mask rectangle (%d, %d)..(%d, %d) leaves the %dx%d canvas", what, k, r[0], r[1], r[2], r[3], dst_h, dst_w);
+    UDH_REQUIRE(masks[k], "%s: frame %d's mask is a null pointer", what, k);
+    sm[(size_t)k] = SeamMask{masks[k], r[0], r[1], r[2] - r[0], r[3] - r[1]};
+  }
+  std::vector<GainMapDev> gm;
+  int rc = maps ? gm_table(maps, rois, n, dst_h, dst_w, gm, what) : UDH_OK;
+  if (rc != UDH_OK) return rc;
   const cudaStream_t st = as_stream(stream);
-  const size_t off_gm = mb_align((size_t)n * sizeof(MosaicFrame)) + mb_align((size_t)n * sizeof(SeamMask));
-  if (gmaps && n > 0) {
-    std::vector<GainMapDev> gm((size_t)n);
-    int rc = gm_table(gmaps, mrois, n, dst_h, dst_w, gm, "udh_mosaic_blend_gainmap_u8");
-    if (rc != UDH_OK) return rc;
-    const cudaError_t e = cudaMemcpyAsync(static_cast<char*>(ws) + off_gm, gm.data(), (size_t)n * sizeof(GainMapDev),
-                                          cudaMemcpyHostToDevice, st);
-    if (e != cudaSuccess) {
-      set_error("udh_mosaic_blend_gainmap_u8: map table copy: %s", cudaGetErrorString(e));
-      return UDH_ECUDA;
-    }
-  }
-  if (masks && n > 0) {
-    std::vector<SeamMask> sm((size_t)n, SeamMask{nullptr, 0, 0, 0, 0});
-    for (int k = 0; k < n; ++k) {
-      const int* r = mrois + 4 * k;
-      if (r[2] <= r[0] || r[3] <= r[1]) continue;
-      UDH_REQUIRE(r[0] >= 0 && r[1] >= 0 && r[2] <= dst_w && r[3] <= dst_h,
-                  "udh_mosaic_blend_masked_u8: frame %d's mask rectangle (%d, %d)..(%d, %d) leaves the %dx%d canvas", k, r[0], r[1],
-                  r[2], r[3], dst_h, dst_w);
-      UDH_REQUIRE(masks[k], "udh_mosaic_blend_masked_u8: frame %d's mask is a null pointer", k);
-      sm[k] = SeamMask{masks[k], r[0], r[1], r[2] - r[0], r[3] - r[1]};
-    }
-    const cudaError_t e = cudaMemcpyAsync(static_cast<char*>(ws) + mb_align((size_t)n * sizeof(MosaicFrame)), sm.data(),
-                                          (size_t)n * sizeof(SeamMask), cudaMemcpyHostToDevice, st);
-    if (e != cudaSuccess) {
-      set_error("udh_mosaic_blend_masked_u8: mask table copy: %s", cudaGetErrorString(e));
-      return UDH_ECUDA;
-    }
-  }
+  char* base = static_cast<char*>(ws);
+  SeamMask* sm_d = reinterpret_cast<SeamMask*>(base + mb_align((size_t)n * sizeof(MosaicFrame)));
+  GainMapDev* gm_d = reinterpret_cast<GainMapDev*>(reinterpret_cast<char*>(sm_d) + mb_align((size_t)n * sizeof(SeamMask)));
   if (n > 0) {
-    std::vector<MosaicFrame> host((size_t)n);
-    for (int k = 0; k < n; ++k) {
-      const int h = sizes[2 * k], w = sizes[2 * k + 1];
-      UDH_REQUIRE(frames[k], "udh_mosaic_blend_u8: frame %d is a null pointer", k);
-      UDH_REQUIRE(h >= 1 && w >= 1 && h < 32767 && w < 32767, "udh_mosaic_blend_u8: frame %d is %dx%d", k, h, w);
-      host[k].src = frames[k];
-      host[k].h = h;
-      host[k].w = w;
-    }
-    // pageable source: the copy is staged before this call returns, so `host` may go
-      const cudaError_t e = cudaMemcpyAsync(ws, host.data(), (size_t)n * sizeof(MosaicFrame), cudaMemcpyHostToDevice, st);
-    if (e != cudaSuccess) {
-      set_error("udh_mosaic_blend_u8: frame table copy: %s", cudaGetErrorString(e));
-      return UDH_ECUDA;
-    }
-    mosaic_invert_kernel<<<(n + 127) / 128, 128, 0, st>>>(M, static_cast<MosaicFrame*>(ws), n);
-    const int rc = check_launch("udh_mosaic_blend_u8 (inverses)");
-    if (rc != UDH_OK) return rc;
+    if ((rc = upload(base, fr, st, what)) != UDH_OK || (masks && (rc = upload(sm_d, sm, st, what)) != UDH_OK) ||
+        (maps && (rc = upload(gm_d, gm, st, what)) != UDH_OK))
+      return rc;
+    invert_kernel<<<(n + 127) / 128, 128, 0, st>>>(M, reinterpret_cast<MosaicFrame*>(base), n);
+    if ((rc = check_launch("udh_mosaic_blend_u8 (inverses)")) != UDH_OK) return rc;
   }
-  const int bh = dst_h < 16 ? dst_h : 16;
-  const int bw = 1024 / bh < dst_w ? 1024 / bh : dst_w;
   const dim3 grid((unsigned)((dst_w + UDH_MOSAIC_TILE_W - 1) / UDH_MOSAIC_TILE_W),
                   (unsigned)((dst_h + UDH_MOSAIC_TILE_H - 1) / UDH_MOSAIC_TILE_H));
-  const MosaicFrame* fr = static_cast<const MosaicFrame*>(ws);
-  if (gmaps) {
-    const SeamMask* sm = masks ? reinterpret_cast<const SeamMask*>(static_cast<const char*>(ws) + mb_align((size_t)n * sizeof(MosaicFrame)))
-                               : nullptr;
-    const GainMapDev* gm = reinterpret_cast<const GainMapDev*>(static_cast<const char*>(ws) + off_gm);
-    const int f32 = 32 * feather;
-    if (masks && c == 3)
-      gainmap_blend_u8_kernel<3, true><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, f32, sm, gm, dst, mask);
-    else if (masks)
-      gainmap_blend_u8_kernel<1, true><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, f32, sm, gm, dst, mask);
-    else if (c == 3)
-      gainmap_blend_u8_kernel<3, false><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, f32, sm, gm, dst, mask);
-    else
-      gainmap_blend_u8_kernel<1, false><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, f32, sm, gm, dst, mask);
-    return check_launch("udh_mosaic_blend_gainmap_u8");
-  }
-  if (masks) {
-    const SeamMask* sm = reinterpret_cast<const SeamMask*>(static_cast<const char*>(ws) + mb_align((size_t)n * sizeof(MosaicFrame)));
-    const int f32 = 32 * feather;
-    if (gains && c == 3)
-      seam_blend_u8_kernel<3, true><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, f32, gains, sm, dst, mask);
-    else if (gains)
-      seam_blend_u8_kernel<1, true><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, f32, gains, sm, dst, mask);
-    else if (c == 3)
-      seam_blend_u8_kernel<3, false><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, f32, nullptr, sm, dst, mask);
-    else
-      seam_blend_u8_kernel<1, false><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, f32, nullptr, sm, dst, mask);
-    return check_launch("udh_mosaic_blend_masked_u8");
-  }
-  if (gains && c == 3)
-    exposure_blend_u8_kernel<3><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, 32 * feather, gains, dst, mask);
-  else if (gains)
-    exposure_blend_u8_kernel<1><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, 32 * feather, gains, dst, mask);
-  else if (c == 3)
-    mosaic_blend_u8_kernel<3><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, 32 * feather, dst, mask);
-  else
-    mosaic_blend_u8_kernel<1><<<grid, 256, 0, st>>>(fr, n, tile_ptr, tile_frames, dst_h, dst_w, bw, 32 * feather, dst, mask);
-  return check_launch("udh_mosaic_blend_u8");
+  const BlendKernel kernel = c == 3 ? blend_kernel<3>(gains, masks, maps) : blend_kernel<1>(gains, masks, maps);
+  kernel<<<grid, 256, 0, st>>>(reinterpret_cast<const MosaicFrame*>(base), n, tile_ptr, tile_frames, dst_h, dst_w, warp_tile_w(dst_h, dst_w),
+                               32 * feather, dst, mask, gains, masks ? sm_d : nullptr, maps ? gm_d : nullptr);
+  return check_launch(what);
 }
 
-extern "C" int udh_mosaic_blend_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, int n, int c,
-                                   const int32_t* tile_ptr, const int32_t* tile_frames, int dst_h, int dst_w, int feather,
-                                   uint8_t* dst, uint8_t* mask, void* ws, size_t ws_bytes, void* stream) {
-  return mosaic_blend(frames, sizes, M, nullptr, n, c, tile_ptr, tile_frames, dst_h, dst_w, feather, dst, mask, ws, ws_bytes, stream);
-}
-
-extern "C" int udh_mosaic_blend_gain_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains, int n,
-                                        int c, const int32_t* tile_ptr, const int32_t* tile_frames, int dst_h, int dst_w, int feather,
-                                        uint8_t* dst, uint8_t* mask, void* ws, size_t ws_bytes, void* stream) {
-  UDH_REQUIRE(gains || n == 0, "udh_mosaic_blend_gain_u8: null gains");
-  return mosaic_blend(frames, sizes, M, gains, n, c, tile_ptr, tile_frames, dst_h, dst_w, feather, dst, mask, ws, ws_bytes, stream);
-}
-
+// The multi-band blend's workspace: the plan's layout, then the map table (after the pyramid, whose offsets do not move).
 extern "C" size_t udh_mosaic_multiband_workspace_bytes(const int32_t* rois, int n, int dst_h, int dst_w, int bands) {
   MultibandPlan p;
-  return mb_plan(rois, nullptr, n, dst_h, dst_w, bands, p) == UDH_OK ? p.total : 0;
+  return mb_plan(nullptr, rois, nullptr, n, dst_h, dst_w, bands, p) == UDH_OK ? p.total + (size_t)n * sizeof(GainMapDev) : 0;
 }
 
 extern "C" int udh_debug_multiband_layout(const int32_t* rois, int n, int dst_h, int dst_w, int bands, size_t off[MB_MAX_BANDS + 1],
                                           int dims[3]) {
   UDH_REQUIRE(off && dims, "udh_debug_multiband_layout: null pointer");
   MultibandPlan p;
-  const int rc = mb_plan(rois, nullptr, n, dst_h, dst_w, bands, p);
+  const int rc = mb_plan(nullptr, rois, nullptr, n, dst_h, dst_w, bands, p);
   if (rc != UDH_OK) return rc;
   for (int i = 0; i <= MB_MAX_BANDS; ++i) off[i] = i <= p.B ? p.off_acc[i] : 0;
   dims[0] = p.B;
@@ -1478,46 +1364,31 @@ extern "C" int udh_debug_multiband_layout(const int32_t* rois, int n, int dst_h,
   return UDH_OK;
 }
 
-static int mosaic_multiband(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains,
-                            const int32_t* rois, int n, int c, int dst_h, int dst_w, int bands, uint8_t* dst, uint8_t* mask, void* ws,
-                            size_t ws_bytes, void* stream, const uint8_t* const* masks = nullptr,
-                            const udh_gain_map* gmaps = nullptr) {
-  UDH_REQUIRE(frames && sizes && M && rois && dst && mask && ws, "udh_mosaic_multiband_u8: null pointer");
-  UDH_REQUIRE(c == 3, "udh_mosaic_multiband_u8: channels must be 3 (got %d)", c);
+extern "C" int udh_mosaic_multiband_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains,
+                                       const udh_gain_map* maps, const uint8_t* const* masks, const int32_t* rois, int n, int c, int dst_h,
+                                       int dst_w, int bands, uint8_t* dst, uint8_t* mask, void* ws, size_t ws_bytes, void* stream) {
+  const char* what = "udh_mosaic_multiband_u8";
+  UDH_REQUIRE(frames && sizes && M && rois && dst && mask && ws, "%s: null pointer", what);
+  UDH_REQUIRE(c == 3, "%s: channels must be 3 (got %d)", what, c);
+  UDH_REQUIRE(!(gains && maps), "%s: gains and maps exclude each other", what);
   MultibandPlan p;
-  int rc = mb_plan(rois, sizes, n, dst_h, dst_w, bands, p);
+  int rc = mb_plan(frames, rois, sizes, n, dst_h, dst_w, bands, p);
   if (rc != UDH_OK) return rc;
-  const size_t need = p.total + (gmaps ? (size_t)n * sizeof(GainMapDev) : 0);
+  const size_t need = p.total + (size_t)n * sizeof(GainMapDev);
   if (ws_bytes < need) {
-    set_error("udh_mosaic_multiband_u8: workspace of %zu bytes, %zu needed", ws_bytes, need);
+    set_error("%s: workspace of %zu bytes, %zu needed", what, ws_bytes, need);
     return UDH_EWS;
   }
-  for (int k = 0; k < n; ++k) {
-    UDH_REQUIRE(frames[k], "udh_mosaic_multiband_u8: frame %d is a null pointer", k);
-    p.fr[k].src = frames[k];
-    if (masks) {
-      UDH_REQUIRE(masks[k], "udh_mosaic_multiband_masked_u8: frame %d's mask is a null pointer", k);
-      p.fr[k].bmask = masks[k];
-    }
+  for (int k = 0; masks && k < n; ++k) {
+    UDH_REQUIRE(masks[k], "%s: frame %d's mask is a null pointer", what, k);
+    p.fr[(size_t)k].bmask = masks[k];
   }
+  std::vector<GainMapDev> gm;
+  if (maps && (rc = gm_table(maps, rois, n, dst_h, dst_w, gm, what)) != UDH_OK) return rc;
   const cudaStream_t st = as_stream(stream);
   char* base = static_cast<char*>(ws);
-  // pageable source: the copy is staged before this call returns, so `p` may go
-  const cudaError_t e = cudaMemcpyAsync(base, p.fr.data(), (size_t)n * sizeof(MultibandFrame), cudaMemcpyHostToDevice, st);
-  if (e != cudaSuccess) {
-    set_error("udh_mosaic_multiband_u8: frame table copy: %s", cudaGetErrorString(e));
-    return UDH_ECUDA;
-  }
-  GainMapDev* gm = reinterpret_cast<GainMapDev*>(base + p.total);
-  if (gmaps) {
-    std::vector<GainMapDev> host((size_t)n);
-    if ((rc = gm_table(gmaps, rois, n, dst_h, dst_w, host, "udh_mosaic_multiband_gainmap_u8")) != UDH_OK) return rc;
-    const cudaError_t e2 = cudaMemcpyAsync(gm, host.data(), (size_t)n * sizeof(GainMapDev), cudaMemcpyHostToDevice, st);
-    if (e2 != cudaSuccess) {
-      set_error("udh_mosaic_multiband_gainmap_u8: map table copy: %s", cudaGetErrorString(e2));
-      return UDH_ECUDA;
-    }
-  }
+  GainMapDev* gm_d = reinterpret_cast<GainMapDev*>(base + p.total);
+  if ((rc = upload(base, p.fr, st, what)) != UDH_OK || (maps && (rc = upload(gm_d, gm, st, what)) != UDH_OK)) return rc;
   const MultibandFrame* fr = reinterpret_cast<const MultibandFrame*>(base);
   uchar4* G = reinterpret_cast<uchar4*>(base + p.off_g);
   int16_t* Wt = reinterpret_cast<int16_t*>(base + p.off_w);
@@ -1525,10 +1396,8 @@ static int mosaic_multiband(const uint8_t* const* frames, const int32_t* sizes, 
   auto R = [&](int i) { return reinterpret_cast<short4*>(base + p.off_r[i]); };
   {
     ProfScope ps(PROF_MB_BASE, st);
-    if (gmaps)
-      gainmap_mb_base_kernel<<<dim3(mb_blocks(p.max_px[0]), (unsigned)n), 256, 0, st>>>(fr, M, gm, G, Wt);
-    else
-      multiband_base_kernel<<<dim3(mb_blocks(p.max_px[0]), (unsigned)n), 256, 0, st>>>(fr, M, gains, G, Wt);
+    (maps ? multiband_base_kernel<true> : multiband_base_kernel<false>)<<<dim3(mb_blocks(p.max_px[0]), (unsigned)n), 256, 0, st>>>(
+        fr, M, gains, gm_d, G, Wt);
     if ((rc = check_launch("udh_mosaic_multiband_u8 (base)")) != UDH_OK) return rc;
   }
   {
@@ -1559,85 +1428,36 @@ static int mosaic_multiband(const uint8_t* const* frames, const int32_t* sizes, 
   return check_launch("udh_mosaic_multiband_u8");
 }
 
-extern "C" int udh_mosaic_multiband_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const int32_t* rois, int n,
-                                       int c, int dst_h, int dst_w, int bands, uint8_t* dst, uint8_t* mask, void* ws, size_t ws_bytes,
-                                       void* stream) {
-  return mosaic_multiband(frames, sizes, M, nullptr, rois, n, c, dst_h, dst_w, bands, dst, mask, ws, ws_bytes, stream);
-}
-
-extern "C" int udh_mosaic_multiband_gain_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains,
-                                            const int32_t* rois, int n, int c, int dst_h, int dst_w, int bands, uint8_t* dst,
-                                            uint8_t* mask, void* ws, size_t ws_bytes, void* stream) {
-  UDH_REQUIRE(gains, "udh_mosaic_multiband_gain_u8: null gains");
-  return mosaic_multiband(frames, sizes, M, gains, rois, n, c, dst_h, dst_w, bands, dst, mask, ws, ws_bytes, stream);
-}
-
 extern "C" size_t udh_mosaic_exposure_workspace_bytes(int n) { return n > 0 ? (size_t)n * sizeof(ExposureFrame) : 0; }
 
 extern "C" int udh_mosaic_exposure_stats_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const int32_t* rois,
                                             int n, const int32_t* pair_ptr, const int32_t* pair_j, int npairs, const double* history,
                                             int feeds, int norms, int dst_h, int dst_w, uint64_t* stats, void* ws, size_t ws_bytes,
                                             void* stream) {
-  UDH_REQUIRE(frames && sizes && M && rois && pair_ptr && pair_j && stats && ws && (feeds == 0 || history),
-              "udh_mosaic_exposure_stats_u8: null pointer");
+  const char* what = "udh_mosaic_exposure_stats_u8";
+  UDH_REQUIRE(frames && sizes && M && rois && pair_ptr && pair_j && stats && ws && (feeds == 0 || history), "%s: null pointer", what);
   UDH_REQUIRE(n >= 1 && n <= UDH_EXPOSURE_MAX_FRAMES && dst_h >= 1 && dst_w >= 1 && dst_h < 32767 && dst_w < 32767,
-              "udh_mosaic_exposure_stats_u8: bad dimensions (n %d of at most %d, canvas %dx%d)", n, UDH_EXPOSURE_MAX_FRAMES, dst_h,
-              dst_w);
+              "%s: bad dimensions (n %d of at most %d, canvas %dx%d)", what, n, UDH_EXPOSURE_MAX_FRAMES, dst_h, dst_w);
   UDH_REQUIRE(npairs >= n && npairs <= n * (n + 1) / 2 && feeds >= 0 && feeds <= UDH_EXPOSURE_MAX_FEEDS,
-              "udh_mosaic_exposure_stats_u8: %d pairs of %d frames, %d feeds (at most %d)", npairs, n, feeds, UDH_EXPOSURE_MAX_FEEDS);
+              "%s: %d pairs of %d frames, %d feeds (at most %d)", what, npairs, n, feeds, UDH_EXPOSURE_MAX_FEEDS);
   if (ws_bytes < udh_mosaic_exposure_workspace_bytes(n)) {
-    set_error("udh_mosaic_exposure_stats_u8: workspace of %zu bytes, %zu needed", ws_bytes, udh_mosaic_exposure_workspace_bytes(n));
+    set_error("%s: workspace of %zu bytes, %zu needed", what, ws_bytes, udh_mosaic_exposure_workspace_bytes(n));
     return UDH_EWS;
   }
   std::vector<ExposureFrame> host((size_t)n);
-  for (int k = 0; k < n; ++k) {
-    const int* r = rois + 4 * k;
-    UDH_REQUIRE(r[0] >= 0 && r[1] >= 0 && r[0] < r[2] && r[1] < r[3] && r[2] <= dst_w && r[3] <= dst_h,
-                "udh_mosaic_exposure_stats_u8: frame %d's ROI (%d, %d)..(%d, %d) is empty or leaves the %dx%d canvas", k, r[0], r[1],
-                r[2], r[3], dst_h, dst_w);
-    UDH_REQUIRE(frames[k], "udh_mosaic_exposure_stats_u8: frame %d is a null pointer", k);
-    ExposureFrame& F = host[k];
-    F.src = frames[k];
-    F.h = sizes[2 * k];
-    F.w = sizes[2 * k + 1];
-    UDH_REQUIRE(F.h >= 1 && F.w >= 1 && F.h < 32767 && F.w < 32767, "udh_mosaic_exposure_stats_u8: frame %d is %dx%d", k, F.h, F.w);
-    F.rx = r[0]; F.ry = r[1]; F.rw = r[2] - r[0]; F.rh = r[3] - r[1];
-    const int bh = F.rh < 16 ? F.rh : 16;
-    F.bw = 1024 / bh < F.rw ? 1024 / bh : F.rw;                      // the ROI warp's tile width, as mb_plan sets it
-  }
+  int rc;
+  for (int k = 0; k < n; ++k)
+    if ((rc = roi_frame(frames, sizes, rois, k, dst_h, dst_w, host[(size_t)k], what)) != UDH_OK) return rc;
   const cudaStream_t st = as_stream(stream);
-  // pageable source: the copy is staged before this call returns, so `host` may go
-  cudaError_t e = cudaMemcpyAsync(ws, host.data(), (size_t)n * sizeof(ExposureFrame), cudaMemcpyHostToDevice, st);
-  if (e == cudaSuccess) e = cudaMemsetAsync(stats, 0, (size_t)npairs * UDH_EXPOSURE_STATS * sizeof(uint64_t), st);
-  if (e != cudaSuccess) {
-    set_error("udh_mosaic_exposure_stats_u8: %s", cudaGetErrorString(e));
-    return UDH_ECUDA;
-  }
+  if ((rc = upload(ws, host, st, what)) != UDH_OK) return rc;
+  UDH_CUDA(cudaMemsetAsync(stats, 0, (size_t)npairs * UDH_EXPOSURE_STATS * sizeof(uint64_t), st));
   ExposureFrame* fr = static_cast<ExposureFrame*>(ws);
-  exposure_invert_kernel<<<(n + 127) / 128, 128, 0, st>>>(M, fr, n);
-  int rc = check_launch("udh_mosaic_exposure_stats_u8 (inverses)");
-  if (rc != UDH_OK) return rc;
+  invert_kernel<<<(n + 127) / 128, 128, 0, st>>>(M, fr, n);
+  if ((rc = check_launch("udh_mosaic_exposure_stats_u8 (inverses)")) != UDH_OK) return rc;
   const dim3 grid((unsigned)((dst_w + EX_TILE_W - 1) / EX_TILE_W), (unsigned)((dst_h + EX_TILE_H - 1) / EX_TILE_H));
   exposure_stats_kernel<<<grid, 256, 0, st>>>(fr, n, pair_ptr, pair_j, history, feeds, norms,
                                               reinterpret_cast<unsigned long long*>(stats));
-  return check_launch("udh_mosaic_exposure_stats_u8");
-}
-
-extern "C" int udh_mosaic_blend_masked_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains,
-                                          const uint8_t* const* masks, const int32_t* rois, int n, int c, const int32_t* tile_ptr,
-                                          const int32_t* tile_frames, int dst_h, int dst_w, int feather, uint8_t* dst, uint8_t* mask,
-                                          void* ws, size_t ws_bytes, void* stream) {
-  UDH_REQUIRE(n == 0 || (masks && rois), "udh_mosaic_blend_masked_u8: null masks or rois");
-  static const uint8_t* const none[1] = {nullptr};
-  return mosaic_blend(frames, sizes, M, gains, n, c, tile_ptr, tile_frames, dst_h, dst_w, feather, dst, mask, ws, ws_bytes, stream,
-                      n ? masks : none, rois);
-}
-
-extern "C" int udh_mosaic_multiband_masked_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const double* gains,
-                                              const uint8_t* const* masks, const int32_t* rois, int n, int c, int dst_h, int dst_w,
-                                              int bands, uint8_t* dst, uint8_t* mask, void* ws, size_t ws_bytes, void* stream) {
-  UDH_REQUIRE(masks, "udh_mosaic_multiband_masked_u8: null masks");
-  return mosaic_multiband(frames, sizes, M, gains, rois, n, c, dst_h, dst_w, bands, dst, mask, ws, ws_bytes, stream, masks);
+  return check_launch(what);
 }
 
 // The host's plan of one seam call: the frame table, the pairs in visiting order with their windows, and the workspace.
@@ -1648,30 +1468,21 @@ struct SeamPlan {
   size_t off_g, off_p, total;
 };
 
-static int seam_plan(const int32_t* rois, const int32_t* sizes, int n, const int32_t* pair_ptr, const int32_t* pair_j, int dst_h,
-                     int dst_w, SeamPlan& p) {
-  UDH_REQUIRE(rois && pair_ptr && (pair_j || !pair_ptr[n]), "udh_mosaic_seam_masks_u8: null pointer");
+static int seam_plan(const uint8_t* const* frames, const int32_t* rois, const int32_t* sizes, int n, const int32_t* pair_ptr,
+                     const int32_t* pair_j, int dst_h, int dst_w, SeamPlan& p) {
+  const char* what = "udh_mosaic_seam_masks_u8";
+  UDH_REQUIRE(rois && pair_ptr && (pair_j || !pair_ptr[n]), "%s: null pointer", what);
   UDH_REQUIRE(n >= 1 && n <= UDH_SEAM_MAX_FRAMES && dst_h >= 1 && dst_w >= 1 && dst_h < 32767 && dst_w < 32767,
-              "udh_mosaic_seam_masks_u8: bad dimensions (n %d of at most %d, canvas %dx%d)", n, UDH_SEAM_MAX_FRAMES, dst_h, dst_w);
+              "%s: bad dimensions (n %d of at most %d, canvas %dx%d)", what, n, UDH_SEAM_MAX_FRAMES, dst_h, dst_w);
   p.fr.assign((size_t)n, SeamFrame{});
   int64_t off = 0;
   for (int k = 0; k < n; ++k) {
-    const int* r = rois + 4 * k;
-    UDH_REQUIRE(r[0] >= 0 && r[1] >= 0 && r[0] < r[2] && r[1] < r[3] && r[2] <= dst_w && r[3] <= dst_h,
-                "udh_mosaic_seam_masks_u8: frame %d's ROI (%d, %d)..(%d, %d) is empty or leaves the %dx%d canvas", k, r[0], r[1], r[2],
-                r[3], dst_h, dst_w);
     SeamFrame& F = p.fr[k];
-    F.rx = r[0]; F.ry = r[1]; F.rw = r[2] - r[0]; F.rh = r[3] - r[1];
-    const int bh = F.rh < 16 ? F.rh : 16;
-    F.bw = 1024 / bh < F.rw ? 1024 / bh : F.rw;                      // the ROI warp's tile width, as mb_plan sets it
+    const int rc = roi_frame(frames, sizes, rois, k, dst_h, dst_w, F, what);
+    if (rc != UDH_OK) return rc;
     F.off = off;
     off += (int64_t)F.rw * F.rh;
     if ((int64_t)F.rw * F.rh > p.max_px) p.max_px = (int64_t)F.rw * F.rh;
-    if (sizes) {
-      F.h = sizes[2 * k];
-      F.w = sizes[2 * k + 1];
-      UDH_REQUIRE(F.h >= 1 && F.w >= 1 && F.h < 32767 && F.w < 32767, "udh_mosaic_seam_masks_u8: frame %d is %dx%d", k, F.h, F.w);
-    }
   }
   UDH_REQUIRE(pair_ptr[0] == 0, "udh_mosaic_seam_masks_u8: pair_ptr[0] is %d", pair_ptr[0]);
   for (int i = 0; i < n; ++i) {
@@ -1699,32 +1510,24 @@ static int seam_plan(const int32_t* rois, const int32_t* sizes, int n, const int
 extern "C" size_t udh_mosaic_seam_workspace_bytes(const int32_t* rois, int n, const int32_t* pair_ptr, const int32_t* pair_j,
                                                   int dst_h, int dst_w) {
   SeamPlan p;
-  return seam_plan(rois, nullptr, n, pair_ptr, pair_j, dst_h, dst_w, p) == UDH_OK ? p.total : 0;
+  return seam_plan(nullptr, rois, nullptr, n, pair_ptr, pair_j, dst_h, dst_w, p) == UDH_OK ? p.total : 0;
 }
 
 extern "C" int udh_mosaic_seam_masks_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const int32_t* rois, int n,
                                         const int32_t* pair_ptr, const int32_t* pair_j, int dst_h, int dst_w, uint8_t* seam,
                                         uint8_t* blend, void* ws, size_t ws_bytes, void* stream) {
-  UDH_REQUIRE(frames && sizes && M && seam && blend && ws, "udh_mosaic_seam_masks_u8: null pointer");
+  const char* what = "udh_mosaic_seam_masks_u8";
+  UDH_REQUIRE(frames && sizes && M && seam && blend && ws, "%s: null pointer", what);
   SeamPlan p;
-  int rc = seam_plan(rois, sizes, n, pair_ptr, pair_j, dst_h, dst_w, p);
+  int rc = seam_plan(frames, rois, sizes, n, pair_ptr, pair_j, dst_h, dst_w, p);
   if (rc != UDH_OK) return rc;
   if (ws_bytes < p.total) {
-    set_error("udh_mosaic_seam_masks_u8: workspace of %zu bytes, %zu needed", ws_bytes, p.total);
+    set_error("%s: workspace of %zu bytes, %zu needed", what, ws_bytes, p.total);
     return UDH_EWS;
-  }
-  for (int k = 0; k < n; ++k) {
-    UDH_REQUIRE(frames[k], "udh_mosaic_seam_masks_u8: frame %d is a null pointer", k);
-    p.fr[k].src = frames[k];
   }
   const cudaStream_t st = as_stream(stream);
   char* base = static_cast<char*>(ws);
-  // pageable source: the copy is staged before this call returns, so `p` may go
-  const cudaError_t e = cudaMemcpyAsync(base, p.fr.data(), (size_t)n * sizeof(SeamFrame), cudaMemcpyHostToDevice, st);
-  if (e != cudaSuccess) {
-    set_error("udh_mosaic_seam_masks_u8: frame table copy: %s", cudaGetErrorString(e));
-    return UDH_ECUDA;
-  }
+  if ((rc = upload(base, p.fr, st, what)) != UDH_OK) return rc;
   const SeamFrame* fr = reinterpret_cast<const SeamFrame*>(base);
   int* ga = reinterpret_cast<int*>(base + p.off_g);
   int* gb = ga + p.max_win;
@@ -1745,28 +1548,6 @@ extern "C" int udh_mosaic_seam_masks_u8(const uint8_t* const* frames, const int3
   }
   seam_blend_mask_kernel<<<dim3(mb_blocks(p.max_px), (unsigned)n), 256, 0, st>>>(fr, seam, blend);
   return check_launch("udh_mosaic_seam_masks_u8 (blend masks)");
-}
-
-extern "C" int udh_mosaic_blend_gainmap_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const udh_gain_map* maps,
-                                           const uint8_t* const* masks, const int32_t* rois, int n, int c, const int32_t* tile_ptr,
-                                           const int32_t* tile_frames, int dst_h, int dst_w, int feather, uint8_t* dst, uint8_t* mask,
-                                           void* ws, size_t ws_bytes, void* stream) {
-  UDH_REQUIRE(n >= 1 && maps && rois, "udh_mosaic_blend_gainmap_u8: no frames, or null maps or rois");
-  return mosaic_blend(frames, sizes, M, nullptr, n, c, tile_ptr, tile_frames, dst_h, dst_w, feather, dst, mask, ws, ws_bytes, stream,
-                      masks, rois, maps);
-}
-
-extern "C" size_t udh_mosaic_multiband_gainmap_workspace_bytes(const int32_t* rois, int n, int dst_h, int dst_w, int bands) {
-  MultibandPlan p;
-  return mb_plan(rois, nullptr, n, dst_h, dst_w, bands, p) == UDH_OK ? p.total + (size_t)n * sizeof(GainMapDev) : 0;
-}
-
-extern "C" int udh_mosaic_multiband_gainmap_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M,
-                                               const udh_gain_map* maps, const uint8_t* const* masks, const int32_t* rois, int n, int c,
-                                               int dst_h, int dst_w, int bands, uint8_t* dst, uint8_t* mask, void* ws, size_t ws_bytes,
-                                               void* stream) {
-  UDH_REQUIRE(maps, "udh_mosaic_multiband_gainmap_u8: null maps");
-  return mosaic_multiband(frames, sizes, M, nullptr, rois, n, c, dst_h, dst_w, bands, dst, mask, ws, ws_bytes, stream, masks, maps);
 }
 
 extern "C" size_t udh_mosaic_exposure_block_workspace_bytes(int n) { return n > 0 ? (size_t)n * sizeof(ExposureBlockFrame) : 0; }
@@ -1791,20 +1572,10 @@ extern "C" int udh_mosaic_exposure_block_stats_u8(const uint8_t* const* frames, 
     return UDH_EWS;
   }
   std::vector<ExposureBlockFrame> host((size_t)n);
+  int rc;
   for (int k = 0; k < n; ++k) {
-    const int* r = rois + 4 * k;
-    UDH_REQUIRE(r[0] >= 0 && r[1] >= 0 && r[0] < r[2] && r[1] < r[3] && r[2] <= dst_w && r[3] <= dst_h,
-                "%s: frame %d's ROI (%d, %d)..(%d, %d) is empty or leaves the %dx%d canvas", what, k, r[0], r[1], r[2], r[3], dst_h,
-                dst_w);
-    UDH_REQUIRE(frames[k], "%s: frame %d is a null pointer", what, k);
-    ExposureBlockFrame& F = host[k];
-    F.src = frames[k];
-    F.h = sizes[2 * k];
-    F.w = sizes[2 * k + 1];
-    UDH_REQUIRE(F.h >= 1 && F.w >= 1 && F.h < 32767 && F.w < 32767, "%s: frame %d is %dx%d", what, k, F.h, F.w);
-    F.rx = r[0]; F.ry = r[1]; F.rw = r[2] - r[0]; F.rh = r[3] - r[1];
-    const int bh = F.rh < 16 ? F.rh : 16;
-    F.bw = 1024 / bh < F.rw ? 1024 / bh : F.rw;                      // the ROI warp's tile width, as mb_plan sets it
+    ExposureBlockFrame& F = host[(size_t)k];
+    if ((rc = roi_frame(frames, sizes, rois, k, dst_h, dst_w, F, what)) != UDH_OK) return rc;
     F.bkw = blocks[4 * k];
     F.bkh = blocks[4 * k + 1];
     F.bpx = blocks[4 * k + 2];
@@ -1815,16 +1586,11 @@ extern "C" int udh_mosaic_exposure_block_stats_u8(const uint8_t* const* frames, 
                 F.bkh, F.bpx, (long long)F.boff, F.rw, F.rh, (long long)nblocks);
   }
   const cudaStream_t st = as_stream(stream);
-  cudaError_t e = cudaMemcpyAsync(ws, host.data(), (size_t)n * sizeof(ExposureBlockFrame), cudaMemcpyHostToDevice, st);
-  if (e == cudaSuccess) e = cudaMemsetAsync(stats, 0, (size_t)nslots * UDH_EXPOSURE_STATS * sizeof(uint64_t), st);
-  if (e != cudaSuccess) {
-    set_error("%s: %s", what, cudaGetErrorString(e));
-    return UDH_ECUDA;
-  }
+  if ((rc = upload(ws, host, st, what)) != UDH_OK) return rc;
+  UDH_CUDA(cudaMemsetAsync(stats, 0, (size_t)nslots * UDH_EXPOSURE_STATS * sizeof(uint64_t), st));
   ExposureBlockFrame* fr = static_cast<ExposureBlockFrame*>(ws);
-  gainblock_invert_kernel<<<(n + 127) / 128, 128, 0, st>>>(M, fr, n);
-  int rc = check_launch("udh_mosaic_exposure_block_stats_u8 (inverses)");
-  if (rc != UDH_OK) return rc;
+  invert_kernel<<<(n + 127) / 128, 128, 0, st>>>(M, fr, n);
+  if ((rc = check_launch("udh_mosaic_exposure_block_stats_u8 (inverses)")) != UDH_OK) return rc;
   const dim3 grid((unsigned)((dst_w + EX_TILE_W - 1) / EX_TILE_W), (unsigned)((dst_h + EX_TILE_H - 1) / EX_TILE_H));
   gainblock_stats_kernel<<<grid, 256, 0, st>>>(fr, n, pair_ptr, pair_j, cell_off, cell_nx, history, nblocks, feeds, norms,
                                                     reinterpret_cast<unsigned long long*>(stats));
@@ -1875,11 +1641,8 @@ extern "C" int udh_exposure_gain_maps(const double* gains, int n, const int32_t*
   }
   const cudaStream_t st = as_stream(stream);
   int4* fb_d = reinterpret_cast<int4*>(static_cast<char*>(ws) + mb_align((size_t)nblocks * channels * sizeof(float)));
-  const cudaError_t e = cudaMemcpyAsync(fb_d, fb.data(), (size_t)n * sizeof(int4), cudaMemcpyHostToDevice, st);
-  if (e != cudaSuccess) {
-    set_error("udh_exposure_gain_maps: %s", cudaGetErrorString(e));
-    return UDH_ECUDA;
-  }
+  const int rc = upload(fb_d, fb, st, "udh_exposure_gain_maps");
+  if (rc != UDH_OK) return rc;
   gainblock_maps_kernel<<<(unsigned)n, 256, 0, st>>>(gains, fb_d, channels, maps, static_cast<float*>(ws));
   return check_launch("udh_exposure_gain_maps");
 }

@@ -668,31 +668,72 @@ def _mask_table(masks, rois, n, what):
     return ptrs, rr
 
 
+def _frames_and_M(frames, M, what, channels):
+    """frames (n CUDA uint8 tensors [h_k,w_k,C], or one [n,h,w,C] tensor) and M [n,3,3] (numpy or tensor) -> (frames as a
+    list, M float64 [n,3,3] numpy, sizes [(h_k, w_k)]), checked: at least one frame, one matrix each, C in channels and the
+    same for every frame."""
+    frames = list(frames.unbind(0)) if isinstance(frames, torch.Tensor) else list(frames)
+    Mh = (M.detach().cpu().numpy() if isinstance(M, torch.Tensor) else np.asarray(M)).astype(np.float64).reshape(-1, 3, 3)
+    n = len(frames)
+    if Mh.shape[0] != n:
+        raise _lib.UdhError("%s: %d matrices for %d frames" % (what, Mh.shape[0], n))
+    if n == 0:
+        raise _lib.UdhError("%s: no frames" % what)
+    for k, f in enumerate(frames):
+        _req(f, torch.uint8, "frames[%d]" % k)
+        if f.dim() != 3 or f.shape[2] not in channels or f.shape[2] != frames[0].shape[2]:
+            raise _lib.UdhError("%s: frames must all be %s (frame %d is %s)"
+                                % (what, " or all ".join("[h,w,%d]" % c for c in channels), k, tuple(f.shape)))
+    return frames, Mh, [(int(f.shape[0]), int(f.shape[1])) for f in frames]
+
+
+class _Fed(object):
+    """frames and M (frame k -> canvas) as the multi-band blend takes them -> the frames it feeds, those whose ROI
+    (mosaic.multiband_rois) meets the canvas, as the ROI entry points take them: n, dev, rois int64 [n,4], take (the fed
+    frames' indices), m = len(take) and, when m > 0, frames [m], ptrs (host array of device pointers), sz int32 [m,2], rr
+    int32 [m,4] (their ROIs) and M_d float64 [m,9] on the device (frame -> ROI)."""
+
+    def __init__(self, frames, M, dst_h, dst_w, what, max_frames=None):
+        from . import mosaic
+        frames, Mh, sizes = _frames_and_M(frames, M, what, (3,))
+        rois, Mr = mosaic.multiband_rois(Mh, sizes, int(dst_h), int(dst_w))
+        self.n, self.dev, self.rois = len(frames), frames[0].device, rois
+        self.take = [k for k in range(self.n) if rois[k, 2] > rois[k, 0] and rois[k, 3] > rois[k, 1]]
+        m = self.m = len(self.take)
+        if max_frames is not None and m > max_frames:
+            raise _lib.UdhError("%s: %d frames meet the canvas (at most %d)" % (what, m, max_frames))
+        if not m:
+            return
+        self.frames = [frames[k] for k in self.take]
+        self.ptrs = (ctypes.c_void_p * m)(*[f.data_ptr() for f in self.frames])
+        self.sz = np.ascontiguousarray(np.array([sizes[k] for k in self.take], np.int32).reshape(m, 2))
+        self.rr = np.ascontiguousarray(rois[self.take].astype(np.int32))
+        self.M_d = torch.from_numpy(np.ascontiguousarray(Mr[self.take].reshape(m, 9))).to(self.dev)
+
+    def fed(self, items, what, name):
+        """A per-frame list [n] -> its entries for the fed frames."""
+        items = list(items)
+        if len(items) != self.n:
+            raise _lib.UdhError("%s: %d %s for %d frames" % (what, len(items), name, self.n))
+        return [items[k] for k in self.take]
+
+
 def mosaic_blend_u8(frames, M, dst_h, dst_w, feather, gains=None, masks=None, gain_maps=None):
     """frames: n CUDA uint8 tensors [h_k,w_k,C] (C = 1 or 3, sizes may differ; or one [n,h,w,C] tensor), M float64 [n,3,3]
     (frame k -> canvas; numpy or tensor) -> (mosaic uint8 [dst_h,dst_w,C], mask uint8 [dst_h,dst_w]): udh_mosaic_blend_u8's
     feathered blend of cv2.warpPerspective(frame k, M_k, (dst_w, dst_h)), bit for bit with oracle/mosaic.py.  The tile
     lists are built on the host (mosaic_tile_lists); the frames are read where they are.  gains ([n] or [n,3], e.g.
-    mosaic_exposure_gains'): each frame's warp value is exposure-compensated first, saturate_u8(rint(v g)) in float64
-    (udh_mosaic_blend_gain_u8).  masks ([n], e.g. mosaic_seam_masks' blend masks): frame k counts only where its mask,
-    a CUDA uint8 [roi_h,roi_w] on its ROI (mosaic.multiband_rois), is set; a frame whose ROI misses the canvas takes None
-    and counts nowhere (udh_mosaic_blend_masked_u8).  gain_maps ([n], e.g. mosaic_exposure_gain_maps'; not with gains):
-    each frame's warp value is compensated by its block gain map resized to its ROI, at the pixel's ROI coordinates,
-    saturate_u8(rint(float32(v) g)) (udh_mosaic_blend_gainmap_u8)."""
+    mosaic_exposure_gains'): each frame's warp value is exposure-compensated first, saturate_u8(rint(v g)) in float64.
+    masks ([n], e.g. mosaic_seam_masks' blend masks): frame k counts only where its mask, a CUDA uint8 [roi_h,roi_w] on its
+    ROI (mosaic.multiband_rois), is set; a frame whose ROI misses the canvas takes None and counts nowhere.  gain_maps ([n],
+    e.g. mosaic_exposure_gain_maps'; not with gains): each frame's warp value is compensated by its block gain map resized
+    to its ROI, at the pixel's ROI coordinates, saturate_u8(rint(float32(v) g))."""
     from . import mosaic
-    frames = list(frames.unbind(0)) if isinstance(frames, torch.Tensor) else list(frames)
-    Mh = (M.detach().cpu().numpy() if isinstance(M, torch.Tensor) else np.asarray(M)).astype(np.float64).reshape(-1, 3, 3)
-    n = len(frames)
-    if Mh.shape[0] != n:
-        raise _lib.UdhError("mosaic_blend_u8: %d matrices for %d frames" % (Mh.shape[0], n))
-    if n == 0:
-        raise _lib.UdhError("mosaic_blend_u8: no frames")
-    for k, f in enumerate(frames):
-        _req(f, torch.uint8, "frames[%d]" % k)
-        if f.dim() != 3 or f.shape[2] not in (1, 3) or f.shape[2] != frames[0].shape[2]:
-            raise _lib.UdhError("mosaic_blend_u8: frames must all be [h,w,1] or all [h,w,3] (frame %d is %s)" % (k, tuple(f.shape)))
-    C, dev = frames[0].shape[2], frames[0].device
-    sizes = [(int(f.shape[0]), int(f.shape[1])) for f in frames]
+    what = "mosaic_blend_u8"
+    frames, Mh, sizes = _frames_and_M(frames, M, what, (1, 3))
+    if gains is not None and gain_maps is not None:
+        raise _lib.UdhError("%s: gains and gain_maps exclude each other" % what)
+    n, C, dev = len(frames), frames[0].shape[2], frames[0].device
     ptr, idx = mosaic_tile_lists(Mh, sizes, int(dst_h), int(dst_w))
     ptr_d = torch.from_numpy(ptr).to(dev)
     idx_d = torch.from_numpy(idx if len(idx) else np.zeros(1, np.int32)).to(dev)
@@ -703,35 +744,17 @@ def mosaic_blend_u8(frames, M, dst_h, dst_w, feather, gains=None, masks=None, ga
     ws = torch.empty(max(nb, 1), device=dev, dtype=torch.uint8)
     ptrs = (ctypes.c_void_p * n)(*[f.data_ptr() for f in frames])
     sz = np.ascontiguousarray(np.array(sizes, np.int32).reshape(n, 2))
-    if gain_maps is not None:
-        if gains is not None:
-            raise _lib.UdhError("mosaic_blend_u8: gains and gain_maps exclude each other")
+    g_d = None if gains is None else _gains(gains, n, dev, what)
+    gm = mp = rr = None
+    if masks is not None or gain_maps is not None:
         rr = np.ascontiguousarray(mosaic.multiband_rois(Mh, sizes, int(dst_h), int(dst_w))[0].astype(np.int32))
-        gm, _keep = _gain_map_table(gain_maps, rr, n, dev, "mosaic_blend_u8")
-        mp = None
-        if masks is not None:
-            mp, rr = _mask_table(masks, rr, n, "mosaic_blend_u8")
-        nb = lib.udh_mosaic_blend_gainmap_workspace_bytes(n)
-        ws = torch.empty(max(nb, 1), device=dev, dtype=torch.uint8)
-        check(lib.udh_mosaic_blend_gainmap_u8(ptrs, sz.ctypes.data, _ptr(M_d), gm, mp, rr.ctypes.data, n, C, _ptr(ptr_d), _ptr(idx_d),
-                                              int(dst_h), int(dst_w), int(feather), _ptr(out), _ptr(mask), _ptr(ws), nb, _stream()),
-              "udh_mosaic_blend_gainmap_u8")
-    elif masks is not None:
-        mp, rr = _mask_table(masks, mosaic.multiband_rois(Mh, sizes, int(dst_h), int(dst_w))[0], n, "mosaic_blend_u8")
-        g_d = None if gains is None else _gains(gains, n, dev, "mosaic_blend_u8")
-        nb = lib.udh_mosaic_blend_masked_workspace_bytes(n)
-        ws = torch.empty(max(nb, 1), device=dev, dtype=torch.uint8)
-        check(lib.udh_mosaic_blend_masked_u8(ptrs, sz.ctypes.data, _ptr(M_d), None if g_d is None else _ptr(g_d), mp, rr.ctypes.data, n,
-                                             C, _ptr(ptr_d), _ptr(idx_d), int(dst_h), int(dst_w), int(feather), _ptr(out), _ptr(mask),
-                                             _ptr(ws), nb, _stream()), "udh_mosaic_blend_masked_u8")
-    elif gains is None:
-        check(lib.udh_mosaic_blend_u8(ptrs, sz.ctypes.data, _ptr(M_d), n, C, _ptr(ptr_d), _ptr(idx_d), int(dst_h), int(dst_w),
-                                      int(feather), _ptr(out), _ptr(mask), _ptr(ws), nb, _stream()), "udh_mosaic_blend_u8")
-    else:
-        g_d = _gains(gains, n, dev, "mosaic_blend_u8")
-        check(lib.udh_mosaic_blend_gain_u8(ptrs, sz.ctypes.data, _ptr(M_d), _ptr(g_d), n, C, _ptr(ptr_d), _ptr(idx_d), int(dst_h),
-                                           int(dst_w), int(feather), _ptr(out), _ptr(mask), _ptr(ws), nb, _stream()),
-              "udh_mosaic_blend_gain_u8")
+    if gain_maps is not None:
+        gm, _keep = _gain_map_table(gain_maps, rr, n, dev, what)
+    if masks is not None:
+        mp, rr = _mask_table(masks, rr, n, what)
+    check(lib.udh_mosaic_blend_u8(ptrs, sz.ctypes.data, _ptr(M_d), _ptr(g_d), gm, mp, None if rr is None else rr.ctypes.data, n, C,
+                                  _ptr(ptr_d), _ptr(idx_d), int(dst_h), int(dst_w), int(feather), _ptr(out), _ptr(mask), _ptr(ws), nb,
+                                  _stream()), "udh_mosaic_blend_u8")
     return out, mask
 
 
@@ -743,80 +766,37 @@ def mosaic_multiband_u8(frames, M, dst_h, dst_w, bands, levels=False, gains=None
     map to finite points with a positive denominator); a frame whose ROI misses the canvas is left out.  levels=True also
     returns the canvas pyramid as the feeds left it: [B' + 1] int16 CUDA tensors [Hp >> i, Wp >> i, 4] (acc, then wacc).
     gains ([n] or [n,3], e.g. mosaic_exposure_gains'): each ROI warp is exposure-compensated before it is fed,
-    saturate_u8(rint(v g)) in float64 (udh_mosaic_multiband_gain_u8), cv2's stitcher order.  masks ([n], e.g.
-    mosaic_seam_masks' blend masks; None for a frame whose ROI misses the canvas): frame k is fed its mask, a CUDA uint8
-    [roi_h,roi_w], in place of its validity mask (udh_mosaic_multiband_masked_u8).  gain_maps ([n], e.g.
-    mosaic_exposure_gain_maps'; not with gains): each ROI warp is compensated by its block gain map resized to the ROI,
-    saturate_u8(rint(float32(v) g)), before it is fed (udh_mosaic_multiband_gainmap_u8)."""
-    from . import mosaic
-    frames = list(frames.unbind(0)) if isinstance(frames, torch.Tensor) else list(frames)
-    Mh = (M.detach().cpu().numpy() if isinstance(M, torch.Tensor) else np.asarray(M)).astype(np.float64).reshape(-1, 3, 3)
-    n = len(frames)
-    if Mh.shape[0] != n:
-        raise _lib.UdhError("mosaic_multiband_u8: %d matrices for %d frames" % (Mh.shape[0], n))
-    if n == 0:
-        raise _lib.UdhError("mosaic_multiband_u8: no frames")
-    for k, f in enumerate(frames):
-        _req(f, torch.uint8, "frames[%d]" % k)
-        if f.dim() != 3 or f.shape[2] != 3:
-            raise _lib.UdhError("mosaic_multiband_u8: frames must be [h,w,3] (frame %d is %s)" % (k, tuple(f.shape)))
-    sizes = [(int(f.shape[0]), int(f.shape[1])) for f in frames]
-    rois, Mr = mosaic.multiband_rois(Mh, sizes, int(dst_h), int(dst_w))
-    take = [k for k in range(n) if rois[k, 2] > rois[k, 0] and rois[k, 3] > rois[k, 1]]
-    dev = frames[0].device
+    saturate_u8(rint(v g)) in float64, cv2's stitcher order.  masks ([n], e.g. mosaic_seam_masks' blend masks; None for a
+    frame whose ROI misses the canvas): frame k is fed its mask, a CUDA uint8 [roi_h,roi_w], in place of its validity
+    mask.  gain_maps ([n], e.g. mosaic_exposure_gain_maps'; not with gains): each ROI warp is compensated by its block gain
+    map resized to the ROI, saturate_u8(rint(float32(v) g)), before it is fed."""
+    what = "mosaic_multiband_u8"
+    fed = _Fed(frames, M, dst_h, dst_w, what)
+    if gains is not None and gain_maps is not None:
+        raise _lib.UdhError("%s: gains and gain_maps exclude each other" % what)
+    m, dev = fed.m, fed.dev
     out = torch.zeros(int(dst_h), int(dst_w), 3, device=dev, dtype=torch.uint8)
     mask = torch.zeros(int(dst_h), int(dst_w), device=dev, dtype=torch.uint8)
-    g_d = None if gains is None else _gains(gains, n, dev, "mosaic_multiband_u8")
-    if not take:
+    g_d = None if gains is None else _gains(gains, fed.n, dev, what)
+    if not m:
         return (out, mask, []) if levels else (out, mask)
-    m = len(take)
-    rr = np.ascontiguousarray(rois[take].astype(np.int32))
-    M_d = torch.from_numpy(np.ascontiguousarray(Mr[take].reshape(m, 9))).to(dev)
-    sz = np.ascontiguousarray(np.array([sizes[k] for k in take], np.int32).reshape(m, 2))
-    ptrs = (ctypes.c_void_p * m)(*[frames[k].data_ptr() for k in take])
-    nb = lib.udh_mosaic_multiband_workspace_bytes(rr.ctypes.data, m, int(dst_h), int(dst_w), int(bands))
+    nb = lib.udh_mosaic_multiband_workspace_bytes(fed.rr.ctypes.data, m, int(dst_h), int(dst_w), int(bands))
     if nb == 0:
-        raise _lib.UdhError("mosaic_multiband_u8: bad arguments (%d frames, canvas %dx%d, %d bands)" % (m, dst_h, dst_w, bands))
+        raise _lib.UdhError("%s: bad arguments (%d frames, canvas %dx%d, %d bands)" % (what, m, dst_h, dst_w, bands))
     ws = torch.empty(nb, device=dev, dtype=torch.uint8)
+    g_d = None if g_d is None else g_d[fed.take].contiguous()
+    gm = mp = None
     if gain_maps is not None:
-        if gains is not None:
-            raise _lib.UdhError("mosaic_multiband_u8: gains and gain_maps exclude each other")
-        gain_maps = list(gain_maps)
-        if len(gain_maps) != n:
-            raise _lib.UdhError("mosaic_multiband_u8: %d gain maps for %d frames" % (len(gain_maps), n))
-        gm, _keep = _gain_map_table([gain_maps[k] for k in take], rr, m, dev, "mosaic_multiband_u8")
-        mp = None
-        if masks is not None:
-            masks = list(masks)
-            if len(masks) != n:
-                raise _lib.UdhError("mosaic_multiband_u8: %d masks for %d frames" % (len(masks), n))
-            mp, _ = _mask_table([masks[k] for k in take], rr, m, "mosaic_multiband_u8")
-        nb = lib.udh_mosaic_multiband_gainmap_workspace_bytes(rr.ctypes.data, m, int(dst_h), int(dst_w), int(bands))
-        ws = torch.empty(nb, device=dev, dtype=torch.uint8)
-        check(lib.udh_mosaic_multiband_gainmap_u8(ptrs, sz.ctypes.data, _ptr(M_d), gm, mp, rr.ctypes.data, m, 3, int(dst_h),
-                                                  int(dst_w), int(bands), _ptr(out), _ptr(mask), _ptr(ws), nb, _stream()),
-              "udh_mosaic_multiband_gainmap_u8")
-    elif masks is not None:
-        masks = list(masks)
-        if len(masks) != n:
-            raise _lib.UdhError("mosaic_multiband_u8: %d masks for %d frames" % (len(masks), n))
-        mp, _ = _mask_table([masks[k] for k in take], rr, m, "mosaic_multiband_u8")
-        g_d = None if g_d is None else g_d[take].contiguous()
-        check(lib.udh_mosaic_multiband_masked_u8(ptrs, sz.ctypes.data, _ptr(M_d), None if g_d is None else _ptr(g_d), mp, rr.ctypes.data,
-                                                 m, 3, int(dst_h), int(dst_w), int(bands), _ptr(out), _ptr(mask), _ptr(ws), nb,
-                                                 _stream()), "udh_mosaic_multiband_masked_u8")
-    elif g_d is None:
-        check(lib.udh_mosaic_multiband_u8(ptrs, sz.ctypes.data, _ptr(M_d), rr.ctypes.data, m, 3, int(dst_h), int(dst_w), int(bands),
-                                          _ptr(out), _ptr(mask), _ptr(ws), nb, _stream()), "udh_mosaic_multiband_u8")
-    else:
-        g_d = g_d[take].contiguous()
-        check(lib.udh_mosaic_multiband_gain_u8(ptrs, sz.ctypes.data, _ptr(M_d), _ptr(g_d), rr.ctypes.data, m, 3, int(dst_h),
-                                               int(dst_w), int(bands), _ptr(out), _ptr(mask), _ptr(ws), nb, _stream()),
-              "udh_mosaic_multiband_gain_u8")
+        gm, _keep = _gain_map_table(fed.fed(gain_maps, what, "gain maps"), fed.rr, m, dev, what)
+    if masks is not None:
+        mp, _ = _mask_table(fed.fed(masks, what, "masks"), fed.rr, m, what)
+    check(lib.udh_mosaic_multiband_u8(fed.ptrs, fed.sz.ctypes.data, _ptr(fed.M_d), _ptr(g_d), gm, mp, fed.rr.ctypes.data, m, 3,
+                                      int(dst_h), int(dst_w), int(bands), _ptr(out), _ptr(mask), _ptr(ws), nb, _stream()),
+          "udh_mosaic_multiband_u8")
     if not levels:
         return out, mask
     off, dims = (ctypes.c_size_t * 11)(), (ctypes.c_int * 3)()
-    check(lib.udh_debug_multiband_layout(rr.ctypes.data, m, int(dst_h), int(dst_w), int(bands), off, dims),
+    check(lib.udh_debug_multiband_layout(fed.rr.ctypes.data, m, int(dst_h), int(dst_w), int(bands), off, dims),
           "udh_debug_multiband_layout")
     B, Hp, Wp = dims
     pyr = []
@@ -830,13 +810,14 @@ def mosaic_multiband_u8(frames, M, dst_h, dst_w, bands, levels=False, gains=None
 EXPOSURE_ALPHA, EXPOSURE_BETA = 0.01, 100.0       # cv2.detail.GainCompensator's weights of the gain and intensity terms
 
 
-def exposure_pairs(rois):
-    """rois [m,4] (x_lo, y_lo, x_hi, y_hi) -> CSR (pair_ptr int32 [m+1], pair_j int32 [P]) of the pairs i <= j whose rectangles
-    intersect (cv2.detail.overlapRoi), the diagonal included, row-major."""
+def roi_pairs(rois, diagonal):
+    """rois [m,4] (x_lo, y_lo, x_hi, y_hi) -> CSR (pair_ptr int32 [m+1], pair_j int32 [P]) of the pairs whose rectangles
+    intersect (cv2.detail.overlapRoi), row-major: i <= j with the diagonal (the exposure statistics' pairs), i < j without
+    (cv2.detail.PairwiseSeamFinder's visiting order)."""
     r = np.asarray(rois, np.int64).reshape(-1, 4)
     x0, y0 = np.maximum(r[:, None, 0], r[None, :, 0]), np.maximum(r[:, None, 1], r[None, :, 1])
     x1, y1 = np.minimum(r[:, None, 2], r[None, :, 2]), np.minimum(r[:, None, 3], r[None, :, 3])
-    hit = np.triu((x0 < x1) & (y0 < y1))
+    hit = np.triu((x0 < x1) & (y0 < y1), 0 if diagonal else 1)
     ptr = np.zeros(len(r) + 1, np.int64)
     ptr[1:] = np.cumsum(hit.sum(1))
     return ptr.astype(np.int32), np.nonzero(hit)[1].astype(np.int32)
@@ -844,55 +825,29 @@ def exposure_pairs(rois):
 
 def exposure_norm_sum(l0, l1, l2):
     """The three 21-bit limb sums of udh_mosaic_exposure_stats_u8's sum q (q = norm 2^52, an integer) -> sum norm: the exact
-    total, rounded to double once (ties to even)."""
+    total, rounded to double once (ties to even).  Scalars give a float; arrays, elementwise, a float64 array."""
+    if np.ndim(l0):
+        return np.array([exposure_norm_sum(*v) for v in zip(l0, l1, l2)], np.float64)
     return math.ldexp(float(int(l0) + (int(l1) << 21) + (int(l2) << 42)), -52)
 
 
-def _exposure_rois(frames, M, dst_h, dst_w, what):
-    from . import mosaic
-    frames = list(frames.unbind(0)) if isinstance(frames, torch.Tensor) else list(frames)
-    Mh = (M.detach().cpu().numpy() if isinstance(M, torch.Tensor) else np.asarray(M)).astype(np.float64).reshape(-1, 3, 3)
-    n = len(frames)
-    if Mh.shape[0] != n:
-        raise _lib.UdhError("%s: %d matrices for %d frames" % (what, Mh.shape[0], n))
-    if n == 0:
-        raise _lib.UdhError("%s: no frames" % what)
-    for k, f in enumerate(frames):
-        _req(f, torch.uint8, "frames[%d]" % k)
-        if f.dim() != 3 or f.shape[2] != 3:
-            raise _lib.UdhError("%s: frames must be [h,w,3] (frame %d is %s)" % (what, k, tuple(f.shape)))
-    sizes = [(int(f.shape[0]), int(f.shape[1])) for f in frames]
-    rois, Mr = mosaic.multiband_rois(Mh, sizes, int(dst_h), int(dst_w))
-    take = [k for k in range(n) if rois[k, 2] > rois[k, 0] and rois[k, 3] > rois[k, 1]]
-    if len(take) > _lib.EXPOSURE_MAX_FRAMES:
-        raise _lib.UdhError("%s: %d frames meet the canvas (at most %d)" % (what, len(take), _lib.EXPOSURE_MAX_FRAMES))
-    return frames, sizes, rois, Mr, take
-
-
-class _ExposureStats(object):
+class _ExposureStats(_Fed):
     """udh_mosaic_exposure_stats_u8 on fixed frames: the device-side frame table, pairs and output, reused by every feed."""
 
     def __init__(self, frames, M, dst_h, dst_w):
-        frames, sizes, rois, Mr, take = _exposure_rois(frames, M, dst_h, dst_w, "mosaic_exposure_stats")
-        self.n, self.take, self.dst = len(frames), take, (int(dst_h), int(dst_w))
-        m = self.m = len(take)
+        _Fed.__init__(self, frames, M, dst_h, dst_w, "mosaic_exposure_stats", _lib.EXPOSURE_MAX_FRAMES)
+        self.dst = (int(dst_h), int(dst_w))
+        m = self.m
         if not m:
             self.i = self.j = np.zeros(0, np.int64)
             return
-        dev = frames[0].device
-        self.frames = [frames[k] for k in take]
-        self.ptrs = (ctypes.c_void_p * m)(*[f.data_ptr() for f in self.frames])
-        self.sz = np.ascontiguousarray(np.array([sizes[k] for k in take], np.int32).reshape(m, 2))
-        self.rr = np.ascontiguousarray(rois[take].astype(np.int32))
-        self.M_d = torch.from_numpy(np.ascontiguousarray(Mr[take].reshape(m, 9))).to(dev)
-        ptr, pj = exposure_pairs(self.rr)
+        ptr, pj = roi_pairs(self.rr, True)
         self.i = np.repeat(np.arange(m), np.diff(ptr)).astype(np.int64)
         self.j = pj.astype(np.int64)
-        self.ptr_d, self.pj_d = torch.from_numpy(ptr).to(dev), torch.from_numpy(pj).to(dev)
-        self.out = torch.empty(len(pj), _lib.EXPOSURE_STATS, device=dev, dtype=torch.int64)
+        self.ptr_d, self.pj_d = torch.from_numpy(ptr).to(self.dev), torch.from_numpy(pj).to(self.dev)
+        self.out = torch.empty(len(pj), _lib.EXPOSURE_STATS, device=self.dev, dtype=torch.int64)
         self.nb = lib.udh_mosaic_exposure_workspace_bytes(m)
-        self.ws = torch.empty(max(self.nb, 1), device=dev, dtype=torch.uint8)
-        self.dev = dev
+        self.ws = torch.empty(max(self.nb, 1), device=self.dev, dtype=torch.uint8)
 
     def __call__(self, history=None, norms=True):
         """history: None or float64 [t,m,3] (the fed frames' gains of feeds 0..t-1) -> uint64 [P,13] numpy."""
@@ -917,7 +872,7 @@ def mosaic_exposure_stats(frames, M, dst_h, dst_w, history=None, norms=True):
     exact and rounded once; 0 without norms), raw uint64 [P,13])."""
     st = _ExposureStats(frames, M, dst_h, dst_w)
     raw = st(history, norms)
-    ns = np.array([[exposure_norm_sum(*r[7:10]), exposure_norm_sum(*r[10:13])] for r in raw]).reshape(-1, 2)
+    ns = np.stack([exposure_norm_sum(*raw[:, 7:10].T), exposure_norm_sum(*raw[:, 10:13].T)], 1)
     return dict(take=st.take, i=st.i, j=st.j, count=raw[:, 0].astype(np.int64), sums=raw[:, 1:7].astype(np.int64).reshape(-1, 2, 3),
                 norms=ns, raw=raw)
 
@@ -984,8 +939,7 @@ def mosaic_exposure_gains(frames, M, dst_h, dst_w, mode="gain", feeds=1):
         raw = st(np.stack(hist) if hist else None, norms=mode == "gain")
         count = raw[:, 0].astype(np.int64)
         if mode == "gain":
-            g = exposure_solve(st.m, st.i, st.j, count, [exposure_norm_sum(*r[7:10]) for r in raw],
-                               [exposure_norm_sum(*r[10:13]) for r in raw])
+            g = exposure_solve(st.m, st.i, st.j, count, exposure_norm_sum(*raw[:, 7:10].T), exposure_norm_sum(*raw[:, 10:13].T))
             g3 = np.repeat(g[:, None], 3, 1)
         else:
             g3 = np.stack([exposure_solve(st.m, st.i, st.j, count, raw[:, 1 + c].astype(np.int64),
@@ -1031,10 +985,10 @@ def _block_axis(ra, ea, bwa, rb, eb, bwb, lo, hi):
 
 def exposure_block_cells(rois, blocks, boff):
     """The block pairs of cv2's block compensator and where udh_mosaic_exposure_block_stats_u8 sums them.  -> dict(pair_ptr,
-    pair_j (the frame pairs i <= j whose ROIs intersect, exposure_pairs), cell_off int64 [P], cell_nx int32 [P], nslots,
+    pair_j (the frame pairs i <= j whose ROIs intersect, roi_pairs), cell_off int64 [P], cell_nx int32 [P], nslots,
     a, b int64 [Q] (every pair of blocks a <= b whose rectangles intersect, a block with itself included), slot int64 [Q])."""
     r = np.asarray(rois, np.int64).reshape(-1, 4)
-    ptr, pj = exposure_pairs(r)
+    ptr, pj = roi_pairs(r, True)
     P = len(pj)
     cell_off, cell_nx = np.zeros(P, np.int64), np.zeros(P, np.int32)
     A, B, S = [], [], []
@@ -1120,30 +1074,17 @@ def exposure_block_solve(row_ptr, col, val, rhs, dev, tol=EXPOSURE_BLOCK_TOL, ma
     return x.cpu().numpy(), int(inf[0]), float(inf[1:2].view(np.float64)[0])
 
 
-def _norm_sums(l0, l1, l2):
-    """exposure_norm_sum over arrays of limb sums (exact in Python integers, rounded once)."""
-    tot = np.asarray(l0, np.uint64).astype(object) + (np.asarray(l1, np.uint64).astype(object) << 21) + \
-        (np.asarray(l2, np.uint64).astype(object) << 42)
-    return np.array([math.ldexp(float(v), -52) for v in tot], np.float64)
-
-
-class _ExposureBlockStats(object):
+class _ExposureBlockStats(_Fed):
     """udh_mosaic_exposure_block_stats_u8 on fixed frames and blocks: tables, cells and output, reused by every feed."""
 
     def __init__(self, frames, M, dst_h, dst_w, block):
         if int(block) < 1:
             raise ValueError("block must be >= 1 (got %r)" % (block,))
-        frames, sizes, rois, Mr, take = _exposure_rois(frames, M, dst_h, dst_w, "mosaic_exposure_gain_maps")
-        self.n, self.take, self.dst = len(frames), take, (int(dst_h), int(dst_w))
-        m = self.m = len(take)
+        _Fed.__init__(self, frames, M, dst_h, dst_w, "mosaic_exposure_gain_maps", _lib.EXPOSURE_MAX_FRAMES)
+        self.dst = (int(dst_h), int(dst_w))
+        m, dev = self.m, self.dev
         if not m:
             return
-        dev = self.dev = frames[0].device
-        self.frames = [frames[k] for k in take]
-        self.ptrs = (ctypes.c_void_p * m)(*[f.data_ptr() for f in self.frames])
-        self.sz = np.ascontiguousarray(np.array([sizes[k] for k in take], np.int32).reshape(m, 2))
-        self.rr = np.ascontiguousarray(rois[take].astype(np.int32))
-        self.M_d = torch.from_numpy(np.ascontiguousarray(Mr[take].reshape(m, 9))).to(dev)
         self.blocks, boff = exposure_block_grid(self.rr, block)
         self.blocks = np.ascontiguousarray(self.blocks)
         self.boff, self.nblocks = np.ascontiguousarray(boff[:-1]), int(boff[-1])
@@ -1179,7 +1120,7 @@ def mosaic_exposure_block_stats(frames, M, dst_h, dst_w, block=32, history=None,
     raw = st(h, norms)
     return dict(take=st.take, blocks=st.blocks, boff=st.boff, a=st.cells["a"], b=st.cells["b"], count=raw[:, 0].astype(np.int64),
                 sums=raw[:, 1:7].astype(np.int64).reshape(-1, 2, 3),
-                norms=np.stack([_norm_sums(*raw[:, 7:10].T), _norm_sums(*raw[:, 10:13].T)], 1), raw=raw)
+                norms=np.stack([exposure_norm_sum(*raw[:, 7:10].T), exposure_norm_sum(*raw[:, 10:13].T)], 1), raw=raw)
 
 
 def mosaic_exposure_block_gains(frames, M, dst_h, dst_w, mode="gain", feeds=1, block=32):
@@ -1203,7 +1144,7 @@ def mosaic_exposure_block_gains(frames, M, dst_h, dst_w, mode="gain", feeds=1, b
         if mode == "gain":
             pos = (count > 0) & (c["a"] != c["b"])              # a block's own mean never enters the system
             sa, sb = np.zeros(len(count)), np.zeros(len(count))
-            sa[pos], sb[pos] = _norm_sums(*raw[pos, 7:10].T), _norm_sums(*raw[pos, 10:13].T)
+            sa[pos], sb[pos] = exposure_norm_sum(*raw[pos, 7:10].T), exposure_norm_sum(*raw[pos, 10:13].T)
             sums = [(sa, sb)]
         else:
             sums = [(raw[:, 1 + ch].astype(np.int64), raw[:, 4 + ch].astype(np.int64)) for ch in range(3)]
@@ -1295,18 +1236,6 @@ def _gain_map_table(gain_maps, rois, n, dev, what):
 
 
 # ------------------------------------------------------------------ seam finding
-def seam_pairs(rois):
-    """rois [m,4] (x_lo, y_lo, x_hi, y_hi) -> CSR (pair_ptr int32 [m+1], pair_j int32 [P]) of the pairs i < j whose rectangles
-    intersect, row-major: cv2.detail.PairwiseSeamFinder's visiting order."""
-    r = np.asarray(rois, np.int64).reshape(-1, 4)
-    x0, y0 = np.maximum(r[:, None, 0], r[None, :, 0]), np.maximum(r[:, None, 1], r[None, :, 1])
-    x1, y1 = np.minimum(r[:, None, 2], r[None, :, 2]), np.minimum(r[:, None, 3], r[None, :, 3])
-    hit = np.triu((x0 < x1) & (y0 < y1), 1)
-    ptr = np.zeros(len(r) + 1, np.int64)
-    ptr[1:] = np.cumsum(hit.sum(1))
-    return ptr.astype(np.int32), np.nonzero(hit)[1].astype(np.int32)
-
-
 def mosaic_seam_masks(frames, M, dst_h, dst_w):
     """frames: n CUDA uint8 RGB tensors [h_k,w_k,3], M float64 [n,3,3] (frame k -> canvas) -> dict(take (the fed frames:
     those whose ROI meets the canvas), rois int64 [n,4] (mosaic.multiband_rois), seam [m], blend [m]): per fed frame its
@@ -1314,16 +1243,12 @@ def mosaic_seam_masks(frames, M, dst_h, dst_w):
     leaves in the multi-band blend's validity masks, and cv2.dilate of that AND the validity, the mask cv2's stitcher feeds
     its blender (udh_mosaic_seam_masks_u8; oracle/seam.py states the rule).  A frame lying inside another one's seam region
     vanishes (an all-zero mask), as in cv2."""
-    frames, sizes, rois, Mr, take = _exposure_rois(frames, M, dst_h, dst_w, "mosaic_seam_masks")
-    out = dict(take=take, rois=rois, seam=[], blend=[])
-    if not take:
+    fed = _Fed(frames, M, dst_h, dst_w, "mosaic_seam_masks", _lib.EXPOSURE_MAX_FRAMES)
+    out = dict(take=fed.take, rois=fed.rois, seam=[], blend=[])
+    if not fed.m:
         return out
-    m, dev = len(take), frames[0].device
-    rr = np.ascontiguousarray(rois[take].astype(np.int32))
-    M_d = torch.from_numpy(np.ascontiguousarray(Mr[take].reshape(m, 9))).to(dev)
-    sz = np.ascontiguousarray(np.array([sizes[k] for k in take], np.int32).reshape(m, 2))
-    ptrs = (ctypes.c_void_p * m)(*[frames[k].data_ptr() for k in take])
-    ptr, pj = seam_pairs(rr)
+    m, dev, rr = fed.m, fed.dev, fed.rr
+    ptr, pj = roi_pairs(rr, False)
     pj = pj if len(pj) else np.zeros(1, np.int32)
     hw = np.stack([rr[:, 3] - rr[:, 1], rr[:, 2] - rr[:, 0]], 1).astype(np.int64)
     off = np.concatenate([[0], np.cumsum(hw[:, 0] * hw[:, 1])])
@@ -1333,8 +1258,8 @@ def mosaic_seam_masks(frames, M, dst_h, dst_w):
     if nb == 0:
         raise _lib.UdhError("mosaic_seam_masks: bad arguments (%d frames, canvas %dx%d)" % (m, dst_h, dst_w))
     ws = torch.empty(nb, device=dev, dtype=torch.uint8)
-    check(lib.udh_mosaic_seam_masks_u8(ptrs, sz.ctypes.data, _ptr(M_d), rr.ctypes.data, m, ptr.ctypes.data, pj.ctypes.data, int(dst_h),
-                                       int(dst_w), _ptr(seam), _ptr(blend), _ptr(ws), nb, _stream()), "udh_mosaic_seam_masks_u8")
+    check(lib.udh_mosaic_seam_masks_u8(fed.ptrs, fed.sz.ctypes.data, _ptr(fed.M_d), rr.ctypes.data, m, ptr.ctypes.data, pj.ctypes.data,
+                                       int(dst_h), int(dst_w), _ptr(seam), _ptr(blend), _ptr(ws), nb, _stream()), "udh_mosaic_seam_masks_u8")
     for k in range(m):
         h, w = (int(v) for v in hw[k])
         out["seam"].append(seam[off[k]:off[k + 1]].view(h, w))
