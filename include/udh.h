@@ -744,6 +744,11 @@ int udh_debug_tc_pool(int numeric_mode, const float* in, float* out, uint32_t* c
 size_t udh_debug_fc1_scratch_bytes(int B, int numeric_mode);
 int udh_debug_fc1(int numeric_mode, const float* x, const float* w, const float* dy, float* y, float* dW, float* dx, void* scratch,
                   int B, void* stream);
+/* fc1 of the P x P-patch regressor in UDH_NUMERIC_FP32 (the only mode above P = 128), F = (P/8)^2 * 128 features, through
+ * exactly the calls the step makes: y[B,1024] = x[B,F] . w[F,1024] (split-K, no bias, no ReLU); with dy[B,1024] != NULL also
+ * dW[F,1024] += x^T . dy (ACCUMULATED, as in the step) and dx[B,F] = dy . w^T.  B and P are checked as udh_cnn_fwd checks
+ * them (P a multiple of 128 up to 1408).  All buffers are the caller's. */
+int udh_debug_fc1_ex(const float* x, const float* w, const float* dy, float* y, float* dW, float* dx, int B, int P, void* stream);
 
 /* ---- debug / test entry points of the fp32 CUDA-core path (UDH_NUMERIC_FP32), the calls the step makes ------------
  * udh_debug_simt_conv: one 3x3 convolution, NHWC fp32, H % 8 == 0, W % 16 == 0.  dgrad == 0: out [B,H,W,cout] =

@@ -181,6 +181,23 @@ def test_fc1_debug_entry_rejects_bad_arguments():
         assert b"unknown numeric_mode" in L.udh_last_error()
 
 
+def test_fc1_ex_debug_entry_rejects_what_the_step_rejects():
+    """udh_debug_fc1_ex (fc1 at any fp32 patch size) checks B and P as udh_cnn_fwd does, and its pointers, before touching
+    the device."""
+    from unsuperviseddeephomographyral2018_b200 import _lib
+    L = _lib.lib
+    p = ctypes.c_void_p(256)                          # never dereferenced: every call below fails its argument checks
+    for B, P, msg in ((0, 128, b"batch must be >= 1"), (-2, 1408, b"batch must be >= 1"), (1, 100, b"multiple of 128"),
+                      (1, 0, b"multiple of 128"), (1, 1536, b"P <= 1408")):
+        assert L.udh_debug_fc1_ex(p, p, p, p, p, p, B, P, None) == _lib.EINVAL, (B, P)
+        assert msg in L.udh_last_error(), (B, P, L.udh_last_error())
+    for i in (0, 1, 3, 4, 5):                         # x, w, y; dW and dx when dy is given
+        a = [p, p, p, p, p, p]
+        a[i] = None
+        assert L.udh_debug_fc1_ex(*a, 2, 1408, None) == _lib.EINVAL, i
+        assert b"udh_debug_fc1_ex: null pointer" in L.udh_last_error()
+
+
 def test_simt_debug_entries_reject_bad_arguments():
     """udh_debug_simt_conv / _wgrad / _pool are exported and check their arguments before touching the device."""
     from unsuperviseddeephomographyral2018_b200 import _lib

@@ -138,6 +138,7 @@ SIGNATURES = {
     "udh_debug_tc_pool": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "udh_debug_fc1_scratch_bytes": (c_size_t, [c_int, c_int]),
     "udh_debug_fc1": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
+    "udh_debug_fc1_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "udh_debug_simt_conv": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                     c_int, c_int, c_int, c_void_p]),
     "udh_debug_simt_wgrad": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,

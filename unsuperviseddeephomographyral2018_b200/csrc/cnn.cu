@@ -191,6 +191,19 @@ extern "C" int udh_debug_fc1(int numeric_mode, const float* x, const float* w, c
   return UDH_OK;
 }
 
+extern "C" int udh_debug_fc1_ex(const float* x, const float* w, const float* dy, float* y, float* dW, float* dx, int B, int P,
+                                void* stream) {
+  TRY(check_cnn_args("udh_debug_fc1_ex", B, P, UDH_NUMERIC_FP32));
+  UDH_REQUIRE(x && w && y && (dy == nullptr || (dW && dx)), "udh_debug_fc1_ex: null pointer");
+  const int feat = (P / 8) * (P / 8) * 128;
+  cudaStream_t st = as_stream(stream);
+  // the fp32 calls of udh_cnn_fwd_ex / udh_cnn_bwd_phase at this patch size
+  UDH_CUDA(cudaMemsetAsync(y, 0, (size_t)B * 1024 * 4, st));
+  TRY(fc1_fwd_simt(x, w, y, B, feat, st));
+  if (dy) TRY(fc1_bwd_simt(x, w, dy, dW, dx, B, feat, st));
+  return UDH_OK;
+}
+
 extern "C" int udh_debug_tc_pool(int numeric_mode, const float* in, float* out, uint32_t* codes, const float* dout, float* din, int B,
                                  int H, int W, int C, void* stream) {
   UDH_REQUIRE(numeric_mode == UDH_NUMERIC_BF16 || numeric_mode == UDH_NUMERIC_BF16X3, "udh_debug_tc_pool: unknown numeric_mode %d",

@@ -71,10 +71,13 @@ def init_flat(seed, patch_size=128):
     specs = param_specs(patch_size)
     flat = np.zeros(total_floats(specs), dtype=np.float32)
     rng = np.random.default_rng(seed)
+    chunk = 1 << 24          # float64 draws per call: the same stream as one call, without a float64 copy of fc1 (32 GB at P = 1408)
     for s in specs.values():
         if s.fan_in:
             lim = np.sqrt(6.0 / (s.fan_in + s.fan_out))
-            flat[s.offset:s.offset + s.size] = rng.uniform(-lim, lim, size=s.size).astype(np.float32)
+            for a in range(0, s.size, chunk):
+                b = min(s.size, a + chunk)
+                flat[s.offset + a:s.offset + b] = rng.uniform(-lim, lim, size=b - a).astype(np.float32)
     return flat
 
 
