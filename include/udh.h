@@ -616,6 +616,31 @@ int udh_mosaic_seam_masks_u8(const uint8_t* const* frames, const int32_t* sizes,
                              const int32_t* pair_ptr, const int32_t* pair_j, int dst_h, int dst_w, uint8_t* seam, uint8_t* blend,
                              void* ws, size_t ws_bytes, void* stream);
 
+/* udh_mosaic_seam_gc_masks_u8: the same call with cv2.detail's GraphCutSeamFinder(COST_COLOR) rule (oracle/seam_gc.py):
+ *   the pairs, the window, s_i and s_j as above; I_i is frame i's ROI warp where the window pixel lies inside its ROI (its
+ *   border values included), 0 outside, likewise I_j, and d = sum_c (I_i - I_j)^2.  The window is a 4-connected graph:
+ *   edge (p, q) carries d(p) + d(q) + 1 both ways, + 1000 unless s_i and s_j hold both p and q; a pixel with s_i and not
+ *   s_j is tied to the source, one with s_j and not s_i to the sink, with 10000.  T is the set of pixels that reach the
+ *   sink in the residual graph of a maximum flow (the same for every maximum flow), S the rest; over the intersection,
+ *   frame j's mask is cleared where p is in S and frame i holds it, frame i's where p is in T and frame j holds it.
+ *   cut (host, optional): npairs int64, each pair's minimum-cut value.  Synchronises; the launches depend on how fast each
+ *   pair's flow settles.  ws: udh_mosaic_seam_gc_workspace_bytes(rois, n, pair_ptr, pair_j, dst_h, dst_w) bytes of device
+ *   memory (0: bad arguments).
+ * udh_debug_grid_mincut: the minimum cut of an h x w grid graph (device int32 planes [h,w]): hcap[y,x] the capacity of
+ *   edge (x, y) - (x + 1, y) both ways (last column ignored), vcap[y,x] of (x, y) - (x, y + 1) (last row ignored), src and
+ *   snk the terminal capacities; every one in [0, 2^24].  T [h,w] uint8 (device): 1 where the pixel reaches the sink in
+ *   the residual graph of a maximum preflow, 0 elsewhere; *cut (host): the cut's capacity; residual (device, optional)
+ *   int32 [5,h,w]: the residual capacities to the right, lower, left and upper neighbour and to the sink.  Synchronises.
+ *   ws: udh_debug_grid_mincut_workspace_bytes(h, w) bytes (0: sides outside 1..32786). */
+size_t udh_mosaic_seam_gc_workspace_bytes(const int32_t* rois, int n, const int32_t* pair_ptr, const int32_t* pair_j, int dst_h,
+                                          int dst_w);
+int udh_mosaic_seam_gc_masks_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const int32_t* rois, int n,
+                                const int32_t* pair_ptr, const int32_t* pair_j, int dst_h, int dst_w, uint8_t* seam, uint8_t* blend,
+                                int64_t* cut, void* ws, size_t ws_bytes, void* stream);
+size_t udh_debug_grid_mincut_workspace_bytes(int h, int w);
+int udh_debug_grid_mincut(const int32_t* hcap, const int32_t* vcap, const int32_t* src, const int32_t* snk, int h, int w, uint8_t* T,
+                          int64_t* cut, int32_t* residual, void* ws, size_t ws_bytes, void* stream);
+
 /* ---- instrumentation read by bench.py -------------------------------------------------------------------------
  * udh_launch_count: kernels this library has launched in this process (monotonic).
  * udh_prof_*: when enabled, every tagged phase is bracketed by CUDA events recorded on the launching stream;

@@ -21,13 +21,15 @@ cv2's rule pulls every gain towards 1, so one feed removes only part of a step; 
 is left (on a sweep with exposures 0.75 / 1 / 1.3, four gain-mode feeds recover the gain ratios to within 1 %).
 --seam voronoi cuts seams between the frames before the blend (cv2.detail's Voronoi seam finder, byte for byte): each
 pixel of an overlap goes to one frame, so the blend no longer averages two drifted frames into a double image across
-the whole overlap; with --blend multiband only the low frequencies are spread across the seam.
+the whole overlap; with --blend multiband only the low frequencies are spread across the seam.  --seam gc_color cuts
+them as cv2.detail's GraphCutSeamFinder(COST_COLOR) does, as the exact minimum cut of each overlap's colour-difference
+graph: the seam runs where the two frames agree.
 
 Writes in --out_dir:
   pairs.txt    `frame_k frame_k+1` and H's nine entries per consecutive pair, as align_images.py's homographies.txt;
   refine.txt   with refinement, `frame_k frame_k+1 rho status levels` per pair, as align_images.py writes it;
   mosaic.txt   `canvas Hc Wc ref r` (` blend multiband B` appended with --blend multiband, then ` compensate MODE F` with
-               --compensate, then ` seam voronoi` with --seam voronoi), then `name kept|dropped` and the nine entries of M_k (frame k -> canvas) per frame,
+               --compensate, then ` seam <finder>` with --seam), then `name kept|dropped` and the nine entries of M_k (frame k -> canvas) per frame,
                '%.9g' of their float32 values; the blend uses those float32 values.  With --compensate each frame line
                ends in its three gains, '%.17g' (exact); so the file reproduces mosaic.jpg.  With a block mode the
                compensate field is ` compensate MODE F B` (B: --compensate_block) and the frame lines carry no gains;
@@ -70,8 +72,9 @@ def build_parser():
     p.add_argument('--compensate_feeds', type=int, default=1,
                    help='feeds of the exposure compensator, 1..16; one feed removes only part of an exposure step (the '
                         'rule pulls every gain towards 1), several (e.g. 4) remove nearly all of it')
-    p.add_argument('--seam', type=str, default='none', choices=['none', 'voronoi'],
-                   help='seams between the frames before the blend: none, or cv2.detail\'s Voronoi seam finder')
+    p.add_argument('--seam', type=str, default='none', choices=['none', 'voronoi', 'gc_color'],
+                   help='seams between the frames before the blend: none, cv2.detail\'s Voronoi seam finder, or its '
+                        'GraphCutSeamFinder(COST_COLOR) as an exact minimum cut')
     p.add_argument('--out_dir', type=str, default='mosaic')
     return p
 

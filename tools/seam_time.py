@@ -7,10 +7,16 @@
     CUDA events over repeated launches (mosaic_time.blend_time);
   * cv2.detail's Voronoi seam finder on the same validity masks (the oracle, CPU) with cv2.setNumThreads(1) and (16);
     the masks are made once and not timed.
+With --finder voronoi gc_color both finders are timed in the same run; gc_color's numbers go under "gc_color":
+  * udh_mosaic_seam_gc_masks_u8 on every pair, one call timed by CUDA events (seconds per sweep; its launches depend on
+    how fast each pair's flow settles), and on the pair with the smallest window alone;
+  * cv2's GraphCutSeamFinder(COST_COLOR) (oracle/seam_gc.cv2_seams, CPU, its default threads) on that one pair: it
+    needs minutes for a whole sweep's windows at these sizes.
 Prints one JSON line with the card name, power limit and maximum SM clock read in the same run.
 
-    python tools/seam_time.py
+    python tools/seam_time.py [--finder voronoi|gc_color ...]
 """
+import argparse
 import ctypes
 import json
 import os
@@ -25,12 +31,14 @@ import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 from oracle import seam as SM  # noqa: E402
+from oracle import seam_gc as GC  # noqa: E402
 from tools import jpeg_time, mosaic_time  # noqa: E402
 from tools.mosaic_time import _p, _stream, events_ms  # noqa: E402
 from unsuperviseddeephomographyral2018_b200 import _lib, mosaic, ops  # noqa: E402
 
 
-def seam_time(dev, M, canvas, reps=5):
+def seam_time(dev, M, canvas, reps=5, finder="voronoi", only=None):
+    """The seam call on every intersecting pair (or only on pair only = (i, j)) and without pairs -> (times, blend masks)."""
     Hc, Wc = canvas
     n = len(dev)
     sizes = [tuple(int(v) for v in t.shape[:2]) for t in dev]
@@ -42,18 +50,34 @@ def seam_time(dev, M, canvas, reps=5):
     area = ((rr[:, 2] - rr[:, 0]) * (rr[:, 3] - rr[:, 1])).astype(np.int64)
     seam = torch.empty(int(area.sum()), dtype=torch.uint8, device="cuda")
     blend = torch.empty_like(seam)
+    gc = finder == "gc_color"
+    pairs = ops.roi_pairs(rr, False)
+    if only is not None:
+        pairs = (np.array([0] * (only[0] + 1) + [1] * (n - only[0]), np.int32), np.array([only[1]], np.int32))
     res = {}
-    for label, (ptr, pj) in (("seam", ops.roi_pairs(rr, False)), ("no_pairs", (np.zeros(n + 1, np.int32), np.zeros(1, np.int32)))):
-        nb = _lib.lib.udh_mosaic_seam_workspace_bytes(rr.ctypes.data, n, ptr.ctypes.data, pj.ctypes.data, Hc, Wc)
+    for label, (ptr, pj) in (("seam", pairs), ("no_pairs", (np.zeros(n + 1, np.int32), np.zeros(1, np.int32)))):
+        ws_bytes = _lib.lib.udh_mosaic_seam_gc_workspace_bytes if gc else _lib.lib.udh_mosaic_seam_workspace_bytes
+        nb = ws_bytes(rr.ctypes.data, n, ptr.ctypes.data, pj.ctypes.data, Hc, Wc)
         ws = torch.empty(nb, dtype=torch.uint8, device="cuda")
-        call = lambda: _lib.check(_lib.lib.udh_mosaic_seam_masks_u8(
-            ptrs, sz.ctypes.data, _p(Mr_d), rr.ctypes.data, n, ptr.ctypes.data, pj.ctypes.data, Hc, Wc, _p(seam), _p(blend), _p(ws), nb,
-            _stream()), "udh_mosaic_seam_masks_u8")
+        args = (ptrs, sz.ctypes.data, _p(Mr_d), rr.ctypes.data, n, ptr.ctypes.data, pj.ctypes.data, Hc, Wc, _p(seam), _p(blend))
+        if gc:
+            call = lambda: _lib.check(_lib.lib.udh_mosaic_seam_gc_masks_u8(*args, None, _p(ws), nb, _stream()), "udh_mosaic_seam_gc_masks_u8")
+        else:
+            call = lambda: _lib.check(_lib.lib.udh_mosaic_seam_masks_u8(*args, _p(ws), nb, _stream()), "udh_mosaic_seam_masks_u8")
         l0 = _lib.lib.udh_launch_count()
-        call()
-        torch.cuda.synchronize()
+        if gc:                                                     # seconds per call: the timed call is the only one
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            call()
+            e1.record()
+            e1.synchronize()
+            res[label + "_ms"] = e0.elapsed_time(e1)
+        else:
+            call()
+            torch.cuda.synchronize()
         res[label + "_launches"] = int(_lib.lib.udh_launch_count() - l0)
-        res[label + "_ms"] = events_ms(call, reps)
+        if not gc:
+            res[label + "_ms"] = events_ms(call, reps)
         if label == "seam":
             res["pairs"] = int(ptr[-1])
             res["workspace_mb"] = nb / 2 ** 20
@@ -75,21 +99,47 @@ def cv2_time(frames, M, canvas):
     return out
 
 
+def gc_time(frames, dev, M, canvas, cv2_pair=True):
+    """The graph-cut finder on the whole sweep and on its smallest pair window, and cv2's on that pair."""
+    r, _ = seam_time(dev, M, canvas, finder="gc_color")
+    print(json.dumps(r), flush=True)
+    _, imgs, masks, tls = SM.fed(frames, M, canvas[0], canvas[1])
+    i, j, (x0, y0, x1, y1) = min(SM.pairs(tls, [m.shape for m in masks]), key=lambda p: (p[2][2] - p[2][0]) * (p[2][3] - p[2][1]))
+    one, _ = seam_time(dev, M, canvas, finder="gc_color", only=(i, j))
+    r.update(small_pair=[i, j], small_pair_window=[y1 - y0 + 2 * SM.GAP, x1 - x0 + 2 * SM.GAP], small_pair_ms=one["pair_loop_ms"],
+             small_pair_launches=one["seam_launches"] - one["no_pairs_launches"])
+    if cv2_pair:
+        t0 = time.perf_counter()
+        GC.cv2_seams([imgs[i], imgs[j]], [masks[i], masks[j]], [tls[i], tls[j]])
+        r["cv2_small_pair_ms"] = (time.perf_counter() - t0) * 1e3
+    print(json.dumps(r), flush=True)
+    return r
+
+
 def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--finder", nargs="+", default=["voronoi"], choices=["voronoi", "gc_color"])
+    ap.add_argument("--no_cv2", action="store_true", help="skip cv2's timing")
+    args = ap.parse_args()
     torch.cuda.set_device(0)
-    out = {"gpu": torch.cuda.get_device_name(0), "card": jpeg_time.card()}
+    out = {"gpu": torch.cuda.get_device_name(0), "card": jpeg_time.card(), "finder": args.finder}
     for n, h, w in ((32, 1080, 1920), (16, 3000, 4000)):
         frames, M, canvas = mosaic_time.placed_sweep(n, h, w)
         dev = [torch.from_numpy(f).cuda() for f in frames]
         r = {"canvas": list(canvas)}
-        s, bm = seam_time(dev, M, canvas)
-        r.update(s)
-        r.update(mosaic_time.blend_time(dev, M, canvas, masks=bm))
-        print(json.dumps(r), flush=True)
-        r.update(cv2_time(frames, M, canvas))
+        if "voronoi" in args.finder:
+            s, bm = seam_time(dev, M, canvas)
+            r.update(s)
+            r.update(mosaic_time.blend_time(dev, M, canvas, masks=bm))
+            print(json.dumps(r), flush=True)
+            if not args.no_cv2:
+                r.update(cv2_time(frames, M, canvas))
+            del bm
+        if "gc_color" in args.finder:
+            r["gc_color"] = gc_time(frames, dev, M, canvas, not args.no_cv2)
         out["sweep_%dx%dx%d" % (n, h, w)] = r
         print(json.dumps(r), flush=True)
-        del frames, dev, bm
+        del frames, dev
         torch.cuda.empty_cache()
     print(json.dumps(out))
 

@@ -19,64 +19,9 @@
 #include <vector>
 
 #include "common.cuh"
+#include "roi_warp.cuh"
 
 namespace udh {
-
-__device__ __forceinline__ void cv_invert3(const double* m, double* t) {
-  auto dm = [](double a, double b) { return __dmul_rn(a, b); };
-  auto cof = [&](int a, int b, int c, int d) { return __dsub_rn(dm(m[a], m[b]), dm(m[c], m[d])); };
-  double det = __dadd_rn(__dsub_rn(dm(m[0], cof(4, 8, 5, 7)), dm(m[1], cof(3, 8, 5, 6))), dm(m[2], cof(3, 7, 4, 6)));
-  if (det == 0.0) {
-    for (int k = 0; k < 9; ++k) t[k] = 0.0;
-    return;
-  }
-  const double d = __ddiv_rn(1.0, det);
-  t[0] = dm(cof(4, 8, 5, 7), d); t[1] = dm(cof(2, 7, 1, 8), d); t[2] = dm(cof(1, 5, 2, 4), d);
-  t[3] = dm(cof(5, 6, 3, 8), d); t[4] = dm(cof(0, 8, 2, 6), d); t[5] = dm(cof(2, 3, 0, 5), d);
-  t[6] = dm(cof(3, 7, 4, 6), d); t[7] = dm(cof(1, 6, 0, 7), d); t[8] = dm(cof(0, 4, 1, 3), d);
-}
-
-__device__ __forceinline__ int wp_fixed(double num, double W) {
-  const double f = fmax(-2147483648.0, fmin(2147483647.0, __dmul_rn(num, W)));
-  return __double2int_rn(f);
-}
-
-// The source position of output pixel (x, y) in 1/32 pixel (X, Y); returns the denominator before 32 / W (0: cv2 lands on
-// source pixel (0, 0)).
-__device__ __forceinline__ double wp_coords(const double* mi, int x, int y, int bw, int& X, int& Y) {
-  const int xb = x - x % bw;
-  const double dxb = (double)xb, dy = (double)y, dx1 = (double)(x - xb);
-  const double X0 = __dadd_rn(__dadd_rn(__dmul_rn(mi[0], dxb), __dmul_rn(mi[1], dy)), mi[2]);
-  const double Y0 = __dadd_rn(__dadd_rn(__dmul_rn(mi[3], dxb), __dmul_rn(mi[4], dy)), mi[5]);
-  const double W0 = __dadd_rn(__dadd_rn(__dmul_rn(mi[6], dxb), __dmul_rn(mi[7], dy)), mi[8]);
-  const double Wd = __dadd_rn(W0, __dmul_rn(mi[6], dx1));
-  const double W = Wd != 0.0 ? __ddiv_rn(32.0, Wd) : 0.0;
-  X = wp_fixed(__dadd_rn(X0, __dmul_rn(mi[0], dx1)), W);
-  Y = wp_fixed(__dadd_rn(Y0, __dmul_rn(mi[3], dx1)), W);
-  return Wd;
-}
-
-// The bilinear value at (X, Y) (1/32 pixel) of an h x w source with C channels: 15-bit weights, taps outside read 0.
-template <int C>
-__device__ __forceinline__ void wp_sample(const uint8_t* __restrict__ s, int h, int w, int X, int Y, int* v) {
-  const int sx = min(max(X >> 5, -32768), 32767), sy = min(max(Y >> 5, -32768), 32767);
-  const int fx = X & 31, fy = Y & 31;
-  const int wt[4] = {(32 - fx) * (32 - fy) * 32, fx * (32 - fy) * 32, (32 - fx) * fy * 32, fx * fy * 32};
-  int acc[C];
-#pragma unroll
-  for (int c = 0; c < C; ++c) acc[c] = 0;
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    const int tx = sx + (k & 1), ty = sy + (k >> 1);
-    if ((unsigned)tx < (unsigned)w && (unsigned)ty < (unsigned)h) {
-      const uint8_t* p = s + ((int64_t)ty * w + tx) * C;
-#pragma unroll
-      for (int c = 0; c < C; ++c) acc[c] += wt[k] * (int)__ldg(p + c);
-    }
-  }
-#pragma unroll
-  for (int c = 0; c < C; ++c) v[c] = (acc[c] + (1 << 14)) >> 15;
-}
 
 template <int C>
 __device__ __forceinline__ void wp_pixel(const uint8_t* __restrict__ s, int h, int w, const double* mi, int x, int y, int bw,
@@ -123,14 +68,6 @@ struct MosaicFrame {
   double mi[9];                   // cv_invert3 of the frame's M (frame -> canvas), filled by invert_kernel
   const uint8_t* src;
   int h, w;
-};
-
-// A frame warped onto its ROI rectangle of the canvas (the multi-band blend's feed, the exposure statistics, the seams):
-// the frame, the ROI (rx, ry, rw, rh) and the ROI warp's tile width.  roi_frame fills it on the host.
-struct RoiFrame {
-  const uint8_t* src;
-  int h, w;
-  int rx, ry, rw, rh, bw;
 };
 
 // Every frame's inverse into its table entry: fr[k].mi = cv_invert3(M_k).
@@ -317,15 +254,6 @@ __device__ __forceinline__ void mb_up_taps(int o, int n, int* t, int* wt) {
 }
 
 __device__ __forceinline__ int mb_sat16(int v) { return min(max(v, -32768), 32767); }
-
-// Frame (s, h, w)'s ROI warp at ROI pixel (sx, sy) (tile width bw): its value, and whether the pixel is valid.
-__device__ __forceinline__ bool mb_roi_warp(const uint8_t* __restrict__ s, int h, int w, const double* mi, int sx, int sy, int bw,
-                                            int* v) {
-  int X, Y;
-  const double Wd = wp_coords(mi, sx, sy, bw, X, Y);
-  wp_sample<3>(s, h, w, X, Y, v);
-  return Wd != 0.0 && X >= 0 && X <= 32 * (w - 1) && Y >= 0 && Y <= 32 * (h - 1);
-}
 
 // Level 0 of every frame: the ROI warp bordered with BORDER_REFLECT, and the 0 / 256 weight with a constant 0 border.
 // gains (null: none) [n][3]: the ROI warp is exposure-compensated first, ex_apply(v, gains[k][c]), as cv2's stitcher
@@ -1029,16 +957,7 @@ __global__ void __launch_bounds__(256) gainblock_maps_kernel(const double* __res
 // turns that into the exact L1 distance (min over x' of g(x') + |x - x'|, a prefix and a suffix minimum) and clears one
 // frame's mask at every pixel of the intersection.  All in int32: SEAM_INF marks "no source" and survives the adds
 // (distances are below 2^17, the window's sides below 32767 + 2 SEAM_GAP).
-constexpr int SEAM_GAP = 10, SEAM_INF = 1 << 30, SEAM_SEGS = 16, SEAM_ROW_THREADS = 256;
-
-struct SeamFrame : RoiFrame {
-  int64_t off;                  // the ROI's element offset in the mask pools
-};
-
-struct SeamRect {                  // a frame's ROI and pool offset, passed by value to the pair kernels
-  int64_t off;
-  int rx, ry, rw, rh;
-};
+constexpr int SEAM_INF = 1 << 30, SEAM_SEGS = 16, SEAM_ROW_THREADS = 256;
 
 // Every frame's ROI validity (udh_mosaic_multiband_u8's mask, mb_roi_warp's rule), 0 / 255, into both pools.
 __global__ void __launch_bounds__(256) seam_valid_kernel(const SeamFrame* __restrict__ fr, const double* __restrict__ M,
@@ -1059,11 +978,6 @@ __global__ void __launch_bounds__(256) seam_valid_kernel(const SeamFrame* __rest
     seam[off + e] = v;
     blend[off + e] = v;
   }
-}
-
-__device__ __forceinline__ bool seam_at(const uint8_t* __restrict__ seam, const SeamRect& r, int cx, int cy) {
-  const int lx = cx - r.rx, ly = cy - r.ry;
-  return (unsigned)lx < (unsigned)r.rw && (unsigned)ly < (unsigned)r.rh && seam[r.off + (int64_t)ly * r.rw + lx] != 0;
 }
 
 // The pair's unique pixels at window pixel (x, y): bit 0 frame a's, bit 1 frame b's (a pixel both masks hold is neither's).
@@ -1469,8 +1383,7 @@ struct SeamPlan {
 };
 
 static int seam_plan(const uint8_t* const* frames, const int32_t* rois, const int32_t* sizes, int n, const int32_t* pair_ptr,
-                     const int32_t* pair_j, int dst_h, int dst_w, SeamPlan& p) {
-  const char* what = "udh_mosaic_seam_masks_u8";
+                     const int32_t* pair_j, int dst_h, int dst_w, SeamPlan& p, const char* what) {
   UDH_REQUIRE(rois && pair_ptr && (pair_j || !pair_ptr[n]), "%s: null pointer", what);
   UDH_REQUIRE(n >= 1 && n <= UDH_SEAM_MAX_FRAMES && dst_h >= 1 && dst_w >= 1 && dst_h < 32767 && dst_w < 32767,
               "%s: bad dimensions (n %d of at most %d, canvas %dx%d)", what, n, UDH_SEAM_MAX_FRAMES, dst_h, dst_w);
@@ -1484,16 +1397,16 @@ static int seam_plan(const uint8_t* const* frames, const int32_t* rois, const in
     off += (int64_t)F.rw * F.rh;
     if ((int64_t)F.rw * F.rh > p.max_px) p.max_px = (int64_t)F.rw * F.rh;
   }
-  UDH_REQUIRE(pair_ptr[0] == 0, "udh_mosaic_seam_masks_u8: pair_ptr[0] is %d", pair_ptr[0]);
+  UDH_REQUIRE(pair_ptr[0] == 0, "%s: pair_ptr[0] is %d", what, pair_ptr[0]);
   for (int i = 0; i < n; ++i) {
-    UDH_REQUIRE(pair_ptr[i + 1] >= pair_ptr[i], "udh_mosaic_seam_masks_u8: pair_ptr decreases at frame %d", i);
+    UDH_REQUIRE(pair_ptr[i + 1] >= pair_ptr[i], "%s: pair_ptr decreases at frame %d", what, i);
     for (int e = pair_ptr[i]; e < pair_ptr[i + 1]; ++e) {
       const int j = pair_j[e];
       UDH_REQUIRE(j > i && j < n && (e == pair_ptr[i] || j > pair_j[e - 1]),
-                  "udh_mosaic_seam_masks_u8: pair (%d, %d) is out of order or range", i, j);
+                  "%s: pair (%d, %d) is out of order or range", what, i, j);
       const SeamFrame &A = p.fr[i], &B = p.fr[j];
       const int iw = std::min(A.rx + A.rw, B.rx + B.rw) - std::max(A.rx, B.rx), ih = std::min(A.ry + A.rh, B.ry + B.rh) - std::max(A.ry, B.ry);
-      UDH_REQUIRE(iw > 0 && ih > 0, "udh_mosaic_seam_masks_u8: the ROIs of pair (%d, %d) do not intersect", i, j);
+      UDH_REQUIRE(iw > 0 && ih > 0, "%s: the ROIs of pair (%d, %d) do not intersect", what, i, j);
       const int64_t ww = iw + 2 * SEAM_GAP, wh = ih + 2 * SEAM_GAP;
       p.max_win = std::max(p.max_win, ww * wh);
       p.max_inner = std::max(p.max_inner, ww * ih);
@@ -1510,7 +1423,7 @@ static int seam_plan(const uint8_t* const* frames, const int32_t* rois, const in
 extern "C" size_t udh_mosaic_seam_workspace_bytes(const int32_t* rois, int n, const int32_t* pair_ptr, const int32_t* pair_j,
                                                   int dst_h, int dst_w) {
   SeamPlan p;
-  return seam_plan(nullptr, rois, nullptr, n, pair_ptr, pair_j, dst_h, dst_w, p) == UDH_OK ? p.total : 0;
+  return seam_plan(nullptr, rois, nullptr, n, pair_ptr, pair_j, dst_h, dst_w, p, "udh_mosaic_seam_masks_u8") == UDH_OK ? p.total : 0;
 }
 
 extern "C" int udh_mosaic_seam_masks_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const int32_t* rois, int n,
@@ -1519,7 +1432,7 @@ extern "C" int udh_mosaic_seam_masks_u8(const uint8_t* const* frames, const int3
   const char* what = "udh_mosaic_seam_masks_u8";
   UDH_REQUIRE(frames && sizes && M && seam && blend && ws, "%s: null pointer", what);
   SeamPlan p;
-  int rc = seam_plan(frames, rois, sizes, n, pair_ptr, pair_j, dst_h, dst_w, p);
+  int rc = seam_plan(frames, rois, sizes, n, pair_ptr, pair_j, dst_h, dst_w, p, what);
   if (rc != UDH_OK) return rc;
   if (ws_bytes < p.total) {
     set_error("%s: workspace of %zu bytes, %zu needed", what, ws_bytes, p.total);
@@ -1548,6 +1461,38 @@ extern "C" int udh_mosaic_seam_masks_u8(const uint8_t* const* frames, const int3
   }
   seam_blend_mask_kernel<<<dim3(mb_blocks(p.max_px), (unsigned)n), 256, 0, st>>>(fr, seam, blend);
   return check_launch("udh_mosaic_seam_masks_u8 (blend masks)");
+}
+
+extern "C" size_t udh_mosaic_seam_gc_workspace_bytes(const int32_t* rois, int n, const int32_t* pair_ptr, const int32_t* pair_j,
+                                                     int dst_h, int dst_w) {
+  SeamPlan p;
+  if (seam_plan(nullptr, rois, nullptr, n, pair_ptr, pair_j, dst_h, dst_w, p, "udh_mosaic_seam_gc_masks_u8") != UDH_OK) return 0;
+  return gc_workspace_bytes(mb_align((size_t)n * sizeof(SeamFrame)), p.max_win, (int64_t)p.pi.size());
+}
+
+// The Voronoi call's plan, validity and blend masks around gc_seam_pairs (seam_gc.cu).
+extern "C" int udh_mosaic_seam_gc_masks_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const int32_t* rois,
+                                           int n, const int32_t* pair_ptr, const int32_t* pair_j, int dst_h, int dst_w, uint8_t* seam,
+                                           uint8_t* blend, int64_t* cut, void* ws, size_t ws_bytes, void* stream) {
+  const char* what = "udh_mosaic_seam_gc_masks_u8";
+  UDH_REQUIRE(frames && sizes && M && seam && blend && ws, "%s: null pointer", what);
+  SeamPlan p;
+  int rc = seam_plan(frames, rois, sizes, n, pair_ptr, pair_j, dst_h, dst_w, p, what);
+  if (rc != UDH_OK) return rc;
+  const size_t off = mb_align((size_t)n * sizeof(SeamFrame)), need = gc_workspace_bytes(off, p.max_win, (int64_t)p.pi.size());
+  if (ws_bytes < need) {
+    set_error("%s: workspace of %zu bytes, %zu needed", what, ws_bytes, need);
+    return UDH_EWS;
+  }
+  const cudaStream_t st = as_stream(stream);
+  char* base = static_cast<char*>(ws);
+  if ((rc = upload(base, p.fr, st, what)) != UDH_OK) return rc;
+  const SeamFrame* fr = reinterpret_cast<const SeamFrame*>(base);
+  seam_valid_kernel<<<dim3(mb_blocks(p.max_px), (unsigned)n), 256, 0, st>>>(fr, M, seam, blend);
+  if ((rc = check_launch("udh_mosaic_seam_gc_masks_u8 (validity)")) != UDH_OK) return rc;
+  if ((rc = gc_seam_pairs(base, off, p.max_win, fr, p.fr, M, seam, p.pi, p.pj, cut, st, what)) != UDH_OK) return rc;
+  seam_blend_mask_kernel<<<dim3(mb_blocks(p.max_px), (unsigned)n), 256, 0, st>>>(fr, seam, blend);
+  return check_launch("udh_mosaic_seam_gc_masks_u8 (blend masks)");
 }
 
 extern "C" size_t udh_mosaic_exposure_block_workspace_bytes(int n) { return n > 0 ? (size_t)n * sizeof(ExposureBlockFrame) : 0; }

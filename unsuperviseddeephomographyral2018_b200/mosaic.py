@@ -42,7 +42,9 @@ dilation of its seam mask meets its validity (cv2's stitcher's blend mask): the 
 frequencies at the seam and spreads only the low ones, instead of averaging the frames across the whole overlap, which
 leaves a semi-transparent double image where the chain drifts; the feathered blend keeps its weights inside each
 frame's region.  The compensator still sees the un-seamed masks, as in cv2's stitcher.  A frame lying inside another
-one's region gets nothing (cv2's result).
+one's region gets nothing (cv2's result).  seam="gc_color" cuts each overlap as cv2.detail's GraphCutSeamFinder
+(COST_COLOR) does instead (oracle/seam_gc.py): along the minimum cut of a graph whose edges cost the two warps' squared
+colour difference, so the seam runs where the frames agree rather than where geometry puts it.
 """
 import numpy as np
 
@@ -146,7 +148,7 @@ def farthest_frame(sizes, G, kept, ref):
 
 
 COMPENSATE = ("none", "gain", "channels", "gain_blocks", "channels_blocks")
-SEAM = ("none", "voronoi")
+SEAM = ("none", "voronoi", "gc_color")
 
 
 def build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None, float32_M=False, blend="feather", bands=5,
@@ -158,8 +160,8 @@ def build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None
     float32, the values a text file of '%.9g' float32 entries gives back.  compensate: "none", "gain" or "channels"
     (ops.mosaic_exposure_gains with compensate_feeds feeds, applied by the blend), or "gain_blocks" / "channels_blocks"
     (ops.mosaic_exposure_gain_maps with blocks of about compensate_block px: a gain map per frame, cv2's
-    BlocksGainCompensator / BlocksChannelsCompensator; gains stay 1).  seam: "none" or "voronoi"
-    (ops.mosaic_seam_masks; each frame blends only inside its blend mask).
+    BlocksGainCompensator / BlocksChannelsCompensator; gains stay 1).  seam: "none", "voronoi" or "gc_color"
+    (ops.mosaic_seam_masks' finder; each frame blends only inside its blend mask).
     -> dict(mosaic uint8 [Hc,Wc,3] RGB, mask uint8 [Hc,Wc], M [N,3,3] frame k -> canvas (float64, float32 values with
     float32_M), kept bool [N], ref, H_pairs [N-1,3,3], refine (rho, status, level_reached) or None, gains float64 [N,3]
     (1 for a dropped frame, all 1 without per-frame compensation), gain_maps [N] (the block modes only: CUDA float32
@@ -187,7 +189,7 @@ def build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None
     if compensate not in COMPENSATE:
         raise ValueError("compensate must be one of %s (got %r)" % (", ".join(COMPENSATE), compensate))
     if seam not in SEAM:
-        raise ValueError("seam must be 'none' or 'voronoi' (got %r)" % (seam,))
+        raise ValueError("seam must be one of %s (got %r)" % (", ".join(SEAM), seam))
     gains = np.ones((len(frames), 3))
     gain_maps = None
     if compensate in ("gain", "channels"):
@@ -197,7 +199,7 @@ def build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None
                                                              compensate_block)
     masks = None
     if seam != "none":
-        masks, ms["seam"] = seam_kept(frames, M, kept, Hc, Wc)
+        masks, ms["seam"] = seam_kept(frames, M, kept, Hc, Wc, seam)
     mosaic, mask, ms["blend"] = blend_kept(frames, M, kept, Hc, Wc, feather, blend, bands,
                                            gains if compensate in ("gain", "channels") else None, masks,
                                            None if gain_maps is None else [gain_maps[k] for k in range(len(frames)) if kept[k]])
@@ -245,15 +247,15 @@ def compensate_blocks_kept(frames, M, kept, Hc, Wc, mode, feeds=1, block=32):
     return maps, e0.elapsed_time(e1)
 
 
-def seam_kept(frames, M, kept, Hc, Wc):
-    """The kept frames' blend masks (ops.mosaic_seam_masks) -> (masks [n_kept]: CUDA uint8 [roi_h,roi_w], None for a frame
+def seam_kept(frames, M, kept, Hc, Wc, finder="voronoi"):
+    """The kept frames' blend masks (ops.mosaic_seam_masks with finder) -> (masks [n_kept]: CUDA uint8 [roi_h,roi_w], None for a frame
     whose ROI misses the canvas; CUDA-event ms)."""
     import torch
     from . import ops
     take = [k for k in range(len(frames)) if kept[k]]
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
-    s = ops.mosaic_seam_masks([frames[k].contiguous() for k in take], np.asarray(M)[take], Hc, Wc)
+    s = ops.mosaic_seam_masks([frames[k].contiguous() for k in take], np.asarray(M)[take], Hc, Wc, finder)
     e1.record()
     e1.synchronize()
     masks = [None] * len(take)

@@ -1236,34 +1236,81 @@ def _gain_map_table(gain_maps, rois, n, dev, what):
 
 
 # ------------------------------------------------------------------ seam finding
-def mosaic_seam_masks(frames, M, dst_h, dst_w):
+SEAM_FINDERS = ("voronoi", "gc_color")
+
+
+def mosaic_seam_masks(frames, M, dst_h, dst_w, finder="voronoi"):
     """frames: n CUDA uint8 RGB tensors [h_k,w_k,3], M float64 [n,3,3] (frame k -> canvas) -> dict(take (the fed frames:
     those whose ROI meets the canvas), rois int64 [n,4] (mosaic.multiband_rois), seam [m], blend [m]): per fed frame its
-    seam mask and blend mask, CUDA uint8 [roi_h,roi_w] (0 / 255), byte for byte what cv2.detail's Voronoi seam finder
-    leaves in the multi-band blend's validity masks, and cv2.dilate of that AND the validity, the mask cv2's stitcher feeds
-    its blender (udh_mosaic_seam_masks_u8; oracle/seam.py states the rule).  A frame lying inside another one's seam region
-    vanishes (an all-zero mask), as in cv2."""
+    seam mask and blend mask, CUDA uint8 [roi_h,roi_w] (0 / 255), and cv2.dilate of that AND the validity, the mask cv2's
+    stitcher feeds its blender.  finder "voronoi": byte for byte what cv2.detail's Voronoi seam finder leaves in the
+    multi-band blend's validity masks (udh_mosaic_seam_masks_u8; oracle/seam.py states the rule).  A frame lying inside
+    another one's seam region vanishes (an all-zero mask), as in cv2.  finder "gc_color": cv2.detail's
+    GraphCutSeamFinder(COST_COLOR) on the uncompensated ROI warps, as the canonical minimum cut of each pair's window
+    (udh_mosaic_seam_gc_masks_u8; oracle/seam_gc.py states the rule), with cut int64 [pairs]: each pair's cut value, the
+    pairs in cv2's visiting order."""
+    if finder not in SEAM_FINDERS:
+        raise ValueError("finder must be one of %s (got %r)" % (", ".join(SEAM_FINDERS), finder))
+    gc = finder == "gc_color"
     fed = _Fed(frames, M, dst_h, dst_w, "mosaic_seam_masks", _lib.EXPOSURE_MAX_FRAMES)
     out = dict(take=fed.take, rois=fed.rois, seam=[], blend=[])
+    if gc:
+        out["cut"] = np.zeros(0, np.int64)
     if not fed.m:
         return out
     m, dev, rr = fed.m, fed.dev, fed.rr
     ptr, pj = roi_pairs(rr, False)
+    npairs = int(ptr[-1])
     pj = pj if len(pj) else np.zeros(1, np.int32)
     hw = np.stack([rr[:, 3] - rr[:, 1], rr[:, 2] - rr[:, 0]], 1).astype(np.int64)
     off = np.concatenate([[0], np.cumsum(hw[:, 0] * hw[:, 1])])
     seam = torch.empty(int(off[-1]), device=dev, dtype=torch.uint8)
     blend = torch.empty(int(off[-1]), device=dev, dtype=torch.uint8)
-    nb = lib.udh_mosaic_seam_workspace_bytes(rr.ctypes.data, m, ptr.ctypes.data, pj.ctypes.data, int(dst_h), int(dst_w))
+    name = "udh_mosaic_seam_gc_masks_u8" if gc else "udh_mosaic_seam_masks_u8"
+    ws_bytes = lib.udh_mosaic_seam_gc_workspace_bytes if gc else lib.udh_mosaic_seam_workspace_bytes
+    nb = ws_bytes(rr.ctypes.data, m, ptr.ctypes.data, pj.ctypes.data, int(dst_h), int(dst_w))
     if nb == 0:
         raise _lib.UdhError("mosaic_seam_masks: bad arguments (%d frames, canvas %dx%d)" % (m, dst_h, dst_w))
     ws = torch.empty(nb, device=dev, dtype=torch.uint8)
-    check(lib.udh_mosaic_seam_masks_u8(fed.ptrs, fed.sz.ctypes.data, _ptr(fed.M_d), rr.ctypes.data, m, ptr.ctypes.data, pj.ctypes.data,
-                                       int(dst_h), int(dst_w), _ptr(seam), _ptr(blend), _ptr(ws), nb, _stream()), "udh_mosaic_seam_masks_u8")
+    args = (fed.ptrs, fed.sz.ctypes.data, _ptr(fed.M_d), rr.ctypes.data, m, ptr.ctypes.data, pj.ctypes.data, int(dst_h), int(dst_w),
+            _ptr(seam), _ptr(blend))
+    if gc:
+        cut = np.zeros(max(npairs, 1), np.int64)
+        check(lib.udh_mosaic_seam_gc_masks_u8(*args, cut.ctypes.data, _ptr(ws), nb, _stream()), name)
+        out["cut"] = cut[:npairs]
+    else:
+        check(lib.udh_mosaic_seam_masks_u8(*args, _ptr(ws), nb, _stream()), name)
     for k in range(m):
         h, w = (int(v) for v in hw[k])
         out["seam"].append(seam[off[k]:off[k + 1]].view(h, w))
         out["blend"].append(blend[off[k]:off[k + 1]].view(h, w))
+    return out
+
+
+def grid_mincut(hcap, vcap, src, snk, residual=False):
+    """The minimum cut of an h x w 4-connected grid graph (udh_debug_grid_mincut): hcap, vcap, src, snk CUDA int32
+    [h,w] (hcap[y,x]: edge (x, y) - (x + 1, y), both ways; vcap[y,x]: edge (x, y) - (x, y + 1); src / snk: terminal
+    capacities; all in [0, 2^24]) -> dict(T CUDA uint8 [h,w]: 1 where the pixel reaches the sink in the residual graph of
+    a maximum preflow, cut: the cut's capacity (int), and with residual=True residual CUDA int32 [5,h,w]: the residual
+    capacities to the right, lower, left and upper neighbour and to the sink)."""
+    for t, nm in ((hcap, "hcap"), (vcap, "vcap"), (src, "src"), (snk, "snk")):
+        _req(t, torch.int32, nm)
+        if t.dim() != 2 or t.shape != hcap.shape:
+            raise _lib.UdhError("grid_mincut: %s must be [h,w] like hcap (got %s)" % (nm, tuple(t.shape)))
+    h, w = (int(v) for v in hcap.shape)
+    nb = lib.udh_debug_grid_mincut_workspace_bytes(h, w)
+    if nb == 0:
+        raise _lib.UdhError("grid_mincut: bad dimensions %dx%d" % (h, w))
+    dev = hcap.device
+    ws = torch.empty(nb, device=dev, dtype=torch.uint8)
+    T = torch.empty((h, w), device=dev, dtype=torch.uint8)
+    res = torch.empty((5, h, w), device=dev, dtype=torch.int32) if residual else None
+    cut = ctypes.c_int64(0)
+    check(lib.udh_debug_grid_mincut(_ptr(hcap), _ptr(vcap), _ptr(src), _ptr(snk), h, w, _ptr(T), ctypes.addressof(cut), _ptr(res), _ptr(ws),
+                                    nb, _stream()), "udh_debug_grid_mincut")
+    out = dict(T=T, cut=int(cut.value))
+    if residual:
+        out["residual"] = res
     return out
 
 
