@@ -638,6 +638,28 @@ int udh_mosaic_seam_gc_masks_u8(const uint8_t* const* frames, const int32_t* siz
                                 const int32_t* pair_ptr, const int32_t* pair_j, int dst_h, int dst_w, uint8_t* seam, uint8_t* blend,
                                 int64_t* cut, void* ws, size_t ws_bytes, void* stream);
 size_t udh_debug_grid_mincut_workspace_bytes(int h, int w);
+/* ---- seams at a reduced resolution (cv2's seam_megapix; oracle/seam_scale.py restates the rule) -----------------------
+ * udh_resize_linear_exact_u8: cv2.resize(src, ..., INTER_LINEAR_EXACT) on n uint8 [src_h,src_w,c] images (c = 1 or 3),
+ *   byte for byte, down or up.  tab (device, int32; ops.linear_exact_table): xs0[dst_w], xs1[dst_w], xc1[dst_w],
+ *   ys0[dst_h], ys1[dst_h], yc1[dst_h]: per output column / row its two source taps and the upper tap's weight in 1/256
+ *   (f = (d + 1/2) scale - 1/2 in float64, c1 = rint((f - floor f) 256), taps clamped to the image); each value is
+ *   (c0' (c0 p00 + c1 p01) + c1' (c0 p10 + c1 p11) + 2^15) >> 16.  n <= 65535, dst_h dst_w < 2^31.
+ * udh_mosaic_seam_upscale_u8: the full-resolution blend masks of seams found at scale (0, 1]: frames, sizes, M frame ->
+ *   ROI (device) and rois (host) as udh_mosaic_seam_masks_u8 takes them (every ROI non-empty); seams [n] (device) frame
+ *   k's seam mask on its seam ROI seam_rois[k] (host int32 [n,4] on the seam_h x seam_w seam canvas; an empty rectangle
+ *   gives an all-zero mask and its pointer is ignored).  blend [sum of roi_h roi_w] (device, udh_mosaic_seam_masks_u8's
+ *   layout) receives, at each ROI pixel (canvas X, Y), the frame's validity (0 / 255) AND the INTER_LINEAR_EXACT sample
+ *   at ((X + 1/2) scale - 1/2, (Y + 1/2) scale - 1/2) of cv2.dilate(seam mask) placed on the seam canvas (0 outside its
+ *   seam ROI), the taps built on the host in float64 and clamped to the seam canvas: graded masks, 1 .. 254 along the
+ *   seams.  Launches 2 (1 when no seam ROI is given).  ws: udh_mosaic_seam_upscale_workspace_bytes(rois, seam_rois, n,
+ *   seam_h, seam_w, scale, dst_h, dst_w) bytes of device memory (0: bad arguments). */
+int udh_resize_linear_exact_u8(const uint8_t* src, const int32_t* tab, uint8_t* dst, int n, int src_h, int src_w, int c, int dst_h,
+                               int dst_w, void* stream);
+size_t udh_mosaic_seam_upscale_workspace_bytes(const int32_t* rois, const int32_t* seam_rois, int n, int seam_h, int seam_w,
+                                               double scale, int dst_h, int dst_w);
+int udh_mosaic_seam_upscale_u8(const uint8_t* const* frames, const int32_t* sizes, const double* M, const int32_t* rois,
+                               const uint8_t* const* seams, const int32_t* seam_rois, int n, int seam_h, int seam_w, double scale,
+                               int dst_h, int dst_w, uint8_t* blend, void* ws, size_t ws_bytes, void* stream);
 int udh_debug_grid_mincut(const int32_t* hcap, const int32_t* vcap, const int32_t* src, const int32_t* snk, int h, int w, uint8_t* T,
                           int64_t* cut, int32_t* residual, void* ws, size_t ws_bytes, void* stream);
 

@@ -23,13 +23,17 @@ is left (on a sweep with exposures 0.75 / 1 / 1.3, four gain-mode feeds recover 
 pixel of an overlap goes to one frame, so the blend no longer averages two drifted frames into a double image across
 the whole overlap; with --blend multiband only the low frequencies are spread across the seam.  --seam gc_color cuts
 them as cv2.detail's GraphCutSeamFinder(COST_COLOR) does, as the exact minimum cut of each overlap's colour-difference
-graph: the seam runs where the two frames agree.
+graph: the seam runs where the two frames agree.  --seam_megapix X finds the seams at a reduced resolution, as cv2's
+stitcher does (its default is 0.1): the frames scaled to about X megapixels (by the first frame's area) with
+INTER_LINEAR_EXACT, the seams found there, and each seam mask resampled back to full resolution (graded along the seam).
+The graph-cut finder's time falls with the pixel count; -1 (the default) keeps full resolution.
 
 Writes in --out_dir:
   pairs.txt    `frame_k frame_k+1` and H's nine entries per consecutive pair, as align_images.py's homographies.txt;
   refine.txt   with refinement, `frame_k frame_k+1 rho status levels` per pair, as align_images.py writes it;
   mosaic.txt   `canvas Hc Wc ref r` (` blend multiband B` appended with --blend multiband, then ` compensate MODE F` with
-               --compensate, then ` seam <finder>` with --seam), then `name kept|dropped` and the nine entries of M_k (frame k -> canvas) per frame,
+               --compensate, then ` seam <finder>` with --seam, ` seam <finder> A` when --seam_megapix gives a seam
+               scale A < 1, '%.17g'), then `name kept|dropped` and the nine entries of M_k (frame k -> canvas) per frame,
                '%.9g' of their float32 values; the blend uses those float32 values.  With --compensate each frame line
                ends in its three gains, '%.17g' (exact); so the file reproduces mosaic.jpg.  With a block mode the
                compensate field is ` compensate MODE F B` (B: --compensate_block) and the frame lines carry no gains;
@@ -75,6 +79,9 @@ def build_parser():
     p.add_argument('--seam', type=str, default='none', choices=['none', 'voronoi', 'gc_color'],
                    help='seams between the frames before the blend: none, cv2.detail\'s Voronoi seam finder, or its '
                         'GraphCutSeamFinder(COST_COLOR) as an exact minimum cut')
+    p.add_argument('--seam_megapix', type=float, default=-1,
+                   help='find the seams on frames scaled to about this many megapixels (cv2\'s seam_megapix; needs --seam); '
+                        '-1: at full resolution')
     p.add_argument('--out_dir', type=str, default='mosaic')
     return p
 
@@ -107,6 +114,8 @@ def run(args, est, decode, encode):
         raise SystemExit("--compensate_feeds must be in 1..16 (got %d)" % args.compensate_feeds)
     if not 1 <= args.compensate_block <= 1024:
         raise SystemExit("--compensate_block must be in 1..1024 (got %d)" % args.compensate_block)
+    if args.seam_megapix > 0 and args.seam == "none":
+        raise SystemExit("--seam_megapix needs --seam")
     names, paths = frame_list(args)
     os.makedirs(args.out_dir, exist_ok=True)
     refining = args.refine_levels != 0
@@ -120,6 +129,8 @@ def run(args, est, decode, encode):
     seaming = args.seam != "none"
     if seaming:
         comp["seam"] = args.seam
+        if args.seam_megapix > 0:
+            comp["seam_megapix"] = args.seam_megapix
     imgs = decode(paths)
     try:
         out = mosaic.build_mosaic(est, imgs, None if args.ref_frame < 0 else args.ref_frame, refine, args.feather,
@@ -137,7 +148,8 @@ def run(args, est, decode, encode):
     lines = ["canvas %d %d ref %d" % (Hc, Wc, out["ref"]) + (" blend multiband %d" % args.bands if args.blend == "multiband" else "") +
              (" compensate %s %d" % (args.compensate, args.compensate_feeds) if compensating else "") +
              (" %d" % args.compensate_block if blocks else "") +
-             (" seam %s" % args.seam if seaming else "")]
+             (" seam %s" % args.seam if seaming else "") +
+             (" %.17g" % out["seam_scale"] if seaming and out.get("seam_scale", 1.0) < 1.0 else "")]
     for k, nm in enumerate(names):
         lines.append(" ".join([nm, "kept" if out["kept"][k] else "dropped"] +
                               ["%.9g" % v for v in align.homography_as_written(out["M"][k])[0]] +

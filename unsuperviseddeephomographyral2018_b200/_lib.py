@@ -207,6 +207,10 @@ SIGNATURES = {
     "udh_debug_grid_mincut_workspace_bytes": (c_size_t, [c_int, c_int]),
     "udh_debug_grid_mincut": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                                       c_size_t, c_void_p]),
+    "udh_resize_linear_exact_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "udh_mosaic_seam_upscale_workspace_bytes": (c_size_t, [c_void_p, c_void_p, c_int, c_int, c_int, c_double, c_int, c_int]),
+    "udh_mosaic_seam_upscale_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_double,
+                                           c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     "udh_mosaic_exposure_block_workspace_bytes": (c_size_t, [c_int]),
     "udh_mosaic_exposure_block_stats_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int64, c_void_p,
                                                    c_void_p, c_int, c_void_p, c_void_p, c_int64, c_void_p, c_int, c_int, c_int, c_int,

@@ -1,6 +1,7 @@
-// The ROI warp helpers the mosaic kernels share (warp_perspective.cu) with the graph-cut seams (seam_gc.cu): cv2's
-// warpPerspective coordinates and taps (the rules: warp_perspective.cu's header), a frame on its ROI rectangle, and the
-// seam masks' pool layout.  The graph-cut seam pass (seam_gc.cu) is declared at the end.
+// The ROI warp helpers the mosaic kernels share (warp_perspective.cu) with the graph-cut seams (seam_gc.cu) and the
+// seam-scale upscale (seam_scale.cu): cv2's warpPerspective coordinates and taps (the rules: warp_perspective.cu's
+// header), a frame on its ROI rectangle and the host helpers that fill and upload its table, and the seam masks' pool
+// layout.  The graph-cut seam pass (seam_gc.cu) is declared at the end.
 #pragma once
 #include <cstdint>
 #include <vector>
@@ -80,6 +81,53 @@ __device__ __forceinline__ bool mb_roi_warp(const uint8_t* __restrict__ s, int h
   const double Wd = wp_coords(mi, sx, sy, bw, X, Y);
   wp_sample<3>(s, h, w, X, Y, v);
   return Wd != 0.0 && X >= 0 && X <= 32 * (w - 1) && Y >= 0 && Y <= 32 * (h - 1);
+}
+
+// ---- host helpers of the ROI-frame entry points ----------------------------------------------------------------------
+inline size_t mb_align(size_t v) { return (v + 255) & ~(size_t)255; }
+
+// The warp's tile width for an h x w output: tiles of up to 16 rows and 1024 pixels.
+inline int warp_tile_w(int h, int w) {
+  const int bh = h < 16 ? h : 16;
+  return 1024 / bh < w ? 1024 / bh : w;
+}
+
+// Frame k's ROI rois[k] (x_lo, y_lo, x_hi, y_hi: non-empty, inside the dst_h x dst_w canvas) -> F, with the frame's
+// pointer and size unless frames and sizes are null (the workspace-size calls leave them unset).  0 or an error.
+inline int roi_frame(const uint8_t* const* frames, const int32_t* sizes, const int32_t* rois, int k, int dst_h, int dst_w, RoiFrame& F,
+                     const char* what) {
+  const int* r = rois + 4 * k;
+  UDH_REQUIRE(r[0] >= 0 && r[1] >= 0 && r[0] < r[2] && r[1] < r[3] && r[2] <= dst_w && r[3] <= dst_h,
+              "%s: frame %d's ROI (%d, %d)..(%d, %d) is empty or leaves the %dx%d canvas", what, k, r[0], r[1], r[2], r[3], dst_h,
+              dst_w);
+  F.rx = r[0]; F.ry = r[1]; F.rw = r[2] - r[0]; F.rh = r[3] - r[1];
+  F.bw = warp_tile_w(F.rh, F.rw);
+  if (frames) {
+    UDH_REQUIRE(frames[k], "%s: frame %d is a null pointer", what, k);
+    F.src = frames[k];
+  }
+  if (sizes) {
+    F.h = sizes[2 * k];
+    F.w = sizes[2 * k + 1];
+    UDH_REQUIRE(F.h >= 1 && F.w >= 1 && F.h < 32767 && F.w < 32767, "%s: frame %d is %dx%d", what, k, F.h, F.w);
+  }
+  return UDH_OK;
+}
+
+// Copies a host table to dst on the device (pageable source: the copy is staged before this returns, so the table may go).
+template <class T>
+inline int upload(void* dst, const std::vector<T>& table, cudaStream_t st, const char* what) {
+  const cudaError_t e = cudaMemcpyAsync(dst, table.data(), table.size() * sizeof(T), cudaMemcpyHostToDevice, st);
+  if (e != cudaSuccess) {
+    set_error("%s: table copy: %s", what, cudaGetErrorString(e));
+    return UDH_ECUDA;
+  }
+  return UDH_OK;
+}
+
+inline unsigned mb_blocks(int64_t px) {
+  const int64_t b = (px + 255) / 256;
+  return (unsigned)(b < 1 ? 1 : b > 4096 ? 4096 : b);
 }
 
 // ---- seam masks: every fed frame's mask on its ROI (rh x rw bytes at element offset off of a pool) ----------------------

@@ -258,7 +258,8 @@ __device__ __forceinline__ int mb_sat16(int v) { return min(max(v, -32768), 3276
 // Level 0 of every frame: the ROI warp bordered with BORDER_REFLECT, and the 0 / 256 weight with a constant 0 border.
 // gains (null: none) [n][3]: the ROI warp is exposure-compensated first, ex_apply(v, gains[k][c]), as cv2's stitcher
 // applies its compensator to the whole warped image before it feeds the blender.  A frame with a blend mask (bmask) takes
-// its weight from that mask instead of the warp's validity.
+// its weight from that mask instead of the warp's validity: mask + 1 where the mask is nonzero, cv2's CV_16S feed (255 ->
+// 256; a graded seam-scale mask weighs 2 .. 255 along its seams).
 // MAP: the ROI warp is compensated by the frame's gain map at each ROI pixel instead (gm_gains, ex_apply_f).
 template <bool MAP>
 __global__ void __launch_bounds__(256) multiband_base_kernel(const MultibandFrame* __restrict__ fr, const double* __restrict__ M,
@@ -285,8 +286,13 @@ __global__ void __launch_bounds__(256) multiband_base_kernel(const MultibandFram
     const int ix = x + ox, iy = y + oy;
     const int sx = mb_reflect(ix, rw), sy = mb_reflect(iy, rh);
     int v[3];
-    bool valid = mb_roi_warp(s, h, w, mi, sx, sy, bw, v) && ix == sx && iy == sy;
-    if (bm) valid = ix == sx && iy == sy && __ldg(bm + (int64_t)sy * rw + sx) != 0;
+    const bool valid = mb_roi_warp(s, h, w, mi, sx, sy, bw, v) && ix == sx && iy == sy;
+    int wt = valid ? 256 : 0;
+    if (bm) {
+      const int b = ix == sx && iy == sy ? __ldg(bm + (int64_t)sy * rw + sx) : 0;
+      wt = b ? b + 1 : 0;
+    }
+    Wt[off + e] = (int16_t)wt;
     if (MAP) {
       float gf[3];
       gm_gains(gmap + k, sx, sy, gf);
@@ -297,7 +303,6 @@ __global__ void __launch_bounds__(256) multiband_base_kernel(const MultibandFram
       for (int c = 0; c < 3; ++c) v[c] = ex_apply(v[c], g[c]);
     }
     G[off + e] = make_uchar4((unsigned char)v[0], (unsigned char)v[1], (unsigned char)v[2], 0);
-    Wt[off + e] = valid ? 256 : 0;
   }
 }
 
@@ -456,47 +461,6 @@ struct MultibandPlan {
   std::vector<MultibandFrame> fr;
 };
 
-static size_t mb_align(size_t v) { return (v + 255) & ~(size_t)255; }
-
-// The warp's tile width for an h x w output: tiles of up to 16 rows and 1024 pixels.
-static int warp_tile_w(int h, int w) {
-  const int bh = h < 16 ? h : 16;
-  return 1024 / bh < w ? 1024 / bh : w;
-}
-
-// Frame k's ROI rois[k] (x_lo, y_lo, x_hi, y_hi: non-empty, inside the dst_h x dst_w canvas) -> F, with the frame's
-// pointer and size unless frames and sizes are null (the workspace-size calls leave them unset).  0 or an error.
-static int roi_frame(const uint8_t* const* frames, const int32_t* sizes, const int32_t* rois, int k, int dst_h, int dst_w, RoiFrame& F,
-                     const char* what) {
-  const int* r = rois + 4 * k;
-  UDH_REQUIRE(r[0] >= 0 && r[1] >= 0 && r[0] < r[2] && r[1] < r[3] && r[2] <= dst_w && r[3] <= dst_h,
-              "%s: frame %d's ROI (%d, %d)..(%d, %d) is empty or leaves the %dx%d canvas", what, k, r[0], r[1], r[2], r[3], dst_h,
-              dst_w);
-  F.rx = r[0]; F.ry = r[1]; F.rw = r[2] - r[0]; F.rh = r[3] - r[1];
-  F.bw = warp_tile_w(F.rh, F.rw);
-  if (frames) {
-    UDH_REQUIRE(frames[k], "%s: frame %d is a null pointer", what, k);
-    F.src = frames[k];
-  }
-  if (sizes) {
-    F.h = sizes[2 * k];
-    F.w = sizes[2 * k + 1];
-    UDH_REQUIRE(F.h >= 1 && F.w >= 1 && F.h < 32767 && F.w < 32767, "%s: frame %d is %dx%d", what, k, F.h, F.w);
-  }
-  return UDH_OK;
-}
-
-// Copies a host table to dst on the device (pageable source: the copy is staged before this returns, so the table may go).
-template <class T>
-static int upload(void* dst, const std::vector<T>& table, cudaStream_t st, const char* what) {
-  const cudaError_t e = cudaMemcpyAsync(dst, table.data(), table.size() * sizeof(T), cudaMemcpyHostToDevice, st);
-  if (e != cudaSuccess) {
-    set_error("%s: table copy: %s", what, cudaGetErrorString(e));
-    return UDH_ECUDA;
-  }
-  return UDH_OK;
-}
-
 // rois [n,4] (x_lo, y_lo, x_hi, y_hi) -> plan (frames and sizes may be null: the frame fields are left unset).  0 or an error.
 static int mb_plan(const uint8_t* const* frames, const int32_t* rois, const int32_t* sizes, int n, int Hc, int Wc, int bands,
                    MultibandPlan& p) {
@@ -550,11 +514,6 @@ static int mb_plan(const uint8_t* const* frames, const int32_t* rois, const int3
   }
   p.total = o;
   return UDH_OK;
-}
-
-static unsigned mb_blocks(int64_t px) {
-  const int64_t b = (px + 255) / 256;
-  return (unsigned)(b < 1 ? 1 : b > 4096 ? 4096 : b);
 }
 
 // ---- exposure compensation: per-pair statistics of the ROI warps (cv2.detail's gain compensators; oracle/exposure.py) ----

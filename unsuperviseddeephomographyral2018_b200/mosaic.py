@@ -2,7 +2,7 @@
 canvas, and blend every frame onto it on the GPU (udh_mosaic_blend_u8, or udh_mosaic_multiband_u8 across frequency bands).
 
     out = build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None, blend="feather", bands=5,
-                       compensate="none", compensate_feeds=1, seam="none")
+                       compensate="none", compensate_feeds=1, seam="none", seam_megapix=None)
     out["mosaic"], out["mask"], out["M"], out["kept"], out["H_pairs"], out["gains"], out["last_ms"]
 
 frames are CUDA uint8 RGB [h_k,w_k,3] tensors in sequence order (sizes may differ); est is an align.HomographyEstimator.
@@ -45,7 +45,19 @@ frame's region.  The compensator still sees the un-seamed masks, as in cv2's sti
 one's region gets nothing (cv2's result).  seam="gc_color" cuts each overlap as cv2.detail's GraphCutSeamFinder
 (COST_COLOR) does instead (oracle/seam_gc.py): along the minimum cut of a graph whose edges cost the two warps' squared
 colour difference, so the seam runs where the frames agree rather than where geometry puts it.
+
+Seam scale, seam_megapix=m (default None: full resolution).  As cv2's stitcher (stitching_detailed's --seam_megapix,
+Stitcher::setSeamEstimationResol), the seams are found on the frames scaled by a = min(1, sqrt(m 1e6 / area of frame 0))
+(seam_scale; oracle/seam_scale.py states the rule): each frame resized by a with INTER_LINEAR_EXACT, the finder on the
+pixel-centre conjugates C(a) M_k C(a)^-1 over a ceil(a Hc) x ceil(a Wc) seam canvas (seam_geometry), and each frame's
+dilated seam mask sampled back at its full-resolution canvas positions, AND its validity: graded blend masks.  The
+multi-band blend weighs a frame mask + 1 there (cv2's feed), the feathered one keeps it where the mask is nonzero.  The
+finder's cost falls with a^2: the graph-cut finder becomes usable on camera-size sweeps.  The seam-scale frames cover up
+to about 1 / (2a) px less at each edge, so a few valid pixels at the mosaic's outer border can get no weight (mask 0
+there, as in cv2).  a = 1 is the full-resolution path.
 """
+import math
+
 import numpy as np
 
 MAX_SIDE = 32766                 # udh_mosaic_blend_u8 takes canvas sides below 32767
@@ -147,12 +159,38 @@ def farthest_frame(sizes, G, kept, ref):
     return far
 
 
+def seam_scale(sizes, megapix):
+    """cv2's seam scale: a = min(1, sqrt(megapix 1e6 / (h0 w0))) of the first frame's size (h0, w0)."""
+    h0, w0 = sizes[0]
+    if not megapix > 0:
+        raise ValueError("seam_megapix must be > 0 (got %r)" % (megapix,))
+    return min(1.0, math.sqrt(float(megapix) * 1e6 / (float(h0) * float(w0))))
+
+
+def centre_map(a):
+    """C(a): a pixel centre -> the centre it maps to in an image resized by a (cv2.resize's own sampling map)."""
+    return np.array([[a, 0.0, a / 2.0 - 0.5], [0.0, a, a / 2.0 - 0.5], [0.0, 0.0, 1.0]])
+
+
+def seam_geometry(M, sizes, Hc, Wc, a):
+    """M [n,3,3] (frame k -> canvas), sizes [(h_k, w_k)] -> (M^s [n,3,3] = C(a) M_k C(a)^-1, the resized frames' sizes
+    [(rint(a h_k), rint(a w_k))], the seam canvas (ceil(a Hc), ceil(a Wc))).  ValueError for a frame resized to nothing."""
+    C = centre_map(a)
+    Ci = np.linalg.inv(C)
+    Ms = np.stack([C @ Mk @ Ci for Mk in np.asarray(M, np.float64).reshape(-1, 3, 3)])
+    small = [(int(np.rint(h * a)), int(np.rint(w * a))) for h, w in sizes]
+    for k, (h, w) in enumerate(small):
+        if h < 1 or w < 1:
+            raise ValueError("frame %d (%dx%d) is empty at seam scale %.17g" % (k, sizes[k][0], sizes[k][1], a))
+    return Ms, small, (int(math.ceil(a * Hc)), int(math.ceil(a * Wc)))
+
+
 COMPENSATE = ("none", "gain", "channels", "gain_blocks", "channels_blocks")
 SEAM = ("none", "voronoi", "gc_color")
 
 
 def build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None, float32_M=False, blend="feather", bands=5,
-                 compensate="none", compensate_feeds=1, seam="none", compensate_block=32):
+                 compensate="none", compensate_feeds=1, seam="none", compensate_block=32, seam_megapix=None):
     """est: align.HomographyEstimator; frames: CUDA uint8 RGB [h_k,w_k,3] tensors in sequence order.  blend: "feather"
     (udh_mosaic_blend_u8 with `feather`) or "multiband" (udh_mosaic_multiband_u8 with `bands`).  refine: None, or a
     dict of est.refine's keyword arguments (levels, iters, eps, max_side) to refine each pair's H.  max_pixels: the canvas
@@ -161,12 +199,14 @@ def build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None
     (ops.mosaic_exposure_gains with compensate_feeds feeds, applied by the blend), or "gain_blocks" / "channels_blocks"
     (ops.mosaic_exposure_gain_maps with blocks of about compensate_block px: a gain map per frame, cv2's
     BlocksGainCompensator / BlocksChannelsCompensator; gains stay 1).  seam: "none", "voronoi" or "gc_color"
-    (ops.mosaic_seam_masks' finder; each frame blends only inside its blend mask).
+    (ops.mosaic_seam_masks' finder; each frame blends only inside its blend mask).  seam_megapix: None (full resolution)
+    or m > 0, the seams found at seam_scale(sizes, m) (a seam is needed).
     -> dict(mosaic uint8 [Hc,Wc,3] RGB, mask uint8 [Hc,Wc], M [N,3,3] frame k -> canvas (float64, float32 values with
     float32_M), kept bool [N], ref, H_pairs [N-1,3,3], refine (rho, status, level_reached) or None, gains float64 [N,3]
     (1 for a dropped frame, all 1 without per-frame compensation), gain_maps [N] (the block modes only: CUDA float32
-    maps, None for a dropped frame or one whose ROI misses the canvas), last_ms {prep, forward, refine, compensate, seam, blend} of
-    CUDA-event time; compensate only when compensating, seam only with seams)."""
+    maps, None for a dropped frame or one whose ROI misses the canvas), seam_scale (a; 1 at full resolution), last_ms {prep,
+    forward, refine, compensate, seam, blend} of CUDA-event time; compensate only when compensating, seam only with seams,
+    covering the resize, the finder and the upscale at a seam scale)."""
     frames = list(frames)
     if len(frames) < 2:
         raise ValueError("a mosaic needs at least two frames (got %d)" % len(frames))
@@ -190,6 +230,9 @@ def build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None
         raise ValueError("compensate must be one of %s (got %r)" % (", ".join(COMPENSATE), compensate))
     if seam not in SEAM:
         raise ValueError("seam must be one of %s (got %r)" % (", ".join(SEAM), seam))
+    if seam_megapix is not None and seam == "none":
+        raise ValueError("seam_megapix needs a seam finder")
+    a = 1.0 if seam_megapix is None else seam_scale(sizes, seam_megapix)
     gains = np.ones((len(frames), 3))
     gain_maps = None
     if compensate in ("gain", "channels"):
@@ -199,11 +242,11 @@ def build_mosaic(est, frames, ref=None, refine=None, feather=64, max_pixels=None
                                                              compensate_block)
     masks = None
     if seam != "none":
-        masks, ms["seam"] = seam_kept(frames, M, kept, Hc, Wc, seam)
+        masks, ms["seam"] = seam_kept(frames, M, kept, Hc, Wc, seam, a)
     mosaic, mask, ms["blend"] = blend_kept(frames, M, kept, Hc, Wc, feather, blend, bands,
                                            gains if compensate in ("gain", "channels") else None, masks,
                                            None if gain_maps is None else [gain_maps[k] for k in range(len(frames)) if kept[k]])
-    out = dict(mosaic=mosaic, mask=mask, M=M, kept=kept, ref=ref, H_pairs=H, refine=refined, gains=gains, last_ms=ms)
+    out = dict(mosaic=mosaic, mask=mask, M=M, kept=kept, ref=ref, H_pairs=H, refine=refined, gains=gains, seam_scale=a, last_ms=ms)
     if gain_maps is not None:
         out["gain_maps"] = gain_maps
     return out
@@ -247,15 +290,15 @@ def compensate_blocks_kept(frames, M, kept, Hc, Wc, mode, feeds=1, block=32):
     return maps, e0.elapsed_time(e1)
 
 
-def seam_kept(frames, M, kept, Hc, Wc, finder="voronoi"):
-    """The kept frames' blend masks (ops.mosaic_seam_masks with finder) -> (masks [n_kept]: CUDA uint8 [roi_h,roi_w], None for a frame
-    whose ROI misses the canvas; CUDA-event ms)."""
+def seam_kept(frames, M, kept, Hc, Wc, finder="voronoi", scale=1.0):
+    """The kept frames' blend masks (ops.mosaic_seam_masks with finder at scale) -> (masks [n_kept]: CUDA uint8 [roi_h,roi_w],
+    None for a frame whose ROI misses the canvas; CUDA-event ms)."""
     import torch
     from . import ops
     take = [k for k in range(len(frames)) if kept[k]]
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
-    s = ops.mosaic_seam_masks([frames[k].contiguous() for k in take], np.asarray(M)[take], Hc, Wc, finder)
+    s = ops.mosaic_seam_masks([frames[k].contiguous() for k in take], np.asarray(M)[take], Hc, Wc, finder, scale)
     e1.record()
     e1.synchronize()
     masks = [None] * len(take)

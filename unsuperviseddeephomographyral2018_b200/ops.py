@@ -360,6 +360,52 @@ def resize_linear_u8(src, dst_h, dst_w):
     return out
 
 
+def linear_exact_table(src_h, src_w, dst_h, dst_w, scale=None):
+    """udh_resize_linear_exact_u8's table (int32): xs0, xs1, xc1, ys0, ys1, yc1 - cv2's INTER_LINEAR_EXACT taps (the rule:
+    oracle/seam_scale.py): per axis the sampling scale is 1 / scale (cv2.resize's fx / fy form) or src / dst (its dsize
+    form), f = (d + 0.5) * that - 0.5 in float64, s = floor(f), c1 = rint((f - s) * 256) (ties to even), taps (s, s + 1),
+    both on pixel 0 when s < 0 and on pixel size - 1 when s + 1 > size - 1.  An output of the source's size is a copy (cv2's
+    rule), the identity table."""
+    def axis(n, N, inv):
+        f = (np.arange(N, dtype=np.float64) + 0.5) * (1.0 / inv) - 0.5
+        s = np.floor(f)
+        c1 = np.rint((f - s) * 256.0)
+        s = s.astype(np.int64)
+        lo, hi = s < 0, s + 1 > n - 1
+        return [np.where(lo, 0, np.where(hi, n - 1, s)), np.where(lo, 0, np.where(hi, n - 1, s + 1)), c1]
+    if min(src_h, src_w, dst_h, dst_w) < 1:
+        raise _lib.UdhError("linear_exact_table: sizes must be >= 1 (got %dx%d -> %dx%d)" % (src_h, src_w, dst_h, dst_w))
+    ix = float(scale) if scale is not None else dst_w / float(src_w)
+    iy = float(scale) if scale is not None else dst_h / float(src_h)
+    if (dst_h, dst_w) == (src_h, src_w):                            # cv2 copies when the size stays, whatever fx says
+        ix = iy = 1.0
+    return np.concatenate([np.asarray(a, np.float64) for a in axis(src_w, dst_w, ix) + axis(src_h, dst_h, iy)]).astype(np.int32)
+
+
+def resize_linear_exact_u8(src, dst_h=None, dst_w=None, scale=None):
+    """uint8 [N,h,w,C] or [h,w,C] CUDA tensor (C = 1 or 3) -> [N,dst_h,dst_w,C] (or [dst_h,dst_w,C]): cv2.resize with
+    INTER_LINEAR_EXACT per image, byte for byte.  Give dst_h and dst_w (cv2.resize(img, (dst_w, dst_h), ...)) or scale
+    (cv2.resize(img, None, fx=scale, fy=scale, ...): the sides are rint(side * scale) and the sampling scale is 1 / scale,
+    which differs from the dsize form's side / dst).  One launch."""
+    _req(src, torch.uint8, "src")
+    batched = src.dim() == 4
+    if src.dim() not in (3, 4) or src.shape[-1] not in (1, 3):
+        raise _lib.UdhError("resize_linear_exact_u8: src must be [N,h,w,C] or [h,w,C] with C = 1 or 3 (got %s)" % (tuple(src.shape),))
+    x = src if batched else src[None]
+    n, h, w, C = (int(v) for v in x.shape)
+    if (scale is None) == (dst_h is None or dst_w is None) or (scale is not None and (dst_h is not None or dst_w is not None)):
+        raise _lib.UdhError("resize_linear_exact_u8: give dst_h and dst_w, or scale")
+    if scale is not None:
+        if not float(scale) > 0:
+            raise _lib.UdhError("resize_linear_exact_u8: scale must be > 0 (got %r)" % (scale,))
+        dst_h, dst_w = int(np.rint(h * float(scale))), int(np.rint(w * float(scale)))
+    tab = torch.from_numpy(linear_exact_table(h, w, int(dst_h), int(dst_w), scale)).to(src.device)
+    out = torch.empty(n, int(dst_h), int(dst_w), C, device=src.device, dtype=torch.uint8)
+    check(lib.udh_resize_linear_exact_u8(_ptr(x), _ptr(tab), _ptr(out), n, h, w, C, int(dst_h), int(dst_w), _stream()),
+          "udh_resize_linear_exact_u8")
+    return out if batched else out[0]
+
+
 def real_prep(I_u8, Ip_u8, luts, img_h, img_w):
     """Full-size uint8 I, I' [B,FH,FW,3] and per-sample value tables luts [B,4,256,3] fp32 (plain I, plain I', augmented I,
     augmented I') -> (I, I_prime, I_aug, I_prime_aug) [B,img_h,img_w,3] fp32: table lookup, then cv2's INTER_AREA
@@ -1239,7 +1285,7 @@ def _gain_map_table(gain_maps, rois, n, dev, what):
 SEAM_FINDERS = ("voronoi", "gc_color")
 
 
-def mosaic_seam_masks(frames, M, dst_h, dst_w, finder="voronoi"):
+def mosaic_seam_masks(frames, M, dst_h, dst_w, finder="voronoi", scale=1.0):
     """frames: n CUDA uint8 RGB tensors [h_k,w_k,3], M float64 [n,3,3] (frame k -> canvas) -> dict(take (the fed frames:
     those whose ROI meets the canvas), rois int64 [n,4] (mosaic.multiband_rois), seam [m], blend [m]): per fed frame its
     seam mask and blend mask, CUDA uint8 [roi_h,roi_w] (0 / 255), and cv2.dilate of that AND the validity, the mask cv2's
@@ -1248,9 +1294,18 @@ def mosaic_seam_masks(frames, M, dst_h, dst_w, finder="voronoi"):
     another one's seam region vanishes (an all-zero mask), as in cv2.  finder "gc_color": cv2.detail's
     GraphCutSeamFinder(COST_COLOR) on the uncompensated ROI warps, as the canonical minimum cut of each pair's window
     (udh_mosaic_seam_gc_masks_u8; oracle/seam_gc.py states the rule), with cut int64 [pairs]: each pair's cut value, the
-    pairs in cv2's visiting order."""
+    pairs in cv2's visiting order.
+    scale a < 1 (mosaic.seam_scale: cv2's seam_megapix) finds the seams at reduced resolution (oracle/seam_scale.py): the
+    frames resized by a (resize_linear_exact_u8), the finder on mosaic.seam_geometry's maps and seam canvas, and each seam
+    mask upscaled to the full ROI (udh_mosaic_seam_upscale_u8): blend [m] on the full ROIs, graded (1 .. 254 along the
+    seams), seam [m] each fed frame's seam mask on its seam ROI ([0,0] where that misses the seam canvas), seam_rois int64
+    [n,4] and scale; cut is the seam-scale finder's."""
     if finder not in SEAM_FINDERS:
         raise ValueError("finder must be one of %s (got %r)" % (", ".join(SEAM_FINDERS), finder))
+    if not 0.0 < float(scale) <= 1.0:
+        raise ValueError("scale must be in (0, 1] (got %r)" % (scale,))
+    if float(scale) < 1.0:
+        return _scaled_seam_masks(frames, M, dst_h, dst_w, finder, float(scale))
     gc = finder == "gc_color"
     fed = _Fed(frames, M, dst_h, dst_w, "mosaic_seam_masks", _lib.EXPOSURE_MAX_FRAMES)
     out = dict(take=fed.take, rois=fed.rois, seam=[], blend=[])
@@ -1284,6 +1339,45 @@ def mosaic_seam_masks(frames, M, dst_h, dst_w, finder="voronoi"):
         h, w = (int(v) for v in hw[k])
         out["seam"].append(seam[off[k]:off[k + 1]].view(h, w))
         out["blend"].append(blend[off[k]:off[k + 1]].view(h, w))
+    return out
+
+
+def _scaled_seam_masks(frames, M, dst_h, dst_w, finder, a):
+    """mosaic_seam_masks at scale a < 1."""
+    from . import mosaic
+    what = "mosaic_seam_masks"
+    frames, Mh, sizes = _frames_and_M(frames, M, what, (3,))
+    Ms, _, (Hs, Ws) = mosaic.seam_geometry(Mh, sizes, int(dst_h), int(dst_w), a)
+    found = mosaic_seam_masks([resize_linear_exact_u8(f, scale=a) for f in frames], Ms, Hs, Ws, finder)
+    fed = _Fed(frames, Mh, dst_h, dst_w, what, _lib.SEAM_MAX_FRAMES)
+    out = dict(take=fed.take, rois=fed.rois, seam=[], blend=[], seam_rois=found["rois"], scale=a)
+    if "cut" in found:
+        out["cut"] = found["cut"]
+    if not fed.m:
+        return out
+    m, dev, rr = fed.m, fed.dev, fed.rr
+    seam_rr = np.zeros((m, 4), np.int32)
+    seam_ptrs = (ctypes.c_void_p * m)()
+    for q, k in enumerate(fed.take):
+        if k in found["take"]:
+            t = found["seam"][found["take"].index(k)]
+            seam_rr[q] = found["rois"][k]
+            seam_ptrs[q] = t.data_ptr()
+        else:
+            t = torch.zeros((0, 0), device=dev, dtype=torch.uint8)
+        out["seam"].append(t)
+    area = (rr[:, 2] - rr[:, 0]).astype(np.int64) * (rr[:, 3] - rr[:, 1])
+    off = np.concatenate([[0], np.cumsum(area)])
+    blend = torch.empty(int(off[-1]), device=dev, dtype=torch.uint8)
+    nb = lib.udh_mosaic_seam_upscale_workspace_bytes(rr.ctypes.data, seam_rr.ctypes.data, m, Hs, Ws, a, int(dst_h), int(dst_w))
+    if nb == 0:
+        raise _lib.UdhError("%s: bad arguments (%d frames, canvas %dx%d, seam canvas %dx%d)" % (what, m, dst_h, dst_w, Hs, Ws))
+    ws = torch.empty(nb, device=dev, dtype=torch.uint8)
+    check(lib.udh_mosaic_seam_upscale_u8(fed.ptrs, fed.sz.ctypes.data, _ptr(fed.M_d), rr.ctypes.data, seam_ptrs, seam_rr.ctypes.data, m,
+                                         Hs, Ws, a, int(dst_h), int(dst_w), _ptr(blend), _ptr(ws), nb, _stream()),
+          "udh_mosaic_seam_upscale_u8")
+    for k in range(m):
+        out["blend"].append(blend[off[k]:off[k + 1]].view(int(rr[k, 3] - rr[k, 1]), int(rr[k, 2] - rr[k, 0])))
     return out
 
 
